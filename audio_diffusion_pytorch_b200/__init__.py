@@ -1,5 +1,5 @@
-"""audio_diffusion_pytorch on B200: the reference's public names (reference __init__.py:1-20)
-for the UNetV0 + VDiffusion/VSampler hot path, executed by hand-written sm_100a kernels.
+"""audio_diffusion_pytorch on H100: the reference's public names (reference __init__.py:1-20)
+for the UNetV0 + VDiffusion/VSampler hot path, executed by hand-written sm_90a kernels.
 
 Every name of the reference's export list is implemented; what is not supported inside one
 (`use_text_conditioning=True`: T5 weights) raises on use instead of silently running something else."""

@@ -1,4 +1,4 @@
-"""Builds libadp_b200.so (sm_100a only) in-tree with nvcc.  No torch involvement: the
+"""Builds libadp_b200.so (sm_90a only) in-tree with nvcc.  No torch involvement: the
 library is a plain C-ABI shared object (include/adp_b200.h) loaded through ctypes."""
 import os
 import subprocess
@@ -10,7 +10,7 @@ CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libadp_b200.so")
 SOURCES = ["common.cu", "conv_gemm.cu", "rowwise.cu", "stem.cu", "mid_conv.cu", "attention.cu", "attention_bwd.cu", "backward.cu", "wgrad.cu", "stem_bwd.cu", "frontend.cu", "verify_f32.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",
 ]
 
@@ -57,7 +57,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     with ThreadPoolExecutor(max_workers=8) as ex:
         objs = list(ex.map(compile_one, _sources()))
-    cmd = [nvcc, "-shared", "-o", LIB_PATH, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [nvcc, "-shared", "-o", LIB_PATH, *objs, "-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -1,7 +1,7 @@
 """ctypes binding of libadp_b200.so (C ABI declared in include/adp_b200.h).
 
 There is deliberately no fallback: if the shared library is missing or the device is not
-sm_100 the product path raises.  Nothing under oracle/ is imported here.
+sm_90 the product path raises.  Nothing under oracle/ is imported here.
 """
 import ctypes as C
 import os

@@ -10,7 +10,7 @@ from .utils import default
 
 
 class _Appended(nn.Module):
-    """Generic AppendChannelsPlugin for a net that is not the B200 U-Net: concatenate, call."""
+    """Generic AppendChannelsPlugin for a net that is not the CUDA U-Net: concatenate, call."""
 
     def __init__(self, net: nn.Module):
         super().__init__()
@@ -21,7 +21,7 @@ class _Appended(nn.Module):
 
 
 def AppendChannelsPlugin(net_t: Callable, channels: int):
-    """reference components.py:162-180.  With the B200 U-Net the concatenation is never
+    """reference components.py:162-180.  With the CUDA U-Net the concatenation is never
     materialised: the stem kernels read `x` and `append_channels` through two base pointers."""
 
     def Net(in_channels: int, out_channels: Optional[int] = None, **kwargs) -> nn.Module:
@@ -50,7 +50,7 @@ def LTPlugin(net_t: Callable, num_filters: int, window_length: int, stride: int)
     """Learned Transform plugin (reference components.py:113-157): a strided learned filterbank
     (Conv1d, reflect padding, bias-free) in front of the net and its transposed counterpart behind
     it; the net runs on `in_channels * num_filters` channels at 1/stride of the rate.  The two
-    filterbank convolutions are PyTorch modules around the net call; with the B200 U-Net inside, its
+    filterbank convolutions are PyTorch modules around the net call; with the CUDA U-Net inside, its
     stem limits apply to the TRANSFORMED widths (in_channels * num_filters <= 8 inputs,
     out_channels * num_filters <= 4 outputs) and are asserted by its constructor."""
 

@@ -1,14 +1,12 @@
-// adp_attention: softmax(q k^T * scale) v, head dim 64, on tcgen05 (a_unet AttentionBase).
+// adp_attention: softmax(q k^T * scale) v, head dim 64, on wgmma (a_unet AttentionBase).
 //
-// One CTA = one (batch, head, 128-query tile); two CTAs are resident per SM so one CTA's
-// softmax overlaps the other's MMAs.  S = Q K^T (128 x 128 keys) and O (128 x 64) accumulate
-// in TMEM.  Each query row is owned by TWO softmax threads (same TMEM lane, one per 64-key
-// half), so the online softmax needs no shuffles: the halves exchange their row max through
-// shared memory once per key tile and their row sums once at the end.
-//   warps 0-7: softmax     S(TMEM, read once) -> max -> ex2 -> P(bf16, swizzled smem);
-//                          O(TMEM) rescaled only when a row max actually moved
-//   warp 8   : TMA producer  Q once; K double-buffered; V single-buffered (it is needed last)
-//   warp 9   : MMA issuer    S = Q K_j^T ; (wait P) ; O += P_j V_j
+// One CTA = one (batch, head, 128-query tile).  Two consumer warpgroups own 64 query rows each:
+// S = Q K_j^T (64 x 128 keys) accumulates in registers, the online softmax runs on the
+// accumulator fragments (a row is spread over the four lanes of a quad: two shuffles per
+// reduction), and P is converted to bf16 in registers and fed straight back as the A operand
+// of O += P V_j (the fp32 accumulator layout of a 64 x 16 slice is the bf16 A-fragment layout).
+//   warps 0-7: consumers   S = Q K^T -> max -> ex2 -> P (registers) -> O += P V
+//   warp 8   : TMA producer  Q once; K and V double-buffered
 // K is the K-major B operand of the first GEMM (keys x d); V is used in place as the
 // MN-major B operand of the second (d contiguous per key), so no transpose is materialised.
 #include "common.cuh"
@@ -21,10 +19,8 @@ constexpr int kKT = 128;       // keys per tile
 constexpr int kD = 64;         // head dim
 constexpr int kQBytes = kQT * kD * 2;          // 16 KB
 constexpr int kKVBytes = kKT * kD * 2;         // 16 KB
-constexpr int kPBytes = kQT * kKT * 2;         // 32 KB (two 64-key swizzle chunks)
-constexpr int kAttnSmem = kQBytes + 2 * kKVBytes + kKVBytes + kPBytes + 1024;   // 97 KB
-constexpr uint32_t kTmemCols = 256;            // S: [0,128)  O: [128,192)
-constexpr int kSoftmaxThreads = 256;
+constexpr int kAttnSmem = kQBytes + 4 * kKVBytes + 1024;   // Q + 2 x (K, V): 81 KB
+constexpr int kAttnThreads = 288;
 
 struct AttnParams {
   __nv_bfloat16* o;
@@ -39,14 +35,11 @@ __device__ __forceinline__ float ex2_approx(float x) {
   return y;
 }
 
-__global__ void __launch_bounds__(320, 2)
+__global__ void __launch_bounds__(kAttnThreads, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                  const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint64_t q_full, s_full, p_full, o_done, v_full, v_empty;
-  __shared__ uint64_t k_full[2], k_empty[2];
-  __shared__ uint32_t tmem_slot;
-  __shared__ float s_xch[2][kQT];
+  __shared__ uint64_t q_full, kv_full[2], kv_empty[2];
 
   pdl_launch_dependents();
   const int warp = warp_id_uniform();
@@ -55,37 +48,23 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   uint8_t* base = smem_raw + ((1024u - (raw & 1023u)) & 1023u);
   uint8_t* q_s = base;
   uint8_t* k_s = q_s + kQBytes;            // [2][16 KB]
-  uint8_t* v_s = k_s + 2 * kKVBytes;       // 16 KB
-  uint8_t* p_s = v_s + kKVBytes;           // 32 KB
+  uint8_t* v_s = k_s + 2 * kKVBytes;       // [2][16 KB]
 
   const int t0 = blockIdx.x * kQT;
   const int h = blockIdx.y;
   const int b = blockIdx.z;
   const int n_tiles = (p.Tk + kKT - 1) / kKT;
 
-  if (warp == 8) {
-    tmem_alloc(&tmem_slot, kTmemCols);
-    tmem_relinquish();
-  } else if (warp == 9 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     mbar_init(&q_full, 1);
-    mbar_init(&s_full, 1);
-    mbar_init(&p_full, kSoftmaxThreads);
-    mbar_init(&o_done, 1);
-    mbar_init(&v_full, 1);
-    mbar_init(&v_empty, 1);
-    for (int s = 0; s < 2; ++s) { mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], 1); }
+    for (int s = 0; s < 2; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 8); }
     fence_mbar_init();
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, tmem_slot, 0);   // warp-uniform for ptxas
-  const uint32_t tmem_s = tmem_base;
   pdl_wait();
-  const uint32_t tmem_o = tmem_base + 128;
 
   if (warp == 8) {
     // whole warp runs the loop (uniform control flow), one elected lane issues: see ptx.cuh
@@ -96,156 +75,112 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     __syncwarp();
     for (int j = 0; j < n_tiles; ++j) {
       const int s = j & 1;
-      mbar_wait(&k_empty[s], ((j >> 1) & 1) ^ 1);
+      mbar_wait(&kv_empty[s], ((j >> 1) & 1) ^ 1);
       if (elect_one()) {
-        mbar_arrive_expect_tx(&k_full[s], kKVBytes);
-        tma_load_3d(k_s + s * kKVBytes, &tmK, &k_full[s], h * kD, j * kKT, b);
-      }
-      __syncwarp();
-      mbar_wait(&v_empty, (j & 1) ^ 1);
-      if (elect_one()) {
-        mbar_arrive_expect_tx(&v_full, kKVBytes);
-        tma_load_3d(v_s, &tmV, &v_full, h * kD, j * kKT, b);
+        mbar_arrive_expect_tx(&kv_full[s], 2 * kKVBytes);
+        tma_load_3d(k_s + s * kKVBytes, &tmK, &kv_full[s], h * kD, j * kKT, b);
+        tma_load_3d(v_s + s * kKVBytes, &tmV, &kv_full[s], h * kD, j * kKT, b);
       }
       __syncwarp();
     }
-  } else if (warp == 9) {
-    constexpr uint32_t idesc_qk = umma_idesc_bf16(kQT, kKT, 0, 0);
-    constexpr uint32_t idesc_pv = umma_idesc_bf16(kQT, kD, 0, 1);   // B (= V) is MN-major
-    mbar_wait(&q_full, 0);
-    const uint64_t q_desc = umma_desc_kmajor<128>(smem_u32(q_s));
-    const uint64_t p_desc = umma_desc_kmajor<128>(smem_u32(p_s));
-    const uint64_t v_desc = umma_desc_mnmajor_sw128(smem_u32(v_s), 1024);
-    for (int j = 0; j < n_tiles; ++j) {
-      const int s = j & 1;
-      mbar_wait(&k_full[s], (j >> 1) & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t k_desc = umma_desc_kmajor<128>(smem_u32(k_s + s * kKVBytes));
-#pragma unroll
-        for (int kk = 0; kk < kD / 16; ++kk)
-          umma_bf16(tmem_s, q_desc + ((kk * 32) >> 4), k_desc + ((kk * 32) >> 4), idesc_qk, kk != 0);
-        umma_commit(&s_full);
-        umma_commit(&k_empty[s]);
-      }
-      __syncwarp();
-      mbar_wait(&p_full, j & 1);
-      mbar_wait(&v_full, j & 1);
-      tc_fence_after();
-      if (elect_one()) {
-#pragma unroll
-        for (int kk = 0; kk < kKT / 16; ++kk)
-          umma_bf16(tmem_o, p_desc + (((kk >> 2) * (kQT * 128) + (kk & 3) * 32) >> 4),
-                    v_desc + ((kk * 16 * 128) >> 4), idesc_pv, (j | kk) != 0);
-        umma_commit(&v_empty);
-        if (j == n_tiles - 1) umma_commit(&o_done);
-      }
-      __syncwarp();
-    }
-  } else {
-    // ------------------------------------------------------------- softmax / epilogue
-    const int half = warp >> 2;                  // which 64 keys of the tile / 32 columns of O
-    const int row = (warp & 3) * 32 + lane;
-    const uint32_t lane_off = static_cast<uint32_t>((warp & 3) * 32) << 16;
-    float m_run = -INFINITY, l_run = 0.f;
-    for (int j = 0; j < n_tiles; ++j) {
-      mbar_wait(&s_full, j & 1);
-      tc_fence_after();
-      const int key0 = j * kKT + half * 64;
-      uint32_t r[64];
-      {
-        uint32_t (&r0)[32] = *reinterpret_cast<uint32_t (*)[32]>(&r[0]);
-        uint32_t (&r1)[32] = *reinterpret_cast<uint32_t (*)[32]>(&r[32]);
-        tmem_ld32(tmem_s + lane_off + half * 64, r0);
-        tmem_ld32(tmem_s + lane_off + half * 64 + 32, r1);
-        tmem_ld_wait();
-      }
-      float m_loc = -INFINITY;
-      if (key0 + 64 <= p.Tk) {
-#pragma unroll
-        for (int i = 0; i < 64; ++i) m_loc = fmaxf(m_loc, __uint_as_float(r[i]));
-      } else {
-#pragma unroll
-        for (int i = 0; i < 64; ++i) {
-          if (key0 + i >= p.Tk) r[i] = 0xff800000u;   // -inf: key outside the sequence
-          m_loc = fmaxf(m_loc, __uint_as_float(r[i]));
-        }
-      }
-      s_xch[half][row] = m_loc;
-      named_bar_sync(2, kSoftmaxThreads);
-      const float m_new = fmaxf(m_run, fmaxf(m_loc, s_xch[half ^ 1][row]));
-      const float alpha = ex2_approx((m_run - m_new) * p.scale_log2);   // 0 on the first tile
-      const float m_scaled = m_new * p.scale_log2;
-      // rescale the running output only if some row of this warp moved its max (the previous
-      // P V is complete: s_full is committed after it)
-      if (j > 0 && __any_sync(0xffffffffu, m_new > m_run)) {
-        uint32_t o[32];
-        tmem_ld32(tmem_o + lane_off + half * 32, o);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-        uint32_t (&o0)[16] = *reinterpret_cast<uint32_t (*)[16]>(&o[0]);
-        uint32_t (&o1)[16] = *reinterpret_cast<uint32_t (*)[16]>(&o[16]);
-        tmem_st16(tmem_o + lane_off + half * 32, o0);
-        tmem_st16(tmem_o + lane_off + half * 32 + 16, o1);
-        tmem_st_wait();
-      }
-      // p = 2^(s*c - m*c) -> bf16 -> swizzled smem chunk `half` (K-major A operand of P V)
-      float l_tile = 0.f;
-      uint8_t* prow = p_s + half * (kQT * 128) + row * 128;
-#pragma unroll
-      for (int piece = 0; piece < 8; ++piece) {
-        uint32_t pk[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float p0 = ex2_approx(__uint_as_float(r[piece * 8 + 2 * i]) * p.scale_log2 - m_scaled);
-          const float p1 = ex2_approx(__uint_as_float(r[piece * 8 + 2 * i + 1]) * p.scale_log2 - m_scaled);
-          pk[i] = pack_bf16(p0, p1);
-          const float2 pr = unpack_bf16(pk[i]);   // sum what the MMA will actually see
-          l_tile += pr.x + pr.y;
-        }
-        *reinterpret_cast<uint4*>(prow + ((piece ^ (row & 7)) << 4)) =
-            make_uint4(pk[0], pk[1], pk[2], pk[3]);
-      }
-      l_run = l_run * alpha + l_tile;
-      m_run = m_new;
-      fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive(&p_full);
-    }
-    // total row sum = sum of the two halves
-    mbar_wait(&o_done, 0);
-    tc_fence_after();
-    s_xch[half][row] = l_run;
-    named_bar_sync(2, kSoftmaxThreads);
-    const float l_tot = l_run + s_xch[half ^ 1][row];
-    const float inv_l = 1.f / l_tot;
-    const int t = t0 + row;
-    if (p.lse != nullptr && half == 0 && t < p.Tq)    // natural-log units (adp_attention_bwd)
-      p.lse[(static_cast<size_t>(b) * gridDim.y + h) * p.Tq + t] =
-          (m_run * p.scale_log2 + log2f(l_tot)) * 0.6931471805599453f;
-    uint32_t o[32];
-    tmem_ld32(tmem_o + lane_off + half * 32, o);
-    tmem_ld_wait();
-    if (t < p.Tq) {
-      __nv_bfloat16* orow = p.o + (static_cast<size_t>(b) * p.Tq + t) * p.ldo + h * kD + half * 32;
-#pragma unroll
-      for (int c = 0; c < 32; c += 8) {
-        uint4 ov;
-        ov.x = pack_bf16(__uint_as_float(o[c]) * inv_l, __uint_as_float(o[c + 1]) * inv_l);
-        ov.y = pack_bf16(__uint_as_float(o[c + 2]) * inv_l, __uint_as_float(o[c + 3]) * inv_l);
-        ov.z = pack_bf16(__uint_as_float(o[c + 4]) * inv_l, __uint_as_float(o[c + 5]) * inv_l);
-        ov.w = pack_bf16(__uint_as_float(o[c + 6]) * inv_l, __uint_as_float(o[c + 7]) * inv_l);
-        *reinterpret_cast<uint4*>(orow + c) = ov;
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 8) {
+  // ------------------------------------------------------------------ consumers (softmax)
+  const int wg = threadIdx.x >> 7;
+  const int row_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // fragment rows row_lo, row_lo + 8
+  const int cq = 2 * (lane & 3);
+  const uint64_t q_desc = gmma_desc_kmajor<128>(smem_u32(q_s) + wg * 64 * 128);
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  float o[kD / 2];
+#pragma unroll
+  for (int i = 0; i < kD / 2; ++i) o[i] = 0.f;
+  mbar_wait(&q_full, 0);
+  for (int j = 0; j < n_tiles; ++j) {
+    const int s = j & 1;
+    mbar_wait(&kv_full[s], (j >> 1) & 1);
+    float sc[kKT / 2];
+    const uint64_t k_desc = gmma_desc_kmajor<128>(smem_u32(k_s + s * kKVBytes));
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kD / 16; ++kk)
+      Wgmma<kKT>::ss<0, 0>(sc, q_desc + ((kk * 32) >> 4), k_desc + ((kk * 32) >> 4), kk != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    acc_fence(sc);
+
+    const int key0 = j * kKT;
+    if (key0 + kKT > p.Tk) {
+#pragma unroll
+      for (int i = 0; i < kKT / 2; ++i)
+        if (key0 + 8 * (i >> 2) + cq + (i & 1) >= p.Tk) sc[i] = -INFINITY;   // key outside the sequence
+    }
+    float m_loc[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int i = 0; i < kKT / 2; ++i) m_loc[(i >> 1) & 1] = fmaxf(m_loc[(i >> 1) & 1], sc[i]);
+    float alpha[2], m_scaled[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      m_loc[r] = fmaxf(m_loc[r], __shfl_xor_sync(0xffffffffu, m_loc[r], 1));
+      m_loc[r] = fmaxf(m_loc[r], __shfl_xor_sync(0xffffffffu, m_loc[r], 2));
+      const float m_new = fmaxf(m_run[r], m_loc[r]);
+      alpha[r] = ex2_approx((m_run[r] - m_new) * p.scale_log2);   // 0 on the first tile
+      m_scaled[r] = m_new * p.scale_log2;
+      m_run[r] = m_new;
+    }
+    if (j > 0) {
+#pragma unroll
+      for (int i = 0; i < kD / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
+    }
+    // p = 2^(s*c - m*c) -> bf16 A fragments of P V (16 keys per fragment)
+    uint32_t pa[kKT / 16][4];
+    float l_tile[2] = {0.f, 0.f};
+#pragma unroll
+    for (int kk = 0; kk < kKT / 16; ++kk) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int i = 8 * kk + 2 * q;
+        const int r = q & 1;
+        const float p0 = ex2_approx(sc[i] * p.scale_log2 - m_scaled[r]);
+        const float p1 = ex2_approx(sc[i + 1] * p.scale_log2 - m_scaled[r]);
+        pa[kk][q] = pack_bf16(p0, p1);
+        const float2 pr = unpack_bf16(pa[kk][q]);   // sum what the MMA will actually see
+        l_tile[r] += pr.x + pr.y;
+      }
+    }
+    l_run[0] = l_run[0] * alpha[0] + l_tile[0];
+    l_run[1] = l_run[1] * alpha[1] + l_tile[1];
+
+    const uint64_t v_desc = gmma_desc_mnmajor_sw128(smem_u32(v_s + s * kKVBytes), 1024);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kKT / 16; ++kk)
+      Wgmma<kD>::rs<1>(o, pa[kk], v_desc + ((kk * 16 * 128) >> 4), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    acc_fence(o);
     __syncwarp();
-    tmem_dealloc(tmem_base, kTmemCols);
+    if (lane == 0) mbar_arrive(&kv_empty[s]);
+  }
+
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
+    l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int t = t0 + row_lo + 8 * r;
+    if (t >= p.Tq) continue;
+    const float inv_l = 1.f / l_run[r];
+    if (p.lse != nullptr && (lane & 3) == 0)    // natural-log units (adp_attention_bwd)
+      p.lse[(static_cast<size_t>(b) * gridDim.y + h) * p.Tq + t] =
+          (m_run[r] * p.scale_log2 + log2f(l_run[r])) * 0.6931471805599453f;
+    __nv_bfloat16* orow = p.o + (static_cast<size_t>(b) * p.Tq + t) * p.ldo + h * kD;
+#pragma unroll
+    for (int jb = 0; jb < kD / 8; ++jb)
+      *reinterpret_cast<uint32_t*>(orow + 8 * jb + cq) =
+          pack_bf16(o[4 * jb + 2 * r] * inv_l, o[4 * jb + 2 * r + 1] * inv_l);
   }
 }
 
@@ -290,7 +225,7 @@ extern "C" int adp_attention(const void* q, const void* k, const void* v, void* 
   p.ldo = ldo;
   p.scale_log2 = scale * 1.4426950408889634f;
   dim3 grid((Tq + kQT - 1) / kQT, H, B);
-  ADP_CUDA(launch_k(attention_kernel, grid, dim3(320), (size_t)kAttnSmem, as_stream(stream), tmQ, tmK, tmV, p));
+  ADP_CUDA(launch_k(attention_kernel, grid, dim3(kAttnThreads), (size_t)kAttnSmem, as_stream(stream), tmQ, tmK, tmV, p));
   ADP_LAUNCH_CHECK();
   return 0;
 }

@@ -10,7 +10,7 @@
 //   attn_dq_kernel      one CTA per (64 queries, head, batch), loops over the key tiles
 // Tensor cores through mma.sync.m16n8k16 (bf16 in, fp32 accumulate): the backward of attention
 // is < 2 % of a training step of the networks this library runs (N <= 1024 tokens), so this
-// kernel is written for exactness and simplicity; the forward is the tcgen05 kernel.
+// kernel is written for exactness and simplicity; the forward is the wgmma kernel.
 #include "common.cuh"
 #include "ptx.cuh"
 

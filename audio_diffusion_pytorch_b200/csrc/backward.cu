@@ -26,7 +26,7 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
 // vpr = C/8 vectors per row).  When vpr < 32 the lanes l, l+vpr, l+2vpr, ... of a warp own the
 // SAME channels: fold their partial sums with shuffles so that one lane per channel touches the
 // block's shared-memory bins (at C = 32 the unfolded version sent 64 threads to every bin and
-// the kernel ran at 5 % of HBM bandwidth, profiles/r2_train_profile_start.txt).
+// the kernel ran far below HBM bandwidth).
 __device__ __forceinline__ bool fold_ok(int vpr) { return vpr < 32 && (32 % vpr) == 0; }
 __device__ __forceinline__ float fold_lanes(float v, int vpr) {
   for (int o = vpr; o < 32; o <<= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -545,7 +545,7 @@ cond_bwd_kernel(const float* __restrict__ dss, int ld_dss, const float* __restri
 static int grid_for(size_t nvec, int B) {
   // every block ends in 2C global atomics: a few hundred blocks in total, each streaming many rows
   size_t g = (nvec + 256 * 4 - 1) / (256 * 4);
-  const size_t cap = 148 * 3 / (B < 8 ? B : 8) + 1;
+  const size_t cap = num_sms() * 3 / (B < 8 ? B : 8) + 1;
   if (g > cap) g = cap;
   if (g < 1) g = 1;
   return static_cast<int>(g);
@@ -602,8 +602,8 @@ extern "C" int adp_ln_film_bwd(const void* dy, const void* x, const float* scale
   // few rows (deep levels): one pass per warp so that every SM gets a block; many rows: persistent
   // blocks (each ends in 3C global atomics)
   const size_t g1 = (static_cast<size_t>(T) + rows_per_block - 1) / rows_per_block;
-  size_t g = g1 * B <= 148 * 2 ? g1 : (static_cast<size_t>(T) + rows_per_block * 4 - 1) / (rows_per_block * 4);
-  const size_t cap = 148 * 4 / (B < 8 ? B : 8) + 1;
+  size_t g = g1 * B <= num_sms() * 2 ? g1 : (static_cast<size_t>(T) + rows_per_block * 4 - 1) / (rows_per_block * 4);
+  const size_t cap = num_sms() * 4 / (B < 8 ? B : 8) + 1;
   if (g > cap) g = cap;
   dim3 grid(static_cast<unsigned>(g < 1 ? 1 : g), B);
   const uint4* pdy = static_cast<const uint4*>(dy);

@@ -69,6 +69,16 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
   return 0;
 }
 
+int num_sms() {
+  static int n[64] = {};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) dev = 0;
+  int& v = n[dev & 63];
+  if (v <= 0 && (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0))
+    v = 132;
+  return v;
+}
+
 }  // namespace adp
 
 extern "C" {
@@ -83,8 +93,8 @@ int adp_device_check(void) {
   int major = 0, minor = 0;
   ADP_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
   ADP_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
-  ADP_CHECK(major == 10, "libadp_b200 needs an sm_100 (B200) device, found sm_%d%d", major,
-            minor);
+  ADP_CHECK(major == 9 && minor == 0, "libadp_b200 is built for sm_90a (H100), found sm_%d%d",
+            major, minor);
   return 0;
 }
 

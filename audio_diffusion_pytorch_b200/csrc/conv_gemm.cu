@@ -1,38 +1,38 @@
-// adp_conv_gemm: persistent shifted-tap GEMM on tcgen05 (see include/adp_b200.h).
+// adp_conv_gemm: persistent shifted-tap GEMM on wgmma (see include/adp_b200.h).
 //
 // GEMM view (swapped w.r.t. the usual conv-as-GEMM so that one accumulator ROW is one time
 // position): D[m = time position, n = output channel] = sum_{tap,k} A[m + off(tap), k] * W[n, tap, k]
 //   A: channels-last activations -> K-major operand.  ONE TMA box of (128 + span) rows per
-//      64-channel chunk serves all taps: tap j is the same smem tile read through a UMMA
-//      descriptor whose start address is advanced by j rows (the 128B swizzle is a function of
-//      the absolute smem address, so row-shifted starts need no re-layout).  Rows outside
-//      [0,T) are zero-filled by TMA = the conv's zero padding.
+//      64-channel chunk serves all taps: tap j is the same smem tile read through a wgmma
+//      descriptor whose start address is advanced by j rows (the swizzle is a function of the
+//      absolute smem address, so row-shifted starts need no re-layout).  Rows outside [0,T)
+//      are zero-filled by TMA = the conv's zero padding.
 //   W: packed weights [N][taps*C_in] -> K-major operand.
 //   A pipeline stage = KC chunks x {A box, one W box per tap} behind ONE full/empty mbarrier
-//      pair, so the single-thread issue loops pay one barrier round trip per KC*taps*4 MMAs.
-//   D: fp32 in TMEM, 128 lanes x BN columns, DOUBLE buffered: the epilogue of tile i drains
-//      buffer i&1 while the MMAs of tile i+1 fill the other one.
-// Persistent: each CTA owns a contiguous range of tiles (n fastest).  Warp roles (192 threads):
-// warp 0 TMA producer + TMEM allocator, warp 1 MMA issuer, warps 2-5 epilogue (TMEM lane
-// quarter = warp & 3).  The epilogue prefetches the residual rows of its tile into registers
-// while the tile's MMAs still run, and keeps GroupNorm partial sums in thread-private smem
-// slots (no shuffles / atomics per tile; one reduction per batch change).
-#include <type_traits>
-
+//      pair, so the issue loops pay one barrier round trip per KC*taps*4 MMAs.
+//   D: fp32 in registers.  Two consumer warpgroups own 64 tile rows each (m64nBNk16 per
+//      warpgroup); one MMA stage stays in flight while the next is issued.
+// Persistent: each CTA owns a contiguous range of tiles (n fastest).  Warp roles (288 threads):
+// warps 0-7 the two consumer warpgroups (MMA issue + epilogue straight from the accumulator
+// registers), warp 8 the TMA producer, which keeps filling the ring while the consumers drain
+// a tile.  GroupNorm partial sums of the output are reduced per warp into per-warp shared-memory
+// slots; one global reduction per batch change.
 #include "common.cuh"
 #include "ptx.cuh"
 
 namespace adp {
 
-// diagnostic switches (adp_debug_set): [0] 3 = CTA-pair (cta_group::2) GEMMs; [2] 1 = weights are not
-// written by the preceding kernels (fetch them before griddepcontrol.wait); [3] CTAs/SM override;
-// [4] bit0 skip MMAs, bit1 skip TMA loads, bit2 skip drain, bit3 exit at entry (timing
-// experiments only); [5] KC override; [6] PDL; [7] 1 = never use the 8-epilogue-warp variant
-int g_debug[8] = {2, 1, 0, 0, 0, 0, 0, 0};
+// diagnostic switches (adp_debug_set): [2] 1 = weights are not written by the preceding kernels
+// (fetch them before griddepcontrol.wait); [3] CTAs/SM override; [5] KC override; [6] PDL
+int g_debug[8] = {0, 0, 0, 0, 0, 0, 0, 0};
 
 constexpr int kBM = 128;
 constexpr int kMaxStages = 8;
 constexpr int kMaxGroups = 8;      // GroupNorm groups handled by the fused statistics
+constexpr int kConsumers = 256;    // two warpgroups
+constexpr int kGemmThreads = kConsumers + 32;
+constexpr int kSmemPerSM = 228 * 1024;
+constexpr int kSmemPerBlock = 227 * 1024;
 
 struct Gemm2Params {
   __nv_bfloat16* out;
@@ -51,9 +51,8 @@ struct Gemm2Params {
   int k_stages;          // stages per tile = (c_in / BK) / kc
   int n_stages;          // ring depth
   int a_sub_bytes, w_sub_bytes, stage_bytes, max_taps;
-  int dbg;
   int early_w;           // weights may be fetched before griddepcontrol.wait
-  // optional GroupNorm-apply + SiLU on the A operand (transform warps rewrite the smem tile)
+  // optional GroupNorm-apply + SiLU on the A operand (the consumers rewrite the smem tile)
   const double* gn_stats;   // fp64 [B][gn_groups][2] of the A tensor
   const float* gn_gamma;
   const float* gn_beta;
@@ -63,19 +62,13 @@ struct Gemm2Params {
 
 struct TileInfo {
   int b, t0, n0, phase, ch0, ntaps, min_off;
-  bool valid;       // CTA pairs: the odd CTA of the last pair may have no rows
 };
 
-// cg = CTAs per tile (1, or 2 for cta_group::2 pairs: `tile` then indexes PAIR tiles of
-// 2*kBM rows and `rank` selects this CTA's 128 of them)
-__device__ __forceinline__ TileInfo tile_info(const Gemm2Params& p, int tile, int BN, int cg = 1,
-                                              int rank = 0) {
+__device__ __forceinline__ TileInfo tile_info(const Gemm2Params& p, int tile, int BN) {
   TileInfo ti;
-  const int m_pair = tile / p.n_tiles_n;
-  const int n_tile = tile - m_pair * p.n_tiles_n;
-  const int m_tile = m_pair * cg + rank;
+  const int m_tile = tile / p.n_tiles_n;
+  const int n_tile = tile - m_tile * p.n_tiles_n;
   ti.b = m_tile / p.tiles_per_batch;
-  ti.valid = ti.b < p.B;
   ti.t0 = (m_tile - ti.b * p.tiles_per_batch) * kBM;
   ti.n0 = n_tile * BN;
   ti.phase = ti.n0 / p.n_pad;
@@ -91,7 +84,7 @@ __device__ __forceinline__ TileInfo tile_info(const Gemm2Params& p, int tile, in
   return ti;
 }
 
-// SiLU with ONE special-function op per element (the transform warps are MUFU-bound):
+// SiLU with ONE special-function op per element (the A-tile transform is MUFU-bound):
 // z*sigmoid(z) = 0.5*z*(1 + tanh(z/2)); tanh.approx error (2^-11) is below bf16 rounding.
 __device__ __forceinline__ float silu_tanh(float z) {
   float t;
@@ -100,477 +93,155 @@ __device__ __forceinline__ float silu_tanh(float z) {
   return fmaf(hz, t, hz);
 }
 
-// thread-private GroupNorm partial sums: slot (value v of group g, epilogue thread et)
-template <int NET>      // NET = epilogue threads per CTA
-struct StatSlots {
-  float* base;   // [2*kMaxGroups][NET]
-  int et;
-  int cur_g;
-  float s, q;
-  __device__ __forceinline__ void flush() {
+// Running per-group (sum, sumsq) of one consumer warp.  Channels arrive in increasing order and
+// the group is warp-uniform: lanes accumulate privately; on a group change the warp reduces with
+// shuffles and lane 0 adds into the warp's OWN shared-memory column.  Each column has a single
+// writer and the columns are summed in warp order, so the statistics do not depend on the
+// order in which warps finish (only the fp64 global reduction across CTAs does).
+struct WarpStats {
+  int cur_g = -1;
+  float s = 0.f, q = 0.f;
+  __device__ __forceinline__ void flush(float (*slots)[8], int w, int lane) {
     if (cur_g >= 0) {
-      base[(2 * cur_g) * NET + et] += s;
-      base[(2 * cur_g + 1) * NET + et] += q;
+      const float ws = warp_sum(s), wq = warp_sum(q);
+      if (lane == 0) { slots[2 * cur_g][w] += ws; slots[2 * cur_g + 1][w] += wq; }
     }
     s = 0.f; q = 0.f;
   }
-  __device__ __forceinline__ void add(float v, int g) {
-    if (g != cur_g) { flush(); cur_g = g; }
+  __device__ __forceinline__ void add(float v, int g, float (*slots)[8], int w, int lane) {
+    if (g != cur_g) { flush(slots, w, lane); cur_g = g; }
     s += v; q += v * v;
   }
 };
 
-// GroupNorm partial sums for group sizes that are neither >= 8 nor 4 (never the case in the
-// reference configurations): straight into the thread-private slots, one element at a time.
-static __device__ __noinline__ void stats_generic(float* slots, int net, int et, int ch, int shift,
-                                                  int gsize, float v0, float v1, float v2, float v3,
-                                                  float v4, float v5, float v6, float v7) {
-  const float v[8] = {v0, v1, v2, v3, v4, v5, v6, v7};
-  for (int i = 0; i < 8; ++i) {
-    const int g = shift >= 0 ? (ch + i) >> shift : (ch + i) / gsize;
-    slots[(2 * g) * net + et] += v[i];
-    slots[(2 * g + 1) * net + et] += v[i] * v[i];
-  }
-}
-
-// EW = epilogue warps: 4 (one per TMEM lane quarter) or, for the long-K shapes that run one CTA
-// per SM with <= one tile per CTA (nothing to overlap the drain with), 8: two warps per lane
-// quarter, each draining half of the tile's columns.
-// CG = 2: CTA PAIRS (cluster of 2 on one TPC, tcgen05 cta_group::2).  One MMA covers 256 rows x BN:
-// each CTA stages its own 128 rows of A but only HALF of the W tile, so the shared-memory fill
-// traffic per output drops from (A + W) to (A + W/2) per CTA -- the deep-level GEMMs are bound by
-// exactly that L2 -> SMEM traffic (profiles/r2_gemm_traffic.txt).  The leader (cluster rank 0)
-// issues every MMA and multicasts the completion to both CTAs' barriers; both CTAs run their own
-// TMA producer (signalling the LEADER's full barrier) and their own epilogue.
-template <int BN, int SW, bool XF, int EW, int CG = 1>
-__global__ void __launch_bounds__(64 + 32 * EW + (XF ? 256 : 0),
-                                  EW == 8 ? 1 : (BN <= 64 ? (XF ? 2 : 3) : (BN <= 128 ? (XF ? 1 : 2) : 1)))
+template <int BN, int SW, bool XF>
+__global__ void __launch_bounds__(kGemmThreads, BN <= 32 ? 3 : (BN <= 64 ? 2 : 1))
 conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
                   const Gemm2Params p) {
   constexpr int BK = SW / 2;
-  constexpr int ACC_COLS = BN < 32 ? 32 : BN;     // TMEM columns per accumulator buffer
-  constexpr int CH = BN < 32 ? 16 : 32;           // epilogue column chunk
-  constexpr int WN = BN / CG;                     // W rows staged by THIS CTA
-  constexpr uint32_t kWTapBytes = WN * SW;        // bytes one W box writes
-  static_assert(CG == 1 || (CG == 2 && !XF), "CTA pairs: plain (non-transform) variant only");
+  constexpr int NACC = BN / 2;                    // accumulator registers per consumer thread
+  constexpr uint32_t kWTapBytes = BN * SW;        // bytes one W box writes
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint64_t full_bar[kMaxStages], empty_bar[kMaxStages], ready_bar[kMaxStages];
-  __shared__ uint64_t acc_full[2], acc_empty[2];
-  __shared__ uint32_t tmem_slot;
-  constexpr int NET = 32 * EW;                    // epilogue threads
-  constexpr int BNW = BN / (EW / 4);              // columns drained by one epilogue warp
-  static_assert(!XF || EW == 4, "the transform variant runs four epilogue warps");
-  static_assert(EW == 4 || BNW >= 32, "8 epilogue warps need >= 32 columns per warp");
-  __shared__ float s_part[2 * kMaxGroups * NET];
-  // per-tile bias / gate of the BN output columns, double buffered like the accumulators:
-  // staged while the tile's MMAs run so the drain never waits on a global load
-  __shared__ __align__(16) float s_bias[2][BN < 32 ? 32 : BN];
-  __shared__ __align__(16) float s_gate[2][BN < 32 ? 32 : BN];
+  __shared__ uint64_t full_bar[kMaxStages], empty_bar[kMaxStages];
+  __shared__ float s_part[2 * kMaxGroups][8];     // (sum, sumsq) per group of the current batch, per consumer warp
   __shared__ __align__(16) float s_coef[XF ? 2 * 1024 : 4];   // (a, d) per input channel of the current batch
 
   pdl_launch_dependents();
-  if (p.dbg & 8) return;      // timing experiment: launch floor of this configuration
   const int warp = warp_id_uniform();
   const int lane = threadIdx.x & 31;
   const uint32_t raw = smem_u32(smem_raw);
   uint8_t* ring = smem_raw + ((1024u - (raw & 1023u)) & 1023u);
 
-  const uint32_t rank = CG == 2 ? cluster_ctarank() : 0u;       // 0 = leader of the pair
-  const int tile_begin = (blockIdx.x / CG) * p.tiles_per_cta;
+  const int tile_begin = blockIdx.x * p.tiles_per_cta;
   int tile_end = tile_begin + p.tiles_per_cta;
   if (tile_end > p.total_tiles) tile_end = p.total_tiles;
 
-  for (int i = threadIdx.x; i < 2 * kMaxGroups * NET; i += blockDim.x) s_part[i] = 0.f;
-  if (warp == 0) {
-    if constexpr (CG == 2) { tmem_alloc_cg2(&tmem_slot, 2 * ACC_COLS); tmem_relinquish_cg2(); }
-    else { tmem_alloc(&tmem_slot, 2 * ACC_COLS); tmem_relinquish(); }
-  } else if (warp == 1 && lane == 0) {
-    // pairs: the leader's full barrier gets its own arrive.expect_tx plus the peer's remote arrive;
-    // the leader's acc_empty collects the epilogue warps of BOTH CTAs
-    for (int s = 0; s < p.n_stages; ++s) {
-      mbar_init(&full_bar[s], CG); mbar_init(&empty_bar[s], 1); mbar_init(&ready_bar[s], 256);
-    }
-    for (int s = 0; s < 2; ++s) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], EW * CG); }
+  if (threadIdx.x < 2 * kMaxGroups * 8) (&s_part[0][0])[threadIdx.x] = 0.f;
+  if (warp == 8 && lane == 0) {
+    for (int s = 0; s < p.n_stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
     fence_mbar_init();
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmW);
   }
-  tc_fence_before();
-  if constexpr (CG == 2) cluster_sync_all();      // the peer's barriers exist before anyone signals them
-  else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, tmem_slot, 0);   // warp-uniform for ptxas
+  __syncthreads();
   // Programmatic dependent launch: this kernel may have started while its predecessor still
   // runs.  Activations / statistics / conditioning come from the predecessor, so every role
   // that reads them calls griddepcontrol.wait first.  The WEIGHTS do not (p.early_w, set by the
   // host only while it captures an inference graph): the producer puts the weight boxes of the
   // first ring stages in flight BEFORE waiting, taking the first-load latency off the
   // critical path of the many short GEMMs that follow an elementwise kernel.
-  if (warp == 0) {
+  if (warp == 8) {
     // ---------------------------------------------------------------------- TMA producer
-    {
-      const uint32_t a_bytes = static_cast<uint32_t>(p.a_rows) * SW;
-      const int total_it = (tile_end - tile_begin) * p.k_stages;
-      int early = 0;
-      if (p.early_w && !(p.dbg & 2)) {
-        early = total_it < p.n_stages ? total_it : p.n_stages;
-        if (elect_one()) {
-          int tile = tile_begin, ks = 0;
-          for (int it = 0; it < early; ++it) {          // stage `it` of the (still empty) ring
-            const TileInfo ti = tile_info(p, tile, BN, CG, rank);
-            uint8_t* st = ring + it * p.stage_bytes;
-            const uint32_t tx_it = static_cast<uint32_t>(p.kc) * (a_bytes + ti.ntaps * kWTapBytes);
-            const uint32_t lead_bar = CG == 2 ? mapa_shared(smem_u32(&full_bar[it]), 0) : 0u;
-            if (rank == 0) mbar_arrive_expect_tx(&full_bar[it], CG * tx_it);
-            else mbar_arrive_cluster(lead_bar);
-            for (int c = 0; c < p.kc; ++c) {
-              const int k0 = (ks * p.kc + c) * BK;
-              uint8_t* wdst = st + p.kc * p.a_sub_bytes + c * p.max_taps * p.w_sub_bytes;
-              for (int tap = 0; tap < ti.ntaps; ++tap) {
-                if constexpr (CG == 2)
-                  tma_load_2d_cg2(wdst + tap * p.w_sub_bytes, &tmW, lead_bar, tap * p.c_in + k0,
-                                  ti.n0 + static_cast<int>(rank) * WN);
-                else
-                  tma_load_2d(wdst + tap * p.w_sub_bytes, &tmW, &full_bar[it], tap * p.c_in + k0, ti.n0);
-              }
-            }
-            if (++ks == p.k_stages) { ks = 0; ++tile; }
+    const uint32_t a_bytes = static_cast<uint32_t>(p.a_rows) * SW;
+    const int total_it = (tile_end - tile_begin) * p.k_stages;
+    int early = 0;
+    if (p.early_w) {
+      early = total_it < p.n_stages ? total_it : p.n_stages;
+      if (elect_one()) {
+        int tile = tile_begin, ks = 0;
+        for (int it = 0; it < early; ++it) {          // stage `it` of the (still empty) ring
+          const TileInfo ti = tile_info(p, tile, BN);
+          uint8_t* st = ring + it * p.stage_bytes;
+          mbar_arrive_expect_tx(&full_bar[it], static_cast<uint32_t>(p.kc) * (a_bytes + ti.ntaps * kWTapBytes));
+          for (int c = 0; c < p.kc; ++c) {
+            const int k0 = (ks * p.kc + c) * BK;
+            uint8_t* wdst = st + p.kc * p.a_sub_bytes + c * p.max_taps * p.w_sub_bytes;
+            for (int tap = 0; tap < ti.ntaps; ++tap)
+              tma_load_2d(wdst + tap * p.w_sub_bytes, &tmW, &full_bar[it], tap * p.c_in + k0, ti.n0);
           }
-        }
-        __syncwarp();
-      }
-      pdl_wait();
-      int s = 0, it = 0;
-      uint32_t ph = 0;
-      for (int tile = tile_begin; tile < tile_end; ++tile) {
-        const TileInfo ti = tile_info(p, tile, BN, CG, rank);
-        const uint32_t tx = static_cast<uint32_t>(p.kc) * (a_bytes + ti.ntaps * kWTapBytes);
-        for (int ks = 0; ks < p.k_stages; ++ks, ++it) {
-          const bool armed = it < early;                 // barrier armed + weights already issued
-          if (!armed) mbar_wait(&empty_bar[s], ph ^ 1);
-          uint8_t* st = ring + s * p.stage_bytes;
-          if (elect_one()) {
-            const uint32_t lead_bar = CG == 2 ? mapa_shared(smem_u32(&full_bar[s]), 0) : 0u;
-            if (p.dbg & 2) {
-              if (rank == 0) mbar_arrive(&full_bar[s]);
-              else mbar_arrive_cluster(lead_bar);
-            } else {
-              if (!armed) {
-                if (rank == 0) mbar_arrive_expect_tx(&full_bar[s], CG * tx);
-                else mbar_arrive_cluster(lead_bar);
-              }
-              for (int c = 0; c < p.kc; ++c) {
-                const int k0 = (ks * p.kc + c) * BK;
-                if constexpr (CG == 2)
-                  tma_load_3d_cg2(st + c * p.a_sub_bytes, &tmA, lead_bar, k0, ti.t0 + ti.min_off, ti.b);
-                else
-                  tma_load_3d(st + c * p.a_sub_bytes, &tmA, &full_bar[s], k0, ti.t0 + ti.min_off, ti.b);
-                if (armed) continue;
-                uint8_t* wdst = st + p.kc * p.a_sub_bytes + c * p.max_taps * p.w_sub_bytes;
-                for (int tap = 0; tap < ti.ntaps; ++tap) {
-                  if constexpr (CG == 2)
-                    tma_load_2d_cg2(wdst + tap * p.w_sub_bytes, &tmW, lead_bar, tap * p.c_in + k0,
-                                    ti.n0 + static_cast<int>(rank) * WN);
-                  else
-                    tma_load_2d(wdst + tap * p.w_sub_bytes, &tmW, &full_bar[s], tap * p.c_in + k0, ti.n0);
-                }
-              }
-            }
-          }
-          __syncwarp();
-          if (++s == p.n_stages) { s = 0; ph ^= 1; }
+          if (++ks == p.k_stages) { ks = 0; ++tile; }
         }
       }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------------ MMA issuer
-    if (rank == 0) {       // pairs: the leader issues for both CTAs
-      constexpr uint32_t idesc = umma_idesc_bf16(kBM * CG, BN, 0, 0);
-      // descriptor of the ring base; byte offsets are added to the 14-bit address field
-      const uint64_t desc0 = umma_desc_kmajor<SW>(smem_u32(ring));
-      const uint32_t stage_u = static_cast<uint32_t>(p.stage_bytes) >> 4;
-      const uint32_t a_sub_u = static_cast<uint32_t>(p.a_sub_bytes) >> 4;
-      const uint32_t w_sub_u = static_cast<uint32_t>(p.w_sub_bytes) >> 4;
-      const uint32_t w_base_u = static_cast<uint32_t>(p.kc) * a_sub_u;
-      int s = 0;
-      uint32_t ph = 0, j = 0;
-      for (int tile = tile_begin; tile < tile_end; ++tile, ++j) {
-        const TileInfo ti = tile_info(p, tile, BN, CG, 0);
-        const uint32_t buf = j & 1;
-        mbar_wait(&acc_empty[buf], ((j >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + buf * ACC_COLS;
-        uint32_t accumulate = 0;
-        for (int ks = 0; ks < p.k_stages; ++ks) {
-          mbar_wait(XF ? &ready_bar[s] : &full_bar[s], ph);
-          tc_fence_after();
-          if (elect_one()) {        // ONE elected thread issues the whole stage and its commit
-            if (!(p.dbg & 1)) {
-              const uint64_t sdesc = desc0 + static_cast<uint64_t>(s * stage_u);
-              for (int c = 0; c < p.kc; ++c) {
-                const uint64_t adesc = sdesc + c * a_sub_u;
-                const uint64_t wdesc = sdesc + w_base_u + c * p.max_taps * w_sub_u;
-                for (int tap = 0; tap < ti.ntaps; ++tap) {
-#pragma unroll
-                  for (int kk = 0; kk < BK / 16; ++kk) {
-                    if constexpr (CG == 2)
-                      umma_bf16_cg2(d_tmem, adesc + ((tap * SW + kk * 32) >> 4),
-                                    wdesc + tap * w_sub_u + ((kk * 32) >> 4), idesc, accumulate);
-                    else
-                      umma_bf16(d_tmem, adesc + ((tap * SW + kk * 32) >> 4),
-                                wdesc + tap * w_sub_u + ((kk * 32) >> 4), idesc, accumulate);
-                    accumulate = 1;
-                  }
-                }
-              }
-            }
-            if constexpr (CG == 2) {
-              umma_commit_cg2(&empty_bar[s], 3);
-              if (ks == p.k_stages - 1) umma_commit_cg2(&acc_full[buf], 3);
-            } else {
-              umma_commit(&empty_bar[s]);
-              if (ks == p.k_stages - 1) umma_commit(&acc_full[buf]);
-            }
-          }
-          accumulate = 1;
-          __syncwarp();
-          if (++s == p.n_stages) { s = 0; ph ^= 1; }
-        }
-      }
-    }
-  } else if (warp < 2 + EW) {
-    // -------------------------------------------------------------------------- epilogue
-    pdl_wait();
-    const int q = warp & 3;                 // TMEM lane quarter this warp may access
-    const int row = q * 32 + lane;
-    const uint32_t lane_addr = static_cast<uint32_t>(q * 32) << 16;
-    const bool do_stats = p.stats != nullptr;
-    const int et = threadIdx.x - 64;        // 0..NET-1 among epilogue threads
-    const int cbeg = ((warp - 2) >> 2) * BNW;   // first tile column of this warp
-    StatSlots<NET> acc{s_part, et, -1, 0.f, 0.f};
-    int cur_b = -1;
-    uint32_t j = 0;
-
-    auto publish_stats = [&](int b_done) {   // all 128 epilogue threads
-      acc.flush();
-      acc.cur_g = -1;
-      named_bar_sync(1, NET);
-      for (int r2 = warp - 2; r2 < 2 * p.groups; r2 += EW) {     // one warp per row of slots
-        const float* rowp = s_part + r2 * NET + lane;
-        float tot = 0.f;
-#pragma unroll
-        for (int i = 0; i < EW; ++i) tot += rowp[32 * i];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) tot += __shfl_xor_sync(0xffffffffu, tot, o);
-        if (lane == 0 && tot != 0.f)
-          atomicAdd(p.stats + static_cast<size_t>(b_done) * 2 * p.groups + r2,
-                    static_cast<double>(tot));
-      }
-      named_bar_sync(1, NET);
-      for (int g2 = 0; g2 < 2 * p.groups; ++g2) s_part[g2 * NET + et] = 0.f;
-    };
-
-    for (int tile = tile_begin; tile < tile_end; ++tile, ++j) {
-      const TileInfo ti = tile_info(p, tile, BN, CG, rank);
-      const uint32_t buf = j & 1;
-      const int t = ti.t0 + row;
-      const bool row_ok = t < p.T && ti.valid;
-      const size_t row_off = (static_cast<size_t>(ti.valid ? ti.b : 0) * p.T + (row_ok ? t : 0)) * p.ldo +
-                             static_cast<size_t>(ti.phase) * p.n_valid;
-      if (do_stats && ti.valid && ti.b != cur_b) {
-        if (cur_b >= 0) publish_stats(cur_b);
-        cur_b = ti.b;
-      }
-      // residual rows of this tile -> registers, while the tile's MMAs are still running
-      uint4 res[BNW / 8];
-      if (p.residual) {
-#pragma unroll
-        for (int i = 0; i < BNW / 8; ++i) {
-          const int ch = ti.ch0 + cbeg + i * 8;
-          res[i] = make_uint4(0, 0, 0, 0);
-          if (row_ok && ch < p.n_valid)
-            res[i] = __ldg(reinterpret_cast<const uint4*>(p.residual + row_off + ch));
-        }
-      }
-      for (int c = et; c < BN; c += NET) {
-        const int ch = ti.ch0 + c;
-        const bool ok = ch < p.n_valid;
-        s_bias[buf][c] = (p.bias && ok) ? __ldg(p.bias + ch) : 0.f;
-        s_gate[buf][c] = (p.gate && ok && ti.valid) ? __ldg(p.gate + static_cast<size_t>(ti.b) * p.ld_gate + ch) : 1.f;
-      }
-      named_bar_sync(2, NET);     // staging visible to all epilogue warps
-      mbar_wait(&acc_full[buf], (j >> 1) & 1);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + buf * ACC_COLS + lane_addr;
-      // Specialised drains for the shapes the network launches (bias, optional residual and
-      // statistics with >= 8-channel groups, every column valid): the generic loop below pays
-      // ~25 instructions of run-time flag tests per 8-channel vector, and the drain of a
-      // short-K tile is issue/fetch bound.
-      auto drain_fast = [&](auto res_c, auto st_c) {
-        constexpr bool RES = decltype(res_c)::value;
-        constexpr bool ST = decltype(st_c)::value;
-#pragma unroll
-        for (int cc = 0; cc < BNW; cc += CH) {
-          const int c0 = cbeg + cc;
-          uint32_t r[CH];
-          if constexpr (CH == 16) tmem_ld16(taddr + c0, r);
-          else tmem_ld32(taddr + c0, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int v8 = 0; v8 < CH / 8; ++v8) {
-            const int ch = ti.ch0 + c0 + v8 * 8;
-            const float4 b0 = *reinterpret_cast<const float4*>(&s_bias[buf][c0 + v8 * 8]);
-            const float4 b1 = *reinterpret_cast<const float4*>(&s_bias[buf][c0 + v8 * 8 + 4]);
-            float v[8];
-            v[0] = __uint_as_float(r[v8 * 8 + 0]) + b0.x; v[1] = __uint_as_float(r[v8 * 8 + 1]) + b0.y;
-            v[2] = __uint_as_float(r[v8 * 8 + 2]) + b0.z; v[3] = __uint_as_float(r[v8 * 8 + 3]) + b0.w;
-            v[4] = __uint_as_float(r[v8 * 8 + 4]) + b1.x; v[5] = __uint_as_float(r[v8 * 8 + 5]) + b1.y;
-            v[6] = __uint_as_float(r[v8 * 8 + 6]) + b1.z; v[7] = __uint_as_float(r[v8 * 8 + 7]) + b1.w;
-            if constexpr (RES) {
-              const uint4 rr = res[(cc + v8 * 8) / 8];
-              const float2 r0 = unpack_bf16(rr.x), r1 = unpack_bf16(rr.y);
-              const float2 r2 = unpack_bf16(rr.z), r3 = unpack_bf16(rr.w);
-              v[0] += r0.x; v[1] += r0.y; v[2] += r1.x; v[3] += r1.y;
-              v[4] += r2.x; v[5] += r2.y; v[6] += r3.x; v[7] += r3.y;
-            }
-            uint4 o;
-            o.x = pack_bf16(v[0], v[1]); o.y = pack_bf16(v[2], v[3]);
-            o.z = pack_bf16(v[4], v[5]); o.w = pack_bf16(v[6], v[7]);
-            if (row_ok) {
-              *reinterpret_cast<uint4*>(p.out + row_off + ch) = o;
-              if constexpr (ST) {      // statistics of the ROUNDED values the next layer reads
-                const float2 q0 = unpack_bf16(o.x), q1 = unpack_bf16(o.y);
-                const float2 q2 = unpack_bf16(o.z), q3 = unpack_bf16(o.w);
-                const float s8 = ((q0.x + q0.y) + (q1.x + q1.y)) + ((q2.x + q2.y) + (q3.x + q3.y));
-                const float q8 = ((q0.x * q0.x + q0.y * q0.y) + (q1.x * q1.x + q1.y * q1.y)) +
-                                 ((q2.x * q2.x + q2.y * q2.y) + (q3.x * q3.x + q3.y * q3.y));
-                const int g = ch >> p.group_shift;
-                if (g != acc.cur_g) { acc.flush(); acc.cur_g = g; }
-                acc.s += s8; acc.q += q8;
-              }
-            }
-          }
-        }
-      };
-      const bool fast = !p.gate && !p.out_fp32 && !(p.dbg & 4) && ti.ch0 + cbeg + BNW <= p.n_valid &&
-                        (!do_stats || p.group_shift >= 3);
-      if (fast) {
-        if (p.residual) {
-          if (do_stats) drain_fast(std::true_type{}, std::true_type{});
-          else drain_fast(std::true_type{}, std::false_type{});
-        } else {
-          if (do_stats) drain_fast(std::false_type{}, std::true_type{});
-          else drain_fast(std::false_type{}, std::false_type{});
-        }
-      }
-#pragma unroll
-      for (int cc = 0; cc < BNW; cc += CH) {
-        if (fast) break;
-        const int c0 = cbeg + cc;
-        if (p.dbg & 4) break;   // timing experiment: skip the drain
-        uint32_t r[CH];
-        if constexpr (CH == 16) tmem_ld16(taddr + c0, r);
-        else tmem_ld32(taddr + c0, r);
-        tmem_ld_wait();
-#pragma unroll
-        for (int v8 = 0; v8 < CH / 8; ++v8) {
-          const int ch = ti.ch0 + c0 + v8 * 8;
-          if (ch >= p.n_valid) continue;           // padded columns (uniform)
-          float v[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[v8 * 8 + i]);
-          {
-            const float4 b0 = *reinterpret_cast<const float4*>(&s_bias[buf][c0 + v8 * 8]);
-            const float4 b1 = *reinterpret_cast<const float4*>(&s_bias[buf][c0 + v8 * 8 + 4]);
-            v[0] += b0.x; v[1] += b0.y; v[2] += b0.z; v[3] += b0.w;
-            v[4] += b1.x; v[5] += b1.y; v[6] += b1.z; v[7] += b1.w;
-          }
-          if (p.gate) {
-            const float4 g0 = *reinterpret_cast<const float4*>(&s_gate[buf][c0 + v8 * 8]);
-            const float4 g1 = *reinterpret_cast<const float4*>(&s_gate[buf][c0 + v8 * 8 + 4]);
-            v[0] *= g0.x; v[1] *= g0.y; v[2] *= g0.z; v[3] *= g0.w;
-            v[4] *= g1.x; v[5] *= g1.y; v[6] *= g1.z; v[7] *= g1.w;
-          }
-          if (p.out_fp32) {
-            if (row_ok) {
-              float* op = reinterpret_cast<float*>(p.out) + row_off + ch;
-              *reinterpret_cast<float4*>(op) = make_float4(v[0], v[1], v[2], v[3]);
-              *reinterpret_cast<float4*>(op + 4) = make_float4(v[4], v[5], v[6], v[7]);
-            }
-            continue;
-          }
-          if (row_ok) {
-            if (p.residual) {
-              const uint4 rr = res[(cc + v8 * 8) / 8];
-              const float2 r0 = unpack_bf16(rr.x), r1 = unpack_bf16(rr.y);
-              const float2 r2 = unpack_bf16(rr.z), r3 = unpack_bf16(rr.w);
-              v[0] += r0.x; v[1] += r0.y; v[2] += r1.x; v[3] += r1.y;
-              v[4] += r2.x; v[5] += r2.y; v[6] += r3.x; v[7] += r3.y;
-            }
-            uint4 o;
-            o.x = pack_bf16(v[0], v[1]); o.y = pack_bf16(v[2], v[3]);
-            o.z = pack_bf16(v[4], v[5]); o.w = pack_bf16(v[6], v[7]);
-            *reinterpret_cast<uint4*>(p.out + row_off + ch) = o;
-            if (do_stats) {  // statistics of the ROUNDED values the next layer will read
-              const float2 q0 = unpack_bf16(o.x), q1 = unpack_bf16(o.y);
-              const float2 q2 = unpack_bf16(o.z), q3 = unpack_bf16(o.w);
-              v[0] = q0.x; v[1] = q0.y; v[2] = q1.x; v[3] = q1.y;
-              v[4] = q2.x; v[5] = q2.y; v[6] = q3.x; v[7] = q3.y;
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] = 0.f;
-          }
-          if (do_stats) {
-            if (p.group_shift >= 3) {          // the whole 8-vector lies in one group
-              float s8 = 0.f, q8 = 0.f;
-#pragma unroll
-              for (int i = 0; i < 8; ++i) { s8 += v[i]; q8 += v[i] * v[i]; }
-              const int g = ch >> p.group_shift;
-              if (g != acc.cur_g) { acc.flush(); acc.cur_g = g; }
-              acc.s += s8; acc.q += q8;
-            } else if (p.group_shift == 2) {   // 4-channel groups: the vector spans g and g + 1
-              const int g = ch >> 2;
-              float* lo = s_part + (2 * g) * NET + et;
-              lo[0] += (v[0] + v[1]) + (v[2] + v[3]);
-              lo[NET] += (v[0] * v[0] + v[1] * v[1]) + (v[2] * v[2] + v[3] * v[3]);
-              lo[2 * NET] += (v[4] + v[5]) + (v[6] + v[7]);
-              lo[3 * NET] += (v[4] * v[4] + v[5] * v[5]) + (v[6] * v[6] + v[7] * v[7]);
-            } else {
-              // rare group sizes: out of line, or this code is unrolled BN/8 times into the
-              // drain loop and the epilogue stalls on instruction fetch
-              stats_generic(s_part, NET, et, ch, p.group_shift, p.group_size, v[0], v[1], v[2], v[3],
-                            v[4], v[5], v[6], v[7]);
-            }
-          }
-        }
-      }
-      // accumulator buffer drained -> hand it back to the MMA warp
-      tc_fence_before();
       __syncwarp();
-      if (lane == 0) {
-        if constexpr (CG == 2) mbar_arrive_cluster(mapa_shared(smem_u32(&acc_empty[buf]), 0));
-        else mbar_arrive(&acc_empty[buf]);
-      }
     }
-    if (do_stats && cur_b >= 0) publish_stats(cur_b);
-  } else if constexpr (XF) {
-    // ------------------------------------------------- transform: a = silu(x*ga + de) in place
-    // 256 threads, two per tile row.  The TMA tile is SW-byte rows with the 16-byte chunks
-    // XOR-swizzled by address bits [7, 7+log2(SW/16)); zero rows (conv padding) stay zero.
     pdl_wait();
-    const int tt = threadIdx.x - (64 + NET);
-    constexpr int CPR = SW / 16;                 // 16-byte chunks per row
-    constexpr int CPT = CPR / 2 > 0 ? CPR / 2 : 1;   // chunks per thread
-    const int gsz = p.c_in / p.gn_groups;
-    const double inv_n = 1.0 / (static_cast<double>(gsz) * p.T);
-    int s = 0, cur_b = -1;
+    int s = 0, it = 0;
     uint32_t ph = 0;
     for (int tile = tile_begin; tile < tile_end; ++tile) {
       const TileInfo ti = tile_info(p, tile, BN);
-      if (ti.b != cur_b) {     // (a, d) of every input channel for this batch element, once
-        named_bar_sync(3, 256);          // previous batch's coefficients no longer in use
-        for (int ch = tt; ch < p.c_in; ch += 256) {
+      const uint32_t tx = static_cast<uint32_t>(p.kc) * (a_bytes + ti.ntaps * kWTapBytes);
+      for (int ks = 0; ks < p.k_stages; ++ks, ++it) {
+        const bool armed = it < early;                 // barrier armed + weights already issued
+        if (!armed) mbar_wait(&empty_bar[s], ph ^ 1);
+        uint8_t* st = ring + s * p.stage_bytes;
+        if (elect_one()) {
+          if (!armed) mbar_arrive_expect_tx(&full_bar[s], tx);
+          for (int c = 0; c < p.kc; ++c) {
+            const int k0 = (ks * p.kc + c) * BK;
+            tma_load_3d(st + c * p.a_sub_bytes, &tmA, &full_bar[s], k0, ti.t0 + ti.min_off, ti.b);
+            if (armed) continue;
+            uint8_t* wdst = st + p.kc * p.a_sub_bytes + c * p.max_taps * p.w_sub_bytes;
+            for (int tap = 0; tap < ti.ntaps; ++tap)
+              tma_load_2d(wdst + tap * p.w_sub_bytes, &tmW, &full_bar[s], tap * p.c_in + k0, ti.n0);
+          }
+        }
+        __syncwarp();
+        if (++s == p.n_stages) { s = 0; ph ^= 1; }
+      }
+    }
+    return;
+  }
+
+  // ------------------------------------------------------------------------------ consumers
+  pdl_wait();
+  const int tid = threadIdx.x;                 // 0..255
+  const int wg = tid >> 7;                     // warpgroup: tile rows [64*wg, 64*wg + 64)
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // fragment rows r0 and r0 + 8
+  const int cq = 2 * (lane & 3);               // fragment column offset inside each 8-column block
+  const bool do_stats = p.stats != nullptr;
+  WarpStats acc_st;
+  int cur_b = -1, coef_b = -1;
+
+  auto publish_stats = [&](int b_done) {       // all 256 consumer threads
+    acc_st.flush(s_part, warp, lane);
+    acc_st.cur_g = -1;
+    named_bar_sync(1, kConsumers);
+    if (tid < 2 * p.groups) {
+      float tot = 0.f;
+#pragma unroll
+      for (int w = 0; w < 8; ++w) { tot += s_part[tid][w]; s_part[tid][w] = 0.f; }
+      if (tot != 0.f) atomicAdd(p.stats + static_cast<size_t>(b_done) * 2 * p.groups + tid, static_cast<double>(tot));
+    }
+    named_bar_sync(1, kConsumers);
+  };
+
+  // descriptor of the ring base; byte offsets are added to the 14-bit address field
+  const uint64_t desc0 = gmma_desc_kmajor<SW>(smem_u32(ring));
+  const uint32_t stage_u = static_cast<uint32_t>(p.stage_bytes) >> 4;
+  const uint32_t a_sub_u = static_cast<uint32_t>(p.a_sub_bytes) >> 4;
+  const uint32_t w_sub_u = static_cast<uint32_t>(p.w_sub_bytes) >> 4;
+  const uint32_t w_base_u = static_cast<uint32_t>(p.kc) * a_sub_u;
+  const uint32_t wg_row_u = static_cast<uint32_t>(wg * 64 * SW) >> 4;
+  int s = 0;
+  uint32_t ph = 0;
+  for (int tile = tile_begin; tile < tile_end; ++tile) {
+    const TileInfo ti = tile_info(p, tile, BN);
+    if constexpr (XF) {
+      if (ti.b != coef_b) {     // (a, d) of every input channel for this batch element, once
+        named_bar_sync(1, kConsumers);          // previous batch's coefficients no longer in use
+        const int gsz = p.c_in / p.gn_groups;
+        const double inv_n = 1.0 / (static_cast<double>(gsz) * p.T);
+        for (int ch = tid; ch < p.c_in; ch += kConsumers) {
           const int g = ch / gsz;
           const double mean = p.gn_stats[(static_cast<size_t>(ti.b) * p.gn_groups + g) * 2] * inv_n;
           const float var = fmaxf(static_cast<float>(
@@ -579,24 +250,35 @@ conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           s_coef[2 * ch] = ga;
           s_coef[2 * ch + 1] = __ldg(p.gn_beta + ch) - static_cast<float>(mean) * ga;
         }
-        named_bar_sync(3, 256);
-        cur_b = ti.b;
+        named_bar_sync(1, kConsumers);
+        coef_b = ti.b;
       }
-      for (int ks = 0; ks < p.k_stages; ++ks) {
-        mbar_wait(&full_bar[s], ph);
+    }
+    float acc[NACC];
+    uint32_t accumulate = 0;
+    int prev_s = -1;
+    for (int ks = 0; ks < p.k_stages; ++ks) {
+      mbar_wait(&full_bar[s], ph);
+      if constexpr (XF) {
+        // a = silu(x*ga + de) in place, two threads per tile row.  The TMA tile is SW-byte rows
+        // with the 16-byte chunks XOR-swizzled by address bits [7, 7+log2(SW/16)); zero rows
+        // (conv padding) stay zero.  Rows are shared by both warpgroups (tap shifts), so all
+        // consumers finish the stage before either issues its MMAs.
+        constexpr int CPR = SW / 16;                 // 16-byte chunks per row
+        constexpr int CPT = CPR / 2 > 0 ? CPR / 2 : 1;   // chunks per thread
         uint8_t* st = ring + s * p.stage_bytes;
         for (int c = 0; c < p.kc; ++c) {
           uint8_t* sub = st + c * p.a_sub_bytes;
           const float* cf = s_coef + (ks * p.kc + c) * BK * 2;
-          for (int rr = tt >> 1; rr < p.a_rows; rr += 128) {
+          for (int rr = tid >> 1; rr < p.a_rows; rr += kConsumers / 2) {
             const int t = ti.t0 + ti.min_off + rr;
             if (t < 0 || t >= p.T) continue;               // TMA zero fill = conv padding
             const uint32_t row_off = static_cast<uint32_t>(rr) * SW;
             const int swz = (row_off >> 7) & (CPR - 1);
 #pragma unroll
             for (int q = 0; q < CPT; ++q) {
-              const int pc = (CPR >= 2) ? (tt & 1) * CPT + q : 0;      // physical chunk
-              if (CPR < 2 && (tt & 1)) continue;
+              const int pc = (CPR >= 2) ? (tid & 1) * CPT + q : 0;      // physical chunk
+              if (CPR < 2 && (tid & 1)) continue;
               const int lc = pc ^ swz;                                  // logical chunk
               uint4* ptr = reinterpret_cast<uint4*>(sub + row_off + pc * 16);
               const uint4 u = *ptr;
@@ -614,67 +296,106 @@ conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           }
         }
         fence_proxy_async_smem();
-        mbar_arrive(&ready_bar[s]);
-        if (++s == p.n_stages) { s = 0; ph ^= 1; }
+        named_bar_sync(1, kConsumers);
+      }
+      wgmma_fence();
+      const uint64_t sdesc = desc0 + static_cast<uint64_t>(s * stage_u);
+      for (int c = 0; c < p.kc; ++c) {
+        const uint64_t adesc = sdesc + c * a_sub_u + wg_row_u;
+        const uint64_t wdesc = sdesc + w_base_u + c * p.max_taps * w_sub_u;
+        for (int tap = 0; tap < ti.ntaps; ++tap) {
+#pragma unroll
+          for (int kk = 0; kk < BK / 16; ++kk) {
+            Wgmma<BN>::template ss<0, 0>(acc, adesc + ((tap * SW + kk * 32) >> 4),
+                                         wdesc + tap * w_sub_u + ((kk * 32) >> 4), accumulate);
+            accumulate = 1;
+          }
+        }
+      }
+      wgmma_commit();
+      // one stage in flight: the previous one has been read -> hand its slot back
+      wgmma_wait<1>();
+      if (prev_s >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev_s]);
+      }
+      prev_s = s;
+      if (++s == p.n_stages) { s = 0; ph ^= 1; }
+    }
+    wgmma_wait<0>();
+    acc_fence(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[prev_s]);
+
+    // ------------------------------------------------------------------------ epilogue
+    if (do_stats && ti.b != cur_b) {
+      if (cur_b >= 0) publish_stats(cur_b);
+      cur_b = ti.b;
+    }
+    const int t_lo = ti.t0 + r0, t_hi = t_lo + 8;
+    const bool ok_lo = t_lo < p.T, ok_hi = t_hi < p.T;
+    const size_t col_off = static_cast<size_t>(ti.phase) * p.n_valid;
+    const size_t off_lo = (static_cast<size_t>(ti.b) * p.T + (ok_lo ? t_lo : 0)) * p.ldo + col_off;
+    const size_t off_hi = (static_cast<size_t>(ti.b) * p.T + (ok_hi ? t_hi : 0)) * p.ldo + col_off;
+    const float* gate_row = p.gate ? p.gate + static_cast<size_t>(ti.b) * p.ld_gate : nullptr;
+#pragma unroll
+    for (int jb = 0; jb < BN / 8; ++jb) {
+      if (ti.ch0 + jb * 8 >= p.n_valid) break;        // padded columns (n_valid % 8 == 0: uniform)
+      const int ch = ti.ch0 + jb * 8 + cq;
+      const float2 bb = p.bias ? make_float2(__ldg(p.bias + ch), __ldg(p.bias + ch + 1)) : make_float2(0.f, 0.f);
+      const float2 gg = gate_row ? make_float2(__ldg(gate_row + ch), __ldg(gate_row + ch + 1)) : make_float2(1.f, 1.f);
+      float v[4];
+      v[0] = (acc[4 * jb + 0] + bb.x) * gg.x; v[1] = (acc[4 * jb + 1] + bb.y) * gg.y;
+      v[2] = (acc[4 * jb + 2] + bb.x) * gg.x; v[3] = (acc[4 * jb + 3] + bb.y) * gg.y;
+      if (p.out_fp32) {
+        float* o = reinterpret_cast<float*>(p.out);
+        if (ok_lo) *reinterpret_cast<float2*>(o + off_lo + ch) = make_float2(v[0], v[1]);
+        if (ok_hi) *reinterpret_cast<float2*>(o + off_hi + ch) = make_float2(v[2], v[3]);
+        continue;
+      }
+      if (p.residual) {
+        if (ok_lo) {
+          const float2 r = unpack_bf16(__ldg(reinterpret_cast<const unsigned int*>(p.residual + off_lo + ch)));
+          v[0] += r.x; v[1] += r.y;
+        }
+        if (ok_hi) {
+          const float2 r = unpack_bf16(__ldg(reinterpret_cast<const unsigned int*>(p.residual + off_hi + ch)));
+          v[2] += r.x; v[3] += r.y;
+        }
+      }
+      const uint32_t o_lo = pack_bf16(v[0], v[1]), o_hi = pack_bf16(v[2], v[3]);
+      if (ok_lo) *reinterpret_cast<uint32_t*>(p.out + off_lo + ch) = o_lo;
+      if (ok_hi) *reinterpret_cast<uint32_t*>(p.out + off_hi + ch) = o_hi;
+      if (do_stats) {      // statistics of the ROUNDED values the next layer reads
+        const float2 q_lo = ok_lo ? unpack_bf16(o_lo) : make_float2(0.f, 0.f);
+        const float2 q_hi = ok_hi ? unpack_bf16(o_hi) : make_float2(0.f, 0.f);
+        if (p.group_shift >= 3) {          // the 8-column block lies in one group: warp-uniform
+          const int g = ch >> p.group_shift;
+          acc_st.add(q_lo.x, g, s_part, warp, lane); acc_st.add(q_lo.y, g, s_part, warp, lane);
+          acc_st.add(q_hi.x, g, s_part, warp, lane); acc_st.add(q_hi.y, g, s_part, warp, lane);
+        } else {                           // groups narrower than 8 channels (rare): lane 0 adds
+          const float q[4] = {q_lo.x, q_lo.y, q_hi.x, q_hi.y};   // every lane's values in lane order
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int cc = ch + (i & 1);
+            const int g = p.group_shift >= 0 ? cc >> p.group_shift : cc / p.group_size;
+            for (int src = 0; src < 32; ++src) {
+              const float v = __shfl_sync(0xffffffffu, q[i], src);
+              const int gs = __shfl_sync(0xffffffffu, g, src);
+              if (lane == 0 && v != 0.f) { s_part[2 * gs][warp] += v; s_part[2 * gs + 1][warp] += v * v; }
+            }
+          }
+        }
       }
     }
   }
-
-  tc_fence_before();
-  if constexpr (CG == 2) cluster_sync_all();   // neither CTA's smem / TMEM / barriers may vanish early
-  else __syncthreads();
-  if (warp == 0) {
-    __syncwarp();
-    if constexpr (CG == 2) tmem_dealloc_cg2(tmem_base, 2 * ACC_COLS);
-    else tmem_dealloc(tmem_base, 2 * ACC_COLS);
-  }
-}
-
-static int num_sms() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
-  }
-  return n;
-}
-
-template <int BN, int SW, bool XF, int EW, int CG = 1>
-static int launch_gemm2_ew(const adp_conv_gemm_args& a, cudaStream_t stream, int occ_in);
-
-// CTA pairs (cta_group::2) are OPT-IN: adp_debug_set(0, 3).  Measured on B200
-// (profiles/r2_gemm_pairs.txt): the pair MMA removes the shared-memory operand-read bound of the
-// 128 x 128 SS-MMA (MMA phase of the L7 conv3 5.5 us instead of 8.1 us), but every ring stage then
-// costs a cross-CTA handshake (multicast commit -> peer producer -> TMA -> leader's barrier,
-// ~1.8 us per round trip) that a 196 KB ring cannot hide: 16.6 us vs 16.2 us end to end.
-template <int BN, int SW, bool XF>
-static bool use_pairs(const adp_conv_gemm_args& a) {
-  if (BN != 128 || SW != 128 || XF || g_debug[0] != 3) return false;
-  const int taps = a.up_factor > 1 ? 2 : a.ntaps;
-  const long m_tiles = (long)a.B * ((a.T + kBM - 1) / kBM);
-  return m_tiles >= 2 && (a.c_in / 64) * taps >= 8;
+  if (do_stats && cur_b >= 0) publish_stats(cur_b);
 }
 
 template <int BN, int SW, bool XF>
 static int launch_gemm2(const adp_conv_gemm_args& a, cudaStream_t stream) {
-  if constexpr (BN == 128 && SW == 128 && !XF) {
-    if (use_pairs<BN, SW, XF>(a)) {
-      const long m_pairs = ((long)a.B * ((a.T + kBM - 1) / kBM) + 1) / 2;
-      const long total = m_pairs * (a.phases * a.n_pad / BN);
-      // <= one pair tile per CTA pair: nothing overlaps the drain -> 8 drain warps
-      if (g_debug[7] == 0 && 2 * total <= 2L * num_sms()) return launch_gemm2_ew<BN, SW, XF, 8, 2>(a, stream, 1);
-      return launch_gemm2_ew<BN, SW, XF, 4, 2>(a, stream, 1);
-    }
-  }
-  return launch_gemm2_ew<BN, SW, XF, 4>(a, stream, 0);
-}
-
-template <int BN, int SW, bool XF, int EW, int CG>
-static int launch_gemm2_ew(const adp_conv_gemm_args& a, cudaStream_t stream, int occ_in) {
   constexpr int BK = SW / 2;
-  constexpr int WN = BN / CG;
+  auto kernel = conv_gemm2_kernel<BN, SW, XF>;
   const int tiles_per_batch = (a.T + kBM - 1) / kBM;
   const bool up = a.up_factor > 1;
   const int max_taps = up ? 2 : a.ntaps;
@@ -684,32 +405,30 @@ static int launch_gemm2_ew(const adp_conv_gemm_args& a, cudaStream_t stream, int
 
   Gemm2Params p;
   p.a_sub_bytes = (a_rows * SW + 1023) / 1024 * 1024;
-  p.w_sub_bytes = (WN * SW + 1023) / 1024 * 1024;
+  p.w_sub_bytes = (BN * SW + 1023) / 1024 * 1024;
   p.max_taps = max_taps;
   const int chunk_bytes = p.a_sub_bytes + max_taps * p.w_sub_bytes;
 
-  // CTAs per SM: the epilogue (4 warps per CTA) is the critical resource of short-K tiles, so
-  // those run 2-3 CTAs per SM; long-K tiles want deep rings of fat stages instead.
+  // CTAs per SM: short-K tiles are bound by the epilogue, which overlaps another CTA's MMAs
+  // when 2-3 CTAs share an SM; long-K tiles want deep rings of fat stages instead.
   const int w_iters = k_chunks * max_taps;
   int occ = 1;
   if (BN <= 64 && w_iters <= 8) occ = 3;
   else if (BN <= 128 && w_iters <= 12) occ = 2;
   if (XF && occ > (BN <= 64 ? 2 : 1)) occ = BN <= 64 ? 2 : 1;
   if (g_debug[3] > 0) occ = g_debug[3];
-  if (occ_in > 0) occ = occ_in;
-  const int tmem_occ = 512 / (2 * (BN < 32 ? 32 : BN));
-  if (occ > tmem_occ) occ = tmem_occ;
-  auto budget_of = [](int o) {
-    return (o == 1 ? (EW == 8 ? 204 : 196) : (o == 2 ? (XF ? 92 : 96) : 60)) * 1024;   // 227 KB - static - 1 KB
-  };  // <= 11 KB static smem/CTA
-  while (occ > 1 && budget_of(occ) < 2 * chunk_bytes) --occ;   // need >= 2 stages in the ring
-  if constexpr (EW == 4 && !XF && BN >= 64 && CG == 1) {
-    // at most ~two tiles per SM: little or nothing overlaps the drain -> one CTA per SM with
-    // 8 drain warps (also when 2 CTAs/SM were possible but every SM gets <= one tile anyway)
-    const long total = (long)a.B * tiles_per_batch * (a.phases * a.n_pad / BN);
-    if (g_debug[7] == 0 && ((occ == 1 && total <= 2L * num_sms()) || total <= (long)num_sms()))
-      return launch_gemm2_ew<BN, SW, XF, 8>(a, stream, 1);
+  static int static_smem = -1;
+  if (static_smem < 0) {
+    cudaFuncAttributes fa;
+    ADP_CUDA(cudaFuncGetAttributes(&fa, kernel));
+    static_smem = static_cast<int>(fa.sharedSizeBytes);
   }
+  auto budget_of = [&](int o) {   // ring bytes per CTA: 1 KB reserved per CTA, 1 KB alignment slack
+    int per_cta = kSmemPerSM / o - 1024;
+    if (per_cta > kSmemPerBlock) per_cta = kSmemPerBlock;
+    return per_cta - static_smem - 1024;
+  };
+  while (occ > 1 && budget_of(occ) < 2 * chunk_bytes) --occ;   // need >= 2 stages in the ring
   const int budget = budget_of(occ);
   // chunks per stage: amortise one mbarrier round trip over >= 8 MMAs where smem allows
   int kc = 1;
@@ -737,12 +456,17 @@ static int launch_gemm2_ew(const adp_conv_gemm_args& a, cudaStream_t stream, int
   {
     const uint64_t dims[2] = {(uint64_t)a.k_total, (uint64_t)a.phases * a.n_pad};
     const uint64_t strides[1] = {(uint64_t)a.k_total * 2};
-    const uint32_t box[2] = {(uint32_t)BK, (uint32_t)WN};
+    const uint32_t box[2] = {(uint32_t)BK, (uint32_t)BN};
     if (int e = make_tmap_bf16(&tmW, a.w, 2, dims, strides, box, SW)) return e;
   }
 
   static SmemAttrCache smem_cache;
-  ADP_CUDA(ensure_dyn_smem(conv_gemm2_kernel<BN, SW, XF, EW, CG>, smem, smem_cache));
+  ADP_CUDA(ensure_dyn_smem(kernel, smem, smem_cache));
+  int occ_hw = 1;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_hw, kernel, kGemmThreads, smem) != cudaSuccess ||
+      occ_hw < 1)
+    occ_hw = 1;
+  if (occ > occ_hw) occ = occ_hw;
 
   p.out = static_cast<__nv_bfloat16*>(a.out);
   p.residual = static_cast<const __nv_bfloat16*>(a.residual);
@@ -767,9 +491,8 @@ static int launch_gemm2_ew(const adp_conv_gemm_args& a, cudaStream_t stream, int
   p.out_fp32 = a.out_fp32;
   p.ld_gate = a.ld_gate > 0 ? a.ld_gate : a.n_valid;
   p.n_tiles_n = a.phases * a.n_pad / BN;
-  p.total_tiles = (a.B * tiles_per_batch + CG - 1) / CG * p.n_tiles_n;   // pair tiles when CG == 2
+  p.total_tiles = a.B * tiles_per_batch * p.n_tiles_n;
   p.a_rows = a_rows;
-  p.dbg = g_debug[4];
   p.early_w = g_debug[2];
   p.gn_stats = a.gn_stats;
   p.gn_gamma = a.gn_gamma;
@@ -777,13 +500,11 @@ static int launch_gemm2_ew(const adp_conv_gemm_args& a, cudaStream_t stream, int
   p.gn_eps = a.gn_eps;
   p.gn_groups = a.gn_groups > 0 ? a.gn_groups : 1;
 
-  // grid in units of CTA groups (single CTAs, or pairs)
-  const int slots = occ * num_sms() / CG;
+  const int slots = occ * num_sms();
   int grid = p.total_tiles < slots ? p.total_tiles : slots;
   p.tiles_per_cta = (p.total_tiles + grid - 1) / grid;
   grid = (p.total_tiles + p.tiles_per_cta - 1) / p.tiles_per_cta;
-  ADP_CUDA(launch_k_cluster(conv_gemm2_kernel<BN, SW, XF, EW, CG>, dim3(grid * CG),
-                            dim3(64 + 32 * EW + (XF ? 256 : 0)), smem, stream, CG, tmA, tmW, p));
+  ADP_CUDA(launch_k(kernel, dim3(grid), dim3(kGemmThreads), smem, stream, tmA, tmW, p));
   ADP_LAUNCH_CHECK();
   return 0;
 }

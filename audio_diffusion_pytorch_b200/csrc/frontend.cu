@@ -251,7 +251,7 @@ extern "C" int adp_resample(const float* x, const float* bank, float* y, int row
                 taps > 0 && half >= 0, "adp_resample: bad sizes");
   const size_t smem = static_cast<size_t>(factor_out) * taps * sizeof(float);
   ADP_CHECK(smem <= 48 * 1024, "adp_resample: filter bank of %zu bytes exceeds 48 KB", smem);
-  ADP_CUDA(launch_k(resample_kernel, dim3(grid_1d(t_out, 256, 148 * 8), rows), dim3(256), smem,
+  ADP_CUDA(launch_k(resample_kernel, dim3(grid_1d(t_out, 256, num_sms() * 8), rows), dim3(256), smem,
                     as_stream(stream), x, bank, y, t, t_out, factor_in, factor_out, taps, half));
   ADP_LAUNCH_CHECK();
   return 0;
@@ -265,7 +265,7 @@ extern "C" int adp_resample_adjoint(const float* dy, const float* bank, float* d
                 taps > 0 && half >= 0, "adp_resample_adjoint: bad sizes");
   const size_t smem = static_cast<size_t>(factor_out) * taps * sizeof(float);
   ADP_CHECK(smem <= 48 * 1024, "adp_resample_adjoint: filter bank of %zu bytes exceeds 48 KB", smem);
-  ADP_CUDA(launch_k(resample_adjoint_kernel, dim3(grid_1d(t, 256, 148 * 8), rows), dim3(256), smem,
+  ADP_CUDA(launch_k(resample_adjoint_kernel, dim3(grid_1d(t, 256, num_sms() * 8), rows), dim3(256), smem,
                     as_stream(stream), dy, bank, dx, t, t_out, factor_in, factor_out, taps, half));
   ADP_LAUNCH_CHECK();
   return 0;
@@ -300,7 +300,7 @@ extern "C" int adp_to_flat(const float* spec, const float* w, float* out, int B,
   ADP_CHECK(spec && w && out, "adp_to_flat: null pointer");
   ADP_CHECK(B > 0 && B <= 65535 && C > 0 && frames > 0 && win > 0 && hop > 0 && pad >= 0 &&
                 t_out == (frames - 1) * hop - 2 * pad + win, "adp_to_flat: bad sizes");
-  ADP_CUDA(launch_k(to_flat_kernel, dim3(grid_1d(t_out, 256, 148 * 8), B), dim3(256), (size_t)0,
+  ADP_CUDA(launch_k(to_flat_kernel, dim3(grid_1d(t_out, 256, num_sms() * 8), B), dim3(256), (size_t)0,
                     as_stream(stream), spec, w, out, C, frames, win, hop, pad, t_out));
   ADP_LAUNCH_CHECK();
   return 0;

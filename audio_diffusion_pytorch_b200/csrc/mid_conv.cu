@@ -3,8 +3,7 @@
 //
 // These levels are HBM-bound: a conv3 is only 6*C flop per byte moved.  The three-kernel path
 // (adp_gn_silu -> adp_conv_gemm -> adp_ln_film) streams the level's tensor through HBM five to
-// seven times and its 128 x C tcgen05 tiles are dominated by per-tile barrier / drain overheads
-// (profiles/r1_gemm_skeleton_v5.txt).  Here GroupNorm-apply + SiLU happens while rows are staged
+// seven times and its 128 x C wgmma tiles are dominated by per-tile barrier / drain overheads.  Here GroupNorm-apply + SiLU happens while rows are staged
 // into smem, the conv is a [rows x 3C] x [3C x C] GEMM on mma.sync.m16n8k16 (A fragments by
 // ldmatrix over overlapping row windows: tap k of row t is smem row t + k; weights as bf16 in
 // smem), and bias, residual, LayerNorm + FiLM and the next GroupNorm's statistics are applied
@@ -14,7 +13,7 @@
 //   * smem rows padded by 16 bytes so ldmatrix (8 rows x 16 B) and the 4-byte residual reads
 //     in accumulator layout are bank-conflict free
 //   * SiLU with one MUFU op (tanh.approx); operands enter the tensor core as bf16 exactly like
-//     on the tcgen05 path of the wider levels
+//     on the wgmma path of the wider levels
 #include "common.cuh"
 #include "ptx.cuh"
 
@@ -62,7 +61,7 @@ struct MidCfg {
 // and output stores, FiLM coefficients of the thread's 8 channels in registers, 3 shuffles per
 // reduction.  (The first version ran the epilogue in the accumulator-fragment layout: 4-byte
 // stores, 4-byte shared-memory residual reads and a shuffle chain per fragment row made the
-// kernel issue/latency bound at 15-40 % of HBM bandwidth, profiles/r2_ncu_mid_conv64.txt.)
+// kernel issue/latency bound well below HBM bandwidth.)
 template <int C, int NTH>
 __global__ void __launch_bounds__(NTH, 512 / NTH) mid_conv_kernel(const adp_narrow_conv_args a) {
   using Cfg = MidCfg<C, NTH>;
@@ -319,8 +318,7 @@ __global__ void __launch_bounds__(NTH, 512 / NTH) mid_conv_kernel(const adp_narr
   }
 }
 
-// 256: measured A/B on B200 (tools/time_mid_threads.py, L2 flushed): 128 x 4 is 5-6 % faster for
-// C = 32 at 16 batch rows, 7-8 % slower for C = 64 at 8, equal elsewhere; no change end to end
+// threads per block (adp_debug_set(8, 128 | 256); A/B timing: tools/time_mid_threads.py)
 int g_mid_threads = 256;
 
 template <int C, int NTH>
@@ -328,9 +326,8 @@ static int launch_mid(const adp_narrow_conv_args& a, cudaStream_t stream) {
   using Cfg = MidCfg<C, NTH>;
   static SmemAttrCache smem_cache;
   ADP_CUDA(ensure_dyn_smem(mid_conv_kernel<C, NTH>, (size_t)Cfg::SMEM, smem_cache));
-  int dev = 0, sms = 148, occ = 1;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  int occ = 1;
+  const int sms = num_sms();
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, mid_conv_kernel<C, NTH>, NTH, Cfg::SMEM) != cudaSuccess ||
       occ < 1)
     occ = 1;

@@ -563,9 +563,9 @@ extern "C" int adp_gn_silu(const void* x, void* y, const double* stats, const fl
   const int vpr = C / 8;
   const bool reg = vpr <= 256 && (vpr & (vpr - 1)) == 0;
   // small tensors (the deep levels) are latency-bound: one vector per thread, many blocks
-  const bool small = static_cast<size_t>(B) * nvec <= static_cast<size_t>(148) * 2048 * 2;
+  const bool small = static_cast<size_t>(B) * nvec <= static_cast<size_t>(num_sms()) * 2048 * 2;
   const int tile = small ? 256 : 1024;
-  dim3 grid(pick_grid(nvec, tile, 148 * 16 / (B < 16 ? B : 16) + 1), B);
+  dim3 grid(pick_grid(nvec, tile, num_sms() * 16 / (B < 16 ? B : 16) + 1), B);
 #define ADP_GN(REG, NV)                                                                         \
   ADP_CUDA(launch_k(gn_silu_kernel<REG, NV>, grid, dim3(256), (size_t)0, as_stream(stream),     \
                     static_cast<const uint4*>(x), static_cast<uint4*>(y), stats, gamma, beta,    \
@@ -585,7 +585,7 @@ extern "C" int adp_gn_stats(const void* x, double* stats, int32_t B, int32_t T, 
   ADP_CHECK(C % 8 == 0 && C <= 2048 && groups > 0 && groups <= 64 && C % groups == 0,
             "adp_gn_stats: C=%d groups=%d unsupported", C, groups);
   const size_t nvec = static_cast<size_t>(T) * (C / 8);
-  dim3 grid(pick_grid(nvec, 256 * 8, 148 * 8 / (B < 8 ? B : 8) + 1), B);
+  dim3 grid(pick_grid(nvec, 256 * 8, num_sms() * 8 / (B < 8 ? B : 8) + 1), B);
   ADP_CUDA(launch_k(gn_stats_kernel, grid, dim3(256), (size_t)0, as_stream(stream),
                     static_cast<const uint4*>(x), stats, (int)T, (int)C, (int)groups));
   ADP_LAUNCH_CHECK();
@@ -626,8 +626,8 @@ extern "C" int adp_ln_film_dual(const void* x, void* y, void* y2, const float* s
   const int unr = vpl <= 2 ? 2 : 1;
   const int rows_per_block = 8 * (32 / lpr) * unr;
   // deep levels have few rows: one pass per warp (all SMs busy) instead of two
-  const bool few = static_cast<size_t>(B) * ((T + rows_per_block - 1) / rows_per_block) <= 148 * 4;
-  dim3 grid(pick_grid(T, few ? rows_per_block : rows_per_block * 2, 148 * 16 / (B < 16 ? B : 16) + 1), B);
+  const bool few = static_cast<size_t>(B) * ((T + rows_per_block - 1) / rows_per_block) <= num_sms() * 4;
+  dim3 grid(pick_grid(T, few ? rows_per_block : rows_per_block * 2, num_sms() * 16 / (B < 16 ? B : 16) + 1), B);
   const uint4* xi = static_cast<const uint4*>(x);
   uint4* yo = static_cast<uint4*>(y);
   cudaStream_t s = as_stream(stream);
@@ -655,7 +655,7 @@ extern "C" int adp_skinny_linear(const float* x, const void* w, const float* bia
   const size_t smem = static_cast<size_t>(kSkinnyRows) * K * sizeof(float);
   static SmemAttrCache smem_cache;
   ADP_CUDA(ensure_dyn_smem(skinny_linear_kernel, smem, smem_cache));
-  dim3 grid(pick_grid(N, 8, 148 * 2), (B + kSkinnyRows - 1) / kSkinnyRows);
+  dim3 grid(pick_grid(N, 8, num_sms() * 2), (B + kSkinnyRows - 1) / kSkinnyRows);
   ADP_CUDA(launch_k(skinny_linear_kernel, grid, dim3(256), smem, as_stream(stream), x,
                     static_cast<const __nv_bfloat16*>(w), bias, y, (int)B, (int)K, (int)N, (int)ldx,
                     (int)ldw, (int)ldy, (int)in_act, (int)out_act));
@@ -674,7 +674,7 @@ extern "C" int adp_time_features(const float* sigma, const float* freqs, float* 
 
 extern "C" int adp_silu_bf16(const float* x, void* y, int64_t n, adp_stream_t stream) {
   ADP_CHECK(x && y && n > 0, "adp_silu_bf16: bad args");
-  ADP_CUDA(launch_k(silu_bf16_kernel, dim3(pick_grid(static_cast<size_t>(n), 256, 148 * 4)),
+  ADP_CUDA(launch_k(silu_bf16_kernel, dim3(pick_grid(static_cast<size_t>(n), 256, num_sms() * 4)),
                     dim3(256), (size_t)0, as_stream(stream), x, static_cast<__nv_bfloat16*>(y), n));
   ADP_LAUNCH_CHECK();
   return 0;
@@ -684,7 +684,7 @@ extern "C" int adp_step_select(const int32_t* step, const int64_t* ctrl, const f
                                float* ab_out, float* ss_out, int64_t ss_elems, adp_stream_t stream) {
   ADP_CHECK(step && ctrl && ab_table && ab_out && ss_out && ss_elems > 0 && ss_elems % 4 == 0,
             "adp_step_select: bad args");
-  ADP_CUDA(launch_k(step_select_kernel, dim3(pick_grid(static_cast<size_t>(ss_elems / 4), 256 * 4, 148 * 4)),
+  ADP_CUDA(launch_k(step_select_kernel, dim3(pick_grid(static_cast<size_t>(ss_elems / 4), 256 * 4, num_sms() * 4)),
                     dim3(256), (size_t)0, as_stream(stream), step, reinterpret_cast<const long long*>(ctrl),
                     ab_table, ab_out, ss_out, ss_elems));
   ADP_LAUNCH_CHECK();
@@ -701,7 +701,7 @@ extern "C" int adp_step_advance(int32_t* step, adp_stream_t stream) {
 extern "C" int adp_inpaint_blend(float* x, const float* source, const float* noise, const uint8_t* mask,
                                  const float* ab, int64_t n, adp_stream_t stream) {
   ADP_CHECK(x && source && noise && mask && ab && n > 0, "adp_inpaint_blend: bad args");
-  ADP_CUDA(launch_k(inpaint_blend_kernel, dim3(pick_grid(static_cast<size_t>(n), 256 * 4, 148 * 8)),
+  ADP_CUDA(launch_k(inpaint_blend_kernel, dim3(pick_grid(static_cast<size_t>(n), 256 * 4, num_sms() * 8)),
                     dim3(256), (size_t)0, as_stream(stream), x, source, noise, mask, ab, n));
   ADP_LAUNCH_CHECK();
   return 0;
@@ -710,7 +710,7 @@ extern "C" int adp_inpaint_blend(float* x, const float* source, const float* noi
 extern "C" int adp_arv_step(float* chan, const float* v, const float* sig_next, int B, int C, int T,
                             adp_stream_t stream) {
   ADP_CHECK(chan && v && sig_next && B > 0 && C > 0 && T > 0, "adp_arv_step: bad args");
-  ADP_CUDA(launch_k(arv_step_kernel, dim3(pick_grid(static_cast<size_t>(B) * T, 256, 148 * 8)), dim3(256),
+  ADP_CUDA(launch_k(arv_step_kernel, dim3(pick_grid(static_cast<size_t>(B) * T, 256, num_sms() * 8)), dim3(256),
                     (size_t)0, as_stream(stream), chan, v, sig_next, B, C, T));
   ADP_LAUNCH_CHECK();
   return 0;
@@ -719,7 +719,7 @@ extern "C" int adp_arv_step(float* chan, const float* v, const float* sig_next, 
 extern "C" int adp_sampler_step(const float* x, const float* v, const float* ab, float* x_next,
                                 int64_t n, adp_stream_t stream) {
   ADP_CHECK(x && v && ab && x_next && n > 0, "adp_sampler_step: bad args");
-  ADP_CUDA(launch_k(sampler_step_kernel, dim3(pick_grid(static_cast<size_t>(n), 256 * 4, 148 * 8)),
+  ADP_CUDA(launch_k(sampler_step_kernel, dim3(pick_grid(static_cast<size_t>(n), 256 * 4, num_sms() * 8)),
                     dim3(256), (size_t)0, as_stream(stream), x, v, ab, x_next, n));
   ADP_LAUNCH_CHECK();
   return 0;

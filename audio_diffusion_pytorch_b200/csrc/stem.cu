@@ -11,9 +11,8 @@ namespace adp {
 // resident blocks (a grid larger than occupancy * SMs would run a second, mostly empty wave)
 template <typename K>
 static int persistent_gx(K kernel, int threads, size_t smem, int B, int n_tiles) {
-  int dev = 0, sms = 148, occ = 1;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  int occ = 1;
+  const int sms = num_sms();
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, threads, smem) != cudaSuccess || occ < 1)
     occ = 1;
   int gx = (occ * sms) / B;
@@ -300,7 +299,7 @@ __global__ void __launch_bounds__(256, 3) stem_out_kernel(const adp_stem_out_arg
 
 // -------------------------------------------------------------------------- narrow_conv
 // C == 8 ConvBlock on the warp-level tensor cores.  A C=8 conv3 is a [T x 24] x [24 x 8] GEMM:
-// far too thin for a tcgen05 tile (M=128 x N>=16 x K=16 with 32-byte TMA rows), but it fits
+// far too thin for a wgmma tile (M=64 x N>=16 x K=16 with 32-byte TMA rows), but it fits
 // mma.sync m16n8k16 exactly: K = tap*8 + ci (24, padded to 32 with zero weights), N = 8.
 //   * GroupNorm+SiLU is applied while staging rows into smem as bf16 (16 bytes per row), so
 //     the A fragment of rows [r, r+16) x taps {0,1} is ONE ldmatrix.x4 over overlapping row

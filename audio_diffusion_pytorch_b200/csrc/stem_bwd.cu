@@ -11,7 +11,7 @@ constexpr int kTB = 256;
 
 // blocks per batch element for the persistent tile loops: ~4 blocks per SM in total
 static int persistent_blocks(int n_tiles, int B) {
-  int g = (148 * 4 + B - 1) / B;
+  int g = (num_sms() * 4 + B - 1) / B;
   if (g > n_tiles) g = n_tiles;
   return g < 1 ? 1 : g;
 }
@@ -33,7 +33,7 @@ narrow_conv_bwd_kernel(const adp_narrow_conv_bwd_args a) {
   const int b = blockIdx.y;
   // persistent over row tiles: the parameter gradients stay in registers / smem and reach global
   // memory with ONE atomic per parameter per block (one block per tile meant 4096 same-address
-  // atomics per parameter and a 130 us kernel, profiles/r2_train_profile_start.txt)
+  // atomics per parameter)
   const int n_tiles = (a.T + kTB - 1) / kTB;
   static_assert(C == 8, "register layout of the weight-gradient accumulators assumes C = 8");
   float gwr[2][C][3], gb[2] = {0.f, 0.f};              // dw[2 co][C ci][3 taps], dbias[2 co]

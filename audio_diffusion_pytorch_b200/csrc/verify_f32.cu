@@ -4,7 +4,7 @@
 // SiLU / GELU / exp).  It exists to check the PROGRAM -- weight packing, LayerNorm folds, phase-folded
 // upsample convs, the concatenated conditioning GEMM, guidance combine, sampler update -- against
 // the reference at fp32 tolerance (rtol 1e-3 / atol 1e-4), which the bf16 storage of the fast
-// path cannot show.  Not a performance path: ~100x slower than the tcgen05 kernels.
+// path cannot show.  Not a performance path: far slower than the tensor-core kernels.
 // Entry points mirror their bf16 counterparts argument for argument (a/w/out/residual/h are fp32).
 #include "common.cuh"
 #include "ptx.cuh"
@@ -302,7 +302,7 @@ __global__ void __launch_bounds__(256) f32_stem_out_kernel(const adp_stem_out_ar
 static int f32_grid(int64_t n) {
   int64_t g = (n + 255) / 256;
   if (g < 1) g = 1;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > num_sms() * 16) g = num_sms() * 16;
   return static_cast<int>(g);
 }
 
@@ -328,7 +328,7 @@ extern "C" int adp_f32_gn_stats(const float* x, double* stats, int B, int T, int
   ADP_CHECK(x && stats && B > 0 && B <= 65535 && T > 0 && C > 0 && groups > 0 && groups <= 64 && C % groups == 0,
             "adp_f32_gn_stats: bad args");
   int gx = f32_grid(static_cast<int64_t>(T) * C);
-  if (gx > 148 * 4) gx = 148 * 4;
+  if (gx > num_sms() * 4) gx = num_sms() * 4;
   ADP_CUDA(launch_k(f32_gn_stats_kernel, dim3(gx, B), dim3(256), (size_t)0, as_stream(stream), x, stats, T, C,
                     groups));
   ADP_LAUNCH_CHECK();
@@ -360,7 +360,7 @@ extern "C" int adp_f32_attention(const float* q, const float* k, const float* v,
   ADP_CHECK(q && k && v && o && B > 0 && H > 0 && Tq > 0 && Tk > 0, "adp_f32_attention: bad args");
   int64_t n = static_cast<int64_t>(B) * H * Tq;
   int64_t g = (n + 127) / 128;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > num_sms() * 16) g = num_sms() * 16;
   ADP_CUDA(launch_k(f32_attention_kernel, dim3(static_cast<int>(g)), dim3(128), (size_t)0, as_stream(stream), q, k,
                     v, o, B, H, Tq, Tk, ldq, ldk, ldv, ldo, scale));
   ADP_LAUNCH_CHECK();

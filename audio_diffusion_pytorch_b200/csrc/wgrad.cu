@@ -1,15 +1,16 @@
-// adp_wgrad: weight-gradient GEMM on tcgen05 (backward of adp_conv_gemm w.r.t. W).
+// adp_wgrad: weight-gradient GEMM on wgmma (backward of adp_conv_gemm w.r.t. W).
 //
 //   dW[n = out channel][k = in channel] += sum_{b,t} G[b, t, g_col0 + n] * X[b, t + off, x_col0 + k]
 //
 // The reduction runs over TIME, which is the strided dimension of both channels-last
 // operands, so both are fed to the tensor core as MN-major tiles exactly as they lie in
 // memory (no transposes): a 64-time-step chunk of G is the A operand (M = 128 out channels =
-// two 64-channel swizzle chunks, LBO apart), the row-shifted chunk of X the B operand
-// (N = BN in channels).  TMA zero-fills rows outside [0,T) (conv padding) and channels beyond
-// the tensor (C < 64), so narrow levels just run padded tiles.  fp32 accumulation in TMEM
-// over the CTA's share of the (batch, time) chunks, then fp32 atomics into dW (split-K over
-// time across CTAs).  Warp roles: 0 TMA producer (+TMEM), 1 MMA issuer, 2-5 epilogue.
+// two 64-channel swizzle chunks, one per consumer warpgroup), the row-shifted chunk of X the B
+// operand (N = BN in channels, 64-channel chunks LBO apart).  TMA zero-fills rows outside
+// [0,T) (conv padding) and channels beyond the tensor (C < 64), so narrow levels just run
+// padded tiles.  fp32 accumulation in registers over the CTA's share of the (batch, time)
+// chunks, then fp32 atomics into dW (split-K over time across CTAs).  Warp roles: 0-7 the two
+// consumer warpgroups, 8 the TMA producer.
 #include "common.cuh"
 #include "ptx.cuh"
 
@@ -18,6 +19,7 @@ namespace adp {
 constexpr int kWgChunk = 64;          // time steps per pipeline stage
 constexpr int kWgBoxBytes = 64 * 128; // one TMA box: 64 rows x 64 channels bf16
 constexpr int kWgMaxStages = 8;
+constexpr int kWgThreads = 288;
 
 struct WgradParams {
   float* dw;
@@ -32,20 +34,17 @@ struct WgradParams {
 // NT = 3: the three taps of a k=3 convolution in ONE launch.  The X box carries 2 extra time rows;
 // tap j is the same smem tile read through a descriptor whose start is advanced by j rows (the
 // 128-byte swizzle is a function of the absolute address, as for the shifted-tap forward GEMM), and
-// accumulates into its own TMEM columns.  G and X are read once instead of three times.
+// accumulates into its own registers.  G and X are read once instead of three times.
 template <int BN, int NT>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(kWgThreads, 1)
 wgrad_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CUtensorMap tmX,
              const WgradParams p) {
   constexpr int NB = BN / 64;
   constexpr int XBOX = NT == 1 ? kWgBoxBytes : 9 * 1024;        // (64 + NT - 1) rows x 128 B, 1 KB-rounded
   constexpr int STAGE_BYTES = 2 * kWgBoxBytes + NB * XBOX;
-  constexpr int TCOLS = NT * BN <= 32 ? 32 : (NT * BN <= 64 ? 64 : (NT * BN <= 128 ? 128 : (NT * BN <= 256 ? 256 : 512)));
-  static_assert(NT * BN <= 512, "accumulators of all taps must fit TMEM");
+  static_assert(NT * BN <= 256, "accumulators of all taps must fit the register file");
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t full_bar[kWgMaxStages], empty_bar[kWgMaxStages];
-  __shared__ uint64_t acc_full;
-  __shared__ uint32_t tmem_slot;
 
   pdl_launch_dependents();
   const int warp = warp_id_uniform();
@@ -59,23 +58,16 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CU
   int chunk_end = chunk_begin + p.chunks_per_split;
   if (chunk_end > p.total_chunks) chunk_end = p.total_chunks;
 
-  if (warp == 0) {
-    tmem_alloc(&tmem_slot, TCOLS);
-    tmem_relinquish();
-  } else if (warp == 1 && lane == 0) {
-    for (int s = 0; s < p.n_stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(&acc_full, 1);
+  if (warp == 8 && lane == 0) {
+    for (int s = 0; s < p.n_stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
     fence_mbar_init();
     tma_prefetch_desc(&tmG);
     tma_prefetch_desc(&tmX);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, tmem_slot, 0);   // warp-uniform for ptxas
   pdl_wait();
 
-  if (warp == 0) {
+  if (warp == 8) {
     // whole warp runs the loop (uniform control flow), one elected lane issues: see ptx.cuh
     int s = 0;
     uint32_t ph = 0;
@@ -98,80 +90,63 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CU
       __syncwarp();
       if (++s == p.n_stages) { s = 0; ph ^= 1; }
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = umma_idesc_bf16(128, BN, 1, 1);     // both operands MN-major
-    // MN-major SW128: 64-channel chunks kWgBoxBytes apart (LBO), 8-row groups 1024 B (SBO)
-    const uint64_t desc0 = umma_desc_mnmajor_sw128(smem_u32(ring), kWgBoxBytes);
-    const uint64_t xdesc0 = umma_desc_mnmajor_sw128(smem_u32(ring) + 2 * kWgBoxBytes, XBOX);
-    int s = 0;
-    uint32_t ph = 0, accumulate = 0;
-    for (int c = chunk_begin; c < chunk_end; ++c) {
-      mbar_wait(&full_bar[s], ph);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t gdesc = desc0 + static_cast<uint64_t>((s * STAGE_BYTES) >> 4);
-        const uint64_t xdesc = xdesc0 + static_cast<uint64_t>((s * STAGE_BYTES) >> 4);
-#pragma unroll
-        for (int tap = 0; tap < NT; ++tap) {
-#pragma unroll
-          for (int kk = 0; kk < kWgChunk / 16; ++kk) {      // 16 time steps per MMA = 2048 B
-            umma_bf16(tmem_base + tap * BN, gdesc + ((kk * 2048) >> 4),
-                      xdesc + ((tap * 128 + kk * 2048) >> 4), idesc, accumulate | (kk != 0));
-          }
-        }
-        umma_commit(&empty_bar[s]);
-        if (c == chunk_end - 1) umma_commit(&acc_full);
-      }
-      accumulate = 1;
-      __syncwarp();
-      if (++s == p.n_stages) { s = 0; ph ^= 1; }
-    }
-    // an empty split still has to release the epilogue
-    if (chunk_end <= chunk_begin && elect_one()) umma_commit(&acc_full);
-  } else {
-    mbar_wait(&acc_full, 0);
-    tc_fence_after();
-    const int q = warp & 3;
-    const int n = n0 + q * 32 + lane;           // this thread's out channel (TMEM lane)
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-#pragma unroll 1
-    for (int tc = 0; tc < NT * BN; tc += 32) {
-      const int tap = tc / BN, c0 = tc - tap * BN;
-      float* drow = p.dw + tap * p.tap_stride + static_cast<size_t>(n < p.n_valid ? n : 0) * p.ldw;
-      uint32_t r[32];
-      tmem_ld32(taddr + tc, r);
-      tmem_ld_wait();
-      if (n < p.n_valid && chunk_end > chunk_begin) {
-        if (gridDim.z == 1 && k0 + c0 + 32 <= p.k_valid && (p.ldw & 3) == 0) {
-          // single writer of this tile (dW is pre-zeroed): plain 16-byte stores
-#pragma unroll
-          for (int i = 0; i < 32; i += 4)
-            *reinterpret_cast<float4*>(drow + k0 + c0 + i) =
-                make_float4(__uint_as_float(r[i]), __uint_as_float(r[i + 1]),
-                            __uint_as_float(r[i + 2]), __uint_as_float(r[i + 3]));
-        } else if (k0 + c0 + 32 <= p.k_valid && (p.ldw & 3) == 0 && (p.tap_stride & 3) == 0) {
-          // split-K over time: 16-byte vector reductions (one per 4 columns instead of four scalar
-          // atomics whose 32 lanes hit 32 different rows = 32 sectors per instruction)
-#pragma unroll
-          for (int i = 0; i < 32; i += 4)
-            atomicAdd(reinterpret_cast<float4*>(drow + k0 + c0 + i),
-                      make_float4(__uint_as_float(r[i]), __uint_as_float(r[i + 1]),
-                                  __uint_as_float(r[i + 2]), __uint_as_float(r[i + 3])));
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const int k = k0 + c0 + i;
-            if (k < p.k_valid) atomicAdd(drow + k, __uint_as_float(r[i]));
-          }
-        }
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
+
+  // -------------------------------------------------------------------------- consumers
+  const int wg = threadIdx.x >> 7;             // out channels [64*wg, 64*wg + 64) of the tile
+  // MN-major SW128: G box of this warpgroup (one 64-channel chunk); X chunks XBOX apart (LBO);
+  // 8-row groups 1024 B apart (SBO); 16 time steps per MMA = 2048 B
+  const uint64_t gdesc0 = gmma_desc_mnmajor_sw128(smem_u32(ring) + wg * kWgBoxBytes, kWgBoxBytes);
+  const uint64_t xdesc0 = gmma_desc_mnmajor_sw128(smem_u32(ring) + 2 * kWgBoxBytes, XBOX);
+  float acc[NT][BN / 2];
+  int s = 0;
+  uint32_t ph = 0, accumulate = 0;
+  for (int c = chunk_begin; c < chunk_end; ++c) {
+    mbar_wait(&full_bar[s], ph);
+    const uint64_t gdesc = gdesc0 + static_cast<uint64_t>((s * STAGE_BYTES) >> 4);
+    const uint64_t xdesc = xdesc0 + static_cast<uint64_t>((s * STAGE_BYTES) >> 4);
+    wgmma_fence();
+#pragma unroll
+    for (int tap = 0; tap < NT; ++tap) {
+#pragma unroll
+      for (int kk = 0; kk < kWgChunk / 16; ++kk)
+        Wgmma<BN>::template ss<1, 1>(acc[tap], gdesc + ((kk * 2048) >> 4),
+                                     xdesc + ((tap * 128 + kk * 2048) >> 4), accumulate | (kk != 0));
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
     __syncwarp();
-    tmem_dealloc(tmem_base, TCOLS);
+    if (lane == 0) mbar_arrive(&empty_bar[s]);
+    accumulate = 1;
+    if (++s == p.n_stages) { s = 0; ph ^= 1; }
+  }
+  if (chunk_end <= chunk_begin) return;        // an empty split contributes nothing
+#pragma unroll
+  for (int tap = 0; tap < NT; ++tap) acc_fence(acc[tap]);
+
+  const bool single = gridDim.z == 1;          // single writer of this tile (dW is pre-zeroed)
+  const bool pairs = (p.ldw & 1) == 0 && (p.tap_stride & 1) == 0;
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int n = n0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * r;
+    if (n >= p.n_valid) continue;
+#pragma unroll
+    for (int tap = 0; tap < NT; ++tap) {
+      float* drow = p.dw + tap * p.tap_stride + static_cast<size_t>(n) * p.ldw;
+#pragma unroll
+      for (int jb = 0; jb < BN / 8; ++jb) {
+        const int k = k0 + 8 * jb + 2 * (lane & 3);
+        const float v0 = acc[tap][4 * jb + 2 * r], v1 = acc[tap][4 * jb + 2 * r + 1];
+        if (k + 1 < p.k_valid && pairs) {
+          if (single) *reinterpret_cast<float2*>(drow + k) = make_float2(v0, v1);
+          else atomicAdd(reinterpret_cast<float2*>(drow + k), make_float2(v0, v1));
+        } else {
+          if (k < p.k_valid) { if (single) drow[k] = v0; else atomicAdd(drow + k, v0); }
+          if (k + 1 < p.k_valid) { if (single) drow[k + 1] = v1; else atomicAdd(drow + k + 1, v1); }
+        }
+      }
+    }
   }
 }
 
@@ -210,9 +185,7 @@ static int launch_wgrad(const adp_wgrad_args& a, cudaStream_t stream) {
   if (n_stages > kWgMaxStages) n_stages = kWgMaxStages;
   p.n_stages = n_stages;
   const int n_tiles = (a.n + 127) / 128, k_tiles = (a.k + BN - 1) / BN;
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = num_sms();
   // split-K over time: every split ends in NT x 128 x BN fp32 reductions into dW.  Narrow outputs
   // (few tiles) need many splits to fill the SMs; wide outputs pay for every split in atomics:
   // cap the total reduction traffic at ~4 M elements and keep >= 4 chunks per CTA
@@ -228,7 +201,7 @@ static int launch_wgrad(const adp_wgrad_args& a, cudaStream_t stream) {
   static SmemAttrCache smem_cache;
   ADP_CUDA(ensure_dyn_smem(wgrad_kernel<BN, NT>, smem, smem_cache));
   dim3 grid(n_tiles, k_tiles, splits);
-  ADP_CUDA(launch_k(wgrad_kernel<BN, NT>, grid, dim3(192), smem, stream, tmG, tmX, p));
+  ADP_CUDA(launch_k(wgrad_kernel<BN, NT>, grid, dim3(kWgThreads), smem, stream, tmG, tmX, p));
   return 0;
 }
 
@@ -245,9 +218,8 @@ extern "C" int adp_wgrad(const adp_wgrad_args* args, adp_stream_t stream) {
   ADP_CHECK(a.g_col0 + a.n <= a.g_cols && a.x_col0 + a.k <= a.x_cols, "adp_wgrad: columns out of range");
   ADP_CHECK(a.ntaps == 0 || a.ntaps == 1 || a.ntaps == 3, "adp_wgrad: ntaps must be 1 or 3");
   cudaStream_t s = as_stream(stream);
-  if (a.ntaps == 3) {        // all taps of a k=3 conv: three accumulators of <= 128 columns in TMEM
+  if (a.ntaps == 3) {        // all taps of a k=3 conv: three register accumulators of 64 columns
     ADP_CHECK(a.tap_stride >= (long long)a.n * a.ldw, "adp_wgrad: tap_stride smaller than one dW slab");
-    if (a.k > 64) return launch_wgrad<128, 3>(a, s);
     return launch_wgrad<64, 3>(a, s);
   }
   if (a.k > 128) return launch_wgrad<256, 1>(a, s);

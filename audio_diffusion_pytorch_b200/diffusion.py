@@ -1,7 +1,7 @@
-"""`diffusion_t` / `sampler_t` plugin slots (reference diffusion.py), B200-native.
+"""`diffusion_t` / `sampler_t` plugin slots (reference diffusion.py), CUDA-native.
 
 VDiffusion and VSampler keep the reference constructors and call signatures
-(reference diffusion.py:68-95, :158-190).  When the wrapped net is the B200 U-Net the
+(reference diffusion.py:68-95, :158-190).  When the wrapped net is the CUDA U-Net the
 per-step arithmetic is fused into the net's last kernel and the loop launches one CUDA
 graph per step; with any other `net` the same algebra runs as the generic fused
 `adp_sampler_step` kernel after the net call.
@@ -76,7 +76,7 @@ class VDiffusion(Diffusion):
     """v-objective diffusion loss (reference diffusion.py:68-95).
 
     RNG contract kept: `sigma_distribution(B)` is drawn first, then `randn_like(x)`, both on
-    x.device.  With the B200 net the noising (`alpha*x + beta*noise`) is fused into the first
+    x.device.  With the CUDA net the noising (`alpha*x + beta*noise`) is fused into the first
     kernel and the MSE against `alpha*noise - beta*x` into the last."""
 
     def __init__(self, net: nn.Module, sigma_distribution: Distribution = UniformDistribution(),
@@ -111,7 +111,7 @@ class ARVDiffusion(Diffusion):
 
     RNG contract kept: `rand((B, 1, num_splits))` first, then `randn_like(x)`, both on x.device.
     The pointwise noising runs as tensor ops (autograd records them for dL/dx); the net is the
-    B200 differentiable program (`B200UNet.forward` under grad mode)."""
+    CUDA differentiable program (`B200UNet.forward` under grad mode)."""
 
     def __init__(self, net: nn.Module, length: int, num_splits: int, loss_fn: Any = F.mse_loss):
         super().__init__()

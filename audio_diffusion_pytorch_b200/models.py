@@ -1,7 +1,7 @@
 """The model classes users instantiate.  Same names, constructor keywords, attribute names
 (`net`, `diffusion`, `sampler`, `to_spectrogram`, `to_flat`) and call signatures as reference
 models.py:22-45 (DiffusionModel), :134-165 (DiffusionUpsampler), :168-224 (DiffusionVocoder);
-the arithmetic behind `net`, `diffusion` and `sampler` is the B200 path.  U-Net weights of a
+the arithmetic behind `net`, `diffusion` and `sampler` is the CUDA path.  U-Net weights of a
 reference model are taken over with `model.net.load_reference_parameters(ref_model.net)`
 (same parameter order and shapes as a_unet's module tree)."""
 from abc import ABC, abstractmethod
@@ -80,7 +80,7 @@ class AdapterBase(nn.Module, ABC):
 class DiffusionAE(DiffusionModel):
     """Diffusion autoencoder (reference models.py:70-131): the encoder's latent is injected at
     `inject_depth` of the U-Net (`InjectChannelsItem`: conv1x1 over cat([x, latent]) + x); training
-    back-propagates into the encoder through the context gradient of the B200 backward program."""
+    back-propagates into the encoder through the context gradient of the CUDA backward program."""
 
     def __init__(self, in_channels: int, channels: Sequence[int], encoder: nn.Module, inject_depth: int,
                  latent_factor: Optional[int] = None, adapter: Optional[nn.Module] = None, **kwargs):

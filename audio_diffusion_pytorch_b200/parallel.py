@@ -161,7 +161,7 @@ class GradSync:
 
 
 class OverlappedDataParallel(torch.nn.Module):
-    """Data parallelism for the training step of the B200 path (SURVEY.md 8e): replicas + ONE
+    """Data parallelism for the training step of the CUDA path (SURVEY.md 8e): replicas + ONE
     gradient average per step over NCCL, overlapped with the hand-written backward program.
 
         ddp = OverlappedDataParallel(model)            # broadcasts rank 0's weights

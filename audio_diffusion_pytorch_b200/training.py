@@ -1,4 +1,4 @@
-"""Differentiable execution of the B200 U-Net: the training step of the hot path
+"""Differentiable execution of the CUDA U-Net: the training step of the hot path
 (reference diffusion.py:82-95, `loss = model(x); loss.backward()`) and the generic
 `v = net(x, sigma, ...)` with autograd support (custom `loss_fn` / `diffusion_t`,
 reference models.py:28,37 and tests/testcustomloss.py:28).
@@ -932,7 +932,7 @@ def fused_v_loss(net: B200UNet, x: Tensor, noise: Tensor, sigmas: Tensor, *,
                  embedding: Optional[Tensor] = None, embedding_scale: float = 1.0,
                  embedding_mask_proba: float = 0.0, channels=None) -> Tensor:
     """mse(net(alpha*x + beta*noise, sigma), alpha*noise - beta*x)  (reference diffusion.py:90-95)."""
-    assert x.is_cuda, "the B200 path runs on a CUDA device only (no CPU fallback)"
+    assert x.is_cuda, "the CUDA path runs on a CUDA device only (no CPU fallback)"
     if net.use_embedding_cfg and embedding_scale != 1.0:
         # guidance inside the training objective = two differentiable evaluations (a_unet CFG
         # plugin); no fused-loss form: take the generic route
@@ -955,7 +955,7 @@ def differentiable_forward(net: B200UNet, x: Tensor, time: Optional[Tensor], *,
                            embedding_scale: float = 1.0, embedding_mask_proba: float = 0.0,
                            append_channels: Optional[Tensor] = None, channels=None) -> Tensor:
     """v = net(x, time, ...) with autograd support (custom loss_fn / diffusion_t)."""
-    assert x.is_cuda, "the B200 path runs on a CUDA device only (no CPU fallback)"
+    assert x.is_cuda, "the CUDA path runs on a CUDA device only (no CPU fallback)"
     cond = _time_cond(net, time, features)
     emb, fixed = _train_embedding(net, x.shape[0], embedding, embedding_mask_proba)
     params = _net_params(net)

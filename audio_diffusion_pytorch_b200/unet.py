@@ -1,5 +1,5 @@
-"""UNetV0 on B200: the reference's `net_t` plugin slot (reference components.py:34-105),
-rebuilt over the sm_100a kernels of libadp_b200.so.
+"""UNetV0 on H100: the reference's `net_t` plugin slot (reference components.py:34-105),
+rebuilt over the sm_90a kernels of libadp_b200.so.
 
 `UNetV0(dim=1, in_channels=..., channels=[...], ...)` takes the reference's kwargs verbatim
 and returns an nn.Module with the reference's call signature
@@ -182,7 +182,7 @@ class B200UNet(nn.Module):
         context_channels = default(context_channels, [0] * n)
         xs = (channels, factors, items, attentions, cross_attentions, context_channels)
         assert all(len(x) == n for x in xs)                       # reference components.py:61
-        assert dim == 1, "the B200 path implements the 1-D (waveform) U-Net"
+        assert dim == 1, "the CUDA path implements the 1-D (waveform) U-Net"
         if use_embedding_cfg:                                     # components.py:66-68
             assert exists(embedding_max_length), "use_embedding_cfg requires embedding_max_length"
         if use_time_conditioning:                                 # components.py:75
@@ -196,7 +196,7 @@ class B200UNet(nn.Module):
         if any(attentions) or any(cross_attentions):
             assert exists(attention_features) and exists(attention_heads), \
                 "AttentionItem requires attention_features and attention_heads"
-            assert attention_features == 64, "the tcgen05 attention kernel is built for head dim 64"
+            assert attention_features == 64, "the attention kernel is built for head dim 64"
         if any(cross_attentions):
             assert exists(embedding_features), "CrossAttentionItem requires embedding_features"
 
@@ -240,10 +240,9 @@ class B200UNet(nn.Module):
         self._storage_sig = None
         self._repack_graph = None
         self.use_cuda_graph = True
-        # GroupNorm+SiLU applied inside the conv GEMM by transform warps (adp_conv_gemm gn_*).
-        # Verified bit-compatible with the two-kernel path but measured SLOWER on the README
-        # config (6.85 vs 6.0 ms / evaluation, profiles/r1_gn_fusion.txt): every N tile repeats
-        # the transform of its A rows, so it only pays for N <= BN.  Off by default.
+        # GroupNorm+SiLU applied to the A tile inside the conv GEMM (adp_conv_gemm gn_*).
+        # Bit-compatible with the two-kernel path, but every N tile repeats the transform of
+        # its A rows, so it only pays for N <= BN.  Off by default.
         self.fuse_groupnorm = False
         # C = 32 / 64 ConvBlocks as ONE fused kernel (GroupNorm+SiLU -> conv3 -> +res -> LN/FiLM ->
         # statistics, csrc/mid_conv.cu) instead of three: those levels are HBM-bound
@@ -379,8 +378,8 @@ class B200UNet(nn.Module):
     @torch.no_grad()
     def _repack(self) -> None:
         """In-place refresh of every packed weight.  The re-layout is ~500 small permute / cast /
-        fold launches whose HOST cost (12 ms per training step, profiles/r2_train_profile_start.txt)
-        dwarfed their device time: sources (the parameters) and destinations (the packs) have
+        fold launches whose HOST cost
+        dwarfs their device time: sources (the parameters) and destinations (the packs) have
         fixed addresses, so the whole sequence is captured once into a CUDA graph and replayed."""
         if not (self.use_cuda_graph and self.net.down.weight.is_cuda):
             _copy_tree(self._packed, self._compute_packed())
@@ -1017,7 +1016,7 @@ class B200UNet(nn.Module):
                 embedding: Optional[Tensor] = None, embedding_scale: float = 1.0,
                 embedding_mask_proba: float = 0.0, channels=None,
                 append_channels: Optional[Tensor] = None) -> Tensor:
-        assert x.is_cuda, "the B200 path runs on a CUDA device only (no CPU fallback)"
+        assert x.is_cuda, "the CUDA path runs on a CUDA device only (no CPU fallback)"
         if self.use_embedding_cfg:
             assert exists(embedding), "ClassiferFreeGuidancePlugin requires embedding"
         ctx_list = [c for c in (channels or []) if exists(c)]
@@ -1050,7 +1049,7 @@ class B200UNet(nn.Module):
                     progress=None, **kwargs) -> Tensor:
         """VSampler's loop (reference diffusion.py:183-188) with the per-step update fused into
         the net's last kernel: one graph launch per step, no host sync inside the loop."""
-        assert x_noisy.is_cuda, "the B200 path runs on a CUDA device only (no CPU fallback)"
+        assert x_noisy.is_cuda, "the CUDA path runs on a CUDA device only (no CPU fallback)"
         self._check_untracked_updates()
         embedding = kwargs.get("embedding")
         scale = kwargs.get("embedding_scale", 1.0)
@@ -1093,7 +1092,7 @@ def _inpaint_loop(self, x_noisy: Tensor, source: Tensor, mask: Tensor, sigmas: T
     re-noised back to the current level), then the known region (mask) is replaced by the source
     noised to that level.  One graph launch + one blend kernel per evaluation; the noise is drawn
     with torch.randn_like(source) in the reference's order."""
-    assert x_noisy.is_cuda, "the B200 path runs on a CUDA device only (no CPU fallback)"
+    assert x_noisy.is_cuda, "the CUDA path runs on a CUDA device only (no CPU fallback)"
     self._check_untracked_updates()
     embedding = kwargs.get("embedding")
     scale = kwargs.get("embedding_scale", 1.0)
@@ -1145,7 +1144,7 @@ def _arv_loop(self, current: Tensor, sigmas: Tensor, progress=None, **kwargs) ->
     sigma_i]) with a noise level PER POSITION (sigmas [N+1, B, 1, T]) and no time conditioning.
     The plan's input buffer holds that concatenation for the whole loop: one graph launch (the
     net) + one adp_arv_step (the update, which also writes sigma_{i+1} into the last channel)."""
-    assert current.is_cuda, "the B200 path runs on a CUDA device only (no CPU fallback)"
+    assert current.is_cuda, "the CUDA path runs on a CUDA device only (no CPU fallback)"
     self._check_untracked_updates()
     embedding = kwargs.get("embedding")
     scale = kwargs.get("embedding_scale", 1.0)
@@ -1203,6 +1202,6 @@ def _pad_to(t: Tensor, n: int) -> Tensor:
 def UNetV0(dim: int, in_channels: int, channels: Sequence[int], factors: Sequence[int],
            items: Sequence[int], **kwargs) -> nn.Module:
     """Drop-in for reference components.py:34 `UNetV0` (same kwargs, asserts and call
-    signature); returns the B200-native module."""
+    signature); returns the CUDA-native module."""
     return B200UNet(dim=dim, in_channels=in_channels, channels=channels, factors=factors,
                     items=items, **kwargs)

@@ -2,6 +2,7 @@
 """bench.py -- audio-seconds/sec of the VSampler on the README U-Net (BASELINE.json).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--config cfg2|cfg3|cfg5] [--impl reference]
+                    [--dump-outputs DIR]
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one complete `model.sample(...)` call on each rank (weak scaling: the per-GPU batch is
@@ -17,10 +18,13 @@ fixed, independent sampling, no collective on the data path).  Prints ONE JSON l
   value     clips*5.4613 s / wall, inputs resident in HBM, device-timed, max over ranks
   e2e       same through the public API from pinned HOST inputs to a HOST result
   roofline  the dominant kernel/shape of the step, timed live with CUDA events in an instrumented
-            eager pass of the same plan; `traffic` = DRAM bytes per launch read from the committed
-            ncu capture named in `traffic_source` (null when that shape has no capture)
+            eager pass of the same plan; bytes and flops per launch computed from the shapes
   cpu_baseline  the reference's eager-PyTorch CPU path (oracle port) on this box's host cores,
             bounded sample, extrapolated (stated in `sample`)
+
+`--dump-outputs DIR` writes what the timed path returned in its last timed step (the sampled audio,
+float32, [batch, 2, 2**18]) as DIR/sample.npy.  Inputs and weights are seeded, so two builds run with
+the same arguments can be compared output for output.
 
 `--impl reference` times only that CPU path (rank 0), same metric/config: each of the K timed
 steps is ONE VSampler step of the config's batch on clips cut to the longest power-of-two length
@@ -54,7 +58,7 @@ VOCODER = dict(mel_n_fft=1024, mel_channels=80, mel_sample_rate=48000, mel_norma
 UPSAMPLER = dict(upsample_factor=16, in_channels=2, **UNET9)
 METRIC = "audio-seconds/sec (2ch, 2^18 len) VSampler 50-step"
 L2_NOTE = ("no explicit flush: one net evaluation streams ~0.9 GB (activations + 435 MB weights), "
-           "far beyond the 126 MB L2")
+           "far beyond the 50 MB L2")
 
 WORKLOADS = {
     "cfg2": dict(batch=8, steps=50, metric=METRIC,
@@ -77,12 +81,9 @@ def workload_config(name: str):
 
 
 def peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as fh:
-            p = json.load(fh)
-        return p["hbm_gbs"], p["bf16_tflops"], p["bf16_tflops_sustained"], "measured"
-    except Exception:
-        return 6650.0, 1590.0, 1400.0, "fallback"
+    """HBM GB/s, dense BF16 TFLOP/s (data sheet) and the BF16 rate the roofline is drawn at.
+    NVIDIA's H100 SXM data sheet: 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 (at up to 700 W)."""
+    return 3350.0, 989.0, 989.0, "H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -271,22 +272,6 @@ def train_step_bench(adp, dev, world, dist, steps, warmup, batch=4):
             "audio_s_per_s": batch * world * CLIP_SECONDS / (float(ms.item()) * 1e-3)}
 
 
-# --------------------------------------------------------------------------- ncu-derived traffic
-def ncu_traffic(kernel_label: str):
-    """DRAM bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum of one `ncu --set full`
-    capture) for a kernel/shape label, from profiles/ncu_traffic.json -- written by
-    tools/ncu_traffic.py from the committed captures.  (None, None) when that shape has none."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as fh:
-            table = json.load(fh)
-        ent = table.get(kernel_label)
-        if ent:
-            return float(ent["dram_bytes"]), ent["source"]
-    except Exception:
-        pass
-    return None, None
-
-
 # stdout carries exactly ONE JSON line: libraries that print to fd 1 from C (NCCL's version
 # banner) are sent to stderr for the duration of the run
 _REAL_STDOUT = None
@@ -314,6 +299,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--profile-ops", action="store_true", help="print the per-kernel table")
     ap.add_argument("--no-train", action="store_true", help="skip the training-step measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's output as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -369,8 +356,10 @@ def main():
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
         return float(ms.item())
 
+    last = {}
+
     def step_device():
-        model.sample(dev_in, num_steps=num_steps, **dev_kw, **kw)
+        last["sample"] = model.sample(dev_in, num_steps=num_steps, **dev_kw, **kw)
 
     def step_e2e():
         x = host_in.to(dev, non_blocking=True)
@@ -383,6 +372,12 @@ def main():
         step_device()
     with ClockSampler(local) as clocks:
         total_ms = timed(step_device, args.steps)
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, t in last.items():
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), t.float().cpu().numpy())
+    last.clear()
     for _ in range(2):
         step_e2e()
     e2e_ms = timed(step_e2e, args.steps)
@@ -448,10 +443,8 @@ def main():
             roof["in_graph_error"] = in_graph_err
         if busy_us is not None:
             roof["kernel_busy_us_per_net_eval"] = busy_us
-        traffic, traffic_src = ncu_traffic(top["name"])
         roof.update({"kernel": top["name"], "launches_per_net_eval": top["count"],
                      "share_of_step": top_share, "peak_source": which,
-                     "traffic": traffic, "traffic_source": traffic_src,
                      "flops_per_launch": top["flops"], "bytes_per_launch": top["bytes"]})
         # whole-step roofline (SURVEY.md 8d): sum over levels of max(flop time, byte time)
         t_bound = sum(max(r["flops"] / (tf_sust * 1e12), r["bytes"] / (hbm * 1e9)) * r["count"]
@@ -481,7 +474,7 @@ def main():
         del model, net, plan
         gtab = table = None
         torch.cuda.empty_cache()
-        line["train_step"] = train_step_bench(adp, dev, world, dist, steps=5, warmup=3)
+        line["train_step"] = train_step_bench(adp, dev, world, dist, steps=args.steps, warmup=warmup)
     if rank == 0 and not args.no_cpu_baseline and world == 1:
         v, per_step, cores, sample = cpu_reference_run(args.config, steps=1, warmup=1, budget_s=25.0, batch=1)
         line["cpu_baseline"] = {"value": v, "unit": "audio-s/s", "cores": cores, "kind": "port",

@@ -1,4 +1,4 @@
-/* adp_b200.h -- C ABI of libadp_b200.so, the sm_100a (B200) kernels behind the
+/* adp_b200.h -- C ABI of libadp_b200.so, the sm_90a (H100) kernels behind the
  * audio_diffusion_pytorch hot path:  UNetV0 forward/backward + VDiffusion + VSampler.
  *
  * The reference (archinetai/audio-diffusion-pytorch) is pure Python and has no FFI; its
@@ -15,7 +15,7 @@
  *  - the caller owns every buffer (incl. workspaces); no entry point allocates or
  *    synchronises, all are CUDA-graph capturable on `stream` (a cudaStream_t).
  *  - return 0 on success, non-zero on error; adp_last_error() describes the last error of
- *    the calling thread.  There is NO CPU fallback: a non-sm_100 device is an error.
+ *    the calling thread.  There is NO CPU fallback: a non-sm_90 device is an error.
  */
 #ifndef ADP_B200_H_
 #define ADP_B200_H_
@@ -33,14 +33,14 @@ enum { ADP_ACT_NONE = 0, ADP_ACT_GELU = 1, ADP_ACT_SILU = 2 };
 
 int adp_version(void);
 const char* adp_last_error(void);
-/* 0 iff the current CUDA device is compute capability 10.x (B200). */
+/* 0 iff the current CUDA device is compute capability 9.0 (H100). */
 int adp_device_check(void);
 /* Diagnostic switches for A/B runs (key 0: GEMM implementation 2=persistent 1=v1; key 1: one
  * A box for all taps; key 2: descriptor base-offset mode).  Not part of the hot path. */
 int adp_debug_set(int key, int value);
 
 /* ---------------------------------------------------------------------------------------
- * adp_conv_gemm: shifted-tap GEMM on tcgen05 tensor cores (TMA -> smem -> UMMA -> TMEM).
+ * adp_conv_gemm: shifted-tap GEMM on wgmma tensor cores (TMA -> smem -> wgmma -> registers).
  *   out[b,t, p*n_valid + n] = epi( sum_tap sum_k  a[b, t + off(p,tap), k] * w[p*n_pad + n, tap*c_in + k] )
  * with rows outside [0,T) reading as zero (TMA out-of-bounds fill = the conv padding).
  * Replaces (a_unet): ConvBlock's Conv1d k=3 p=1 (ResnetItem), Downsample Conv1d k=s=f (as a
@@ -111,7 +111,7 @@ int adp_ln_film_dual(const void* x, void* y, void* y2, const float* scale_shift,
 
 /* o = softmax(q k^T * scale) v per (batch, head), head dim 64 -- a_unet AttentionBase.
  * q: bf16 [B][Tq][ldq] (head h at columns [h*64,(h+1)*64)), k/v likewise over Tk rows,
- * o: bf16 [B][Tq][ldo].  tcgen05 flash attention (S and O accumulators in TMEM).
+ * o: bf16 [B][Tq][ldo].  wgmma flash attention (S and O accumulators in registers).
  * lse: optional fp32 [B][H][Tq] = log sum_k exp(scale * q.k) per row (kept by the training
  * forward for adp_attention_bwd), or NULL. */
 int adp_attention(const void* q, const void* k, const void* v, void* o, int32_t B, int32_t H,
@@ -306,7 +306,7 @@ int adp_to_flat_bwd(const float* spec, const float* w, const float* dout, float*
  * The data gradient of every conv / linear is adp_conv_gemm with transposed packed weights.
  */
 
-/* dW[n][k] += sum_{b,t} g[b][t][g_col0+n] * x[b][t+off][x_col0+k]  (tcgen05, both operands
+/* dW[n][k] += sum_{b,t} g[b][t][g_col0+n] * x[b][t+off][x_col0+k]  (wgmma, both operands
  * consumed MN-major in place; rows outside [0,T) read as zero).  Backward of adp_conv_gemm
  * w.r.t. one tap of W. */
 typedef struct adp_wgrad_args {

@@ -10,7 +10,7 @@ ORACLE = os.path.join(ROOT, "oracle")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run with -m gpu")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100); run with -m gpu")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -1,4 +1,4 @@
-"""Whole-path parity on the GPU: the B200 UNetV0 / VSampler / model wrappers against
+"""Whole-path parity on the GPU: the CUDA UNetV0 / VSampler / model wrappers against
  (a) the committed golden vectors (made by oracle/make_golden.py from the UNMODIFIED
      reference files running on the a_unet shim), and
  (b) the CPU oracle port evaluated here on the same seeded inputs,
@@ -10,7 +10,7 @@ v = x + gate*branch with |branch| << |x| at initialisation, so two metrics are b
   * rel-L2 error of v                      <= 1e-4   (10x inside the north star's fp32 rtol)
   * rel-L2 error of the branch (v - skip)  <= BRANCH_TOL = 1.2e-2 = 2x the error of the fp32
     oracle itself evaluated under bf16 autocast on CPU (5.8e-3 on the same metric, stored
-    in the golden file as bf16_err_branch).  Measured on B200: 3.0e-3 (tiny), 4.4e-3 (README)."""
+    in the golden file as bf16_err_branch)."""
 import os
 
 import numpy as np
@@ -169,7 +169,7 @@ def test_upsampler_and_vocoder_sample_vs_golden(adp, oracle_port, golden_dir):
 
 
 def test_sampler_algebra_generic_net(adp, golden_dir):
-    """VSampler around an arbitrary net (not the B200 U-Net): pins the fused step kernel."""
+    """VSampler around an arbitrary net (not the CUDA U-Net): pins the fused step kernel."""
     g = load(golden_dir, "sampler_toy.npz")
 
     class Toy(torch.nn.Module):

@@ -91,7 +91,8 @@ def test_conv_gemm_fp32_out(ops):
 
 
 @pytest.mark.parametrize("B,T,C,co", [(2, 512, 64, 64), (2, 300, 128, 128), (1, 256, 32, 32),
-                                      (2, 100, 256, 256), (1, 128, 16, 16)])
+                                      (2, 100, 256, 256), (1, 128, 16, 16), (8, 256, 1024, 1024),
+                                      (3, 128, 512, 256)])
 def test_conv_gemm_conv3(ops, B, T, C, co):
     x = bf(rnd(B, T, C, seed=4))
     w = bf(rnd(co, C, 3, scale=(3 * C) ** -0.5, seed=5))
@@ -416,55 +417,3 @@ def test_conv_gemm_fused_groupnorm_silu(ops, B, T, C, co):
     ref = F.conv1d(a, w.float(), bias, padding=1).transpose(1, 2) + res.float()
     assert_close(out, ref, 2 ** -6, 3e-2, f"fused gn+silu conv3 C{C}")
     assert_close(stats, stats_of(out, groups), 1e-4, 1e-2, "fused gn stats")
-
-
-@pytest.mark.parametrize("B,T,C,co,taps,extras", [
-    (8, 256, 1024, 1024, 3, "res+stats"),    # README L7 conv3: 64 pair tiles, one per CTA pair (8 drain warps)
-    (8, 1024, 512, 512, 3, "res+stats"),     # README L5 conv3: 128 pair tiles -> two per pair (TMEM double buffer)
-    (3, 128, 512, 256, 3, "res+stats"),      # odd number of M tiles: the last pair's second CTA has no rows
-    (2, 200, 1024, 128, 3, "res+stats"),     # ragged T: row masks differ between the two CTAs of a pair
-    (1, 1024, 512, 1536, 1, "bias"),         # qkv projection (1 tap)
-    (2, 384, 512, 256, 1, "gate+res"),       # MergeModulate epilogue
-    (4, 640, 1024, 1024, 3, "early"),        # weight boxes issued before griddepcontrol.wait
-])
-def test_conv_gemm_cta_pairs(ops, B, T, C, co, taps, extras):
-    """tcgen05 cta_group::2: a pair of CTAs shares the W tile (each stages half of it) and the leader
-    issues M = 256 MMAs.  Checked against fp32 PyTorch AND bit-for-bit against the single-CTA path
-    (same tile shape, same accumulation order)."""
-    from audio_diffusion_pytorch_b200 import _lib
-    L = _lib.lib()
-    x = bf(rnd(B, T, C, seed=4))
-    w = bf(rnd(co, C, taps, scale=(taps * C) ** -0.5, seed=5))
-    bias = rnd(co, seed=6)
-    res = bf(rnd(B, T, co, seed=7)) if "res" in extras else None
-    gate = rnd(B, co, seed=8) if "gate" in extras else None
-    groups = 8
-    wp = ops.pack_conv(w)
-    tp = (-1, 0, 1) if taps == 3 else (0,)
-    outs, sts = [], []
-    for mode in (0, 3):              # 3 = opt into CTA pairs (csrc/conv_gemm.cu use_pairs)
-        L.adp_debug_set(0, mode)
-        L.adp_debug_set(2, 1 if "early" in extras else 0)
-        try:
-            st = torch.zeros(B, groups, 2, dtype=torch.float64, device=DEV) if "stats" in extras else None
-            out = torch.full((B, T, co), float("nan"), dtype=torch.bfloat16, device=DEV)
-            for _ in range(2):
-                if st is not None:
-                    st.zero_()
-                ops.conv_gemm(x, wp, out, c_in=C, n_valid=co, taps=tp, bias=bias, residual=res, gate=gate,
-                              stats=st, groups=groups, block_n=128)
-            torch.cuda.synchronize()
-            outs.append(out)
-            sts.append(st)
-        finally:
-            L.adp_debug_set(0, 0)
-            L.adp_debug_set(2, 0)
-    ref = F.conv1d(x.float().transpose(1, 2), w.float(), bias, padding=taps // 2).transpose(1, 2)
-    if gate is not None:
-        ref = ref * gate[:, None, :]
-    if res is not None:
-        ref = ref + res.float()
-    assert_close(outs[1], ref, 2 ** -7, 1e-2, f"pair GEMM B{B} T{T} K{C} N{co} taps{taps} {extras}")
-    assert torch.equal(outs[0], outs[1]), "CTA-pair result differs from the single-CTA result"
-    if sts[1] is not None:
-        assert_close(sts[1], stats_of(outs[1], groups), 1e-4, 1e-2, "pair GEMM stats")

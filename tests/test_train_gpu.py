@@ -1,4 +1,4 @@
-"""Training step parity: fused VDiffusion loss + hand-written backward of the B200 U-Net against
+"""Training step parity: fused VDiffusion loss + hand-written backward of the CUDA U-Net against
 torch.autograd through the CPU oracle (same weights, same x / noise / sigma): attention-free
 nets (BASELINE cfg4/cfg5 shape), nets with AttentionItem / CrossAttentionItem (README config,
 cfg3), the 9-level shape, custom loss functions through the differentiable net forward, the
@@ -438,7 +438,7 @@ def test_autoregressive_loss_and_gradients(oracle_port):
 
 
 def test_learned_transform_plugin(oracle_port):
-    """LTPlugin (reference components.py:113-157) around the B200 net: forward / 3-step sample
+    """LTPlugin (reference components.py:113-157) around the CUDA net: forward / 3-step sample
     against the oracle and, through the differentiable net (the filterbanks are PyTorch modules on
     both sides of it: d(input) of the hand-written backward feeds the encoder), the loss and every
     gradient incl. the two filterbanks."""
