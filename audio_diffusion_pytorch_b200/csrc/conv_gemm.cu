@@ -16,7 +16,8 @@
 // warps 0-7 the two consumer warpgroups (MMA issue + epilogue straight from the accumulator
 // registers), warp 8 the TMA producer, which keeps filling the ring while the consumers drain
 // a tile.  GroupNorm partial sums of the output are reduced per warp into per-warp shared-memory
-// slots; one global reduction per batch change.
+// slots (per-lane registers for groups narrower than 8 channels); one global reduction per batch
+// change.
 #include "common.cuh"
 #include "ptx.cuh"
 
@@ -111,6 +112,45 @@ struct WarpStats {
   __device__ __forceinline__ void add(float v, int g, float (*slots)[8], int w, int lane) {
     if (g != cur_g) { flush(slots, w, lane); cur_g = g; }
     s += v; q += v * v;
+  }
+};
+
+// Running per-group (sum, sumsq) for power-of-two groups narrower than 8 channels.  With at most
+// kMaxGroups groups such a tensor has n_valid <= 32, so a tile holds at most four valid 8-column
+// blocks and the group of each accumulator element follows from the lane, the unrolled block jb
+// and the column parity: a lane's column pair lies in one group for sizes 2 and 4 (slot jb),
+// and for size 1 only block 0 is valid (slot = parity).  Lanes accumulate privately while the
+// tile's first channel ch0 stays the same; flush() reduces over the lane bits that share a group
+// with a fixed butterfly, and one lane per group adds into the warp's own shared-memory column
+// (one writer per column, as in WarpStats).
+struct NarrowStats {
+  int ch0 = -1;
+  float s[4] = {0.f, 0.f, 0.f, 0.f}, q[4] = {0.f, 0.f, 0.f, 0.f};
+  __device__ __forceinline__ void add(int k, float v) { s[k] += v; q[k] += v * v; }
+  __device__ __forceinline__ void flush(float (*slots)[8], int w, int lane, int shift, int groups) {
+    if (ch0 >= 0) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        float a = s[k], b = q[k];
+#pragma unroll
+        for (int o = 4; o < 32; o <<= 1) {      // the 8 fragment rows of the lane quad
+          a += __shfl_xor_sync(0xffffffffu, a, o);
+          b += __shfl_xor_sync(0xffffffffu, b, o);
+        }
+        if (shift == 2) {                        // size 4: lanes 2i and 2i+1 share the group
+          a += __shfl_xor_sync(0xffffffffu, a, 1);
+          b += __shfl_xor_sync(0xffffffffu, b, 1);
+        }
+        const int col = shift == 0 ? ch0 + 2 * lane + k : ch0 + 8 * k + 2 * (lane & 3);
+        const int g = col >> shift;
+        if (lane < 4 && (shift != 2 || !(lane & 1)) && (shift != 0 || k < 2) && g < groups) {
+          slots[2 * g][w] += a;
+          slots[2 * g + 1][w] += b;
+        }
+        s[k] = 0.f; q[k] = 0.f;
+      }
+    }
+    ch0 = -1;
   }
 };
 
@@ -209,12 +249,18 @@ conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // fragment rows r0 and r0 + 8
   const int cq = 2 * (lane & 3);               // fragment column offset inside each 8-column block
   const bool do_stats = p.stats != nullptr;
+  // narrow power-of-two groups keep per-lane registers only where they fit without spills
+  // (BN <= 64, no A-operand transform); other tiles take the per-block path of other group sizes
+  constexpr bool kNarrowRegs = BN <= 64 && !XF;
+  const bool narrow = kNarrowRegs && p.group_shift >= 0 && p.group_shift < 3;
   WarpStats acc_st;
+  NarrowStats nar_st;
   int cur_b = -1, coef_b = -1;
 
   auto publish_stats = [&](int b_done) {       // all 256 consumer threads
     acc_st.flush(s_part, warp, lane);
     acc_st.cur_g = -1;
+    if (narrow) nar_st.flush(s_part, warp, lane, p.group_shift, p.groups);
     named_bar_sync(1, kConsumers);
     if (tid < 2 * p.groups) {
       float tot = 0.f;
@@ -332,6 +378,10 @@ conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       if (cur_b >= 0) publish_stats(cur_b);
       cur_b = ti.b;
     }
+    if (narrow && ti.ch0 != nar_st.ch0) {        // the slots are bound to the tile's channels
+      nar_st.flush(s_part, warp, lane, p.group_shift, p.groups);
+      nar_st.ch0 = ti.ch0;
+    }
     const int t_lo = ti.t0 + r0, t_hi = t_lo + 8;
     const bool ok_lo = t_lo < p.T, ok_hi = t_hi < p.T;
     const size_t col_off = static_cast<size_t>(ti.phase) * p.n_valid;
@@ -373,17 +423,31 @@ conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           const int g = ch >> p.group_shift;
           acc_st.add(q_lo.x, g, s_part, warp, lane); acc_st.add(q_lo.y, g, s_part, warp, lane);
           acc_st.add(q_hi.x, g, s_part, warp, lane); acc_st.add(q_hi.y, g, s_part, warp, lane);
-        } else {                           // groups narrower than 8 channels (rare): lane 0 adds
-          const float q[4] = {q_lo.x, q_lo.y, q_hi.x, q_hi.y};   // every lane's values in lane order
+        } else if (narrow) {
+          if (p.group_shift == 0) {
+            nar_st.add(0, q_lo.x); nar_st.add(0, q_hi.x);
+            nar_st.add(1, q_lo.y); nar_st.add(1, q_hi.y);
+          } else if (jb < 4) {             // n_valid <= 32: later blocks are padding
+            nar_st.add(jb, q_lo.x); nar_st.add(jb, q_lo.y);
+            nar_st.add(jb, q_hi.x); nar_st.add(jb, q_hi.y);
+          }
+        } else {   // group size not a power of two, or narrow at BN > 64 (no benchmarked shape):
+                   // column sums over the warp's rows, then lane 0 adds the block's 8 columns
+          float cs[2] = {q_lo.x + q_hi.x, q_lo.y + q_hi.y};
+          float cs2[2] = {q_lo.x * q_lo.x + q_hi.x * q_hi.x, q_lo.y * q_lo.y + q_hi.y * q_hi.y};
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int cc = ch + (i & 1);
-            const int g = p.group_shift >= 0 ? cc >> p.group_shift : cc / p.group_size;
-            for (int src = 0; src < 32; ++src) {
-              const float v = __shfl_sync(0xffffffffu, q[i], src);
-              const int gs = __shfl_sync(0xffffffffu, g, src);
-              if (lane == 0 && v != 0.f) { s_part[2 * gs][warp] += v; s_part[2 * gs + 1][warp] += v * v; }
+          for (int e = 0; e < 2; ++e)
+#pragma unroll
+            for (int o = 4; o < 32; o <<= 1) {
+              cs[e] += __shfl_xor_sync(0xffffffffu, cs[e], o);
+              cs2[e] += __shfl_xor_sync(0xffffffffu, cs2[e], o);
             }
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const float v = __shfl_sync(0xffffffffu, cs[i & 1], i >> 1);
+            const float v2 = __shfl_sync(0xffffffffu, cs2[i & 1], i >> 1);
+            const int g = (ti.ch0 + jb * 8 + i) / p.group_size;
+            if (lane == 0) { s_part[2 * g][warp] += v; s_part[2 * g + 1][warp] += v2; }
           }
         }
       }
