@@ -125,7 +125,9 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CU
 #pragma unroll
   for (int tap = 0; tap < NT; ++tap) acc_fence(acc[tap]);
 
-  const bool single = gridDim.z == 1;          // single writer of this tile (dW is pre-zeroed)
+  // dW += the product.  With one split this thread is the only writer of its elements: a plain
+  // read-modify-write instead of atomics
+  const bool single = gridDim.z == 1;
   const bool pairs = (p.ldw & 1) == 0 && (p.tap_stride & 1) == 0;
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
@@ -139,11 +141,16 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CU
         const int k = k0 + 8 * jb + 2 * (lane & 3);
         const float v0 = acc[tap][4 * jb + 2 * r], v1 = acc[tap][4 * jb + 2 * r + 1];
         if (k + 1 < p.k_valid && pairs) {
-          if (single) *reinterpret_cast<float2*>(drow + k) = make_float2(v0, v1);
-          else atomicAdd(reinterpret_cast<float2*>(drow + k), make_float2(v0, v1));
+          float2* d2 = reinterpret_cast<float2*>(drow + k);
+          if (single) {
+            const float2 o = *d2;
+            *d2 = make_float2(o.x + v0, o.y + v1);
+          } else {
+            atomicAdd(d2, make_float2(v0, v1));
+          }
         } else {
-          if (k < p.k_valid) { if (single) drow[k] = v0; else atomicAdd(drow + k, v0); }
-          if (k + 1 < p.k_valid) { if (single) drow[k + 1] = v1; else atomicAdd(drow + k + 1, v1); }
+          if (k < p.k_valid) { if (single) drow[k] += v0; else atomicAdd(drow + k, v0); }
+          if (k + 1 < p.k_valid) { if (single) drow[k + 1] += v1; else atomicAdd(drow + k + 1, v1); }
         }
       }
     }

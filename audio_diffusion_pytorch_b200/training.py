@@ -56,6 +56,223 @@ def _zeros(shape, dev, dtype=torch.float32):
     return torch.zeros(shape, device=dev, dtype=dtype)
 
 
+S_CAT = 2 ** -0.5          # SkipCat scales the skip branch before the 1x1 merge conv
+
+
+def _master(w: Tensor) -> Tensor:
+    """fp32 copy of a weight for the host-side packers (an fp64 weight stays fp64, so the
+    packing algebra can be checked exactly on the CPU)."""
+    w = w.detach()
+    return w if w.dtype == torch.float64 else w.float()
+
+
+# ------------------------------------------------------------------ host packers and folds
+def pack_ln_folded_dgrad(*pairs) -> Tensor:
+    """Data-gradient pack of projections run with their input LayerNorm's affine folded in:
+    pairs (W_i [N_i, C], gamma_i [C]) -> pack of cat_i(W_i diag(gamma_i))^T, [C, sum N_i]."""
+    wf = torch.cat([_master(w) * _master(g)[None, :] for w, g in pairs], 0)
+    return ops.pack_linear(wf.t().contiguous())
+
+
+def pack_upsample_dgrad(w: Tensor, f: int) -> Tensor:
+    """Upsample conv (nearest x f, then Conv1d k=3 p=1, w [Co, C, 3]) backward w.r.t. its low-res
+    input: one 3-tap GEMM over the [B, T, f*Co] view of the output gradient.  Tap j reads
+    low-res row q + j - 1; column block p holds the transposed phase-p weights."""
+    Co, C = w.shape[0], w.shape[1]
+    w = _master(w)
+    w0, w1, w2 = w[:, :, 0], w[:, :, 1], w[:, :, 2]
+    wd = torch.zeros(3, C, f * Co, dtype=w.dtype, device=w.device)
+    wd[2, :, 0:Co] = w0.t()                          # forward off -1 (phase 0, slot 0)
+    wd[1, :, 0:Co] = (w1 + w2).t()
+    wd[1, :, (f - 1) * Co:f * Co] = (w0 + w1).t()
+    wd[0, :, (f - 1) * Co:f * Co] = w2.t()          # forward off +1 (last phase, slot 1)
+    for p_ in range(1, f - 1):
+        wd[1, :, p_ * Co:(p_ + 1) * Co] = (w0 + w1 + w2).t()
+    return ops._pad_rows(wd.permute(1, 0, 2).reshape(C, 3 * f * Co), ops.round_up(C, 16))
+
+
+def upsample_wgrad_slots(f: int):
+    """[(phase, slot, row offset)] of the per-phase weight-gradient GEMMs of an upsample conv
+    (f >= 2): slot s of phase p multiplies the same low-res input rows as the forward phase
+    weights in slot s (see ops.pack_upsample_conv)."""
+    out = []
+    for p_ in range(f):
+        slots = [(0, -1), (1, 0)] if p_ == 0 else ([(0, 0), (1, 1)] if p_ == f - 1 else [(0, 0)])
+        out += [(p_, s_, off) for s_, off in slots]
+    return out
+
+
+def fold_upsample_wgrad(gwc: Tensor, f: int) -> Tensor:
+    """Per-phase, per-slot gradients gwc [f, 2, Co, C] -> the conv's weight gradient [Co, C, 3]."""
+    g0 = gwc[0, 0] + gwc[f - 1, 0]
+    g1 = gwc[0, 1] + gwc[f - 1, 0]
+    g2 = gwc[0, 1] + gwc[f - 1, 1]
+    for p_ in range(1, f - 1):
+        g0, g1, g2 = g0 + gwc[p_, 0], g1 + gwc[p_, 0], g2 + gwc[p_, 0]
+    return torch.stack([g0, g1, g2], dim=-1)
+
+
+def pack_down_dgrad(w: Tensor) -> Tensor:
+    """Downsample conv (k = stride = f, w [C, ci, f]) backward w.r.t. its input: a linear GEMM
+    writing the [B, T/f, f*ci] view; pack rows are ordered [tap][ci]."""
+    C, ci, f = w.shape
+    return ops.pack_linear(w.detach().permute(0, 2, 1).reshape(C, f * ci).t().contiguous())
+
+
+def pack_skipcat_dgrad(w_merge: Tensor, rp: int):
+    """SkipCat merge (1x1 conv over cat([skip * S_CAT, y]), w_merge [Co, 2*Co, 1]) backward:
+    (pack for d skip, pack for d y), block-diagonal over rp positions per row."""
+    Co = w_merge.shape[0]
+    wm = _master(w_merge)[:, :, 0]
+    wd_c1 = ops.pack_linear(torch.block_diag(*[wm[:, :Co].t() * S_CAT] * rp).contiguous())
+    wd_c2 = ops.pack_linear(torch.block_diag(*[wm[:, Co:].t()] * rp).contiguous())
+    return wd_c1, wd_c2
+
+
+def skipcat_weight_grad(blk1: Tensor, blk2: Tensor, rp: int, Co: int) -> Tensor:
+    """Weight gradients of the paired-position merge GEMMs [rp*Co, rp*Co] -> the merge conv's
+    [Co, 2*Co]: the diagonal blocks (same position in and out) sum to the 1x1 conv's gradient."""
+    g1 = blk1.view(rp, Co, rp, Co).diagonal(dim1=0, dim2=2).sum(-1) * S_CAT
+    g2 = blk2.view(rp, Co, rp, Co).diagonal(dim1=0, dim2=2).sum(-1)
+    return torch.cat([g1, g2], dim=1)
+
+
+def unfold_level0_grads(w_merge: Tensor, w_up: Tensor, b_up: Tensor, dw_up: Tensor, db_up: Tensor,
+                        dwa: Tensor, dba: Tensor, w_ad: Optional[Tensor] = None,
+                        b_ad: Optional[Tensor] = None) -> Dict[str, Tensor]:
+    """Level-0 SkipCat runs in the stem kernels with the merge conv folded into the upsample conv
+    (Wc2 W_up, Wc2 b_up + b_merge) and the skip adapter (S_CAT Wc1 W_ad, ...).  From the
+    gradients of the folded weights (dw_up [Co, C, 3], db_up, dwa [Co, Ci], dba) recover those of
+    merge / up / adapter, keyed by module and parameter name."""
+    Co = w_merge.shape[0]
+    wm = _master(w_merge)[:, :, 0]
+    wc1, wc2 = wm[:, :Co], wm[:, Co:]
+    w_up, b_up = _master(w_up), _master(b_up)
+    g = {"up.weight": torch.einsum("om,ock->mck", wc2, dw_up), "up.bias": wc2.t() @ db_up}
+    d_wc2 = torch.einsum("ock,mck->om", dw_up, w_up) + torch.outer(db_up, b_up)
+    if w_ad is not None:
+        w_ad, b_ad = _master(w_ad)[:, :, 0], _master(b_ad)
+        g["adapter.weight"] = S_CAT * (wc1.t() @ dwa)
+        g["adapter.bias"] = S_CAT * (wc1.t() @ dba)
+        d_wc1 = S_CAT * (dwa @ w_ad.t() + torch.outer(dba, b_ad))
+    else:
+        d_wc1 = S_CAT * dwa
+    g["merge.weight"] = torch.cat([d_wc1, d_wc2], dim=1)
+    g["merge.bias"] = db_up.clone()
+    return g
+
+
+def pack_inject_dgrad(w: Tensor, C: int, ctx_pad: int):
+    """InjectChannelsItem (1x1 conv over cat([x, ctx]), w [C, C + n_ctx, 1]) backward:
+    (pack for d x, pack for d ctx with the context channels zero-padded to ctx_pad)."""
+    n_ctx = w.shape[1] - C
+    wd_x = ops.pack_linear(w.detach()[:, :C, 0].t().contiguous())
+    wc = _master(w)[:, C:, 0].t()
+    wpad = torch.zeros(ctx_pad, C, dtype=wc.dtype, device=w.device)
+    wpad[:n_ctx] = wc
+    return wd_x, ops.pack_linear(wpad)
+
+
+# ------------------------------------------------------------------------ launch sequences
+def conv3_bwd(dy: Tensor, a_in: Tensor, gw: Tensor, da: Tensor, wd: Tensor, C: int):
+    """dy: grad of the conv output; a_in: its input; writes da, accumulates dW (3 taps)."""
+    ops.wgrad(dy, a_in, gw, n=C, k=C, off=-1, ntaps=3)
+    ops.conv_gemm(dy, wd, da, c_in=C, n_valid=C, taps=(-1, 0, 1))
+
+
+def upsample_bwd(dys: Tensor, x_last: Tensor, wd_up: Tensor, gw: Tensor, db: Tensor, dx_last: Tensor,
+                 f: int) -> None:
+    """Backward of the up conv x_last [B, Tl, C] -> y [B, f*Tl, Co], given dys = dL/dy.
+    f >= 2: gw is the per-phase accumulator [f, 2, Co, C] (fold_upsample_wgrad), wd_up from
+    pack_upsample_dgrad.  f = 1: a plain k=3 conv, gw [3, Co, C], wd_up = ops.pack_conv_dgrad.
+    Accumulates gw and db (bias), writes dx_last."""
+    B, Tl, C = x_last.shape
+    Co = dys.shape[-1]
+    ops.colsum(dys, db)
+    if f > 1:
+        for p_, s_, off in upsample_wgrad_slots(f):
+            ops.wgrad(dys.view(B, Tl, f * Co), x_last, gw[p_, s_], n=Co, k=C, off=off, g_col0=p_ * Co)
+        ops.conv_gemm(dys.view(B, Tl, f * Co), wd_up, dx_last, c_in=f * Co, n_valid=C, taps=(-1, 0, 1))
+    else:
+        ops.wgrad(dys, x_last, gw, n=Co, k=C, off=-1, ntaps=3)
+        ops.conv_gemm(dys, wd_up, dx_last, c_in=Co, n_valid=C, taps=(-1, 0, 1))
+
+
+def downsample_bwd(d: Tensor, x_in: Tensor, wd_down: Tensor, gw_down: Tensor, db_down: Tensor,
+                   d_xin: Tensor, d_skip: Tensor, f: int, wgrad_done=None) -> None:
+    """Backward of the down conv x_in [B, T, ci] -> [B, T/f, C] (k = stride = f), given d = its
+    output gradient.  Accumulates gw_down ([C, f*ci], [co][tap][ci]) and db_down; writes
+    d_xin = dgrad + d_skip (the gradient reaching the level input through the skip path).
+    wgrad_done() runs once the weight gradients are complete."""
+    B, Tl, C = d.shape
+    kdim = f * x_in.shape[-1]
+    ops.colsum(d, db_down)
+    ops.wgrad(d, x_in.view(B, Tl, kdim), gw_down, n=C, k=kdim, off=0)
+    if wgrad_done is not None:
+        wgrad_done()
+    ops.conv_gemm(d, wd_down, d_xin.view(B, Tl, kdim), c_in=C, n_valid=kdim,
+                  residual=d_skip.view(B, Tl, kdim))
+
+
+def skipcat_bwd(d_out: Tensor, skip: Tensor, y_up: Tensor, wd_c1: Tensor, wd_c2: Tensor, gw_cat: Tensor,
+                db_cat: Tensor, blk1: Tensor, blk2: Tensor, dys: Tensor, d_skip: Tensor, rp: int) -> None:
+    """Backward of out = merge(cat([skip * S_CAT, y_up])) on [B, T, Co] tensors, rp positions per
+    GEMM row.  Accumulates db_cat and the block products blk1 / blk2 [rp*Co, rp*Co], writes
+    gw_cat [Co, 2*Co] (from blk1 / blk2), dys and d_skip."""
+    B, T, Co = d_out.shape
+
+    def rows(t):
+        return t.view(B, T // rp, rp * Co)
+    ops.colsum(d_out, db_cat)
+    ops.wgrad(rows(d_out), rows(skip), blk1, n=rp * Co, k=rp * Co)
+    ops.wgrad(rows(d_out), rows(y_up), blk2, n=rp * Co, k=rp * Co)
+    gw_cat.copy_(skipcat_weight_grad(blk1, blk2, rp, Co))
+    ops.conv_gemm(rows(d_out), wd_c2, rows(dys), c_in=rp * Co, n_valid=rp * Co)
+    ops.conv_gemm(rows(d_out), wd_c1, rows(d_skip), c_in=rp * Co, n_valid=rp * Co)
+
+
+def inject_bwd(d_out: Tensor, x: Tensor, ctxb: Tensor, dctxb: Tensor, wd_x: Tensor, wd_c: Tensor,
+               gw: Tensor, db: Tensor, dx: Tensor, n_ctx: int) -> Tensor:
+    """Backward of out = conv1x1(cat([x, ctx])) + x (InjectChannelsItem).  ctxb / dctxb: the
+    context and its gradient [B, T, ctx_pad]; dctxb is ACCUMULATED in place (the items of one
+    depth share it).  Accumulates gw [C, C + n_ctx] and db; writes and returns dx."""
+    C = x.shape[-1]
+    ops.colsum(d_out, db)
+    ops.wgrad(d_out, x, gw[:, :C], n=C, k=C)
+    ops.wgrad(d_out, ctxb, gw[:, C:], n=C, k=n_ctx)
+    ops.conv_gemm(d_out, wd_c, dctxb, c_in=C, n_valid=ctxb.shape[-1], residual=dctxb)
+    ops.conv_gemm(d_out, wd_x, dx, c_in=C, n_valid=C, residual=d_out)   # + the identity path
+    return dx
+
+
+def resnet_item_bwd(dy: Tensor, x: Tensor, h: Tensor, rr: Tensor, a1: Tensor, a2: Tensor, x_stats: Tensor,
+                    h_stats: Tensor, gn1, gn2, wd1: Tensor, wd2: Tensor, gw1: Tensor, gw2: Tensor, dgn1, dgn2,
+                    db1: Tensor, db2: Tensor, S1: Tensor, S2: Tensor, work, groups: int, film=None) -> Tensor:
+    """Backward of a ResnetItem (C >= 32) and its ModulationItem:
+        h = conv1(SiLU(GN1(x))), rr = conv2(SiLU(GN2(h))) + x, y = LN(rr) (1 + scale) + shift.
+    Saved forward tensors: a1 = SiLU(GN1(x)), a2 = SiLU(GN2(h)), GroupNorm statistics x_stats,
+    h_stats.  gn1 / gn2 = (gamma, beta); wd1 / wd2 = ops.pack_conv_dgrad packs.  Accumulates the
+    parameter gradients gw1 / gw2 ([3, C, C] tap-major), dgn1 / dgn2 = (dgamma, dbeta), db1 / db2;
+    S1 / S2 are the GroupNorm backward sums.  work = (dr, dh, dx, dxh, da) bf16 [B, T, C]
+    buffers.  film = (scale_shift, d scale_shift, row stride, eps) of the ModulationItem, or None
+    without one (dy is then dL/drr).  Returns dx."""
+    dr, dh, dx, dxh, da = work
+    C = x.shape[-1]
+    if film is not None:
+        ss, dss, ss_stride, eps = film
+        ops.ln_film_bwd(dy, rr, ss, ss_stride, dr, dss=dss, dss_stride=ss_stride, colsum=db2, eps=eps)
+    else:
+        dr = dy
+        ops.colsum(dy, db2)
+    conv3_bwd(dr, a2, gw2, da, wd2, C)
+    ops.gn_silu_bwd(da, h, h_stats, gn2[0], gn2[1], dxh, dgn2[0], dgn2[1], S2, groups)
+    ops.gn_bwd_apply(dxh, h, h_stats, S2, dh, groups, colsum=db1)
+    conv3_bwd(dh, a1, gw1, da, wd1, C)
+    ops.gn_silu_bwd(da, x, x_stats, gn1[0], gn1[1], dxh, dgn1[0], dgn1[1], S1, groups)
+    ops.gn_bwd_apply(dxh, x, x_stats, S1, dx, groups, dres=dr)
+    return dx
+
+
 def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin: bool) -> _TrainPlan:
     """mode 'loss': noising + MSE fused (VDiffusion); 'v': plain net forward, backward from dL/dv.
     M = embedding tokens (0 without CrossAttentionItems)."""
@@ -113,8 +330,12 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
     refreshers: List = []                  # re-pack the dgrad weights in place after a weight update
 
     def packed_dgrad(make):
+        """make() -> one pack or a tuple of packs, re-made in place by the refreshers."""
         t = make()
-        refreshers.append(lambda t=t, make=make: t.copy_(make()))
+        if isinstance(t, tuple):
+            refreshers.append(lambda t=t, make=make: [a.copy_(b) for a, b in zip(t, make())])
+        else:
+            refreshers.append(lambda t=t, make=make: t.copy_(make()))
         return t
 
     grads: Dict[int, Tensor] = {}          # id(param) -> fp32 gradient (PyTorch layout / packed)
@@ -168,11 +389,6 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
             delta_ws[0] = _zeros((B * heads * Tl,), dev)
         return delta_ws[0]
 
-    def conv3_bwd(dy: Tensor, a_in: Tensor, gw: Tensor, da: Tensor, wd: Tensor, C: int):
-        """dy: grad of the conv output; a_in: its input; writes da, accumulates dW (3 taps)."""
-        ops.wgrad(dy, a_in, gw, n=C, k=C, off=-1, ntaps=3)
-        ops.conv_gemm(dy, wd, da, c_in=C, n_valid=C, taps=(-1, 0, 1))
-
     # ---- AttentionItem / CrossAttentionItem (a_unet): x + to_out(softmax(q k^T / 8) v)
     def attention_block(x: Tensor, xn: Tensor, ap: Dict, am, cross: bool, Tl: int, C: int,
                         out_stats: Optional[Tensor]):
@@ -196,11 +412,8 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
                                                   bias=ap["b_qkv"]))
             plan.fwd.append(lambda: ops.attention(q, k, v, o, heads, att_scale, lse=lse))
 
-            def make_wd():
-                wf = torch.cat([am.to_q.weight.detach().float() * g1.detach().float()[None, :],
-                                am.to_kv.weight.detach().float() * g2.detach().float()[None, :]], 0)
-                return ops.pack_linear(wf.t().contiguous())          # [C, 3*mid]
-            wd_qkv = packed_dgrad(make_wd)
+            wd_qkv = packed_dgrad(lambda: pack_ln_folded_dgrad((am.to_q.weight, g1),
+                                                               (am.to_kv.weight, g2)))   # [C, 3*mid]
             gwf, dbf = gbuf((3 * mid, C)), gbuf((3 * mid,))
 
             def bwd(dy2: Tensor) -> Tensor:
@@ -223,10 +436,8 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
             plan.fwd.append(lambda: ops.conv_gemm(xn, ap["w_q"], q, c_in=C, n_valid=mid, bias=ap["b_q"]))
             plan.fwd.append(lambda: ops.attention(q, kv[..., :mid], kv[..., mid:], o, heads, att_scale,
                                                   lse=lse))
-            wd_q = packed_dgrad(lambda: ops.pack_linear(
-                (am.to_q.weight.detach().float() * g1.detach().float()[None, :]).t().contiguous()))
-            wd_kv = packed_dgrad(lambda: ops.pack_linear(
-                (am.to_kv.weight.detach().float() * g2.detach().float()[None, :]).t().contiguous()))
+            wd_q = packed_dgrad(lambda: pack_ln_folded_dgrad((am.to_q.weight, g1)))
+            wd_kv = packed_dgrad(lambda: pack_ln_folded_dgrad((am.to_kv.weight, g2)))
             gwq, dbq = gbuf((mid, C)), gbuf((mid,))
             gwkv, dbkv = gbuf((2 * mid, E)), gbuf((2 * mid,))
 
@@ -322,22 +533,14 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
                 gw = {"w1": grad_for(r_.conv1.weight, (3, C, C), (1, 2, 0)),
                       "w2": grad_for(r_.conv2.weight, (3, C, C), (1, 2, 0))}
 
-                def bwd(dy, x=x, h=h, rr=rr, a1=a1, a2=a2, ss=ss, dss=dss, xs=x_stats, hs=h_stats,
-                        ip=ip, dr=dr, dh=dh, dx=dx, dxh=dxh, da=da, S1=S1, S2=S2, dgn1=dgn1,
-                        dgn2=dgn2, db1=db1, db2=db2, wd1=wd1, wd2=wd2, gw=gw, C=C):
-                    if mod:
-                        ops.ln_film_bwd(dy, rr, ss, ss_stride, dr, dss=dss, dss_stride=ss_stride,
-                                        colsum=db2, eps=net.MOD_LN_EPS)
-                    else:
-                        dr = dy
-                        ops.colsum(dy, db2)
-                    conv3_bwd(dr, a2, gw["w2"], da, wd2, C)
-                    ops.gn_silu_bwd(da, h, hs, ip["gn2"][0], ip["gn2"][1], dxh, dgn2[0], dgn2[1], S2, G)
-                    ops.gn_bwd_apply(dxh, h, hs, S2, dh, G, colsum=db1)
-                    conv3_bwd(dh, a1, gw["w1"], da, wd1, C)
-                    ops.gn_silu_bwd(da, x, xs, ip["gn1"][0], ip["gn1"][1], dxh, dgn1[0], dgn1[1], S1, G)
-                    ops.gn_bwd_apply(dxh, x, xs, S1, dx, G, dres=dr)
-                    return dx
+                film = (ss, dss, ss_stride, net.MOD_LN_EPS) if mod else None
+
+                def bwd(dy, x=x, h=h, rr=rr, a1=a1, a2=a2, xs=x_stats, hs=h_stats, ip=ip,
+                        work=(dr, dh, dx, dxh, da), S1=S1, S2=S2, dgn1=dgn1, dgn2=dgn2, db1=db1,
+                        db2=db2, wd1=wd1, wd2=wd2, gw=gw, film=film):
+                    return resnet_item_bwd(dy, x, h, rr, a1, a2, xs, hs, ip["gn1"], ip["gn2"], wd1, wd2,
+                                           gw["w1"], gw["w2"], dgn1, dgn2, db1, db2, S1, S2, work, G,
+                                           film=film)
             if mod:
                 grads[id(im.modulation.proj.weight)] = ("cond_w", ip["ss_off"], 2 * C)
                 grads[id(im.modulation.proj.bias)] = ("cond_b", ip["ss_off"], 2 * C)
@@ -357,24 +560,13 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
                     x, jp["w_x"], yi, c_in=C, n_valid=C, residual=tmp, stats=st, groups=G))
                 gw_inj = grad_for(conv.weight, (C, C + n_ctx, 1)).view(C, C + n_ctx)
                 db_inj = grad_for(conv.bias)
-                wd_x = packed_dgrad(lambda conv=conv, C=C: ops.pack_linear(
-                    conv.weight.detach()[:, :C, 0].t().contiguous()))
-
-                def make_wd_c(conv=conv, C=C, ctx_pad=ctx_pad, n_ctx=n_ctx):
-                    w = torch.zeros(ctx_pad, C, device=dev)
-                    w[:n_ctx] = conv.weight.detach().float()[:, C:, 0].t()
-                    return ops.pack_linear(w)
-                wd_c = packed_dgrad(make_wd_c)
+                wd_x, wd_c = packed_dgrad(lambda conv=conv, C=C, ctx_pad=ctx_pad: pack_inject_dgrad(
+                    conv.weight, C, ctx_pad))
 
                 def inj_bwd(d_out, x=x, ctxb=ctxb, dctxb=dctxb, gw_inj=gw_inj, db_inj=db_inj, wd_x=wd_x,
-                            wd_c=wd_c, dyi=dyi, C=C, n_ctx=n_ctx, ctx_pad=ctx_pad):
-                    ops.colsum(d_out, db_inj)
-                    ops.wgrad(d_out, x, gw_inj[:, :C], n=C, k=C)
-                    ops.wgrad(d_out, ctxb, gw_inj[:, C:], n=C, k=n_ctx)
-                    # d context, summed over the items of this depth (in place through the residual)
-                    ops.conv_gemm(d_out, wd_c, dctxb, c_in=C, n_valid=ctx_pad, residual=dctxb)
-                    ops.conv_gemm(d_out, wd_x, dyi, c_in=C, n_valid=C, residual=d_out)   # + the identity path
-                    return dyi
+                            wd_c=wd_c, dyi=dyi, n_ctx=n_ctx):
+                    # d context is summed over the items of this depth (in place through the residual)
+                    return inject_bwd(d_out, x, ctxb, dctxb, wd_x, wd_c, gw_inj, db_inj, dyi, n_ctx)
                 chain.append(inj_bwd)
                 x, x_stats = yi, inj_stats
             for kind, am in (("att", im.attention), ("cross", im.cross)):
@@ -417,8 +609,7 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
             kdim = lv.factor * lv.in_ch
             plan.fwd.append(lambda: ops.conv_gemm(x_in.view(B, Tl, kdim), Lp["down_w"], x0, c_in=kdim,
                                                   n_valid=C, bias=Lp["down_b"], stats=st0, groups=G))
-            wd_down = packed_dgrad(lambda: ops.pack_linear(
-                lv.down.weight.detach().permute(0, 2, 1).reshape(C, kdim).t().contiguous()))
+            wd_down = packed_dgrad(lambda: pack_down_dgrad(lv.down.weight))
             # [co][tap][ci] (the [B, T/f, f*C] view) -> PyTorch [co][ci][tap]
             gw_down = grad_for(lv.down.weight, (C, lv.factor, lv.in_ch), (0, 2, 1)).view(C, kdim)
         x, st, items_down_bwd = run_items(x0, st0, Lp["items_down"], lv.items_down, lv, Tl, li=i)
@@ -429,7 +620,6 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
             x, st, inner = level(i + 1, skip, Tl)
         cur["inner_end"] = cursor[0]
         x, st, items_up_bwd = run_items(x, st, Lp["items_up"], lv.items_up, lv, Tl, li=i)
-        s_cat = 2 ** -0.5
         if mod:
             gate = ss_all[:, Lp["gate_off"]:]
             dgate = dss_all[:, Lp["gate_off"]:]
@@ -446,22 +636,14 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
             dwa, dba = gbuf((Co, Ci)), gbuf((Co,))
 
             def unfold_level0():
-                wm = lv.merge.weight.detach().float()[:, :, 0]
-                wc1, wc2 = wm[:, :Co], wm[:, Co:]
-                w_up, b_up = lv.up.weight.detach().float(), lv.up.bias.detach().float()
-                grads[id(lv.up.weight)] = torch.einsum("om,ock->mck", wc2, dw_up)
-                grads[id(lv.up.bias)] = wc2.t() @ db_up
-                d_wc2 = torch.einsum("ock,mck->om", dw_up, w_up) + torch.outer(db_up, b_up)
-                if lv.adapter is not None:
-                    w_ad = lv.adapter.weight.detach().float()[:, :, 0]
-                    b_ad = lv.adapter.bias.detach().float()
-                    grads[id(lv.adapter.weight)] = s_cat * (wc1.t() @ dwa)
-                    grads[id(lv.adapter.bias)] = s_cat * (wc1.t() @ dba)
-                    d_wc1 = s_cat * (dwa @ w_ad.t() + torch.outer(dba, b_ad))
-                else:
-                    d_wc1 = s_cat * dwa
-                grads[id(lv.merge.weight)] = torch.cat([d_wc1, d_wc2], dim=1)
-                grads[id(lv.merge.bias)] = db_up.clone()
+                ad = lv.adapter
+                g = unfold_level0_grads(lv.merge.weight, lv.up.weight, lv.up.bias, dw_up, db_up, dwa, dba,
+                                        ad.weight if ad is not None else None,
+                                        ad.bias if ad is not None else None)
+                for mod_name, m in (("up", lv.up), ("merge", lv.merge), ("adapter", ad)):
+                    if m is not None:
+                        grads[id(m.weight)] = g[mod_name + ".weight"]
+                        grads[id(m.bias)] = g[mod_name + ".bias"]
             finals.append(unfold_level0)
         else:
             db_up = grad_for(lv.up.bias)
@@ -506,50 +688,17 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
             plan.fwd.append(lambda: ops.conv_gemm(x_last, Lp["up_w"], y_up.view(B, Tl, f * Co), c_in=C,
                                                   n_valid=Co, up_factor=f, bias=Lp["up_b"]))
 
-            def make_wd_up():
-                w = lv.up.weight.detach().float()
-                w0, w1, w2 = w[:, :, 0], w[:, :, 1], w[:, :, 2]
-                wd = torch.zeros(3, C, f * Co, device=dev)      # taps read dys rows q-1, q, q+1
-                wd[2, :, 0:Co] = w0.t()                          # forward off -1 (phase 0, slot 0)
-                wd[1, :, 0:Co] = (w1 + w2).t()
-                wd[1, :, (f - 1) * Co:f * Co] = (w0 + w1).t()
-                wd[0, :, (f - 1) * Co:f * Co] = w2.t()          # forward off +1 (last phase, slot 1)
-                for p_ in range(1, f - 1):
-                    wd[1, :, p_ * Co:(p_ + 1) * Co] = (w0 + w1 + w2).t()
-                return ops._pad_rows(wd.permute(1, 0, 2).reshape(C, 3 * f * Co), ops.round_up(C, 16))
-            wd_up = packed_dgrad(make_wd_up)
-            gwc = gbuf((f, 2, Co, C))
-
-            def up_wgrad():
-                for p_ in range(f):
-                    slots = [(0, -1), (1, 0)] if p_ == 0 else ([(0, 0), (1, 1)] if p_ == f - 1 else [(0, 0)])
-                    for s_, off in slots:
-                        ops.wgrad(dys.view(B, Tl, f * Co), x_last, gwc[p_, s_], n=Co, k=C, off=off,
-                                  g_col0=p_ * Co)
+            wd_up = packed_dgrad(lambda: pack_upsample_dgrad(lv.up.weight, f))
+            gw_up = gbuf((f, 2, Co, C))
 
             def up_final():
-                g0 = gwc[0, 0] + gwc[f - 1, 0]
-                g1 = gwc[0, 1] + gwc[f - 1, 0]
-                g2 = gwc[0, 1] + gwc[f - 1, 1]
-                for p_ in range(1, f - 1):
-                    g0, g1, g2 = g0 + gwc[p_, 0], g1 + gwc[p_, 0], g2 + gwc[p_, 0]
-                grads[id(lv.up.weight)] = torch.stack([g0, g1, g2], dim=-1)
+                grads[id(lv.up.weight)] = fold_upsample_wgrad(gw_up, f)
             finals.append(up_final)
-
-            def up_dgrad():
-                ops.conv_gemm(dys.view(B, Tl, f * Co), wd_up, dx_last, c_in=f * Co, n_valid=C,
-                              taps=(-1, 0, 1))
         else:
             plan.fwd.append(lambda: ops.conv_gemm(x_last, Lp["up_w"], y_up, c_in=C, n_valid=Co,
                                                   taps=(-1, 0, 1), bias=Lp["up_b"]))
             wd_up = packed_dgrad(lambda: ops.pack_conv_dgrad(lv.up.weight.detach()))
-            gw3 = grad_for(lv.up.weight, (3, Co, C), (1, 2, 0))
-
-            def up_wgrad():
-                ops.wgrad(dys, x_last, gw3, n=Co, k=C, off=-1, ntaps=3)
-
-            def up_dgrad():
-                ops.conv_gemm(dys, wd_up, dx_last, c_in=Co, n_valid=C, taps=(-1, 0, 1))
+            gw_up = grad_for(lv.up.weight, (3, Co, C), (1, 2, 0))
         if mod:
             plan.fwd.append(lambda: ops.skip_gate(y_up, x_in, gate, out, ost, G))
             d_skip_of = lambda d_out: d_out      # noqa: E731  (the skip path's gradient is d_out itself)
@@ -573,30 +722,18 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
             if rp > 1:
                 plan.fwd.append(lambda: ops.gn_stats(out, ost, G))
             wm_ = lv.merge.weight
-            wd_c1 = packed_dgrad(lambda: ops.pack_linear(torch.block_diag(
-                *[wm_.detach().float()[:, :Co, 0].t() * s_cat] * rp).contiguous()))
-            wd_c2 = packed_dgrad(lambda: ops.pack_linear(torch.block_diag(
-                *[wm_.detach().float()[:, Co:, 0].t()] * rp).contiguous()))
+            wd_c1, wd_c2 = packed_dgrad(lambda: pack_skipcat_dgrad(wm_, rp))
             gw_cat = grad_for(wm_, (Co, 2 * Co, 1)).view(Co, 2 * Co)
             db_cat = grad_for(lv.merge.bias)
             blk1, blk2 = gbuf((rp * Co, rp * Co)), gbuf((rp * Co, rp * Co))
             d_skip_of = lambda d_out: d_skip     # noqa: E731
 
             def merge_bwd(d_out: Tensor) -> None:
-                ops.colsum(d_out, db_cat)
-                ops.wgrad(rows(d_out), rows(x_in), blk1, n=rp * Co, k=rp * Co)
-                ops.wgrad(rows(d_out), rows(y_up), blk2, n=rp * Co, k=rp * Co)
-                # the diagonal blocks of the paired-position products sum to the 1x1 conv's gradient
-                gw_cat[:, :Co].copy_(blk1.view(rp, Co, rp, Co).diagonal(dim1=0, dim2=2).sum(-1) * s_cat)
-                gw_cat[:, Co:].copy_(blk2.view(rp, Co, rp, Co).diagonal(dim1=0, dim2=2).sum(-1))
-                ops.conv_gemm(rows(d_out), wd_c2, rows(dys), c_in=rp * Co, n_valid=rp * Co)
-                ops.conv_gemm(rows(d_out), wd_c1, rows(d_skip), c_in=rp * Co, n_valid=rp * Co)
+                skipcat_bwd(d_out, x_in, y_up, wd_c1, wd_c2, gw_cat, db_cat, blk1, blk2, dys, d_skip, rp)
 
         def backward_level(d_out: Tensor) -> Tensor:
             merge_bwd(d_out)
-            ops.colsum(dys, db_up)
-            up_wgrad()
-            up_dgrad()
+            upsample_bwd(dys, x_last, wd_up, gw_up, db_up, dx_last, f)
             d = dx_last
             for b_ in reversed(items_up_bwd):
                 d = b_(d)
@@ -605,13 +742,10 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
                 d = inner(d)
             for b_ in reversed(items_down_bwd):
                 d = b_(d)
-            ops.colsum(d, db_down)
-            kdim = lv.factor * lv.in_ch
-            ops.wgrad(d, x_in.view(B, Tl, kdim), gw_down, n=C, k=kdim, off=0)
-            plan.mark((cur["entry"], cur["down_end"] if inner is not None else cur["exit"]))
-            # gradient w.r.t. the level input = dgrad(down conv) + the skip path (d_out)
-            ops.conv_gemm(d, wd_down, d_xin.view(B, Tl, kdim), c_in=C, n_valid=kdim,
-                          residual=d_skip_of(d_out).view(B, Tl, kdim))
+            # gradient w.r.t. the level input = dgrad(down conv) + the skip path
+            downsample_bwd(d, x_in, wd_down, gw_down, db_down, d_xin, d_skip_of(d_out), lv.factor,
+                           wgrad_done=lambda: plan.mark((cur["entry"],
+                                                         cur["down_end"] if inner is not None else cur["exit"])))
             return d_xin
 
         cur["exit"] = cursor[0]

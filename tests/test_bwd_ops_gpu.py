@@ -46,9 +46,12 @@ def stats_of(y, groups):
                                          (2, 1000, 256, 256, 0), (1, 64, 1024, 512, 1),
                                          (3, 100, 8, 32, 0), (2, 4096, 64, 64, -1)])
 def test_wgrad(ops, B, T, n, k, off):
+    """The contract is dw += g^T x: the gradient arenas and the upsample per-phase slots rely on
+    accumulation, so dw starts from non-zero values of the size of the product."""
     g = bf(rnd(B, T, n, seed=1))
     x = bf(rnd(B, T, k, seed=2))
-    dw = torch.zeros(n, k, device=DEV)
+    dw0 = rnd(n, k, scale=(B * T) ** 0.5, seed=3)
+    dw = dw0.clone()
     ops.wgrad(g, x, dw, n=n, k=k, off=off)
     xs = torch.zeros_like(x.float())
     if off == 0:
@@ -57,7 +60,7 @@ def test_wgrad(ops, B, T, n, k, off):
         xs[:, :-off] = x.float()[:, off:]
     else:
         xs[:, -off:] = x.float()[:, :off]
-    ref = torch.einsum("btn,btk->nk", g.float(), xs)
+    ref = dw0 + torch.einsum("btn,btk->nk", g.float(), xs)
     close(dw, ref, 2e-3, 1e-3, f"wgrad n{n} k{k} off{off}")
 
 
@@ -330,12 +333,14 @@ def test_stem_input_gradient(ops, adapter):
 @pytest.mark.parametrize("B,T,n,k", [(2, 256, 64, 64), (2, 300, 128, 128), (1, 100, 32, 32), (4, 256, 1024, 1024),
                                      (3, 1000, 256, 512), (2, 4096, 8, 32), (1, 64, 512, 96)])
 def test_wgrad_three_taps_fused(ops, B, T, n, k):
-    """The three taps of a k=3 convolution in one launch (row-shifted views of one X box)."""
+    """The three taps of a k=3 convolution in one launch (row-shifted views of one X box),
+    accumulated into a non-zero dw."""
     g = bf(rnd(B, T, n, seed=11))
     x = bf(rnd(B, T, k, seed=12))
-    dw = torch.zeros(3, n, k, device=DEV)
+    dw0 = rnd(3, n, k, scale=(B * T) ** 0.5, seed=13)
+    dw = dw0.clone()
     ops.wgrad(g, x, dw, n=n, k=k, off=-1, ntaps=3)
     xp = F.pad(x.float(), (0, 0, 1, 1))                      # zero rows at t = -1 and t = T
     for tap in range(3):
-        ref = torch.einsum("btn,btk->nk", g.float(), xp[:, tap:tap + T])
+        ref = dw0[tap] + torch.einsum("btn,btk->nk", g.float(), xp[:, tap:tap + T])
         close(dw[tap], ref, 1e-2, 1e-3, f"fused wgrad tap {tap} B{B} T{T} n{n} k{k}")

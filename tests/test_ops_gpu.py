@@ -51,23 +51,43 @@ def stats_of(y, groups):
 
 
 # ------------------------------------------------------------------------- conv_gemm
-@pytest.mark.parametrize("B,T,cin,n", [
-    (2, 256, 64, 64),      # SW128, one k-chunk
-    (2, 384, 128, 256),    # SW128, two k-chunks, wide N
-    (1, 128, 32, 32),      # SW64
-    (3, 200, 16, 48),      # SW32, ragged T, n_pad 48
-    (2, 40, 64, 8),        # T < tile, n_valid 8 (padded to 16)
-    (1, 1024, 512, 1536),  # qkv-sized
-    (2, 130, 1024, 128),   # long K pipeline (16 chunks > stages), ragged T
-])
-def test_conv_gemm_linear(ops, B, T, cin, n):
+_LINEAR = [
+    (2, 256, 64, 64, None),        # SW128, one k-chunk
+    (2, 384, 128, 256, None),      # SW128, two k-chunks, wide N
+    (1, 128, 32, 32, None),        # SW64
+    (3, 200, 16, 48, None),        # SW32, ragged T, n_pad 48
+    (2, 40, 64, 8, None),          # T < tile, n_valid 8 (padded to 16)
+    (1, 1024, 512, 1536, None),    # qkv-sized
+    (2, 130, 1024, 128, None),     # long K pipeline (16 chunks > stages), ragged T
+    # backward-only contracts: a residual read from a separate tensor, or from `out` itself (the
+    # in-place accumulation of the cross-attention / injected-context gradients), and narrow
+    # n_valid = f * ci dgrad outputs with the skip gradient as residual
+    (2, 256, 64, 64, "residual"),
+    (3, 200, 64, 32, "residual"),  # n_valid 32, ragged T
+    (3, 200, 128, 48, "residual"),  # n_valid 48
+    (2, 256, 64, 64, "inplace"),
+    (3, 200, 64, 32, "inplace"),
+    (2, 40, 128, 48, "inplace"),
+    (2, 130, 1024, 768, "inplace"),  # K/V dgrad -> LayerNorm(embedding) gradient, long K
+]
+
+
+@pytest.mark.parametrize("B,T,cin,n,res", _LINEAR,
+                         ids=["-".join(str(v) for v in case if v is not None) for case in _LINEAR])
+def test_conv_gemm_linear(ops, B, T, cin, n, res):
     a = bf(rnd(B, T, cin, seed=1))
     w = bf(rnd(n, cin, scale=cin ** -0.5, seed=2))
     bias = rnd(n, seed=3)
     out = torch.full((B, T, n), float("nan"), dtype=torch.bfloat16, device=DEV)
-    ops.conv_gemm(a, ops.pack_linear(w), out, c_in=cin, n_valid=n, bias=bias)
-    ref = a.float() @ w.float().t() + bias
-    assert_close(out, ref, 2 ** -7, 1e-2, f"linear B{B} T{T} K{cin} N{n}")
+    residual = None
+    if res is not None:
+        residual = bf(rnd(B, T, n, seed=4))
+        if res == "inplace":
+            out.copy_(residual)
+            residual = out
+    ref = a.float() @ w.float().t() + bias + (0.0 if residual is None else residual.float())
+    ops.conv_gemm(a, ops.pack_linear(w), out, c_in=cin, n_valid=n, bias=bias, residual=residual)
+    assert_close(out, ref, 2 ** -7, 1e-2, f"linear B{B} T{T} K{cin} N{n} {res or ''}")
 
 
 @pytest.mark.parametrize("block_n", [16, 32, 64, 128, 256])
