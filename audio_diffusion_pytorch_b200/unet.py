@@ -213,6 +213,10 @@ class B200UNet(nn.Module):
         self.use_modulation = use_modulation
         for c in self.channels:
             assert c % resnet_groups == 0 and c % 8 == 0, "channels must be multiples of 8 and groups"
+        # every ResnetItem conv GEMM sums the GroupNorm statistics of its output in its epilogue,
+        # which holds at most 8 groups (csrc/conv_gemm.cu kMaxGroups)
+        assert 1 <= resnet_groups <= 8, \
+            f"resnet_groups={resnet_groups}: the conv GEMM's fused GroupNorm statistics support at most 8 groups"
         assert self.out_channels <= 4 and self.in_channels <= 8, "stem kernels: in<=8, out<=4 channels"
 
         # registration order mirrors a_unet: time plugin, cfg plugin, then the recursive blocks
@@ -662,8 +666,7 @@ class B200UNet(nn.Module):
             narrow = C == 8 and not self._verify_fp32
             # thin levels (C = 32, 64) are HBM-bound: one fused ConvBlock kernel (mid_conv.cu)
             # instead of gn_silu -> conv_gemm (-> ln_film)
-            thin = narrow or (self.fuse_thin_levels and C in (32, 64) and (C // G) % 4 == 0
-                              and not self._verify_fp32)
+            thin = narrow or (self.fuse_thin_levels and C in (32, 64) and not self._verify_fp32)
             for idx, ip in enumerate(items_p):
                 ss = ss_all[:, ip["ss_off"]:] if mod else None
                 has_att, has_cross, has_inj = "att" in ip, "cross" in ip, "inj" in ip

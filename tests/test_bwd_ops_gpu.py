@@ -36,6 +36,12 @@ def ops():
     return ops
 
 
+def group_ids(cases):
+    """pytest ids of cases whose last entry is the GroupNorm group count; 8 groups (the default
+    of UNetV0) is left out of the id."""
+    return ["-".join(str(v) for v in c[:-1]) + ("" if c[-1] == 8 else f"-g{c[-1]}") for c in cases]
+
+
 def stats_of(y, groups):
     B, T, Cc = y.shape
     yg = y.double().reshape(B, T, groups, Cc // groups)
@@ -75,9 +81,16 @@ def test_wgrad_column_views(ops):
     close(dw, ref, 2e-3, 1e-3, "wgrad column view")
 
 
-@pytest.mark.parametrize("B,T,C", [(2, 1000, 8), (2, 512, 32), (2, 300, 64), (1, 256, 512), (2, 128, 1024)])
-def test_gn_silu_backward(ops, B, T, C):
-    groups = 8
+# the per-channel coefficients (gn_coeffs), the per-group S sums of gn_silu_bwd and their
+# broadcast back to channels in gn_bwd_apply all index by channel / group size
+_GN_BWD = [(2, 1000, 8, 8), (2, 512, 32, 8), (2, 300, 64, 8), (1, 256, 512, 8), (2, 128, 1024, 8),
+           (2, 1000, 8, 1), (2, 1000, 8, 2), (2, 1000, 8, 4), (2, 512, 32, 2), (2, 512, 32, 16),
+           (2, 300, 64, 1), (2, 300, 64, 4), (2, 300, 64, 16), (2, 300, 64, 64), (1, 256, 512, 2),
+           (2, 128, 1024, 1), (2, 128, 1024, 4), (2, 128, 1024, 16), (2, 128, 1024, 64)]
+
+
+@pytest.mark.parametrize("B,T,C,groups", _GN_BWD, ids=group_ids(_GN_BWD))
+def test_gn_silu_backward(ops, B, T, C, groups):
     x = bf(rnd(B, T, C, seed=5) * 1.5 + 0.3)
     da = bf(rnd(B, T, C, seed=6))
     dres = bf(rnd(B, T, C, seed=7))
@@ -93,9 +106,9 @@ def test_gn_silu_backward(ops, B, T, C):
     cs = torch.zeros(C, device=DEV)
     ops.gn_silu_bwd(da, x, stats, gamma.detach(), beta.detach(), dxh, dg, db, S, groups)
     ops.gn_bwd_apply(dxh, x, stats, S, dx, groups, dres=dres, colsum=cs)
-    close(dx, xr.grad + dres.float(), 2 ** -6, 2e-3, f"gn bwd dx C{C}")
-    close(dg, gamma.grad, 1e-2, 2e-3, f"gn bwd dgamma C{C}")
-    close(db, beta.grad, 1e-2, 2e-3, f"gn bwd dbeta C{C}")
+    close(dx, xr.grad + dres.float(), 2 ** -6, 2e-3, f"gn bwd dx C{C} G{groups}")
+    close(dg, gamma.grad, 1e-2, 2e-3, f"gn bwd dgamma C{C} G{groups}")
+    close(db, beta.grad, 1e-2, 2e-3, f"gn bwd dbeta C{C} G{groups}")
     # the column sum is taken from the unrounded fp32 values (it feeds a bias gradient)
     close(cs, (xr.grad + dres.float()).sum(dim=(0, 1)), 2e-3, 2e-3, "gn bwd colsum")
 
@@ -117,24 +130,35 @@ def test_ln_film_backward(ops, B, T, C):
     close(cs, xr.grad.sum(dim=(0, 1)), 2e-3, 2e-3, "ln_film bwd colsum")
 
 
-def test_colsum_and_skip_gate(ops):
-    B, T, C, groups = 2, 700, 64, 8
+def _colsum_and_skip_gate(ops, C, groups):
+    B, T = 2, 700
     y, skip, dout = bf(rnd(B, T, C, seed=13)), bf(rnd(B, T, C, seed=14)), bf(rnd(B, T, C, seed=15))
-    gate = rnd(B, 72, seed=16)[:, :C]          # strided view, like a slice of ss_all
+    gate = rnd(B, C + 8, seed=16)[:, :C]       # strided view, like a slice of ss_all
     out = torch.empty_like(y)
     stats = torch.zeros(B, groups, 2, dtype=torch.float64, device=DEV)
     ops.skip_gate(y, skip, gate, out, stats, groups)
     ref = skip.float() + gate[:, None, :] * y.float()
     close(out, ref, 2 ** -7, 1e-3, "skip_gate out")
-    close(stats, stats_of(out, groups), 1e-4, 1e-6, "skip_gate stats")
+    close(stats, stats_of(out, groups), 1e-4, 1e-6, f"skip_gate stats C{C} G{groups}")
     dys = torch.empty_like(y)
-    dgate = torch.zeros(B, 72, device=DEV)
+    dgate = torch.zeros(B, C + 8, device=DEV)
     ops.skip_gate_bwd(dout, y, gate, dys, dgate[:, :C])
     close(dys, gate[:, None, :] * dout.float(), 2 ** -7, 1e-3, "skip_gate_bwd dys")
     close(dgate[:, :C], (dout.float() * y.float()).sum(1), 1e-3, 1e-3, "skip_gate_bwd dgate")
     cs = torch.zeros(C, device=DEV)
     ops.colsum(dout, cs, gate)
     close(cs, (dout.float() * gate[:, None, :]).sum(dim=(0, 1)), 1e-3, 1e-3, "colsum gated")
+
+
+def test_colsum_and_skip_gate(ops):
+    _colsum_and_skip_gate(ops, 64, 8)
+
+
+# the skip_gate statistics sum each group's per-channel sums: other group counts, also at C = 1024
+@pytest.mark.parametrize("C,groups", [(64, 1), (64, 4), (64, 16), (64, 64), (1024, 8), (1024, 1), (1024, 4),
+                                      (1024, 16), (1024, 64)])
+def test_colsum_and_skip_gate_groups(ops, C, groups):
+    _colsum_and_skip_gate(ops, C, groups)
 
 
 @pytest.mark.parametrize("B,want_dcond", [(4, True), (8, True), (19, True), (4, False), (32, False),
@@ -155,8 +179,8 @@ def test_cond_bwd(ops, B, want_dcond):
         close(dcond, dss @ w.float(), 1e-3, 1e-4, "cond_bwd dcond")
 
 
-def test_narrow_conv_backward(ops):
-    B, T, C, groups = 2, 3000, 8, 8
+def _narrow_conv_backward(ops, groups):
+    B, T, C = 2, 3000, 8
     x = bf(rnd(B, T, C, seed=20) * 1.3 + 0.2)
     dy = bf(rnd(B, T, C, seed=21))
     gamma = (rnd(C, seed=22) * 0.2 + 1.0).requires_grad_()
@@ -175,11 +199,21 @@ def test_narrow_conv_backward(ops):
     ops.narrow_conv_bwd(dy, x, stats, gamma.detach(), beta.detach(), w.detach(), dxh, dg, db, S, dw,
                         dbias, groups)
     ops.gn_bwd_apply(dxh, x, stats, S, dx, groups)
-    close(dx, xr.grad, 2 ** -6, 3e-3, "narrow bwd dx")
+    close(dx, xr.grad, 2 ** -6, 3e-3, f"narrow bwd dx G{groups}")
     close(dw, w.grad, 1e-2, 2e-3, "narrow bwd dw")
     close(dbias, bias.grad, 1e-3, 1e-3, "narrow bwd dbias")
-    close(dg, gamma.grad, 1e-2, 2e-3, "narrow bwd dgamma")
-    close(db, beta.grad, 1e-2, 2e-3, "narrow bwd dbeta")
+    close(dg, gamma.grad, 1e-2, 2e-3, f"narrow bwd dgamma G{groups}")
+    close(db, beta.grad, 1e-2, 2e-3, f"narrow bwd dbeta G{groups}")
+
+
+def test_narrow_conv_backward(ops):
+    _narrow_conv_backward(ops, 8)
+
+
+# the C = 8 GroupNorm coefficients and the per-group S sums of narrow_conv_bwd at other group counts
+@pytest.mark.parametrize("groups", [1, 2, 4])
+def test_narrow_conv_backward_groups(ops, groups):
+    _narrow_conv_backward(ops, groups)
 
 
 @pytest.mark.parametrize("cx,ca,co,c0,f", [(2, 0, 2, 8, 1), (2, 2, 2, 8, 1), (1, 1, 1, 32, 4)])

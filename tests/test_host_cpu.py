@@ -81,6 +81,24 @@ def test_product_path_refuses_to_run_on_cpu():
         model.sample(torch.randn(1, 2, 64), num_steps=2)
 
 
+_GROUPS = [([16, 32, 64], 16, False), ([32, 64, 128], 32, False),
+           ([8, 32, 64], 1, True), ([8, 32, 64], 2, True), ([8, 32, 64], 4, True), ([8, 32, 64], 8, True)]
+
+
+@pytest.mark.parametrize("channels,groups,ok", _GROUPS, ids=[f"c{c[0]}-g{g}" for c, g, _ in _GROUPS])
+def test_resnet_groups_beyond_the_fused_statistics_are_refused(channels, groups, ok):
+    """The conv GEMM sums GroupNorm statistics for at most 8 groups: the constructor refuses more
+    instead of failing inside the first forward."""
+    import audio_diffusion_pytorch_b200 as adp
+    kw = dict(dim=1, in_channels=2, channels=channels, factors=[1, 4, 4], items=[1, 1, 1],
+              resnet_groups=groups)
+    if ok:
+        assert adp.UNetV0(**kw).groups == groups
+    else:
+        with pytest.raises(AssertionError, match="at most 8 groups"):
+            adp.UNetV0(**kw)
+
+
 def test_resampler_matches_the_oracle(oracle_port):
     """utils.resample (cached polyphase bank) == the oracle's windowed-sinc resampler, which
     make_golden.py proved bit-identical to the reference's."""

@@ -43,6 +43,12 @@ def ops():
     return ops
 
 
+def group_ids(cases):
+    """pytest ids of cases whose last entry is the GroupNorm group count; 8 groups (the default
+    of UNetV0) is left out of the id."""
+    return ["-".join(str(v) for v in c[:-1]) + ("" if c[-1] == 8 else f"-g{c[-1]}") for c in cases]
+
+
 def stats_of(y, groups):
     """(sum, sumsq) per (batch, group) of a channels-last tensor."""
     B, T, Cc = y.shape
@@ -193,28 +199,52 @@ def test_conv_gemm_upsample(ops, B, T, ci, co, f):
 
 
 # -------------------------------------------------------------------------- row-wise
-@pytest.mark.parametrize("B,T,C", [(2, 1000, 8), (2, 512, 32), (2, 300, 64), (1, 256, 512),
-                                   (2, 128, 1024), (2, 100, 192)])
-def test_gn_silu_and_stats(ops, B, T, C):
+# gn_silu keeps the coefficients of a thread's 8 channels in registers when C/8 is a power of two
+# (one shared group for group sizes >= 8, a per-channel lookup below) and in smem otherwise
+# (C = 192); gn_stats bins every channel by c / group size.  The last two shapes sit on either
+# side of gn_silu's latency-bound `small` launch.
+_GN = [(2, 1000, 8, 8), (2, 512, 32, 8), (2, 300, 64, 8), (1, 256, 512, 8), (2, 128, 1024, 8),
+       (2, 100, 192, 8),
+       (2, 1000, 8, 1), (2, 1000, 8, 2), (2, 1000, 8, 4),
+       (2, 300, 64, 1), (2, 300, 64, 2), (2, 300, 64, 4), (2, 300, 64, 16), (2, 300, 64, 64),
+       (2, 200, 256, 1), (2, 200, 256, 4), (2, 200, 256, 16), (2, 200, 256, 64),
+       (2, 128, 1024, 1), (2, 128, 1024, 2), (2, 128, 1024, 16), (2, 128, 1024, 64),
+       (2, 100, 192, 1), (2, 100, 192, 4), (2, 100, 192, 24), (2, 16384, 192, 4),
+       (2, 2048, 512, 2), (2, 8192, 512, 2)]
+
+
+@pytest.mark.parametrize("B,T,C,groups", _GN, ids=group_ids(_GN))
+def test_gn_silu_and_stats(ops, B, T, C, groups):
     x = bf(rnd(B, T, C, seed=16) * 1.5 + 0.3)
     gamma, beta = rnd(C, seed=17) * 0.2 + 1.0, rnd(C, seed=18) * 0.2
-    groups = 8
     stats = torch.zeros(B, groups, 2, dtype=torch.float64, device=DEV)
     ops.gn_stats(x, stats, groups)
-    assert_close(stats, stats_of(x, groups), 1e-4, 1e-2, f"gn_stats C{C}")
+    assert_close(stats, stats_of(x, groups), 1e-4, 1e-2, f"gn_stats C{C} G{groups}")
     y = torch.empty_like(x)
     ops.gn_silu(x, y, stats, gamma, beta, groups, 1e-5)
     ref = F.silu(F.group_norm(x.float().transpose(1, 2), groups, gamma, beta, 1e-5)).transpose(1, 2)
-    assert_close(y, ref, 2 ** -7, 1e-2, f"gn_silu C{C}")
+    assert_close(y, ref, 2 ** -7, 1e-2, f"gn_silu C{C} G{groups}")
 
 
-@pytest.mark.parametrize("B,T,C,film", [(2, 1000, 8, True), (2, 512, 32, True), (2, 300, 64, True),
-                                        (1, 256, 512, True), (2, 128, 1024, True),
-                                        (2, 64, 768, False), (2, 100, 128, False)])
-def test_ln_film(ops, B, T, C, film):
+# ln_film's statistics: group sizes < 8 (C <= 256) bin per channel (PER_CH); wider groups fold
+# the lpg = size/8 lanes of a group with a shuffle tree over the lpr lanes of a row, which has
+# three regimes: lpg < lpr, lpg == lpr (C = 64 at 1 group, C = 1024 at 4) and lpg > lpr (C = 1024
+# at 1 or 2 groups: one group spans several vectors per lane).  C = 768 at 2 groups has
+# lpg = 48, not a multiple of lpr = 32, and takes the per-lane path.
+_LN = [(2, 1000, 8, True, 8), (2, 512, 32, True, 8), (2, 300, 64, True, 8), (1, 256, 512, True, 8),
+       (2, 128, 1024, True, 8), (2, 64, 768, False, 8), (2, 100, 128, False, 8),
+       (2, 1000, 8, True, 2), (2, 1000, 16, True, 8), (2, 1000, 16, True, 1), (2, 512, 32, True, 1),
+       (2, 300, 64, True, 1), (2, 300, 64, True, 2), (2, 300, 64, True, 16),
+       (2, 200, 256, True, 1), (2, 200, 256, True, 4), (2, 200, 256, True, 64),
+       (1, 256, 512, True, 1),
+       (2, 128, 1024, True, 1), (2, 128, 1024, True, 2), (2, 128, 1024, True, 4),
+       (2, 128, 1024, True, 16), (2, 128, 1024, True, 32), (2, 64, 768, False, 2)]
+
+
+@pytest.mark.parametrize("B,T,C,film,groups", _LN, ids=group_ids(_LN))
+def test_ln_film(ops, B, T, C, film, groups):
     x = bf(rnd(B, T, C, seed=19) * 2.0 + 0.5)
     ss = rnd(B, 2 * C, seed=20) * 0.3 if film else None
-    groups = 8
     stats = torch.zeros(B, groups, 2, dtype=torch.float64, device=DEV)
     y = torch.empty_like(x)
     ops.ln_film(x, y, ss, 2 * C if film else 0, stats, groups, 1e-6)
@@ -222,23 +252,28 @@ def test_ln_film(ops, B, T, C, film):
     if film:
         ref = ref * (1 + ss[:, None, :C]) + ss[:, None, C:]
     assert_close(y, ref, 2 ** -7, 1e-2, f"ln_film C{C}")
-    assert_close(stats, stats_of(y, groups), 1e-4, 1e-2, f"ln_film stats C{C}")
+    assert_close(stats, stats_of(y, groups), 1e-4, 1e-2, f"ln_film stats C{C} G{groups}")
 
 
-@pytest.mark.parametrize("B,T,C", [(2, 300, 1024), (2, 257, 512), (1, 1000, 64), (2, 128, 256)])
-def test_ln_film_dual(ops, B, T, C):
+_LN_DUAL = [(2, 300, 1024, 8), (2, 257, 512, 8), (1, 1000, 64, 8), (2, 128, 256, 8),
+            (2, 300, 1024, 1), (2, 300, 1024, 4), (2, 300, 1024, 32), (2, 257, 512, 2),
+            (1, 1000, 64, 1), (1, 1000, 64, 16), (2, 128, 256, 64), (2, 500, 16, 8), (2, 500, 16, 4)]
+
+
+@pytest.mark.parametrize("B,T,C,groups", _LN_DUAL, ids=group_ids(_LN_DUAL))
+def test_ln_film_dual(ops, B, T, C, groups):
     """Modulation + attention pre-norm in one pass: y2 must equal LayerNorm of the STORED y."""
     x = bf(rnd(B, T, C, seed=26) * 2.0 + 0.5)
     ss = rnd(B, 2 * C, seed=27) * 0.3
-    stats = torch.zeros(B, 8, 2, dtype=torch.float64, device=DEV)
+    stats = torch.zeros(B, groups, 2, dtype=torch.float64, device=DEV)
     y, y2 = torch.empty_like(x), torch.empty_like(x)
-    ops.ln_film(x, y, ss, 2 * C, stats, 8, 1e-6, y2=y2, eps2=1e-5)
+    ops.ln_film(x, y, ss, 2 * C, stats, groups, 1e-6, y2=y2, eps2=1e-5)
     y_single = torch.empty_like(x)
-    ops.ln_film(x, y_single, ss, 2 * C, None, 8, 1e-6)
+    ops.ln_film(x, y_single, ss, 2 * C, None, groups, 1e-6)
     assert torch.equal(y, y_single), "dual pass changed the first output"
     ref2 = F.layer_norm(y.float(), (C,), eps=1e-5)
     assert_close(y2, ref2, 2 ** -7, 1e-2, f"ln_film_dual y2 C{C}")
-    assert_close(stats, stats_of(y, 8), 1e-4, 1e-2, f"ln_film_dual stats C{C}")
+    assert_close(stats, stats_of(y, groups), 1e-4, 1e-2, f"ln_film_dual stats C{C} G{groups}")
 
 
 @pytest.mark.parametrize("B,K,N,in_act,out_act", [(8, 1024, 1024, 0, 1), (3, 264, 1024, 0, 1),
@@ -275,9 +310,16 @@ def test_sampler_step(ops):
 
 
 # ----------------------------------------------------------------------------- stems
-@pytest.mark.parametrize("cx,ca,c0,f,noised", [(2, 0, 8, 1, False), (2, 2, 8, 1, True),
-                                               (1, 1, 32, 4, False), (2, 0, 64, 2, True)])
-def test_stem_in(ops, cx, ca, c0, f, noised):
+# c0 = 8 with groups dividing 8 bins per-channel register sums by channel / (8 / groups) at the
+# end (block_stats8); other widths accumulate per group as the channels stream by (GroupStatAcc)
+_STEM_IN = [(2, 0, 8, 1, False, 8), (2, 2, 8, 1, True, 8), (1, 1, 32, 4, False, 8), (2, 0, 64, 2, True, 8),
+            (2, 0, 8, 1, False, 1), (2, 2, 8, 1, True, 2), (2, 0, 8, 1, False, 4),
+            (1, 1, 32, 4, False, 1), (1, 1, 32, 4, False, 4), (1, 1, 32, 4, False, 16),
+            (2, 0, 64, 2, True, 1), (2, 0, 64, 2, True, 4), (2, 0, 64, 2, True, 16)]
+
+
+@pytest.mark.parametrize("cx,ca,c0,f,noised,groups", _STEM_IN, ids=group_ids(_STEM_IN))
+def test_stem_in(ops, cx, ca, c0, f, noised, groups):
     B, T = 2, 1000 * f
     x = rnd(B, cx, T, seed=27)
     app = rnd(B, ca, T, seed=28) if ca else None
@@ -286,7 +328,6 @@ def test_stem_in(ops, cx, ca, c0, f, noised):
     beta = torch.rand(B, device=DEV) if noised else None
     w = rnd(c0, cx + ca, f, scale=((cx + ca) * f) ** -0.5, seed=30)
     bias = rnd(c0, seed=31)
-    groups = 8
     stats = torch.zeros(B, groups, 2, dtype=torch.float64, device=DEV)
     out = torch.empty(B, T // f, c0, dtype=torch.bfloat16, device=DEV)
     ops.stem_in(x, w, bias, out, f, append=app, noise=noise, alpha=alpha, beta=beta, stats=stats,
@@ -296,7 +337,7 @@ def test_stem_in(ops, cx, ca, c0, f, noised):
         xin = torch.cat([xin, app], dim=1)
     ref = F.conv1d(xin, w, bias, stride=f).transpose(1, 2)
     assert_close(out, ref, 2 ** -7, 1e-2, f"stem_in cx{cx} ca{ca} c0{c0} f{f}")
-    assert_close(stats, stats_of(out, groups), 1e-4, 1e-2, "stem_in stats")
+    assert_close(stats, stats_of(out, groups), 1e-4, 1e-2, f"stem_in stats c0{c0} G{groups}")
 
 
 @pytest.mark.parametrize("cx,ca,co,c0,f,mode", [(2, 0, 2, 8, 1, "v"), (2, 0, 2, 8, 1, "sample"),
@@ -358,10 +399,16 @@ def test_stem_out(ops, cx, ca, co, c0, f, mode):
         assert_close(dv, 2 * (ref_v - vt[:, :co]) / ref_v.numel(), 1e-3, 1e-8, "dv")
 
 
-@pytest.mark.parametrize("C", [8, 32, 64])
-@pytest.mark.parametrize("film,res", [(False, False), (True, True), (False, True)])
-def test_narrow_conv(ops, film, res, C):
-    B, T, groups = 2, 3000, 8
+# the GroupNorm coefficients of the input (per channel, from its group) and the statistics of the
+# output (C = 8: per channel then binned; C = 32 / 64: per half-vector of 4 channels)
+_NARROW = [(f, r, C, 8) for f, r in [(False, False), (True, True), (False, True)] for C in (8, 32, 64)] + \
+    [(True, True, 8, G) for G in (1, 2, 4)] + [(True, True, 32, G) for G in (1, 2, 4)] + \
+    [(True, True, 64, G) for G in (1, 2, 4, 16)]
+
+
+@pytest.mark.parametrize("film,res,C,groups", _NARROW, ids=group_ids(_NARROW))
+def test_narrow_conv(ops, film, res, C, groups):
+    B, T = 2, 3000
     x = bf(rnd(B, T, C, seed=41) * 1.3 + 0.2)
     stats_in = stats_of(x, groups).contiguous()
     gamma, beta = rnd(C, seed=42) * 0.2 + 1.0, rnd(C, seed=43) * 0.2
@@ -386,8 +433,8 @@ def test_narrow_conv(ops, film, res, C):
         ref = F.layer_norm(ref, (C,), eps=1e-6) * (1 + ss[:, None, :C]) + ss[:, None, C:]
     # activations AND weights enter the tensor core as bf16 (like every wider level), and the
     # LayerNorm of the film variant rescales the error by 1/std of an 8-channel row
-    assert_close(y, ref, 2 ** -7, 3e-2 if film else 1e-2, f"narrow_conv film={film}")
-    assert_close(stats_out, stats_of(y, groups), 1e-4, 1e-2, "narrow_conv stats")
+    assert_close(y, ref, 2 ** -7, 3e-2 if film else 1e-2, f"narrow_conv C{C} G{groups} film={film}")
+    assert_close(stats_out, stats_of(y, groups), 1e-4, 1e-2, f"narrow_conv stats C{C} G{groups}")
 
 
 # -------------------------------------------------------------------------- attention
@@ -416,24 +463,32 @@ def test_attention(ops, B, H, Tq, Tk):
     assert_close(o, ref, 2 ** -6, 2e-2, f"attention B{B} H{H} Tq{Tq} Tk{Tk}")
 
 
-@pytest.mark.parametrize("B,T,C,co", [(2, 512, 64, 64), (2, 300, 128, 128), (1, 256, 32, 32),
-                                      (2, 100, 256, 256), (1, 128, 16, 16), (2, 1000, 1024, 128),
-                                      (8, 2048, 64, 64)])
-def test_conv_gemm_fused_groupnorm_silu(ops, B, T, C, co):
+# (B, T, C, co, GroupNorm groups of the input, statistics groups of the output): the A-tile
+# transform reads its own group count, independent of the epilogue's
+_FUSED_GN = [(2, 512, 64, 64, 8, 8), (2, 300, 128, 128, 8, 8), (1, 256, 32, 32, 8, 8),
+             (2, 100, 256, 256, 8, 8), (1, 128, 16, 16, 8, 8), (2, 1000, 1024, 128, 8, 8),
+             (8, 2048, 64, 64, 8, 8),
+             (2, 512, 64, 64, 1, 4), (2, 300, 128, 128, 4, 1), (1, 128, 16, 16, 4, 2),
+             (2, 100, 256, 256, 1, 8), (2, 1000, 1024, 128, 4, 2)]
+
+
+@pytest.mark.parametrize("B,T,C,co,gn_groups,groups", _FUSED_GN,
+                         ids=["-".join(str(v) for v in c[:4]) + ("" if c[4:] == (8, 8) else f"-gn{c[4]}-g{c[5]}")
+                              for c in _FUSED_GN])
+def test_conv_gemm_fused_groupnorm_silu(ops, B, T, C, co, gn_groups, groups):
     """ConvBlock in one kernel: conv3(SiLU(GroupNorm(x))) with the normalisation applied to the
     smem A tile by the transform warps (zero padding must stay zero after the activation)."""
-    groups = 8
     x = bf(rnd(B, T, C, seed=60) * 1.5 + 0.3)
     gamma, beta = rnd(C, seed=61) * 0.2 + 1.0, rnd(C, seed=62) * 0.2
     w = bf(rnd(co, C, 3, scale=(3 * C) ** -0.5, seed=63))
     bias = rnd(co, seed=64)
     res = bf(rnd(B, T, co, seed=65))
-    stats_x = stats_of(x, groups).contiguous()
+    stats_x = stats_of(x, gn_groups).contiguous()
     stats = torch.zeros(B, groups, 2, dtype=torch.float64, device=DEV)
     out = torch.empty(B, T, co, dtype=torch.bfloat16, device=DEV)
     ops.conv_gemm(x, ops.pack_conv(w), out, c_in=C, n_valid=co, taps=(-1, 0, 1), bias=bias,
-                  residual=res, stats=stats, groups=groups, gn=(stats_x, gamma, beta, groups, 1e-5))
-    a = bf(F.silu(F.group_norm(x.float().transpose(1, 2), groups, gamma, beta, 1e-5))).float()
+                  residual=res, stats=stats, groups=groups, gn=(stats_x, gamma, beta, gn_groups, 1e-5))
+    a = bf(F.silu(F.group_norm(x.float().transpose(1, 2), gn_groups, gamma, beta, 1e-5))).float()
     ref = F.conv1d(a, w.float(), bias, padding=1).transpose(1, 2) + res.float()
-    assert_close(out, ref, 2 ** -6, 3e-2, f"fused gn+silu conv3 C{C}")
-    assert_close(stats, stats_of(out, groups), 1e-4, 1e-2, "fused gn stats")
+    assert_close(out, ref, 2 ** -6, 3e-2, f"fused gn+silu conv3 C{C} gn_groups {gn_groups}")
+    assert_close(stats, stats_of(out, groups), 1e-4, 1e-2, f"fused gn stats co{co} G{groups}")

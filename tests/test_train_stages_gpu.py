@@ -210,14 +210,19 @@ def stats_of(y, groups):
     return torch.stack([yg.sum(dim=(1, 3)), (yg * yg).sum(dim=(1, 3))], dim=-1).contiguous()
 
 
+_ITEM = [(2, 512, 64, 8), (2, 256, 512, 8), (2, 5, 64, 8), (3, 203, 512, 8),
+         (2, 512, 64, 1), (2, 512, 64, 4), (3, 203, 512, 1), (3, 203, 512, 4)]
+
+
 @pytest.mark.parametrize("mod", [False, True])
-@pytest.mark.parametrize("B,T,C", [(2, 512, 64), (2, 256, 512), (2, 5, 64), (3, 203, 512)])
-def test_resnet_item_stage(tr, ops, B, T, C, mod):
+@pytest.mark.parametrize("B,T,C,G", _ITEM,
+                         ids=["-".join(str(v) for v in c[:3]) + ("" if c[3] == 8 else f"-g{c[3]}") for c in _ITEM])
+def test_resnet_item_stage(tr, ops, B, T, C, G, mod):
     """training.resnet_item_bwd (the C >= 32 item path) against autograd of
     GroupNorm -> SiLU -> conv3 -> GroupNorm -> SiLU -> conv3 + x (-> LayerNorm (1 + scale) + shift).
     The saved activations (a1, h, a2, rr) are the bf16-rounded values of that fp32 forward, as
     the training forward stores them."""
-    G, gn_eps, ln_eps = 8, 1e-5, 1e-6
+    gn_eps, ln_eps = 1e-5, 1e-6
     x = bf(rnd(B, T, C, seed=17) * 1.5 + 0.3)
     w1 = bf(rnd(C, C, 3, scale=(3 * C) ** -0.5, seed=18)).float()
     w2 = bf(rnd(C, C, 3, scale=(3 * C) ** -0.5, seed=19)).float()
@@ -256,7 +261,7 @@ def test_resnet_item_stage(tr, ops, B, T, C, mod):
     dx = tr.resnet_item_bwd(dy, x, h, rr, a1, a2, stats_of(x, G), stats_of(h, G), (g1, be1), (g2, be2),
                             ops.pack_conv_dgrad(w1), ops.pack_conv_dgrad(w2), gw1, gw2, dgn1, dgn2, db1, db2,
                             S1, S2, work, G, film=film)
-    ck = Checks(f"item B{B} T{T} C{C} mod{int(mod)}")
+    ck = Checks(f"item B{B} T{T} C{C} G{G} mod{int(mod)}")
     ck.act(dx, xr.grad, "dx")
     ck.acc(gw1.permute(1, 2, 0), w1r.grad, "dw1")
     ck.acc(gw2.permute(1, 2, 0), w2r.grad, "dw2")
