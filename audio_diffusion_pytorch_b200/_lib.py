@@ -100,7 +100,9 @@ def lib() -> C.CDLL:
         "adp_ln_film": [vp, vp, vp, i32, vp, i32, i32, i32, i32, f32, vp],
         "adp_ln_film_dual": [vp, vp, vp, vp, i32, vp, i32, i32, i32, i32, f32, f32, vp],
         "adp_attention": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, f32, vp, vp],
+        "adp_attention_hd": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, f32, vp, vp],
         "adp_attention_bwd": [C.POINTER(AttentionBwdArgs), vp],
+        "adp_attention_bwd_hd": [C.POINTER(AttentionBwdArgs), i32, vp],
         "adp_ln_fold_bwd": [vp, vp, vp, vp, i32, vp, vp, vp, vp, i32, i32, vp],
         "adp_skinny_linear": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp],
         "adp_time_features": [vp, vp, vp, i32, i32, i32, vp],
@@ -120,6 +122,7 @@ def lib() -> C.CDLL:
         "adp_f32_gn_silu": [vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp],
         "adp_f32_ln_film": [vp, vp, vp, vp, i32, i32, i32, i32, f32, f32, vp],
         "adp_f32_attention": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, f32, vp],
+        "adp_f32_attention_hd": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, f32, vp],
         "adp_f32_linear": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp],
         "adp_f32_silu": [vp, vp, C.c_int64, vp],
         "adp_f32_stem_in": [C.POINTER(StemInArgs), vp],
@@ -162,4 +165,5 @@ EXPORTS = ["adp_version", "adp_last_error", "adp_device_check", "adp_conv_gemm",
            "adp_stem_in_bwd", "adp_attention_bwd", "adp_ln_fold_bwd", "adp_inpaint_blend", "adp_arv_step", "adp_resample", "adp_resample_adjoint",
            "adp_mel_spectrogram", "adp_to_flat", "adp_to_flat_bwd", "adp_f32_conv_gemm", "adp_f32_gn_stats",
            "adp_f32_gn_silu", "adp_f32_ln_film", "adp_f32_attention", "adp_f32_linear", "adp_f32_silu",
-           "adp_f32_stem_in", "adp_f32_stem_out", "adp_step_select", "adp_step_advance"]
+           "adp_f32_stem_in", "adp_f32_stem_out", "adp_step_select", "adp_step_advance",
+           "adp_attention_hd", "adp_attention_bwd_hd", "adp_f32_attention_hd"]

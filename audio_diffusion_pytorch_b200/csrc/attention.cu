@@ -1,4 +1,5 @@
-// adp_attention: softmax(q k^T * scale) v, head dim 64, on wgmma (a_unet AttentionBase).
+// adp_attention: softmax(q k^T * scale) v, head dim D in {32, 64, 128}, on wgmma (a_unet
+// AttentionBase).
 //
 // One CTA = one (batch, head, 128-query tile).  Two consumer warpgroups own 64 query rows each:
 // S = Q K_j^T (64 x 128 keys) accumulates in registers, the online softmax runs on the
@@ -9,6 +10,12 @@
 //   warp 8   : TMA producer  Q once; K and V double-buffered
 // K is the K-major B operand of the first GEMM (keys x d); V is used in place as the
 // MN-major B operand of the second (d contiguous per key), so no transpose is materialised.
+//
+// Head dims: a tile row is split into swizzle-wide column chunks, each its own TMA box and
+// stored [128 rows][kSW bytes] one after the other.  D = 64 is one 128-byte chunk; D = 128 is
+// two (the QK^T loop steps the K-major descriptors into the second chunk after four k-steps,
+// and the MN-major V descriptor reaches it through LBO); D = 32 is one 64-byte chunk with
+// 64-byte swizzle.
 #include "common.cuh"
 #include "ptx.cuh"
 
@@ -16,11 +23,16 @@ namespace adp {
 
 constexpr int kQT = 128;       // query rows per CTA
 constexpr int kKT = 128;       // keys per tile
-constexpr int kD = 64;         // head dim
-constexpr int kQBytes = kQT * kD * 2;          // 16 KB
-constexpr int kKVBytes = kKT * kD * 2;         // 16 KB
-constexpr int kAttnSmem = kQBytes + 4 * kKVBytes + 1024;   // Q + 2 x (K, V): 81 KB
 constexpr int kAttnThreads = 288;
+
+template <int D>
+struct AttnShape {
+  static constexpr int kSW = D * 2 < 128 ? D * 2 : 128;   // swizzle / chunk width (bytes)
+  static constexpr int kChunks = D * 2 / kSW;               // column chunks per row
+  static constexpr int kQBytes = kQT * D * 2;               // 16 KB at D = 64
+  static constexpr int kKVBytes = kKT * D * 2;              // 16 KB at D = 64
+  static constexpr int kSmem = kQBytes + 4 * kKVBytes + 1024;   // Q + 2 x (K, V): 81 KB at D = 64
+};
 
 struct AttnParams {
   __nv_bfloat16* o;
@@ -35,9 +47,26 @@ __device__ __forceinline__ float ex2_approx(float x) {
   return y;
 }
 
+// descriptor offset (16-byte units) of k-step kk (16 columns) in a chunked K-major tile of
+// `rows` rows: chunk kk / (kSW / 32), then 32 bytes per k-step inside the chunk
+template <int SW>
+__device__ __forceinline__ uint32_t kstep_off(int kk, int rows) {
+  constexpr int kPerChunk = SW / 32;
+  return static_cast<uint32_t>((kk / kPerChunk) * rows * SW + (kk % kPerChunk) * 32) >> 4;
+}
+
+template <int D>
+__device__ __forceinline__ uint64_t v_desc_mnmajor(uint32_t addr) {
+  if constexpr (D == 32) return gmma_desc_mnmajor_sw64(addr, kKT * 64);
+  else return gmma_desc_mnmajor_sw128(addr, D == 64 ? 1024 : kKT * 128);
+}
+
+template <int D>
 __global__ void __launch_bounds__(kAttnThreads, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                  const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
+  using S = AttnShape<D>;
+  constexpr int kSW = S::kSW, kQBytes = S::kQBytes, kKVBytes = S::kKVBytes;
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t q_full, kv_full[2], kv_empty[2];
 
@@ -47,8 +76,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   const uint32_t raw = smem_u32(smem_raw);
   uint8_t* base = smem_raw + ((1024u - (raw & 1023u)) & 1023u);
   uint8_t* q_s = base;
-  uint8_t* k_s = q_s + kQBytes;            // [2][16 KB]
-  uint8_t* v_s = k_s + 2 * kKVBytes;       // [2][16 KB]
+  uint8_t* k_s = q_s + kQBytes;            // [2][kKVBytes]
+  uint8_t* v_s = k_s + 2 * kKVBytes;       // [2][kKVBytes]
 
   const int t0 = blockIdx.x * kQT;
   const int h = blockIdx.y;
@@ -70,7 +99,9 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     // whole warp runs the loop (uniform control flow), one elected lane issues: see ptx.cuh
     if (elect_one()) {
       mbar_arrive_expect_tx(&q_full, kQBytes);
-      tma_load_3d(q_s, &tmQ, &q_full, h * kD, t0, b);
+#pragma unroll
+      for (int c = 0; c < S::kChunks; ++c)
+        tma_load_3d(q_s + c * kQT * kSW, &tmQ, &q_full, h * D + c * (kSW / 2), t0, b);
     }
     __syncwarp();
     for (int j = 0; j < n_tiles; ++j) {
@@ -78,8 +109,11 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       mbar_wait(&kv_empty[s], ((j >> 1) & 1) ^ 1);
       if (elect_one()) {
         mbar_arrive_expect_tx(&kv_full[s], 2 * kKVBytes);
-        tma_load_3d(k_s + s * kKVBytes, &tmK, &kv_full[s], h * kD, j * kKT, b);
-        tma_load_3d(v_s + s * kKVBytes, &tmV, &kv_full[s], h * kD, j * kKT, b);
+#pragma unroll
+        for (int c = 0; c < S::kChunks; ++c) {
+          tma_load_3d(k_s + s * kKVBytes + c * kKT * kSW, &tmK, &kv_full[s], h * D + c * (kSW / 2), j * kKT, b);
+          tma_load_3d(v_s + s * kKVBytes + c * kKT * kSW, &tmV, &kv_full[s], h * D + c * (kSW / 2), j * kKT, b);
+        }
       }
       __syncwarp();
     }
@@ -90,21 +124,21 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   const int wg = threadIdx.x >> 7;
   const int row_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // fragment rows row_lo, row_lo + 8
   const int cq = 2 * (lane & 3);
-  const uint64_t q_desc = gmma_desc_kmajor<128>(smem_u32(q_s) + wg * 64 * 128);
+  const uint64_t q_desc = gmma_desc_kmajor<kSW>(smem_u32(q_s) + wg * 64 * kSW);
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
-  float o[kD / 2];
+  float o[D / 2];
 #pragma unroll
-  for (int i = 0; i < kD / 2; ++i) o[i] = 0.f;
+  for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
   mbar_wait(&q_full, 0);
   for (int j = 0; j < n_tiles; ++j) {
     const int s = j & 1;
     mbar_wait(&kv_full[s], (j >> 1) & 1);
     float sc[kKT / 2];
-    const uint64_t k_desc = gmma_desc_kmajor<128>(smem_u32(k_s + s * kKVBytes));
+    const uint64_t k_desc = gmma_desc_kmajor<kSW>(smem_u32(k_s + s * kKVBytes));
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < kD / 16; ++kk)
-      Wgmma<kKT>::ss<0, 0>(sc, q_desc + ((kk * 32) >> 4), k_desc + ((kk * 32) >> 4), kk != 0);
+    for (int kk = 0; kk < D / 16; ++kk)
+      Wgmma<kKT>::ss<0, 0>(sc, q_desc + kstep_off<kSW>(kk, kQT), k_desc + kstep_off<kSW>(kk, kKT), kk != 0);
     wgmma_commit();
     wgmma_wait<0>();
     acc_fence(sc);
@@ -130,7 +164,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     }
     if (j > 0) {
 #pragma unroll
-      for (int i = 0; i < kD / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
+      for (int i = 0; i < D / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
     }
     // p = 2^(s*c - m*c) -> bf16 A fragments of P V (16 keys per fragment)
     uint32_t pa[kKT / 16][4];
@@ -151,11 +185,11 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     l_run[0] = l_run[0] * alpha[0] + l_tile[0];
     l_run[1] = l_run[1] * alpha[1] + l_tile[1];
 
-    const uint64_t v_desc = gmma_desc_mnmajor_sw128(smem_u32(v_s + s * kKVBytes), 1024);
+    const uint64_t v_desc = v_desc_mnmajor<D>(smem_u32(v_s + s * kKVBytes));
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < kKT / 16; ++kk)
-      Wgmma<kD>::rs<1>(o, pa[kk], v_desc + ((kk * 16 * 128) >> 4), 1);
+      Wgmma<D>::template rs<1>(o, pa[kk], v_desc + ((kk * 16 * kSW) >> 4), 1);
     wgmma_commit();
     wgmma_wait<0>();
     acc_fence(o);
@@ -176,9 +210,9 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     if (p.lse != nullptr && (lane & 3) == 0)    // natural-log units (adp_attention_bwd)
       p.lse[(static_cast<size_t>(b) * gridDim.y + h) * p.Tq + t] =
           (m_run[r] * p.scale_log2 + log2f(l_run[r])) * 0.6931471805599453f;
-    __nv_bfloat16* orow = p.o + (static_cast<size_t>(b) * p.Tq + t) * p.ldo + h * kD;
+    __nv_bfloat16* orow = p.o + (static_cast<size_t>(b) * p.Tq + t) * p.ldo + h * D;
 #pragma unroll
-    for (int jb = 0; jb < kD / 8; ++jb)
+    for (int jb = 0; jb < D / 8; ++jb)
       *reinterpret_cast<uint32_t*>(orow + 8 * jb + cq) =
           pack_bf16(o[4 * jb + 2 * r] * inv_l, o[4 * jb + 2 * r + 1] * inv_l);
   }
@@ -188,35 +222,32 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
 
 using namespace adp;
 
-extern "C" int adp_attention(const void* q, const void* k, const void* v, void* o, int32_t B,
-                             int32_t H, int32_t Tq, int32_t Tk, int32_t ldq, int32_t ldk,
-                             int32_t ldv, int32_t ldo, float scale, float* lse,
-                             adp_stream_t stream) {
-  ADP_CHECK(q && k && v && o, "adp_attention: null pointer");
-  ADP_CHECK(B > 0 && H > 0 && Tq > 0 && Tk > 0, "adp_attention: bad sizes");
-  ADP_CHECK(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0 && ldq >= H * kD &&
-                ldk >= H * kD && ldv >= H * kD && ldo >= H * kD,
-            "adp_attention: row pitches must be multiples of 8 and >= heads*64");
-  ADP_CHECK(scale > 0.f, "adp_attention: scale must be positive");
+namespace {
+
+template <int D>
+int attention_launch(const void* q, const void* k, const void* v, void* o, int32_t B, int32_t H,
+                     int32_t Tq, int32_t Tk, int32_t ldq, int32_t ldk, int32_t ldv, int32_t ldo,
+                     float scale, float* lse, adp_stream_t stream) {
+  using S = AttnShape<D>;
   CUtensorMap tmQ, tmK, tmV;
-  const uint32_t box[3] = {(uint32_t)kD, (uint32_t)kQT, 1};
+  const uint32_t box[3] = {(uint32_t)(S::kSW / 2), (uint32_t)kQT, 1};
   {
-    const uint64_t dims[3] = {(uint64_t)H * kD, (uint64_t)Tq, (uint64_t)B};
+    const uint64_t dims[3] = {(uint64_t)H * D, (uint64_t)Tq, (uint64_t)B};
     const uint64_t str[2] = {(uint64_t)ldq * 2, (uint64_t)Tq * ldq * 2};
-    if (int e = make_tmap_bf16(&tmQ, q, 3, dims, str, box, 128)) return e;
+    if (int e = make_tmap_bf16(&tmQ, q, 3, dims, str, box, S::kSW)) return e;
   }
   {
-    const uint64_t dims[3] = {(uint64_t)H * kD, (uint64_t)Tk, (uint64_t)B};
+    const uint64_t dims[3] = {(uint64_t)H * D, (uint64_t)Tk, (uint64_t)B};
     const uint64_t str[2] = {(uint64_t)ldk * 2, (uint64_t)Tk * ldk * 2};
-    if (int e = make_tmap_bf16(&tmK, k, 3, dims, str, box, 128)) return e;
+    if (int e = make_tmap_bf16(&tmK, k, 3, dims, str, box, S::kSW)) return e;
   }
   {
-    const uint64_t dims[3] = {(uint64_t)H * kD, (uint64_t)Tk, (uint64_t)B};
+    const uint64_t dims[3] = {(uint64_t)H * D, (uint64_t)Tk, (uint64_t)B};
     const uint64_t str[2] = {(uint64_t)ldv * 2, (uint64_t)Tk * ldv * 2};
-    if (int e = make_tmap_bf16(&tmV, v, 3, dims, str, box, 128)) return e;
+    if (int e = make_tmap_bf16(&tmV, v, 3, dims, str, box, S::kSW)) return e;
   }
   static SmemAttrCache smem_cache;
-  ADP_CUDA(ensure_dyn_smem(attention_kernel, (size_t)kAttnSmem, smem_cache));
+  ADP_CUDA(ensure_dyn_smem(attention_kernel<D>, (size_t)S::kSmem, smem_cache));
   AttnParams p;
   p.o = static_cast<__nv_bfloat16*>(o);
   p.lse = lse;
@@ -225,7 +256,37 @@ extern "C" int adp_attention(const void* q, const void* k, const void* v, void* 
   p.ldo = ldo;
   p.scale_log2 = scale * 1.4426950408889634f;
   dim3 grid((Tq + kQT - 1) / kQT, H, B);
-  ADP_CUDA(launch_k(attention_kernel, grid, dim3(kAttnThreads), (size_t)kAttnSmem, as_stream(stream), tmQ, tmK, tmV, p));
+  ADP_CUDA(launch_k(attention_kernel<D>, grid, dim3(kAttnThreads), (size_t)S::kSmem, as_stream(stream), tmQ, tmK, tmV, p));
   ADP_LAUNCH_CHECK();
   return 0;
+}
+
+}  // namespace
+
+extern "C" int adp_attention_hd(const void* q, const void* k, const void* v, void* o, int32_t B,
+                                int32_t H, int32_t head_dim, int32_t Tq, int32_t Tk, int32_t ldq,
+                                int32_t ldk, int32_t ldv, int32_t ldo, float scale, float* lse,
+                                adp_stream_t stream) {
+  ADP_CHECK(head_dim == 32 || head_dim == 64 || head_dim == 128,
+            "adp_attention: head_dim %d not supported (32, 64 or 128)", head_dim);
+  ADP_CHECK(q && k && v && o, "adp_attention: null pointer");
+  ADP_CHECK(B > 0 && H > 0 && Tq > 0 && Tk > 0, "adp_attention: bad sizes");
+  const int64_t w = static_cast<int64_t>(H) * head_dim;
+  ADP_CHECK(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0 && ldq >= w &&
+                ldk >= w && ldv >= w && ldo >= w,
+            "adp_attention: row pitches must be multiples of 8 and >= heads*head_dim (%d*%d)", H,
+            head_dim);
+  ADP_CHECK(scale > 0.f, "adp_attention: scale must be positive");
+  if (head_dim == 32)
+    return attention_launch<32>(q, k, v, o, B, H, Tq, Tk, ldq, ldk, ldv, ldo, scale, lse, stream);
+  if (head_dim == 128)
+    return attention_launch<128>(q, k, v, o, B, H, Tq, Tk, ldq, ldk, ldv, ldo, scale, lse, stream);
+  return attention_launch<64>(q, k, v, o, B, H, Tq, Tk, ldq, ldk, ldv, ldo, scale, lse, stream);
+}
+
+extern "C" int adp_attention(const void* q, const void* k, const void* v, void* o, int32_t B,
+                             int32_t H, int32_t Tq, int32_t Tk, int32_t ldq, int32_t ldk,
+                             int32_t ldv, int32_t ldo, float scale, float* lse,
+                             adp_stream_t stream) {
+  return adp_attention_hd(q, k, v, o, B, H, 64, Tq, Tk, ldq, ldk, ldv, ldo, scale, lse, stream);
 }

@@ -146,11 +146,25 @@ f32_ln_film_kernel(const float* __restrict__ x, float* __restrict__ y, float* __
   }
 }
 
-// softmax(q k^T * scale) v, head dim 64; one thread per (b, head, query), online softmax
+// a load ptxas may not hoist out of a loop
+__device__ __forceinline__ float ld_nc_volatile(const float* p) {
+  float v;
+  asm volatile("ld.global.nc.f32 %0, [%1];" : "=f"(v) : "l"(p));
+  return v;
+}
+
+// softmax(q k^T * scale) v, head dim D; one thread per (b, head, query), online softmax.  For
+// D <= 64 the scaled query and the output accumulator live in registers.  At D = 128 both would
+// not fit: the thread makes one pass over the keys per 64-column half of the output, keeps only
+// that half's accumulator, and re-reads the (L1-resident) query for every key.  Both passes
+// compute the same scores and softmax statistics.
+template <int D>
 __global__ void __launch_bounds__(128)
 f32_attention_kernel(const float* __restrict__ q, const float* __restrict__ k, const float* __restrict__ v,
                      float* __restrict__ o, int B, int H, int Tq, int Tk, int ldq, int ldk, int ldv, int ldo,
                      float scale) {
+  constexpr bool kQInRegs = D <= 64;
+  constexpr int kDO = kQInRegs ? D : 64;   // output columns per pass
   pdl_launch_dependents();
   pdl_wait();
   const int64_t total = static_cast<int64_t>(B) * H * Tq;
@@ -159,28 +173,40 @@ f32_attention_kernel(const float* __restrict__ q, const float* __restrict__ k, c
     const int tq = static_cast<int>(i % Tq);
     const int h = static_cast<int>((i / Tq) % H);
     const int b = static_cast<int>(i / (static_cast<int64_t>(Tq) * H));
-    const float* qr = q + (static_cast<int64_t>(b) * Tq + tq) * ldq + h * 64;
-    float qv[64], acc[64];
+    const float* qr = q + (static_cast<int64_t>(b) * Tq + tq) * ldq + h * D;
+    float qv[kQInRegs ? D : 1];
+    if constexpr (kQInRegs) {
 #pragma unroll
-    for (int d = 0; d < 64; ++d) { qv[d] = qr[d] * scale; acc[d] = 0.f; }
-    float mx = -INFINITY, l = 0.f;
-    for (int j = 0; j < Tk; ++j) {
-      const float* kr = k + (static_cast<int64_t>(b) * Tk + j) * ldk + h * 64;
-      float s = 0.f;
-#pragma unroll
-      for (int d = 0; d < 64; ++d) s = fmaf(qv[d], kr[d], s);
-      const float mn = fmaxf(mx, s);
-      const float corr = expf(mx - mn), pj = expf(s - mn);
-      l = l * corr + pj;
-      const float* vr = v + (static_cast<int64_t>(b) * Tk + j) * ldv + h * 64;
-#pragma unroll
-      for (int d = 0; d < 64; ++d) acc[d] = acc[d] * corr + pj * vr[d];
-      mx = mn;
+      for (int d = 0; d < D; ++d) qv[d] = qr[d] * scale;
     }
-    float* orow = o + (static_cast<int64_t>(b) * Tq + tq) * ldo + h * 64;
-    const float inv = 1.f / l;
+    for (int c0 = 0; c0 < D; c0 += kDO) {
+      float acc[kDO];
 #pragma unroll
-    for (int d = 0; d < 64; ++d) orow[d] = acc[d] * inv;
+      for (int d = 0; d < kDO; ++d) acc[d] = 0.f;
+      float mx = -INFINITY, l = 0.f;
+      for (int j = 0; j < Tk; ++j) {
+        const float* kr = k + (static_cast<int64_t>(b) * Tk + j) * ldk + h * D;
+        float s = 0.f;
+        if constexpr (kQInRegs) {
+#pragma unroll
+          for (int d = 0; d < D; ++d) s = fmaf(qv[d], kr[d], s);
+        } else {
+#pragma unroll
+          for (int d = 0; d < D; ++d) s = fmaf(ld_nc_volatile(qr + d) * scale, kr[d], s);
+        }
+        const float mn = fmaxf(mx, s);
+        const float corr = expf(mx - mn), pj = expf(s - mn);
+        l = l * corr + pj;
+        const float* vr = v + (static_cast<int64_t>(b) * Tk + j) * ldv + h * D + c0;
+#pragma unroll
+        for (int d = 0; d < kDO; ++d) acc[d] = acc[d] * corr + pj * vr[d];
+        mx = mn;
+      }
+      float* orow = o + (static_cast<int64_t>(b) * Tq + tq) * ldo + h * D + c0;
+      const float inv = 1.f / l;
+#pragma unroll
+      for (int d = 0; d < kDO; ++d) orow[d] = acc[d] * inv;
+    }
   }
 }
 
@@ -355,16 +381,29 @@ extern "C" int adp_f32_ln_film(const float* x, float* y, float* y2, const float*
   return 0;
 }
 
-extern "C" int adp_f32_attention(const float* q, const float* k, const float* v, float* o, int B, int H, int Tq,
-                                 int Tk, int ldq, int ldk, int ldv, int ldo, float scale, adp_stream_t stream) {
+extern "C" int adp_f32_attention_hd(const float* q, const float* k, const float* v, float* o, int B, int H,
+                                    int head_dim, int Tq, int Tk, int ldq, int ldk, int ldv, int ldo, float scale,
+                                    adp_stream_t stream) {
+  ADP_CHECK(head_dim == 32 || head_dim == 64 || head_dim == 128,
+            "adp_f32_attention: head_dim %d not supported (32, 64 or 128)", head_dim);
   ADP_CHECK(q && k && v && o && B > 0 && H > 0 && Tq > 0 && Tk > 0, "adp_f32_attention: bad args");
+  const int64_t w = static_cast<int64_t>(H) * head_dim;
+  ADP_CHECK(ldq >= w && ldk >= w && ldv >= w && ldo >= w,
+            "adp_f32_attention: row pitches must be >= heads*head_dim (%d*%d)", H, head_dim);
   int64_t n = static_cast<int64_t>(B) * H * Tq;
   int64_t g = (n + 127) / 128;
   if (g > num_sms() * 16) g = num_sms() * 16;
-  ADP_CUDA(launch_k(f32_attention_kernel, dim3(static_cast<int>(g)), dim3(128), (size_t)0, as_stream(stream), q, k,
-                    v, o, B, H, Tq, Tk, ldq, ldk, ldv, ldo, scale));
+  auto kern = head_dim == 32 ? f32_attention_kernel<32>
+              : head_dim == 128 ? f32_attention_kernel<128> : f32_attention_kernel<64>;
+  ADP_CUDA(launch_k(kern, dim3(static_cast<int>(g)), dim3(128), (size_t)0, as_stream(stream), q, k, v, o, B, H,
+                    Tq, Tk, ldq, ldk, ldv, ldo, scale));
   ADP_LAUNCH_CHECK();
   return 0;
+}
+
+extern "C" int adp_f32_attention(const float* q, const float* k, const float* v, float* o, int B, int H, int Tq,
+                                 int Tk, int ldq, int ldk, int ldv, int ldo, float scale, adp_stream_t stream) {
+  return adp_f32_attention_hd(q, k, v, o, B, H, 64, Tq, Tk, ldq, ldk, ldv, ldo, scale, stream);
 }
 
 extern "C" int adp_f32_linear(const float* x, const float* w, const float* bias, float* y, int B, int K, int N,

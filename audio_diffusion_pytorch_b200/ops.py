@@ -251,26 +251,32 @@ def ln_film(x: Tensor, y: Tensor, scale_shift: Optional[Tensor] = None, ss_strid
     return y
 
 
+def _hd_tag(head_dim: int) -> str:
+    # trace labels name the head dim only when it is not the default 64
+    return "" if head_dim == 64 else f" D={head_dim}"
+
+
 def attention(q: Tensor, k: Tensor, v: Tensor, o: Tensor, heads: int, scale: float,
-              lse: Optional[Tensor] = None) -> Tensor:
-    """q: bf16 view [B, Tq, >=heads*64] (row pitch = stride(1)); k, v over Tk rows.
-    lse: optional fp32 [B, heads, Tq] output (kept for attention_bwd)."""
+              lse: Optional[Tensor] = None, head_dim: int = 64) -> Tensor:
+    """q: bf16 view [B, Tq, >=heads*head_dim] (row pitch = stride(1)); k, v over Tk rows.
+    head_dim: 32, 64 or 128.  lse: optional fp32 [B, heads, Tq] output (kept for attention_bwd)."""
     B, Tq = q.shape[0], q.shape[1]
     Tk = k.shape[1]
+    D, tag = head_dim, _hd_tag(head_dim)
     if q.dtype == torch.float32:
         assert lse is None, "the fp32 verification mode covers inference only"
-        _launch(lambda: _lib.lib().adp_f32_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), B,
-                                                     heads, Tq, Tk, q.stride(1), k.stride(1), v.stride(1),
-                                                     o.stride(1), scale, _stream()),
-                "adp_f32_attention", lambda: (f"f32_attention[B={B} H={heads} Tq={Tq} Tk={Tk}]",
-                                              4.0 * B * heads * Tq * Tk * 64, 0))
+        _launch(lambda: _lib.lib().adp_f32_attention_hd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
+                                                        B, heads, D, Tq, Tk, q.stride(1), k.stride(1),
+                                                        v.stride(1), o.stride(1), scale, _stream()),
+                "adp_f32_attention", lambda: (f"f32_attention[B={B} H={heads} Tq={Tq} Tk={Tk}{tag}]",
+                                              4.0 * B * heads * Tq * Tk * D, 0))
         return o
-    _launch(lambda: _lib.lib().adp_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
-                                             B, heads, Tq, Tk, q.stride(1), k.stride(1),
-                                             v.stride(1), o.stride(1), scale, _p(lse), _stream()),
+    _launch(lambda: _lib.lib().adp_attention_hd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
+                                                B, heads, D, Tq, Tk, q.stride(1), k.stride(1),
+                                                v.stride(1), o.stride(1), scale, _p(lse), _stream()),
             "adp_attention",
-            lambda: (f"attention[B={B} H={heads} Tq={Tq} Tk={Tk}]", 4.0 * B * heads * Tq * Tk * 64,
-                     (2 * B * Tq + 2 * B * Tk) * heads * 64 * 2))
+            lambda: (f"attention[B={B} H={heads} Tq={Tq} Tk={Tk}{tag}]", 4.0 * B * heads * Tq * Tk * D,
+                     (2 * B * Tq + 2 * B * Tk) * heads * D * 2))
     return o
 
 
@@ -639,8 +645,8 @@ def stem_in_bwd(dout: Tensor, x: Tensor, dw: Tensor, dbias: Tensor, f: int, *,
 
 
 def attention_bwd(q: Tensor, k: Tensor, v: Tensor, o: Tensor, d_o: Tensor, lse: Tensor, delta: Tensor,
-                  dq: Tensor, dk: Tensor, dv: Tensor, heads: int, scale: float) -> None:
-    """Backward of `attention`; all bf16 views [B, T, >=heads*64], lse / delta fp32 [B, heads, Tq]."""
+                  dq: Tensor, dk: Tensor, dv: Tensor, heads: int, scale: float, head_dim: int = 64) -> None:
+    """Backward of `attention`; all bf16 views [B, T, >=heads*head_dim], lse / delta fp32 [B, heads, Tq]."""
     a = AttentionBwdArgs()
     a.q, a.k, a.v, a.o, a.d_o = q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), d_o.data_ptr()
     a.lse, a.delta = lse.data_ptr(), delta.data_ptr()
@@ -650,9 +656,10 @@ def attention_bwd(q: Tensor, k: Tensor, v: Tensor, o: Tensor, d_o: Tensor, lse: 
     a.lddq, a.lddk, a.lddv = dq.stride(1), dk.stride(1), dv.stride(1)
     a.scale = scale
     B, Tq, Tk = a.B, a.Tq, a.Tk
-    _launch(lambda: _lib.lib().adp_attention_bwd(C.byref(a), _stream()), "adp_attention_bwd",
-            lambda: (f"attention_bwd[B={B} H={heads} Tq={Tq} Tk={Tk}]", 14.0 * B * heads * Tq * Tk * 64,
-                     (4 * B * Tq + 4 * B * Tk) * heads * 64 * 2))
+    D, tag = head_dim, _hd_tag(head_dim)
+    _launch(lambda: _lib.lib().adp_attention_bwd_hd(C.byref(a), D, _stream()), "adp_attention_bwd",
+            lambda: (f"attention_bwd[B={B} H={heads} Tq={Tq} Tk={Tk}{tag}]", 14.0 * B * heads * Tq * Tk * D,
+                     (4 * B * Tq + 4 * B * Tk) * heads * D * 2))
 
 
 def ln_fold_bwd(w: Tensor, g: Tensor, b: Tensor, dwf: Tensor, dbf: Tensor, dw: Tensor, dg: Tensor,

@@ -284,8 +284,9 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
     bf16 = torch.bfloat16
     loss_mode = mode == "loss"
     heads = net.heads or 0
-    mid = heads * 64
-    att_scale = 64 ** -0.5
+    D = net.head_features or 64
+    mid = heads * D
+    att_scale = D ** -0.5
 
     def act(*shape):
         return torch.empty(*shape, dtype=bf16, device=dev)
@@ -410,7 +411,7 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
             q, k, v = qkv[..., :mid], qkv[..., mid:2 * mid], qkv[..., 2 * mid:]
             plan.fwd.append(lambda: ops.conv_gemm(xn, ap["w_qkv"], qkv, c_in=C, n_valid=3 * mid,
                                                   bias=ap["b_qkv"]))
-            plan.fwd.append(lambda: ops.attention(q, k, v, o, heads, att_scale, lse=lse))
+            plan.fwd.append(lambda: ops.attention(q, k, v, o, heads, att_scale, lse=lse, head_dim=D))
 
             wd_qkv = packed_dgrad(lambda: pack_ln_folded_dgrad((am.to_q.weight, g1),
                                                                (am.to_kv.weight, g2)))   # [C, 3*mid]
@@ -420,7 +421,8 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
                 ops.conv_gemm(dy2, wd_out, d_o, c_in=C, n_valid=mid)
                 ops.wgrad(dy2, o, gw_out, n=C, k=mid)
                 ops.attention_bwd(q, k, v, o, d_o, lse, delta_ws[0], dqkv[..., :mid],
-                                  dqkv[..., mid:2 * mid], dqkv[..., 2 * mid:], heads, att_scale)
+                                  dqkv[..., mid:2 * mid], dqkv[..., 2 * mid:], heads, att_scale,
+                                  head_dim=D)
                 ops.conv_gemm(dqkv, wd_qkv, dxn, c_in=3 * mid, n_valid=C)
                 ops.wgrad(dqkv, xn, gwf, n=3 * mid, k=C)
                 ops.colsum(dqkv, dbf)
@@ -435,7 +437,7 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
                                                   bias=ap["b_kv"]))
             plan.fwd.append(lambda: ops.conv_gemm(xn, ap["w_q"], q, c_in=C, n_valid=mid, bias=ap["b_q"]))
             plan.fwd.append(lambda: ops.attention(q, kv[..., :mid], kv[..., mid:], o, heads, att_scale,
-                                                  lse=lse))
+                                                  lse=lse, head_dim=D))
             wd_q = packed_dgrad(lambda: pack_ln_folded_dgrad((am.to_q.weight, g1)))
             wd_kv = packed_dgrad(lambda: pack_ln_folded_dgrad((am.to_kv.weight, g2)))
             gwq, dbq = gbuf((mid, C)), gbuf((mid,))
@@ -445,7 +447,7 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
                 ops.conv_gemm(dy2, wd_out, d_o, c_in=C, n_valid=mid)
                 ops.wgrad(dy2, o, gw_out, n=C, k=mid)
                 ops.attention_bwd(q, kv[..., :mid], kv[..., mid:], o, d_o, lse, delta_ws[0], dq,
-                                  dkv[..., :mid], dkv[..., mid:], heads, att_scale)
+                                  dkv[..., :mid], dkv[..., mid:], heads, att_scale, head_dim=D)
                 ops.conv_gemm(dq, wd_q, dxn, c_in=mid, n_valid=C)
                 ops.wgrad(dq, xn, gwq, n=mid, k=C)
                 ops.colsum(dq, dbq)

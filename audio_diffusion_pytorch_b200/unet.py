@@ -161,6 +161,7 @@ class B200UNet(nn.Module):
     GN_EPS = 1e-5      # nn.GroupNorm default (a_unet ConvBlock)
     ATT_LN_EPS = 1e-5  # nn.LayerNorm default (a_unet Attention norms)
     MOD_LN_EPS = 1e-6  # a_unet Modulation LayerNorm
+    HEAD_DIMS = (32, 64, 128)   # attention_features the attention kernels are built for
 
     def __init__(self, dim: int, in_channels: int, channels: Sequence[int],
                  factors: Sequence[int], items: Sequence[int],
@@ -196,7 +197,9 @@ class B200UNet(nn.Module):
         if any(attentions) or any(cross_attentions):
             assert exists(attention_features) and exists(attention_heads), \
                 "AttentionItem requires attention_features and attention_heads"
-            assert attention_features == 64, "the attention kernel is built for head dim 64"
+            assert attention_features in self.HEAD_DIMS, \
+                f"attention_features={attention_features}: the attention kernels support head dims " \
+                f"{', '.join(map(str, self.HEAD_DIMS))}"
         if any(cross_attentions):
             assert exists(embedding_features), "CrossAttentionItem requires embedding_features"
 
@@ -741,7 +744,8 @@ class B200UNet(nn.Module):
                     pool.put(tmp)
                     pool.put(x)
                     x, x_stats = out_i, inj_stats
-                mid = (self.heads or 0) * 64
+                D = self.head_features or 64
+                mid = (self.heads or 0) * D
                 for kind in ("att", "cross"):
                     if kind not in ip:
                         continue
@@ -759,9 +763,9 @@ class B200UNet(nn.Module):
                         qkv = pool.get(Bh, Tl, 3 * mid)
                         plan.add(lambda xn=xn, qkv=qkv, ap=ap: ops.conv_gemm(
                             xn, ap["w_qkv"], qkv, c_in=C, n_valid=3 * mid, bias=ap["b_qkv"]))
-                        plan.add(lambda qkv=qkv, o=o: ops.attention(
+                        plan.add(lambda qkv=qkv, o=o, D=D: ops.attention(
                             qkv[..., :mid], qkv[..., mid:2 * mid], qkv[..., 2 * mid:], o, self.heads,
-                            64 ** -0.5))
+                            D ** -0.5, head_dim=D))
                         pool.put(qkv)
                     else:
                         # context K/V do not depend on x or sigma: in sampling mode they are
@@ -777,8 +781,8 @@ class B200UNet(nn.Module):
                             plan.en, ap["w_kv"], kv, c_in=E, n_valid=2 * mid, bias=ap["b_kv"]))
                         plan.add(lambda xn=xn, q=q, ap=ap: ops.conv_gemm(
                             xn, ap["w_q"], q, c_in=C, n_valid=mid, bias=ap["b_q"]))
-                        plan.add(lambda q=q, kv=kv, o=o: ops.attention(
-                            q, kv[..., :mid], kv[..., mid:], o, self.heads, 64 ** -0.5))
+                        plan.add(lambda q=q, kv=kv, o=o, D=D: ops.attention(
+                            q, kv[..., :mid], kv[..., mid:], o, self.heads, D ** -0.5, head_dim=D))
                         pool.put(q)
                     plan.add(lambda o=o, y2=y2, x=x, ap=ap, os_=out_stats: ops.conv_gemm(
                         o, ap["w_out"], y2, c_in=mid, n_valid=C, residual=x, stats=os_, groups=G))

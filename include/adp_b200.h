@@ -110,6 +110,7 @@ int adp_ln_film_dual(const void* x, void* y, void* y2, const float* scale_shift,
                      int32_t groups, float eps, float eps2, adp_stream_t stream);
 
 /* o = softmax(q k^T * scale) v per (batch, head), head dim 64 -- a_unet AttentionBase.
+ * Same as adp_attention_hd(..., head_dim = 64, ...).
  * q: bf16 [B][Tq][ldq] (head h at columns [h*64,(h+1)*64)), k/v likewise over Tk rows,
  * o: bf16 [B][Tq][ldo].  wgmma flash attention (S and O accumulators in registers).
  * lse: optional fp32 [B][H][Tq] = log sum_k exp(scale * q.k) per row (kept by the training
@@ -117,6 +118,12 @@ int adp_ln_film_dual(const void* x, void* y, void* y2, const float* scale_shift,
 int adp_attention(const void* q, const void* k, const void* v, void* o, int32_t B, int32_t H,
                   int32_t Tq, int32_t Tk, int32_t ldq, int32_t ldk, int32_t ldv, int32_t ldo,
                   float scale, float* lse, adp_stream_t stream);
+/* adp_attention at head dim head_dim in {32, 64, 128}: head h at columns
+ * [h*head_dim,(h+1)*head_dim); pitches multiples of 8 and >= H*head_dim.  Any other head_dim
+ * is an error (nothing is launched). */
+int adp_attention_hd(const void* q, const void* k, const void* v, void* o, int32_t B, int32_t H,
+                     int32_t head_dim, int32_t Tq, int32_t Tk, int32_t ldq, int32_t ldk,
+                     int32_t ldv, int32_t ldo, float scale, float* lse, adp_stream_t stream);
 
 /* y[b][n] = out_act( sum_k in_act(x[b][k]) * w[n][k] + bias[n] ),  B <= 64 rows.
  * The step-conditioning linears: NumberEmbedder.to_out, TimeConditioningPlugin MLP,
@@ -261,6 +268,9 @@ int adp_f32_ln_film(const float* x, float* y, float* y2, const float* scale_shif
                     int T, int C, float eps, float eps2, adp_stream_t stream);
 int adp_f32_attention(const float* q, const float* k, const float* v, float* o, int B, int H, int Tq, int Tk,
                       int ldq, int ldk, int ldv, int ldo, float scale, adp_stream_t stream);
+/* adp_f32_attention at head dim head_dim in {32, 64, 128} (adp_f32_attention: 64) */
+int adp_f32_attention_hd(const float* q, const float* k, const float* v, float* o, int B, int H, int head_dim,
+                         int Tq, int Tk, int ldq, int ldk, int ldv, int ldo, float scale, adp_stream_t stream);
 /* y[b,n] = act_out(sum_k act_in(x[b,k]) * w[n,k] + bias[n])  (shadows adp_skinny_linear) */
 int adp_f32_linear(const float* x, const float* w, const float* bias, float* y, int B, int K, int N, int ldx,
                    int ldw, int ldy, int in_act, int out_act, adp_stream_t stream);
@@ -377,6 +387,9 @@ typedef struct adp_attention_bwd_args {
   float scale;
 } adp_attention_bwd_args;
 int adp_attention_bwd(const adp_attention_bwd_args* args, adp_stream_t stream);
+/* adp_attention_bwd at head dim head_dim in {32, 64, 128} (adp_attention_bwd: 64); head h at
+ * columns [h*head_dim,(h+1)*head_dim) of every tensor, pitches >= H*head_dim. */
+int adp_attention_bwd_hd(const adp_attention_bwd_args* args, int32_t head_dim, adp_stream_t stream);
 
 /* The attention projections run with their LayerNorm affine folded in (Wf = W diag(g),
  * bf = W b).  Unfolds the gradients: dw[N][C] = dwf*g + dbf (x) b (stored); dg[C] += colsum(dwf o W);
