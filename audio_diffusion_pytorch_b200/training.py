@@ -33,7 +33,7 @@ import torch.nn.functional as F
 from torch import Tensor
 
 from . import ops
-from .unet import B200UNet, LevelParams, _pad_to
+from .unet import B200UNet, LevelParams, _ForwardWalk, _capture, _pad_to
 
 
 class _TrainPlan:
@@ -320,13 +320,6 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
     # ---- statistics + gradient arenas
     n_items = sum(len(lv.items_down) + len(lv.items_up) for lv in levels)
     arena = torch.zeros(7 * n_items + 4 * len(levels) + 8, B, G, 2, dtype=torch.float64, device=dev)
-    slot = [0]
-
-    def new_stats():
-        s = arena[slot[0]]
-        slot[0] += 1
-        return s
-
     plan.fwd.append(lambda: (arena.zero_(), plan.loss_sum.zero_()))
     refreshers: List = []                  # re-pack the dgrad weights in place after a weight update
 
@@ -383,6 +376,10 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
     if M:
         en, den = act(B, M, E), torch.zeros(B, M, E, dtype=bf16, device=dev)
         plan.fwd.append(lambda: ops.ln_film(plan.embedding, en, None, 0, None, G, net.ATT_LN_EPS))
+    # the forward launches; every intermediate the backward reads stays live
+    walk = _ForwardWalk(net, P, plan.fwd.append, B, arena, ss_all, keep=True, ctx=plan.ctx,
+                        embedding=plan.embedding, add_ctx=plan.fwd.append, en=en)
+    new_stats = walk.new_stats
     delta_ws = [None]    # shared fp32 workspace of adp_attention_bwd, sized for the largest item
 
     def delta_for(Tl: int) -> Tensor:
@@ -390,13 +387,11 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
             delta_ws[0] = _zeros((B * heads * Tl,), dev)
         return delta_ws[0]
 
-    # ---- AttentionItem / CrossAttentionItem (a_unet): x + to_out(softmax(q k^T / 8) v)
-    def attention_block(x: Tensor, xn: Tensor, ap: Dict, am, cross: bool, Tl: int, C: int,
-                        out_stats: Optional[Tensor]):
-        """x: the item's input (residual); xn = LayerNorm(x) (affine folded into the projections).
-        Appends the forward launches; returns (y2, backward closure dy2 -> dx)."""
-        o, y2 = act(B, Tl, mid), act(B, Tl, C)
-        lse = _zeros((B, heads, Tl), dev)
+    # ---- AttentionItem / CrossAttentionItem (a_unet): y = x + to_out(softmax(q k^T / sqrt(D)) v)
+    def attention_backward(a: Dict, am, cross: bool, Tl: int, C: int):
+        """a: the tensors of the walk's forward (x, xn = LayerNorm(x) with the affine folded into the
+        projections, q / k / v, o, lse).  Returns the backward closure dy -> dx."""
+        x, xn, q, k, v, o, lse = a["x"], a["xn"], a["q"], a["k"], a["v"], a["o"], a["lse"]
         delta_for(Tl)
         wo = am.to_out.weight
         wd_out = packed_dgrad(lambda: ops.pack_linear(wo.detach().t().contiguous()))
@@ -407,12 +402,7 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
         dWq, dWkv = grad_for(am.to_q.weight), grad_for(am.to_kv.weight)
         dg1, db1, dg2, db2 = grad_for(g1), grad_for(b1), grad_for(g2), grad_for(b2)
         if not cross:
-            qkv, dqkv = act(B, Tl, 3 * mid), act(B, Tl, 3 * mid)
-            q, k, v = qkv[..., :mid], qkv[..., mid:2 * mid], qkv[..., 2 * mid:]
-            plan.fwd.append(lambda: ops.conv_gemm(xn, ap["w_qkv"], qkv, c_in=C, n_valid=3 * mid,
-                                                  bias=ap["b_qkv"]))
-            plan.fwd.append(lambda: ops.attention(q, k, v, o, heads, att_scale, lse=lse, head_dim=D))
-
+            dqkv = act(B, Tl, 3 * mid)
             wd_qkv = packed_dgrad(lambda: pack_ln_folded_dgrad((am.to_q.weight, g1),
                                                                (am.to_kv.weight, g2)))   # [C, 3*mid]
             gwf, dbf = gbuf((3 * mid, C)), gbuf((3 * mid,))
@@ -431,13 +421,7 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
                 ops.ln_film_bwd(dxn, x, None, 0, dx, dres=dy2, eps=net.ATT_LN_EPS)
                 return dx
         else:
-            q, kv = act(B, Tl, mid), act(B, M, 2 * mid)
             dq, dkv = act(B, Tl, mid), act(B, M, 2 * mid)
-            plan.fwd.append(lambda: ops.conv_gemm(en, ap["w_kv"], kv, c_in=E, n_valid=2 * mid,
-                                                  bias=ap["b_kv"]))
-            plan.fwd.append(lambda: ops.conv_gemm(xn, ap["w_q"], q, c_in=C, n_valid=mid, bias=ap["b_q"]))
-            plan.fwd.append(lambda: ops.attention(q, kv[..., :mid], kv[..., mid:], o, heads, att_scale,
-                                                  lse=lse, head_dim=D))
             wd_q = packed_dgrad(lambda: pack_ln_folded_dgrad((am.to_q.weight, g1)))
             wd_kv = packed_dgrad(lambda: pack_ln_folded_dgrad((am.to_kv.weight, g2)))
             gwq, dbq = gbuf((mid, C)), gbuf((mid,))
@@ -446,7 +430,7 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
             def bwd(dy2: Tensor) -> Tensor:
                 ops.conv_gemm(dy2, wd_out, d_o, c_in=C, n_valid=mid)
                 ops.wgrad(dy2, o, gw_out, n=C, k=mid)
-                ops.attention_bwd(q, kv[..., :mid], kv[..., mid:], o, d_o, lse, delta_ws[0], dq,
+                ops.attention_bwd(q, k, v, o, d_o, lse, delta_ws[0], dq,
                                   dkv[..., :mid], dkv[..., mid:], heads, att_scale, head_dim=D)
                 ops.conv_gemm(dq, wd_q, dxn, c_in=mid, n_valid=C)
                 ops.wgrad(dq, xn, gwq, n=mid, k=C)
@@ -459,136 +443,80 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
                 ops.ln_fold_bwd(am.to_kv.weight, g2, b2, gwkv, dbkv, dWkv, dg2, db2)
                 ops.ln_film_bwd(dxn, x, None, 0, dx, dres=dy2, eps=net.ATT_LN_EPS)
                 return dx
-        plan.fwd.append(lambda: ops.conv_gemm(o, ap["w_out"], y2, c_in=mid, n_valid=C, residual=x,
-                                              stats=out_stats, groups=G))
-        return y2, bwd
+        return bwd
 
-    # ---- one chain of [ResnetItem, ModulationItem, AttentionItem?, CrossAttentionItem?]
-    def run_items(x: Tensor, x_stats: Tensor, items_p: List[Dict], items_m, lv: LevelParams, Tl: int,
-                  li: int = 0):
-        C = lv.ch
-        narrow = C == 8
-        bwds: List = []
-        for ip, im in zip(items_p, items_m):
-            r_ = im.resnet
-            ss = ss_all[:, ip["ss_off"]:] if mod else None
-            dss = dss_all[:, ip["ss_off"]:] if mod else None
-            has_att, has_cross, has_inj = im.attention is not None, im.cross is not None, im.inject is not None
-            h_stats = new_stats()
-            y_stats = None if (has_att or has_cross or has_inj) else new_stats()
-            S1, S2 = new_stats(), new_stats()
-            h, rr = act(B, Tl, C), act(B, Tl, C)
-            # without a ModulationItem the ResnetItem's output is the item's output: conv2 writes
-            # it (and its GroupNorm statistics) directly
-            y = act(B, Tl, C) if mod else rr
-            rs = None if mod else y_stats
-            xn_first = act(B, Tl, C) if ((has_att or has_cross) and not has_inj and mod) else None
-            dgn1 = (grad_for(r_.gn1.weight), grad_for(r_.gn1.bias))
-            dgn2 = (grad_for(r_.gn2.weight), grad_for(r_.gn2.bias))
-            db1, db2 = grad_for(r_.conv1.bias), grad_for(r_.conv2.bias)
-            dr, dh, dx, dxh = act(B, Tl, C), act(B, Tl, C), act(B, Tl, C), act(B, Tl, C)
+    # ---- backward of one [ResnetItem, ModulationItem, InjectChannelsItem?, AttentionItem?,
+    # CrossAttentionItem?] from the tensors of the walk's forward
+    def item_backward(rec, ip: Dict, im, C: int, Tl: int, li: int):
+        res, inj, atts = rec
+        r_ = im.resnet
+        x, h, rr, ss = res["x"], res["h"], res["r"], res["ss"]
+        xs, hs = res["x_stats"], res["h_stats"]
+        dss = dss_all[:, ip["ss_off"]:] if mod else None
+        S1, S2 = new_stats(), new_stats()
+        dgn1 = (grad_for(r_.gn1.weight), grad_for(r_.gn1.bias))
+        dgn2 = (grad_for(r_.gn2.weight), grad_for(r_.gn2.bias))
+        db1, db2 = grad_for(r_.conv1.bias), grad_for(r_.conv2.bias)
+        dr, dh, dx, dxh = act(B, Tl, C), act(B, Tl, C), act(B, Tl, C), act(B, Tl, C)
+        if C == 8:
+            dw1, dw2 = grad_for(r_.conv1.weight), grad_for(r_.conv2.weight)
+            db_scratch = gbuf((C,))
 
-            def modulation_fwd(rr=rr, y=y, ss=ss, ys=y_stats, xn=xn_first):
-                ops.ln_film(rr, y, ss, ss_stride, ys, G, net.MOD_LN_EPS, y2=xn, eps2=net.ATT_LN_EPS)
-            if narrow:
-                dw1, dw2 = grad_for(r_.conv1.weight), grad_for(r_.conv2.weight)
-                db_scratch = gbuf((C,))
-                plan.fwd.append(lambda x=x, h=h, s=x_stats, hs=h_stats, ip=ip: ops.narrow_conv(
-                    x, h, s, ip["gn1"][0], ip["gn1"][1], ip["w1"], ip["b1"], G, stats_out=hs))
-                plan.fwd.append(lambda x=x, h=h, rr=rr, hs=h_stats, ip=ip, rs=rs: ops.narrow_conv(
-                    h, rr, hs, ip["gn2"][0], ip["gn2"][1], ip["w2"], ip["b2"], G, residual=x, stats_out=rs))
+            def bwd(dy):
                 if mod:
-                    plan.fwd.append(modulation_fwd)
+                    ops.ln_film_bwd(dy, rr, ss, ss_stride, dr, dss=dss, dss_stride=ss_stride, eps=net.MOD_LN_EPS)
+                d_r = dr if mod else dy
+                ops.narrow_conv_bwd(d_r, h, hs, ip["gn2"][0], ip["gn2"][1], ip["w2"], dxh, dgn2[0],
+                                    dgn2[1], S2, dw2, db2, G)
+                ops.gn_bwd_apply(dxh, h, hs, S2, dh, G, colsum=db1)   # fp32 sum, pre-rounding
+                ops.narrow_conv_bwd(dh, x, xs, ip["gn1"][0], ip["gn1"][1], ip["w1"], dxh, dgn1[0],
+                                    dgn1[1], S1, dw1, db_scratch, G)
+                ops.gn_bwd_apply(dxh, x, xs, S1, dx, G, dres=d_r)
+                return dx
+        else:
+            a1, a2 = res["a1"], res["a2"]
+            wd1 = packed_dgrad(lambda: ops.pack_conv_dgrad(r_.conv1.weight.detach()))
+            wd2 = packed_dgrad(lambda: ops.pack_conv_dgrad(r_.conv2.weight.detach()))
+            work = (dr, dh, dx, dxh, act(B, Tl, C))
+            # [tap][co][ci] accumulators of the fused 3-tap wgrad -> PyTorch [co][ci][tap]
+            gw1 = grad_for(r_.conv1.weight, (3, C, C), (1, 2, 0))
+            gw2 = grad_for(r_.conv2.weight, (3, C, C), (1, 2, 0))
+            film = (ss, dss, ss_stride, net.MOD_LN_EPS) if mod else None
 
-                def bwd(dy, x=x, h=h, rr=rr, ss=ss, dss=dss, xs=x_stats, hs=h_stats, ip=ip, dr=dr,
-                        dh=dh, dx=dx, dxh=dxh, S1=S1, S2=S2, dgn1=dgn1, dgn2=dgn2, dw1=dw1, dw2=dw2,
-                        db1=db1, db2=db2, db_scratch=db_scratch):
-                    if mod:
-                        ops.ln_film_bwd(dy, rr, ss, ss_stride, dr, dss=dss, dss_stride=ss_stride,
-                                        eps=net.MOD_LN_EPS)
-                    else:
-                        dr = dy
-                    ops.narrow_conv_bwd(dr, h, hs, ip["gn2"][0], ip["gn2"][1], ip["w2"], dxh, dgn2[0],
-                                        dgn2[1], S2, dw2, db2, G)
-                    ops.gn_bwd_apply(dxh, h, hs, S2, dh, G, colsum=db1)   # fp32 sum, pre-rounding
-                    ops.narrow_conv_bwd(dh, x, xs, ip["gn1"][0], ip["gn1"][1], ip["w1"], dxh, dgn1[0],
-                                        dgn1[1], S1, dw1, db_scratch, G)
-                    ops.gn_bwd_apply(dxh, x, xs, S1, dx, G, dres=dr)
-                    return dx
-            else:
-                a1, a2 = act(B, Tl, C), act(B, Tl, C)
-                wd1 = packed_dgrad(lambda r_=r_: ops.pack_conv_dgrad(r_.conv1.weight.detach()))
-                wd2 = packed_dgrad(lambda r_=r_: ops.pack_conv_dgrad(r_.conv2.weight.detach()))
-                plan.fwd.append(lambda x=x, a1=a1, s=x_stats, ip=ip: ops.gn_silu(
-                    x, a1, s, ip["gn1"][0], ip["gn1"][1], G, net.GN_EPS))
-                plan.fwd.append(lambda a1=a1, h=h, hs=h_stats, ip=ip: ops.conv_gemm(
-                    a1, ip["w1"], h, c_in=C, n_valid=C, taps=(-1, 0, 1), bias=ip["b1"], stats=hs, groups=G))
-                plan.fwd.append(lambda a2=a2, h=h, hs=h_stats, ip=ip: ops.gn_silu(
-                    h, a2, hs, ip["gn2"][0], ip["gn2"][1], G, net.GN_EPS))
-                plan.fwd.append(lambda x=x, a2=a2, rr=rr, ip=ip, rs=rs: ops.conv_gemm(
-                    a2, ip["w2"], rr, c_in=C, n_valid=C, taps=(-1, 0, 1), bias=ip["b2"], residual=x,
-                    stats=rs, groups=G))
-                if mod:
-                    plan.fwd.append(modulation_fwd)
-                da = act(B, Tl, C)
-                # [tap][co][ci] accumulators of the fused 3-tap wgrad -> PyTorch [co][ci][tap]
-                gw = {"w1": grad_for(r_.conv1.weight, (3, C, C), (1, 2, 0)),
-                      "w2": grad_for(r_.conv2.weight, (3, C, C), (1, 2, 0))}
+            def bwd(dy):
+                return resnet_item_bwd(dy, x, h, rr, a1, a2, xs, hs, ip["gn1"], ip["gn2"], wd1, wd2, gw1, gw2,
+                                       dgn1, dgn2, db1, db2, S1, S2, work, G, film=film)
+        if mod:
+            grads[id(im.modulation.proj.weight)] = ("cond_w", ip["ss_off"], 2 * C)
+            grads[id(im.modulation.proj.bias)] = ("cond_b", ip["ss_off"], 2 * C)
+        chain = [bwd]
+        if inj is not None:
+            # a_unet InjectChannelsItem: conv1x1(cat([x, ctx])) + x, W = [W_x | W_c]
+            conv, ctxb, dctxb = im.inject, inj["ctx"], plan.dctx[li]
+            n_ctx, ctx_pad = conv.weight.shape[1] - C, ctxb.shape[-1]
+            dyi = act(B, Tl, C)
+            gw_inj = grad_for(conv.weight, (C, C + n_ctx, 1)).view(C, C + n_ctx)
+            db_inj = grad_for(conv.bias)
+            wd_x, wd_c = packed_dgrad(lambda: pack_inject_dgrad(conv.weight, C, ctx_pad))
+            # d context is summed over the items of this depth (in place through the residual)
+            chain.append(lambda d_out: inject_bwd(d_out, inj["x"], ctxb, dctxb, wd_x, wd_c, gw_inj, db_inj, dyi,
+                                                  n_ctx))
+        kinds = [(kind, am) for kind, am in (("att", im.attention), ("cross", im.cross)) if am is not None]
+        for a, (kind, am) in zip(atts, kinds):
+            chain.append(attention_backward(a, am, kind == "cross", Tl, C))
 
-                film = (ss, dss, ss_stride, net.MOD_LN_EPS) if mod else None
+        def item_bwd(dy):
+            for fn in reversed(chain):
+                dy = fn(dy)
+            return dy
+        return item_bwd
 
-                def bwd(dy, x=x, h=h, rr=rr, a1=a1, a2=a2, xs=x_stats, hs=h_stats, ip=ip,
-                        work=(dr, dh, dx, dxh, da), S1=S1, S2=S2, dgn1=dgn1, dgn2=dgn2, db1=db1,
-                        db2=db2, wd1=wd1, wd2=wd2, gw=gw, film=film):
-                    return resnet_item_bwd(dy, x, h, rr, a1, a2, xs, hs, ip["gn1"], ip["gn2"], wd1, wd2,
-                                           gw["w1"], gw["w2"], dgn1, dgn2, db1, db2, S1, S2, work, G,
-                                           film=film)
-            if mod:
-                grads[id(im.modulation.proj.weight)] = ("cond_w", ip["ss_off"], 2 * C)
-                grads[id(im.modulation.proj.bias)] = ("cond_b", ip["ss_off"], 2 * C)
-            chain = [bwd]
-            x, x_stats = y, y_stats
-            xn = xn_first
-            if has_inj:
-                # a_unet InjectChannelsItem: conv1x1(cat([x, ctx])) + x, W = [W_x | W_c]
-                jp, conv = ip["inj"], im.inject
-                ctxb, dctxb = plan.ctx[li], plan.dctx[li]
-                n_ctx, ctx_pad = conv.weight.shape[1] - C, ctxb.shape[-1]
-                tmp, yi, dyi = act(B, Tl, C), act(B, Tl, C), act(B, Tl, C)
-                inj_stats = None if (has_att or has_cross) else new_stats()
-                plan.fwd.append(lambda ctxb=ctxb, jp=jp, tmp=tmp, x=x: ops.conv_gemm(
-                    ctxb, jp["w_c"], tmp, c_in=ctxb.shape[-1], n_valid=C, bias=jp["b"], residual=x))
-                plan.fwd.append(lambda x=x, jp=jp, tmp=tmp, yi=yi, st=inj_stats: ops.conv_gemm(
-                    x, jp["w_x"], yi, c_in=C, n_valid=C, residual=tmp, stats=st, groups=G))
-                gw_inj = grad_for(conv.weight, (C, C + n_ctx, 1)).view(C, C + n_ctx)
-                db_inj = grad_for(conv.bias)
-                wd_x, wd_c = packed_dgrad(lambda conv=conv, C=C, ctx_pad=ctx_pad: pack_inject_dgrad(
-                    conv.weight, C, ctx_pad))
-
-                def inj_bwd(d_out, x=x, ctxb=ctxb, dctxb=dctxb, gw_inj=gw_inj, db_inj=db_inj, wd_x=wd_x,
-                            wd_c=wd_c, dyi=dyi, n_ctx=n_ctx):
-                    # d context is summed over the items of this depth (in place through the residual)
-                    return inject_bwd(d_out, x, ctxb, dctxb, wd_x, wd_c, gw_inj, db_inj, dyi, n_ctx)
-                chain.append(inj_bwd)
-                x, x_stats = yi, inj_stats
-            for kind, am in (("att", im.attention), ("cross", im.cross)):
-                if am is None:
-                    continue
-                last = kind == "cross" or not has_cross
-                ost = new_stats() if last else None
-                if xn is None:                       # second attention of the item: its own pre-norm
-                    xn = act(B, Tl, C)
-                    plan.fwd.append(lambda x=x, xn=xn: ops.ln_film(x, xn, None, 0, None, G, net.ATT_LN_EPS))
-                x, att_bwd = attention_block(x, xn, ip[kind], am, kind == "cross", Tl, C, ost)
-                x_stats, xn = ost, None
-                chain.append(att_bwd)
-
-            def item_bwd(dy, chain=chain):
-                for fn in reversed(chain):
-                    dy = fn(dy)
-                return dy
-            bwds.append(item_bwd)
-        return x, x_stats, bwds
+    # ---- one item chain: the walk's forward (output statistics of every item, the last one
+    # included) and one backward closure per item
+    def run_items(x: Tensor, x_stats: Tensor, items_p: List[Dict], items_m, lv: LevelParams, Tl: int, li: int):
+        x, x_stats, recs = walk.items(x, x_stats, items_p, lv.ch, Tl, li, last_needs_stats=True)
+        return x, x_stats, [item_backward(rec, ip, im, lv.ch, Tl, li)
+                            for rec, ip, im in zip(recs, items_p, items_m)]
 
     # ---- recursive level walk; returns (output tensor, its stats, backward closure)
     def level(i: int, x_in: Optional[Tensor], T_in: int):
@@ -600,20 +528,18 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
         # contiguous ranges; the backward finishes them in the order up, inner, down and
         # announces each range through plan.mark (overlapped gradient all-reduce, parallel.py)
         cur = {"entry": cursor[0]}
-        x0, st0 = act(B, Tl, C), new_stats()
         db_down = grad_for(lv.down.bias)
         if i == 0:
+            x0, st0 = walk.pool.get(B, Tl, C), new_stats()
             dw_down = grad_for(lv.down.weight)
             plan.fwd.append(lambda: ops.stem_in(plan.x, Lp["down_w"], Lp["down_b"], x0, lv.factor,
                                                 append=plan.append, noise=plan.noise, alpha=plan.alpha,
                                                 beta=plan.beta, stats=st0, groups=G))
         else:
-            kdim = lv.factor * lv.in_ch
-            plan.fwd.append(lambda: ops.conv_gemm(x_in.view(B, Tl, kdim), Lp["down_w"], x0, c_in=kdim,
-                                                  n_valid=C, bias=Lp["down_b"], stats=st0, groups=G))
+            x0, st0 = walk.down(lv, Lp, x_in, Tl)
             wd_down = packed_dgrad(lambda: pack_down_dgrad(lv.down.weight))
             # [co][tap][ci] (the [B, T/f, f*C] view) -> PyTorch [co][ci][tap]
-            gw_down = grad_for(lv.down.weight, (C, lv.factor, lv.in_ch), (0, 2, 1)).view(C, kdim)
+            gw_down = grad_for(lv.down.weight, (C, lv.factor, lv.in_ch), (0, 2, 1)).view(C, lv.factor * lv.in_ch)
         x, st, items_down_bwd = run_items(x0, st0, Lp["items_down"], lv.items_down, lv, Tl, li=i)
         cur["down_end"] = cursor[0]
         inner = None
@@ -682,14 +608,11 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
             cur["exit"] = cursor[0]
             return None, None, backward_level0
 
-        # levels >= 1: up conv writes y (pre-gate), skip_gate merges with the level's input
+        # levels >= 1: the up conv writes y_up (pre-gate), the merge combines it with the level's input
         f, Co = lv.factor, lv.out_ch
-        y_up, out, ost = act(B, T_in, Co), act(B, T_in, Co), new_stats()
+        out, ost, y_up = walk.up_merge(lv, Lp, x_last, x_in, Tl, T_in)
         dys, dx_last, d_xin = act(B, T_in, Co), act(B, Tl, C), act(B, T_in, lv.in_ch)
         if f > 1:
-            plan.fwd.append(lambda: ops.conv_gemm(x_last, Lp["up_w"], y_up.view(B, Tl, f * Co), c_in=C,
-                                                  n_valid=Co, up_factor=f, bias=Lp["up_b"]))
-
             wd_up = packed_dgrad(lambda: pack_upsample_dgrad(lv.up.weight, f))
             gw_up = gbuf((f, 2, Co, C))
 
@@ -697,32 +620,16 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
                 grads[id(lv.up.weight)] = fold_upsample_wgrad(gw_up, f)
             finals.append(up_final)
         else:
-            plan.fwd.append(lambda: ops.conv_gemm(x_last, Lp["up_w"], y_up, c_in=C, n_valid=Co,
-                                                  taps=(-1, 0, 1), bias=Lp["up_b"]))
             wd_up = packed_dgrad(lambda: ops.pack_conv_dgrad(lv.up.weight.detach()))
             gw_up = grad_for(lv.up.weight, (3, Co, C), (1, 2, 0))
         if mod:
-            plan.fwd.append(lambda: ops.skip_gate(y_up, x_in, gate, out, ost, G))
             d_skip_of = lambda d_out: d_out      # noqa: E731  (the skip path's gradient is d_out itself)
 
             def merge_bwd(d_out: Tensor) -> None:
                 ops.skip_gate_bwd(d_out, y_up, gate, dys, dgate)
         else:
-            # SkipCat: out = (s Wc1) skip + Wc2 y_up + bc as two accumulating GEMMs; an 8-channel
-            # level is processed two positions per row against block-diagonal weights (K >= 16)
-            rp = max(1, 16 // Co)
-            assert T_in % rp == 0, "SkipCat merge of an 8-channel level needs an even length"
-
-            def rows(t):
-                return t.view(B, T_in // rp, rp * Co)
-            tmp, d_skip = act(B, T_in, Co), act(B, T_in, Co)
-            plan.fwd.append(lambda: ops.conv_gemm(rows(x_in), Lp["cat_w1"], rows(tmp), c_in=rp * Co,
-                                                  n_valid=rp * Co, bias=Lp["cat_b"]))
-            plan.fwd.append(lambda: ops.conv_gemm(rows(y_up), Lp["cat_w2"], rows(out), c_in=rp * Co,
-                                                  n_valid=rp * Co, residual=rows(tmp),
-                                                  stats=ost if rp == 1 else None, groups=G))
-            if rp > 1:
-                plan.fwd.append(lambda: ops.gn_stats(out, ost, G))
+            rp = max(1, 16 // Co)                # positions per GEMM row of the SkipCat merge
+            d_skip = act(B, T_in, Co)
             wm_ = lv.merge.weight
             wd_c1, wd_c2 = packed_dgrad(lambda: pack_skipcat_dgrad(wm_, rp))
             gw_cat = grad_for(wm_, (Co, 2 * Co, 1)).view(Co, 2 * Co)
@@ -754,7 +661,6 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
         return out, ost, backward_level
 
     _, _, backward0 = level(0, None, T)
-    assert slot[0] <= arena.shape[0]
     plan.flat = flat
     plan.refreshers, plan.version = refreshers, net._version()
     plan.grads, plan.finals, plan.specs = grads, finals, specs
@@ -786,46 +692,29 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
 def _refresh_dgrad_packs(plan: _TrainPlan, net: B200UNet) -> None:
     """Transposed / tap-reversed weight packs of the data-gradient GEMMs after a weight update:
     captured into a CUDA graph on first use (same reasoning as B200UNet._repack)."""
+    def refresh():
+        for r in plan.refreshers:
+            r()
     if not net.use_cuda_graph:
-        for r in plan.refreshers:
-            r()
-        return
-    if getattr(plan, "refresh_graph", None) is None:
-        for r in plan.refreshers:
-            r()
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            for r in plan.refreshers:
-                r()
-        plan.refresh_graph = g
+        refresh()
+    elif getattr(plan, "refresh_graph", None) is None:
+        refresh()
+        plan.refresh_graph = _capture(refresh)
     else:
         plan.refresh_graph.replay()
 
 
 def _run(plan: _TrainPlan, which: str, use_graph: bool) -> None:
-    """Eager on the first call, captured on the second, replayed afterwards."""
+    """Eager on the first call, captured on the second, replayed afterwards (which: 'f' / 'b')."""
     prog = (lambda: [f() for f in plan.fwd]) if which == "f" else plan.backward_program
-    runs = plan.runs_f if which == "f" else plan.runs_b
-    graph = plan.graph_f if which == "f" else plan.graph_b
+    runs = getattr(plan, "runs_" + which)
     if not use_graph or runs == 0:
         prog()
-    elif graph is None:
-        g = torch.cuda.CUDAGraph()
-        torch.cuda.synchronize()
-        with torch.cuda.graph(g):
-            prog()
-        if which == "f":
-            plan.graph_f = g
-        else:
-            plan.graph_b = g
-        g.replay()
     else:
-        graph.replay()
-    if which == "f":
-        plan.runs_f += 1
-    else:
-        plan.runs_b += 1
+        if getattr(plan, "graph_" + which) is None:
+            setattr(plan, "graph_" + which, _capture(prog))
+        getattr(plan, "graph_" + which).replay()
+    setattr(plan, "runs_" + which, runs + 1)
 
 
 def _run_backward_synced(plan: _TrainPlan, net: B200UNet, sync) -> None:

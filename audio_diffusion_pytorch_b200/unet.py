@@ -155,6 +155,241 @@ class _Plan:
             fn()
 
 
+def _capture(run: Callable[[], None], early_weights: bool = False) -> torch.cuda.CUDAGraph:
+    """run() captured into a CUDA graph (not executed).  early_weights: no kernel in the graph
+    writes the packed weights, so the GEMMs may fetch them before their programmatic-dependency
+    wait (conv_gemm.cu, early_w)."""
+    torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    if early_weights:
+        _lib.lib().adp_debug_set(2, 1)
+    try:
+        with torch.cuda.graph(g):
+            run()
+    finally:
+        if early_weights:
+            _lib.lib().adp_debug_set(2, 0)
+    return g
+
+
+class _ForwardWalk:
+    """Emits the trunk's forward launches, shared by the inference / sampling plans
+    (B200UNet._build_plan) and the training plan (training.build_train_plan): the item chains,
+    the down conv of levels >= 1 and their up conv + merge.  Each caller walks the levels itself
+    and owns the level-0 stems, the conditioning and its static I/O.  Every emitter returns the
+    tensors it used; the training plan builds its backward from them.
+
+    keep=False: dead activations are reused, and the fusions that never write a tensor are used
+    (FiLM in the narrow / thin-level conv, the thin-level kernel, the GroupNorm A-transform, the
+    merge gate in the up-conv epilogue).  keep=True: every buffer stays live, every tensor the
+    backward reads is written, and attention keeps its log-sum-exp."""
+
+    def __init__(self, net: "B200UNet", P: Dict, add: Callable, Bh: int, stats: Tensor, ss_all: Tensor,
+                 keep: bool, ctx: Dict[int, Tensor], embedding: Optional[Tensor], add_ctx: Callable,
+                 en: Optional[Tensor] = None):
+        self.net, self.P, self.add, self.Bh, self.keep = net, P, add, Bh, keep
+        self.pool = _Pool(net.net.down.weight.device, reuse=not keep, dtype=net._act_dtype())
+        self.stats, self.n_stats = stats, 0
+        self.ss_all, self.ss_stride, self.mod = ss_all, ss_all.shape[1], net.use_modulation
+        self.ctx, self.embedding, self.add_ctx = ctx, embedding, add_ctx
+        self.en = en         # LayerNorm(embedding), shared by all cross-attentions; made on first use
+        self.G = net.groups
+        self.D = net.head_features or 64
+        self.mid = (net.heads or 0) * self.D
+
+    def new_stats(self) -> Tensor:
+        s = self.stats[self.n_stats]
+        self.n_stats += 1
+        return s
+
+    def items(self, x: Tensor, x_stats: Tensor, items_p: List[Dict], C: int, Tl: int, li: int,
+              last_needs_stats: bool):
+        """One item chain of level li; returns (output, its statistics, one record per item)."""
+        recs = []
+        for idx, ip in enumerate(items_p):
+            want_stats = idx < len(items_p) - 1 or last_needs_stats
+            x, x_stats, rec = self.item(x, x_stats, ip, C, Tl, li, want_stats)
+            recs.append(rec)
+        return x, x_stats, recs
+
+    def item(self, x: Tensor, x_stats: Tensor, ip: Dict, C: int, Tl: int, li: int, want_stats: bool):
+        """[ResnetItem, ModulationItem?, InjectChannelsItem?, AttentionItem?, CrossAttentionItem?];
+        returns (output, its statistics, (resnet record, inject record or None, attention records))."""
+        has_att, has_cross, has_inj = "att" in ip, "cross" in ip, "inj" in ip
+        y_stats = self.new_stats() if (want_stats and not (has_att or has_cross or has_inj)) else None
+        res = self._resnet(x, x_stats, ip, C, Tl, y_stats, (has_att or has_cross) and not has_inj)
+        x, x_stats, xn = res["y"], y_stats, res["xn"]
+        inj = None
+        if has_inj:
+            x_stats = self.new_stats() if (want_stats and not (has_att or has_cross)) else None
+            inj = self._inject(x, ip["inj"], C, Tl, li, x_stats)
+            x = inj["y"]
+        atts = []
+        for kind in ("att", "cross"):
+            if kind in ip:
+                x_stats = self.new_stats() if (want_stats and (kind == "cross" or not has_cross)) else None
+                atts.append(self._attention(x, xn, ip[kind], kind == "cross", C, Tl, x_stats))
+                x, xn = atts[-1]["y"], None
+        return x, x_stats, (res, inj, atts)
+
+    def _resnet(self, x: Tensor, x_stats: Tensor, ip: Dict, C: int, Tl: int, y_stats: Optional[Tensor],
+                pre_norm: bool) -> Dict:
+        """ResnetItem + ModulationItem.  pre_norm: the Modulation pass also writes the following
+        attention's LayerNorm (xn) when it runs as its own kernel."""
+        net, pool, add, G, Bh, mod = self.net, self.pool, self.add, self.G, self.Bh, self.mod
+        narrow = C == 8 and not net.verify_fp32
+        # thin levels (C = 32, 64) are HBM-bound: one fused ConvBlock kernel (mid_conv.cu)
+        # instead of gn_silu -> conv_gemm (-> ln_film)
+        fused = not self.keep and (narrow or (net.fuse_thin_levels and C in (32, 64) and not net.verify_fp32))
+        ss = self.ss_all[:, ip["ss_off"]:] if mod else None
+        (g1, be1), (g2, be2) = ip["gn1"], ip["gn2"]
+        h_stats = self.new_stats()
+        h = pool.get(Bh, Tl, C)
+        r = a1 = a2 = xn = None
+        if narrow or fused:
+            w1, w2 = (ip["w1"], ip["w2"]) if narrow else (ip["w1_raw"], ip["w2_raw"])
+            p1, p2 = (None, None) if narrow else (ip["w1_mid"], ip["w2_mid"])
+            add(lambda: ops.narrow_conv(x, h, x_stats, g1, be1, w1, ip["b1"], G, stats_out=h_stats,
+                                        gn_eps=net.GN_EPS, w_packed=p1))
+        if fused:               # the Modulation runs in conv2's epilogue
+            y = pool.get(Bh, Tl, C)
+            add(lambda: ops.narrow_conv(h, y, h_stats, g2, be2, w2, ip["b2"], G, residual=x, scale_shift=ss,
+                                        ss_stride=self.ss_stride, stats_out=y_stats, gn_eps=net.GN_EPS,
+                                        ln_eps=net.MOD_LN_EPS, w_packed=p2))
+        else:
+            r = pool.get(Bh, Tl, C)
+            y = pool.get(Bh, Tl, C) if mod else r
+            # use_modulation=False: the ResnetItem's output IS the item's output, so its
+            # GroupNorm statistics come out of conv2's epilogue
+            rs = None if mod else y_stats
+            if narrow:
+                add(lambda: ops.narrow_conv(h, r, h_stats, g2, be2, w2, ip["b2"], G, residual=x, stats_out=rs))
+            elif net.fuse_groupnorm and not self.keep:
+                # ConvBlock = ONE kernel: GroupNorm+SiLU applied to the smem A tile
+                add(lambda: ops.conv_gemm(x, ip["w1"], h, c_in=C, n_valid=C, taps=(-1, 0, 1), bias=ip["b1"],
+                                          stats=h_stats, groups=G, gn=(x_stats, g1, be1, G, net.GN_EPS)))
+                add(lambda: ops.conv_gemm(h, ip["w2"], r, c_in=C, n_valid=C, taps=(-1, 0, 1), bias=ip["b2"],
+                                          residual=x, stats=rs, groups=G, gn=(h_stats, g2, be2, G, net.GN_EPS)))
+            else:
+                a1 = pool.get(Bh, Tl, C)
+                add(lambda: ops.gn_silu(x, a1, x_stats, g1, be1, G, net.GN_EPS))
+                add(lambda: ops.conv_gemm(a1, ip["w1"], h, c_in=C, n_valid=C, taps=(-1, 0, 1), bias=ip["b1"],
+                                          stats=h_stats, groups=G))
+                pool.put(a1)
+                a2 = pool.get(Bh, Tl, C)
+                add(lambda: ops.gn_silu(h, a2, h_stats, g2, be2, G, net.GN_EPS))
+                add(lambda: ops.conv_gemm(a2, ip["w2"], r, c_in=C, n_valid=C, taps=(-1, 0, 1), bias=ip["b2"],
+                                          residual=x, stats=rs, groups=G))
+                pool.put(a2)
+            if mod:
+                xn = pool.get(Bh, Tl, C) if pre_norm else None
+                # Modulation and the following attention pre-norm in ONE pass over the rows
+                add(lambda: ops.ln_film(r, y, ss, self.ss_stride, y_stats, G, net.MOD_LN_EPS, y2=xn,
+                                        eps2=net.ATT_LN_EPS))
+                pool.put(r)
+        pool.put(h)
+        pool.put(x)             # a level's skip is the chain's *output*, never an item input
+        return dict(x=x, x_stats=x_stats, h=h, h_stats=h_stats, r=r, a1=a1, a2=a2, y=y, ss=ss, xn=xn)
+
+    def _inject(self, x: Tensor, jp: Dict, C: int, Tl: int, li: int, y_stats: Optional[Tensor]) -> Dict:
+        """InjectChannelsItem: conv1x1(cat([x, ctx])) + x as two accumulating GEMMs
+        (W = [W_x | W_c]): tmp = ctx W_c^T + b + x ; y = x W_x^T + tmp."""
+        pool, ctxb = self.pool, self.ctx[li]
+        tmp, y = pool.get(self.Bh, Tl, C), pool.get(self.Bh, Tl, C)
+        self.add(lambda: ops.conv_gemm(ctxb, jp["w_c"], tmp, c_in=ctxb.shape[-1], n_valid=C, bias=jp["b"],
+                                       residual=x))
+        self.add(lambda: ops.conv_gemm(x, jp["w_x"], y, c_in=C, n_valid=C, residual=tmp, stats=y_stats,
+                                       groups=self.G))
+        pool.put(tmp)
+        pool.put(x)
+        return dict(x=x, y=y, ctx=ctxb)
+
+    def _attention(self, x: Tensor, xn: Optional[Tensor], ap: Dict, cross: bool, C: int, Tl: int,
+                   y_stats: Optional[Tensor]) -> Dict:
+        """AttentionItem / CrossAttentionItem: y = x + to_out(softmax(q k^T / sqrt(D)) v) with
+        q, k, v projected from xn = LayerNorm(x) (affine folded into the projections); xn None:
+        the LayerNorm runs here."""
+        net, pool, add, Bh, mid, D = self.net, self.pool, self.add, self.Bh, self.mid, self.D
+        o, y = pool.get(Bh, Tl, mid), pool.get(Bh, Tl, C)
+        if xn is None:
+            xn = pool.get(Bh, Tl, C)
+            add(lambda: ops.ln_film(x, xn, None, 0, None, self.G, net.ATT_LN_EPS))
+        lse = torch.zeros(Bh, net.heads, Tl, device=x.device) if self.keep else None
+        qkv = kv = None
+        if not cross:
+            qkv = pool.get(Bh, Tl, 3 * mid)
+            q, k, v = qkv[..., :mid], qkv[..., mid:2 * mid], qkv[..., 2 * mid:]
+            add(lambda: ops.conv_gemm(xn, ap["w_qkv"], qkv, c_in=C, n_valid=3 * mid, bias=ap["b_qkv"]))
+        else:
+            # context K/V do not depend on x or sigma: in sampling mode they are projected ONCE per
+            # sample() call (plan.pre), not once per step
+            E, M = net.embedding_features, self.embedding.shape[1]
+            q = pool.get(Bh, Tl, mid)
+            if self.en is None:
+                self.en = torch.empty(Bh, M, E, dtype=pool.dtype, device=x.device)
+                self.add_ctx(lambda en=self.en: ops.ln_film(self.embedding, en, None, 0, None, self.G,
+                                                            net.ATT_LN_EPS))
+            en = self.en
+            kv = torch.empty(Bh, M, 2 * mid, dtype=pool.dtype, device=x.device)
+            k, v = kv[..., :mid], kv[..., mid:]
+            self.add_ctx(lambda: ops.conv_gemm(en, ap["w_kv"], kv, c_in=E, n_valid=2 * mid, bias=ap["b_kv"]))
+            add(lambda: ops.conv_gemm(xn, ap["w_q"], q, c_in=C, n_valid=mid, bias=ap["b_q"]))
+        add(lambda: ops.attention(q, k, v, o, net.heads, D ** -0.5, lse=lse, head_dim=D))
+        pool.put(q if cross else qkv)
+        add(lambda: ops.conv_gemm(o, ap["w_out"], y, c_in=mid, n_valid=C, residual=x, stats=y_stats,
+                                  groups=self.G))
+        pool.put(xn)
+        pool.put(o)
+        pool.put(x)
+        return dict(x=x, xn=xn, q=q, k=k, v=v, kv=kv, qkv=qkv, o=o, lse=lse, y=y)
+
+    def down(self, lv: "LevelParams", Lp: Dict, x_in: Tensor, Tl: int) -> Tuple[Tensor, Tensor]:
+        """Down conv of a level >= 1 (k = stride = factor over the [Bh, Tl, f*ci] view)."""
+        x, st, kdim = self.pool.get(self.Bh, Tl, lv.ch), self.new_stats(), lv.factor * lv.in_ch
+        self.add(lambda: ops.conv_gemm(x_in.view(self.Bh, Tl, kdim), Lp["down_w"], x, c_in=kdim, n_valid=lv.ch,
+                                       bias=Lp["down_b"], stats=st, groups=self.G))
+        return x, st
+
+    def up_merge(self, lv: "LevelParams", Lp: Dict, x: Tensor, x_in: Tensor, Tl: int, T_in: int):
+        """Up conv of a level >= 1's chain output x and its merge with the level input x_in:
+        MergeModulate's gate or SkipCat.  Returns (output, its statistics, y_up = the up conv's
+        own output, None when the gate runs in its epilogue)."""
+        pool, add, G, Bh, f, C, Co = self.pool, self.add, self.G, self.Bh, lv.factor, lv.ch, lv.out_ch
+        out, ost = pool.get(Bh, T_in, Co), self.new_stats()
+        gate = self.ss_all[:, Lp["gate_off"]:] if self.mod else None
+        geom = dict(up_factor=f) if f > 1 else dict(taps=(-1, 0, 1))
+
+        def phases(t):          # [Bh, T_in, Co] as the [Bh, Tl, f*Co] output of the upsample GEMM
+            return t.view(Bh, Tl, f * Co)
+        if self.mod and not self.keep:
+            add(lambda: ops.conv_gemm(x, Lp["up_w"], phases(out), c_in=C, n_valid=Co, bias=Lp["up_b"],
+                                      residual=phases(x_in), gate=gate, stats=ost, groups=G, **geom))
+            pool.put(x)
+            return out, ost, None
+        y_up, tmp = pool.get(Bh, T_in, Co), None
+        add(lambda: ops.conv_gemm(x, Lp["up_w"], phases(y_up), c_in=C, n_valid=Co, bias=Lp["up_b"], **geom))
+        if self.mod:
+            add(lambda: ops.skip_gate(y_up, x_in, gate, out, ost, G))
+        else:
+            # SkipCat: tmp = Wc1 (skip * s) + bc; out = Wc2 y_up + tmp.  The tensor-core GEMM needs
+            # K >= 16: an 8-channel level runs two positions per row against block-diagonal weights
+            rp = max(1, 16 // Co)
+            assert T_in % rp == 0, "SkipCat merge of an 8-channel level needs an even length"
+            tmp = pool.get(Bh, T_in, Co)
+
+            def rows(t):
+                return t.view(Bh, T_in // rp, rp * Co)
+            add(lambda: ops.conv_gemm(rows(x_in), Lp["cat_w1"], rows(tmp), c_in=rp * Co, n_valid=rp * Co,
+                                      bias=Lp["cat_b"]))
+            add(lambda: ops.conv_gemm(rows(y_up), Lp["cat_w2"], rows(out), c_in=rp * Co, n_valid=rp * Co,
+                                      residual=rows(tmp), stats=ost if rp == 1 else None, groups=G))
+            if rp > 1:           # the epilogue's group mapping does not see the paired layout
+                add(lambda: ops.gn_stats(out, ost, G))
+        for t in (y_up, tmp, x):
+            pool.put(t)
+        return out, ost, y_up
+
+
 class B200UNet(nn.Module):
     """See module docstring.  Reference parity notes per block are in include/adp_b200.h."""
 
@@ -393,11 +628,7 @@ class B200UNet(nn.Module):
             return
         if self._repack_graph is None:
             _copy_tree(self._packed, self._compute_packed())       # eager once: allocator warm
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                _copy_tree(self._packed, self._compute_packed())
-            self._repack_graph = g
+            self._repack_graph = _capture(lambda: _copy_tree(self._packed, self._compute_packed()))
         else:
             self._repack_graph.replay()
 
@@ -601,7 +832,6 @@ class B200UNet(nn.Module):
         dev = self.net.down.weight.device
         P = self.packed()
         plan = _Plan()
-        pool = _Pool(dev, reuse=True, dtype=self._act_dtype())
         G, Fm = self.groups, self.features
         levels = self.levels()
         total_f = 1
@@ -622,20 +852,11 @@ class B200UNet(nn.Module):
         plan.ctx = {i: torch.zeros(Bh, (T // _prod(self.factors[:i + 1])), ops.round_up(c, 16),
                                    dtype=adt, device=dev)
                     for i, c in enumerate(self.context_channels) if c > 0}
-        plan.en = None                       # LayerNorm(embedding), shared by all cross-attentions
         plan.pre = []                        # step-invariant launches of a sampling plan
-        add_ctx = plan.pre.append if mode == "sample" else plan.add
 
         # ---- statistics arena (zeroed once per forward)
         n_slots = 2 + sum(3 * (len(lv.items_down) + len(lv.items_up)) + 3 for lv in levels)
         arena = torch.zeros(n_slots, Bh, G, 2, dtype=torch.float64, device=dev)
-        slot_i = [0]
-
-        def new_stats() -> Tensor:
-            s = arena[slot_i[0]]
-            slot_i[0] += 1
-            return s
-
         if mode == "sample":
             # the step's conditioning rows and alpha/beta are picked ON THE DEVICE from tables by a
             # step counter, so the captured graph is identical for every step (the host only
@@ -659,228 +880,53 @@ class B200UNet(nn.Module):
         else:
             ss_all = torch.zeros(Bh, 8, device=dev)
             plan.use_features_in = False
-        ss_stride = ss_all.shape[1]
-        mod = self.use_modulation
-
-        # ---- one item chain
-        def run_items(x: Tensor, x_stats: Tensor, items_p: List[Dict], lv: LevelParams, Tl: int,
-                      last_needs_stats: bool, li: int = 0) -> Tuple[Tensor, Optional[Tensor]]:
-            C = lv.ch
-            narrow = C == 8 and not self._verify_fp32
-            # thin levels (C = 32, 64) are HBM-bound: one fused ConvBlock kernel (mid_conv.cu)
-            # instead of gn_silu -> conv_gemm (-> ln_film)
-            thin = narrow or (self.fuse_thin_levels and C in (32, 64) and not self._verify_fp32)
-            for idx, ip in enumerate(items_p):
-                ss = ss_all[:, ip["ss_off"]:] if mod else None
-                has_att, has_cross, has_inj = "att" in ip, "cross" in ip, "inj" in ip
-                item_last = idx == len(items_p) - 1
-                want_stats = (not item_last) or last_needs_stats
-                mod_stats = new_stats() if (want_stats and not (has_att or has_cross or has_inj)) else None
-                h_stats = new_stats()
-                if thin:
-                    h = pool.get(Bh, Tl, C)
-                    y = pool.get(Bh, Tl, C)
-                    w1, w2 = (ip["w1"], ip["w2"]) if narrow else (ip["w1_raw"], ip["w2_raw"])
-                    p1, p2 = (None, None) if narrow else (ip["w1_mid"], ip["w2_mid"])
-                    plan.add(lambda x=x, h=h, s=x_stats, hs=h_stats, ip=ip, w1=w1, p1=p1: ops.narrow_conv(
-                        x, h, s, ip["gn1"][0], ip["gn1"][1], w1, ip["b1"], G, stats_out=hs,
-                        gn_eps=self.GN_EPS, w_packed=p1))
-                    plan.add(lambda x=x, h=h, y=y, hs=h_stats, ms=mod_stats, ip=ip, ss=ss, w2=w2, p2=p2:
-                             ops.narrow_conv(h, y, hs, ip["gn2"][0], ip["gn2"][1], w2, ip["b2"], G,
-                                             residual=x, scale_shift=ss, ss_stride=ss_stride, stats_out=ms,
-                                             gn_eps=self.GN_EPS, ln_eps=self.MOD_LN_EPS, w_packed=p2))
-                    pool.put(h)
-                else:
-                    h = pool.get(Bh, Tl, C)
-                    r = pool.get(Bh, Tl, C)
-                    y = pool.get(Bh, Tl, C) if mod else None
-                    # use_modulation=False: the ResnetItem's output IS the item's output, so its
-                    # GroupNorm statistics come out of conv2's epilogue
-                    rs = None if mod else mod_stats
-                    if self.fuse_groupnorm:
-                        # ConvBlock = ONE kernel: GroupNorm+SiLU applied to the smem A tile
-                        plan.add(lambda x=x, h=h, s=x_stats, hs=h_stats, ip=ip: ops.conv_gemm(
-                            x, ip["w1"], h, c_in=C, n_valid=C, taps=(-1, 0, 1), bias=ip["b1"], stats=hs,
-                            groups=G, gn=(s, ip["gn1"][0], ip["gn1"][1], G, self.GN_EPS)))
-                        plan.add(lambda x=x, h=h, r=r, hs=h_stats, ip=ip, rs=rs: ops.conv_gemm(
-                            h, ip["w2"], r, c_in=C, n_valid=C, taps=(-1, 0, 1), bias=ip["b2"], residual=x,
-                            stats=rs, groups=G, gn=(hs, ip["gn2"][0], ip["gn2"][1], G, self.GN_EPS)))
-                    else:
-                        a = pool.get(Bh, Tl, C)
-                        plan.add(lambda x=x, a=a, s=x_stats, ip=ip: ops.gn_silu(
-                            x, a, s, ip["gn1"][0], ip["gn1"][1], G, self.GN_EPS))
-                        plan.add(lambda a=a, h=h, hs=h_stats, ip=ip: ops.conv_gemm(
-                            a, ip["w1"], h, c_in=C, n_valid=C, taps=(-1, 0, 1), bias=ip["b1"], stats=hs,
-                            groups=G))
-                        plan.add(lambda a=a, h=h, hs=h_stats, ip=ip: ops.gn_silu(
-                            h, a, hs, ip["gn2"][0], ip["gn2"][1], G, self.GN_EPS))
-                        plan.add(lambda x=x, a=a, r=r, ip=ip, rs=rs: ops.conv_gemm(
-                            a, ip["w2"], r, c_in=C, n_valid=C, taps=(-1, 0, 1), bias=ip["b2"], residual=x,
-                            stats=rs, groups=G))
-                        pool.put(a)
-                    xn_first = pool.get(Bh, Tl, C) if ((has_att or has_cross) and not has_inj and mod) else None
-                    if mod:
-                        # Modulation and the following attention pre-norm in ONE pass over the rows
-                        plan.add(lambda r=r, y=y, ss=ss, ms=mod_stats, xn=xn_first: ops.ln_film(
-                            r, y, ss, ss_stride, ms, G, self.MOD_LN_EPS, y2=xn, eps2=self.ATT_LN_EPS))
-                        pool.put(r)
-                    else:
-                        y = r
-                    pool.put(h)
-                # the item's input is dead now (a level's skip is the chain's *output*)
-                pool.put(x)
-                x, x_stats = y, mod_stats
-                if has_inj:
-                    # InjectChannelsItem: conv1x1(cat([x, ctx])) + x as two accumulating GEMMs
-                    # (W = [W_x | W_c]): tmp = ctx W_c^T + b + x ; out = x W_x^T + tmp
-                    jp = ip["inj"]
-                    ctxb = plan.ctx[li]
-                    tmp, out_i = pool.get(Bh, Tl, C), pool.get(Bh, Tl, C)
-                    inj_stats = new_stats() if (want_stats and not (has_att or has_cross)) else None
-                    plan.add(lambda ctxb=ctxb, jp=jp, tmp=tmp, x=x: ops.conv_gemm(
-                        ctxb, jp["w_c"], tmp, c_in=ctxb.shape[-1], n_valid=C, bias=jp["b"], residual=x))
-                    plan.add(lambda x=x, jp=jp, tmp=tmp, o=out_i, st=inj_stats: ops.conv_gemm(
-                        x, jp["w_x"], o, c_in=C, n_valid=C, residual=tmp, stats=st, groups=G))
-                    pool.put(tmp)
-                    pool.put(x)
-                    x, x_stats = out_i, inj_stats
-                D = self.head_features or 64
-                mid = (self.heads or 0) * D
-                for kind in ("att", "cross"):
-                    if kind not in ip:
-                        continue
-                    ap = ip[kind]
-                    is_last_att = kind == "cross" or not has_cross
-                    out_stats = new_stats() if (want_stats and is_last_att) else None
-                    o = pool.get(Bh, Tl, mid)
-                    y2 = pool.get(Bh, Tl, C)
-                    if not thin and xn_first is not None:
-                        xn, xn_first = xn_first, None      # produced by the fused Modulation pass
-                    else:
-                        xn = pool.get(Bh, Tl, C)
-                        plan.add(lambda x=x, xn=xn: ops.ln_film(x, xn, None, 0, None, G, self.ATT_LN_EPS))
-                    if kind == "att":
-                        qkv = pool.get(Bh, Tl, 3 * mid)
-                        plan.add(lambda xn=xn, qkv=qkv, ap=ap: ops.conv_gemm(
-                            xn, ap["w_qkv"], qkv, c_in=C, n_valid=3 * mid, bias=ap["b_qkv"]))
-                        plan.add(lambda qkv=qkv, o=o, D=D: ops.attention(
-                            qkv[..., :mid], qkv[..., mid:2 * mid], qkv[..., 2 * mid:], o, self.heads,
-                            D ** -0.5, head_dim=D))
-                        pool.put(qkv)
-                    else:
-                        # context K/V do not depend on x or sigma: in sampling mode they are
-                        # projected ONCE per sample() call (plan.pre), not once per step
-                        E = self.embedding_features
-                        q = pool.get(Bh, Tl, mid)
-                        if plan.en is None:
-                            plan.en = torch.empty(Bh, M, E, dtype=adt, device=dev)
-                            add_ctx(lambda: ops.ln_film(plan.embedding, plan.en, None, 0, None, G,
-                                                        self.ATT_LN_EPS))
-                        kv = torch.empty(Bh, M, 2 * mid, dtype=adt, device=dev)
-                        add_ctx(lambda kv=kv, ap=ap: ops.conv_gemm(
-                            plan.en, ap["w_kv"], kv, c_in=E, n_valid=2 * mid, bias=ap["b_kv"]))
-                        plan.add(lambda xn=xn, q=q, ap=ap: ops.conv_gemm(
-                            xn, ap["w_q"], q, c_in=C, n_valid=mid, bias=ap["b_q"]))
-                        plan.add(lambda q=q, kv=kv, o=o, D=D: ops.attention(
-                            q, kv[..., :mid], kv[..., mid:], o, self.heads, D ** -0.5, head_dim=D))
-                        pool.put(q)
-                    plan.add(lambda o=o, y2=y2, x=x, ap=ap, os_=out_stats: ops.conv_gemm(
-                        o, ap["w_out"], y2, c_in=mid, n_valid=C, residual=x, stats=os_, groups=G))
-                    pool.put(xn)
-                    pool.put(o)
-                    pool.put(x)
-                    x, x_stats = y2, out_stats
-            return x, x_stats
+        walk = _ForwardWalk(self, P, plan.add, Bh, arena, ss_all, keep=False, ctx=plan.ctx,
+                            embedding=plan.embedding,
+                            add_ctx=plan.pre.append if mode == "sample" else plan.add)
+        pool = walk.pool
 
         # ---- recursive level walk
         def run_level(i: int, x_in: Optional[Tensor], T_in: int) -> Tuple[Tensor, Optional[Tensor]]:
-            """Returns the level's output [Bh, T_in, out_ch] (+ its stats) for i >= 1;
-            level 0 writes plan.v / x_next itself."""
+            """Returns the level's output [Bh, T_in, out_ch] (+ its stats) for i >= 1 and the
+            output of level 0's item chain (the input of stem_out) for i = 0."""
             lv, Lp = levels[i], P["levels"][i]
             Tl = T_in // lv.factor
-            C = lv.ch
             innermost = i == len(levels) - 1
-            x = pool.get(Bh, Tl, C)
-            st = new_stats()
             if i == 0:
+                x, st = pool.get(Bh, Tl, lv.ch), walk.new_stats()
                 for half in range(Bh // B):
                     plan.add(lambda half=half, x=x, st=st: ops.stem_in(
                         plan.x, Lp["down_w"], Lp["down_b"], x[half * B:(half + 1) * B], lv.factor,
                         append=plan.append, stats=st[half * B:(half + 1) * B], groups=G))
             else:
-                plan.add(lambda x=x, st=st: ops.conv_gemm(
-                    x_in.view(Bh, Tl, lv.factor * lv.in_ch), Lp["down_w"], x, c_in=lv.factor * lv.in_ch,
-                    n_valid=C, bias=Lp["down_b"], stats=st, groups=G))
-            x, st = run_items(x, st, Lp["items_down"], lv, Tl, last_needs_stats=innermost, li=i)
+                x, st = walk.down(lv, Lp, x_in, Tl)
+            x, st, _ = walk.items(x, st, Lp["items_down"], lv.ch, Tl, i, last_needs_stats=innermost)
             if not innermost:
                 skip = x
                 x, st = run_level(i + 1, skip, Tl)
                 pool.put(skip)
-            x, st = run_items(x, st, Lp["items_up"], lv, Tl, last_needs_stats=False, li=i)
-            gate = ss_all[:, Lp["gate_off"]:] if mod else None
+            x, st, _ = walk.items(x, st, Lp["items_up"], lv.ch, Tl, i, last_needs_stats=False)
             if i == 0:
-                plan.h0 = x
-                plan.gate0 = gate if mod else torch.ones(Bh, 8, device=dev)
-                plan.level0 = (lv, Lp)
                 return x, None
-            out = pool.get(Bh, T_in, lv.out_ch)
-            ost = new_stats()
-            if not mod:
-                # SkipCat: y = upsample conv (+ bias); tmp = Wc1 (skip * s) + bc; out = Wc2 y + tmp
-                Co = lv.out_ch
-                rr = max(1, 16 // Co)
-                assert T_in % rr == 0, "SkipCat merge of an 8-channel level needs an even length"
-                y_up, tmp = pool.get(Bh, T_in, Co), pool.get(Bh, T_in, Co)
-
-                def rows(t, rr=rr, Co=Co):
-                    return t.view(Bh, T_in // rr, rr * Co)
-                if lv.factor > 1:
-                    plan.add(lambda x=x, y_up=y_up: ops.conv_gemm(
-                        x, Lp["up_w"], y_up.view(Bh, Tl, lv.factor * lv.out_ch), c_in=C, n_valid=lv.out_ch,
-                        up_factor=lv.factor, bias=Lp["up_b"]))
-                else:
-                    plan.add(lambda x=x, y_up=y_up: ops.conv_gemm(
-                        x, Lp["up_w"], y_up, c_in=C, n_valid=lv.out_ch, taps=(-1, 0, 1), bias=Lp["up_b"]))
-                plan.add(lambda tmp=tmp: ops.conv_gemm(rows(x_in), Lp["cat_w1"], rows(tmp), c_in=rr * Co,
-                                                      n_valid=rr * Co, bias=Lp["cat_b"]))
-                plan.add(lambda y_up=y_up, tmp=tmp, out=out, ost=ost: ops.conv_gemm(
-                    rows(y_up), Lp["cat_w2"], rows(out), c_in=rr * Co, n_valid=rr * Co, residual=rows(tmp),
-                    stats=ost if rr == 1 else None, groups=G))
-                if rr > 1:           # the epilogue's group mapping does not see the paired layout
-                    plan.add(lambda out=out, ost=ost: ops.gn_stats(out, ost, G))
-                pool.put(y_up)
-                pool.put(tmp)
-                pool.put(x)
-                return out, ost
-            if lv.factor > 1:
-                plan.add(lambda x=x, out=out, ost=ost: ops.conv_gemm(
-                    x, Lp["up_w"], out.view(Bh, Tl, lv.factor * lv.out_ch), c_in=C, n_valid=lv.out_ch,
-                    up_factor=lv.factor, bias=Lp["up_b"], residual=x_in.view(Bh, Tl, lv.factor * lv.out_ch),
-                    gate=gate, stats=ost, groups=G))
-            else:
-                plan.add(lambda x=x, out=out, ost=ost: ops.conv_gemm(
-                    x, Lp["up_w"], out, c_in=C, n_valid=lv.out_ch, taps=(-1, 0, 1), bias=Lp["up_b"],
-                    residual=x_in, gate=gate, stats=ost, groups=G))
-            pool.put(x)
+            out, ost, _ = walk.up_merge(lv, Lp, x, x_in, Tl, T_in)
             return out, ost
 
-        run_level(0, None, T)
-        lv0, L0 = plan.level0
+        h0, _ = run_level(0, None, T)
+        lv0, L0 = levels[0], P["levels"][0]
+        gate0 = ss_all[:, L0["gate_off"]:] if self.use_modulation else torch.ones(Bh, 8, device=dev)
 
         def final():
             kw = dict(append=plan.append, w_adapt=L0.get("adapt_w"), b_adapt=L0.get("adapt_b"),
                       cfg_scale=plan.cfg_scale)
             if mode == "sample":   # v and the VSampler update in one pass; x advanced in place
-                ops.stem_out(plan.h0, plan.x, L0["up_w"], L0["up_b"], plan.gate0, lv0.factor,
-                             x_next=plan.x, ab=plan.ab, **kw)
+                ops.stem_out(h0, plan.x, L0["up_w"], L0["up_b"], gate0, lv0.factor, x_next=plan.x, ab=plan.ab,
+                             **kw)
             else:
-                ops.stem_out(plan.h0, plan.x, L0["up_w"], L0["up_b"], plan.gate0, lv0.factor,
-                             v_out=plan.v, **kw)
+                ops.stem_out(h0, plan.x, L0["up_w"], L0["up_b"], gate0, lv0.factor, v_out=plan.v, **kw)
         plan.add(final)
         if mode == "sample":
             plan.add(lambda: ops.step_advance(plan.step))
         plan.workspace_bytes = pool.total_bytes
-        assert slot_i[0] <= n_slots
         return plan
 
     def _plan(self, B: int, T: int, Bh: int, M: int, mode: str, baked: Tuple = ()) -> _Plan:
@@ -918,18 +964,8 @@ class B200UNet(nn.Module):
                 plan.run_eager()
             plan.n_kernels = len(tr.records)
         else:
-            g = torch.cuda.CUDAGraph()
-            torch.cuda.synchronize()
-            # inside the captured graph no kernel writes the packed weights, so the GEMMs may
-            # fetch them before their programmatic-dependency wait (conv_gemm.cu, early_w)
-            _lib.lib().adp_debug_set(2, 1)
-            try:
-                with torch.cuda.graph(g):
-                    plan.run_eager()
-            finally:
-                _lib.lib().adp_debug_set(2, 0)
-            plan.graph = g
-            g.replay()
+            plan.graph = _capture(plan.run_eager, early_weights=True)
+            plan.graph.replay()
         plan.runs += 1
 
     def _execute_steps(self, plan: _Plan, n: int) -> None:
@@ -941,16 +977,10 @@ class B200UNet(nn.Module):
         while n > 0:
             if (self.use_cuda_graph and S > 1 and n >= S and plan.graph is not None):
                 if plan.multi_graph is None or plan.multi_steps != S:
-                    g = torch.cuda.CUDAGraph()
-                    torch.cuda.synchronize()
-                    _lib.lib().adp_debug_set(2, 1)
-                    try:
-                        with torch.cuda.graph(g):
-                            for _ in range(S):
-                                plan.run_eager()
-                    finally:
-                        _lib.lib().adp_debug_set(2, 0)
-                    plan.multi_graph, plan.multi_steps = g, S
+                    def steps():
+                        for _ in range(S):
+                            plan.run_eager()
+                    plan.multi_graph, plan.multi_steps = _capture(steps, early_weights=True), S
                 plan.multi_graph.replay()
                 plan.runs += S
                 n -= S
