@@ -1,0 +1,805 @@
+"""Checks every kernel launch of a real program against an fp64 restatement of what it computes.
+
+`Shadow` replaces the launch functions of `ops` (as tests/test_launch_programs_cpu.py's Recorder
+does) by wrappers that, around each launch, synchronise, snapshot every storage the arguments
+touch, run the real kernel (or, with `fake=True`, write the restatement itself, so whole programs
+run on the CPU), and then compare everything the launch wrote with an fp64 reference computed from
+the snapshot -- the exact inputs the kernel saw, with the real buffer aliasing (`residual is out`,
+`stem_out(x_next=plan.x)`).  Errors do not carry from launch to launch, so every kernel is held to
+its own bound at the shape and on the activations the program gives it.
+
+Bounds (err = |got - ref| element-wise, `absref` = the same operation applied to absolute
+values: conv of |a| with |w|, P |V|, ...):
+    bf16 outputs   err <= 2^-7 |ref| + tau absref
+                   tau = 2^-8 where the kernel rounds an internal operand to bf16 (the GroupNorm +
+                   SiLU A operand of the fused conv GEMM and of narrow_conv, attention's P),
+                   tau = 2^-12 elsewhere
+    fp32 outputs   err <= 1e-5 |ref| + 2^-14 absref
+    statistics     the launch's contribution (after - before) against stats_of() of the kernel's
+                   own rounded output, within 1e-4 of sum|x| and sum x^2; the variance the
+                   consumers derive, E[x^2] - mean^2, within 1e-3 (var + 1e-5) of a two-pass fp64
+                   variance (GroupNorm normalises by sqrt(var + 1e-5); the plain relative error
+                   of the variance is recorded as `.var_rel`, unbounded: a single-pass variance
+                   of a near-constant group, var << mean^2, keeps only a few digits)
+    copies         bitwise
+Every launch also checks that read-only arguments are bitwise unchanged and that no byte of a
+written tensor's storage outside the written view changed.
+
+Checked kinds are the launches of the inference and sampling programs; the training backward
+and the vocoder / sampler front-end launches are listed in UNCHECKED, and a program that reaches
+one of them under Shadow fails instead of passing unchecked.
+"""
+import inspect
+import math
+from typing import Callable, Dict, FrozenSet, List, Tuple
+
+import torch
+
+from audio_diffusion_pytorch_b200 import ops
+
+F64 = torch.float64
+TAU_BF16_OPERAND = 2.0 ** -8
+TAU_FP32_ACC = 2.0 ** -12
+BF16_REL = 2.0 ** -7
+FP32_REL, FP32_TAU = 1e-5, 2.0 ** -14
+STATS_TOL = 1e-4
+VAR_TOL = 1e-3
+GN_EPS = 1e-5                    # every statistics slot feeds a GroupNorm: it divides by sqrt(var + eps)
+ROW_TILE = 64                    # rows left stale by the mutation: half the conv GEMM's 128-row M tile
+
+UNCHECKED = {
+    # training backward (training.py's plans)
+    "wgrad": "training backward", "gn_silu_bwd": "training backward",
+    "gn_bwd_apply": "training backward", "ln_film_bwd": "training backward",
+    "colsum": "training backward", "skip_gate_bwd": "training backward",
+    "cond_bwd": "training backward", "narrow_conv_bwd": "training backward",
+    "stem_out_bwd": "training backward", "stem_in_bwd": "training backward",
+    "attention_bwd": "training backward", "ln_fold_bwd": "training backward",
+    "to_flat_bwd": "training backward",
+    # inference launches outside the sampling programs of UNetV0
+    "skip_gate": "keep=True plans and use_modulation=False nets only",
+    "fir_resample": "vocoder / upsampler front-end", "mel_spectrogram": "vocoder front-end",
+    "to_flat": "vocoder front-end", "inpaint_blend": "VInpainter loop", "arv_step": "ARVSampler loop",
+}
+
+
+class CheckError(AssertionError):
+    pass
+
+
+def launching_functions() -> List[str]:
+    """Every function of `ops` that launches a kernel (calls ops._launch)."""
+    out = []
+    for name, fn in inspect.getmembers(ops, inspect.isfunction):
+        if fn.__module__ == ops.__name__ and not name.startswith("_") and "_launch(" in inspect.getsource(fn):
+            out.append(name)
+    return sorted(out)
+
+
+# ------------------------------------------------------------------------------ outputs
+class Val:
+    """A stored output: `view(args)` is the written view; ref / absref fp64 of its shape (or a
+    callable(post args) -> (ref, absref) when the reference reads another output of the launch)."""
+
+    def __init__(self, name, view, ref, absref=None, tau=TAU_FP32_ACC, exact=False):
+        self.name, self.view, self.ref, self.absref, self.tau, self.exact = name, view, ref, absref, tau, exact
+        self.acc = False
+
+
+class Stat:
+    """fp64 GroupNorm statistics [B, G, 2] accumulated (+=) by the launch over src(post args)."""
+
+    def __init__(self, name, view, src, groups):
+        self.name, self.view, self.src, self.groups = name, view, src, groups
+        self.acc = True
+
+
+def arg(name):
+    return lambda a: a[name]
+
+
+def stats_of(y: torch.Tensor, groups: int) -> torch.Tensor:
+    """(sum, sumsq) per (batch, group) of a channels-last tensor [B, T, C], fp64."""
+    B, T, Cc = y.shape
+    yg = y.to(F64).reshape(B, T, groups, Cc // groups)
+    return torch.stack([yg.sum(dim=(1, 3)), (yg * yg).sum(dim=(1, 3))], dim=-1)
+
+
+def _silu(x):
+    return x * torch.sigmoid(x)
+
+
+def _gelu(x):
+    return 0.5 * x * (1.0 + torch.erf(x / math.sqrt(2.0)))
+
+
+def _gn_coef(stats, gamma, beta, groups, eps, T, C):
+    """(scale, shift) [B, 1, C] of GroupNorm from the statistics slots the kernel reads."""
+    st = stats.to(F64)
+    n = float(T * (C // groups))
+    mean = st[..., 0] / n
+    var = (st[..., 1] / n - mean * mean).clamp_min(0.0)
+    rep = C // groups
+    mean, var = mean.repeat_interleave(rep, dim=1), var.repeat_interleave(rep, dim=1)
+    ga = gamma.to(F64)[None] / torch.sqrt(var + eps)
+    return ga[:, None, :], (beta.to(F64)[None] - mean * ga)[:, None, :]
+
+
+def _conv3(a, w3, bias=None):
+    """a [T, Ci] fp64, w3 [3, Co, Ci] (tap -1, 0, +1), zero padding -> [T, Co]."""
+    T = a.shape[0]
+    z = a.new_zeros(1, a.shape[1])
+    ap = torch.cat([z, a, z])
+    out = ap[0:T] @ w3[0].t() + ap[1:T + 1] @ w3[1].t() + ap[2:T + 2] @ w3[2].t()
+    return out if bias is None else out + bias
+
+
+def _layer_norm(x, eps):
+    """(LayerNorm(x), its std, its absref (|x| + mean|x|) / std): the centring cancels, so an
+    output's rounding error scales with the row's magnitude, not with the output itself."""
+    mean = x.mean(-1, keepdim=True)
+    var = ((x - mean) ** 2).mean(-1, keepdim=True)
+    std = torch.sqrt(var + eps)
+    return (x - mean) / std, std, (x.abs() + x.abs().mean(-1, keepdim=True)) / std
+
+
+# ----------------------------------------------------------------------------- checkers
+def c_conv_gemm(a, ctx):
+    x, w, out = a["a"], a["w"], a["out"]
+    assert x.dtype == torch.bfloat16, "the fp32 verification mode is not checked here"
+    B, T, _ = x.shape
+    c_in, n_valid, taps, up = a["c_in"], a["n_valid"], tuple(a["taps"]), a["up_factor"]
+    phases = up if up > 1 else 1
+    n_pad = w.shape[0] // phases
+    W = w.to(F64).reshape(phases, n_pad, w.shape[1])[:, :n_valid]
+    xa = x[..., :c_in].to(F64)
+    tau = TAU_FP32_ACC
+    if a["gn"] is not None:
+        gst, gg, gb, gG, geps = a["gn"]
+        sc, sh = _gn_coef(gst, gg, gb, gG, geps, T, c_in)
+        xa = _silu(xa * sc + sh)
+        tau = TAU_BF16_OPERAND
+    bias = a["bias"].to(F64)[:n_valid] if a["bias"] is not None else None
+    gate = a["gate"].to(F64)[:, :n_valid][:, None, None, :] if a["gate"] is not None else None
+
+    def shifted(t, off):
+        if off == 0:
+            return t
+        z = t.new_zeros(t.shape[0], abs(off), t.shape[2])
+        return torch.cat([t[:, off:], z], 1) if off > 0 else torch.cat([z, t[:, :off]], 1)
+
+    ref = xa.new_zeros(B, T, phases, n_valid)
+    absr = torch.zeros_like(ref)
+    xabs = xa.abs()
+    Wabs = W.abs()
+    for p in range(phases):
+        if up > 1:
+            offs = (-1, 0) if p == 0 else ((0, 1) if p == up - 1 else (0,))
+        else:
+            offs = taps
+        for j, off in enumerate(offs):
+            Wt, Wa = W[p, :, j * c_in:(j + 1) * c_in], Wabs[p, :, j * c_in:(j + 1) * c_in]
+            ref[:, :, p] += shifted(xa, off) @ Wt.t()
+            absr[:, :, p] += shifted(xabs, off) @ Wa.t()
+    if bias is not None:
+        ref += bias
+        absr += bias.abs()
+    if gate is not None:
+        ref *= gate
+        absr *= gate.abs()
+    if a["residual"] is not None and out.dtype != torch.float32:
+        r = a["residual"][..., :phases * n_valid].to(F64).reshape(B, T, phases, n_valid)
+        ref += r
+        absr += r.abs()
+    ncols = phases * n_valid
+
+    def view(args):
+        return args["out"][..., :ncols]
+    outs = [Val("out", view, ref.reshape(B, T, ncols), absr.reshape(B, T, ncols), tau)]
+    if a["stats"] is not None:
+        outs.append(Stat("stats", arg("stats"),
+                         lambda p: p["out"][..., :ncols].reshape(B, T * phases, n_valid), a["groups"]))
+    return outs
+
+
+def c_gn_silu(a, ctx):
+    x = a["x"]
+    B, T, C = x.shape
+    sc, sh = _gn_coef(a["stats"], a["gamma"], a["beta"], a["groups"], a["eps"], T, C)
+    z = x.to(F64) * sc + sh
+    return [Val("y", arg("y"), _silu(z), 1.2 * ((x.to(F64) * sc).abs() + sh.abs()))]
+
+
+def c_gn_stats(a, ctx):
+    return [Stat("stats", arg("stats"), arg("x"), a["groups"])]
+
+
+def c_ln_film(a, ctx):
+    x = a["x"]
+    B, T, C = x.shape
+    xn, _, lnabs = _layer_norm(x.to(F64), a["eps"])
+    ref, absr = xn, lnabs
+    if a["scale_shift"] is not None:
+        ss = a["scale_shift"].to(F64)
+        s, t = ss[:, None, :C], ss[:, None, C:2 * C]
+        ref, absr = xn * (1 + s) + t, lnabs * (1 + s).abs() + t.abs()
+    outs = [Val("y", arg("y"), ref, absr)]
+    if a["y2"] is not None:
+        def ref2(p, eps2=a["eps2"]):
+            y2, _, y2abs = _layer_norm(p["y"].to(F64), eps2)
+            return y2, y2abs
+        outs.append(Val("y2", arg("y2"), ref2))
+    if a["stats_out"] is not None:
+        outs.append(Stat("stats_out", arg("stats_out"), arg("y"), a["groups"]))
+    return outs
+
+
+def c_attention(a, ctx):
+    q, k, v = a["q"], a["k"], a["v"]
+    H, D, scale = a["heads"], a["head_dim"], a["scale"]
+    B, Tq, Tk, mid = q.shape[0], q.shape[1], k.shape[1], a["heads"] * a["head_dim"]
+    ref = torch.empty(B, Tq, mid, dtype=F64, device=q.device)
+    absr = torch.empty_like(ref)
+    lse = torch.empty(B, H, Tq, dtype=F64, device=q.device) if a["lse"] is not None else None
+    lse_abs = torch.empty_like(lse) if lse is not None else None
+    for b in range(B):                 # one batch element at a time: S is [H, Tq, Tk] in fp64
+        Q = q[b, :, :mid].to(F64).reshape(Tq, H, D).transpose(0, 1)
+        K = k[b, :, :mid].to(F64).reshape(Tk, H, D).transpose(0, 1)
+        V = v[b, :, :mid].to(F64).reshape(Tk, H, D).transpose(0, 1)
+        S = (Q @ K.transpose(1, 2)) * scale
+        P = torch.softmax(S, dim=-1)
+        ref[b] = (P @ V).transpose(0, 1).reshape(Tq, mid)
+        absr[b] = (P @ V.abs()).transpose(0, 1).reshape(Tq, mid)
+        if lse is not None:
+            lse[b] = torch.logsumexp(S, dim=-1)
+            lse_abs[b] = S.abs().amax(-1)
+    outs = [Val("o", lambda p: p["o"][..., :mid], ref, absr, TAU_BF16_OPERAND)]
+    if lse is not None:
+        outs.append(Val("lse", arg("lse"), lse, lse_abs))
+    return outs
+
+
+def c_skinny_linear(a, ctx):
+    x, w, K, N = a["x"], a["w"], a["K"], a["N"]
+    acts = {ops.ACT_NONE: (lambda t: t, 1.0), ops.ACT_GELU: (_gelu, 1.2), ops.ACT_SILU: (_silu, 1.2)}
+    fin, gin = acts[a["in_act"]]
+    fout, gout = acts[a["out_act"]]
+    xi = fin(x[:, :K].to(F64))
+    W = w[:N, :K].to(F64)
+    pre = xi @ W.t()
+    absr = xi.abs() @ W.abs().t()
+    if a["bias"] is not None:
+        pre = pre + a["bias"].to(F64)[:N]
+        absr = absr + a["bias"].to(F64)[:N].abs()
+    return [Val("y", lambda p: p["y"][:, :N], fout(pre), gout * absr)]
+
+
+def c_time_features(a, ctx):
+    s, fr, out = a["sigma"].to(F64), a["freqs"].to(F64), a["out"]
+    B, nf = s.shape[0], fr.shape[0]
+    arg_ = s[:, None] * fr[None] * (2 * math.pi)
+    ref = torch.zeros(B, out.shape[1], dtype=F64, device=out.device)
+    absr = torch.zeros_like(ref)
+    ref[:, 0], absr[:, 0] = s, s.abs()
+    ref[:, 1:1 + nf], ref[:, 1 + nf:1 + 2 * nf] = arg_.sin(), arg_.cos()
+    absr[:, 1:1 + nf] = absr[:, 1 + nf:1 + 2 * nf] = arg_.abs()
+    return [Val("out", lambda p: p["out"][:B], ref, absr)]
+
+
+def c_silu_bf16(a, ctx):
+    x = a["x"].to(F64)
+    return [Val("y", arg("y"), _silu(x).reshape(a["y"].shape), 1.2 * x.abs().reshape(a["y"].shape))]
+
+
+def _stem_input(a):
+    """cat([alpha x + beta noise, append]) fp64 [B, cin, T] (VDiffusion noising in the stems)."""
+    x = a["x"].to(F64)
+    if a["noise"] is not None:
+        x = a["alpha"].to(F64)[:, None, None] * x + a["beta"].to(F64)[:, None, None] * a["noise"].to(F64)
+    if a["append"] is not None:
+        x = torch.cat([x, a["append"].to(F64)], dim=1)
+    return x
+
+
+def c_stem_in(a, ctx):
+    xin, w, f = _stem_input(a), a["w"].to(F64), a["f"]
+    B, cin, T = xin.shape
+    c0 = w.shape[0]
+    xr = xin.reshape(B, cin, T // f, f).permute(0, 2, 1, 3).reshape(B, T // f, cin * f)
+    Wm = w.reshape(c0, cin * f)
+    ref, absr = xr @ Wm.t(), xr.abs() @ Wm.abs().t()
+    if a["bias"] is not None:
+        ref, absr = ref + a["bias"].to(F64), absr + a["bias"].to(F64).abs()
+    outs = [Val("out", arg("out"), ref, absr)]
+    if a["stats"] is not None:
+        outs.append(Stat("stats", arg("stats"), arg("out"), a["groups"]))
+    return outs
+
+
+def c_stem_out(a, ctx):
+    if a["loss_sum"] is not None or a["dv"] is not None:
+        raise NotImplementedError("stem_out's training loss outputs are not checked here")
+    h, f = a["h"], a["f"]
+    xin = _stem_input(a)
+    B, _, T = xin.shape
+    w = a["w"].to(F64)
+    co = w.shape[0]
+    w3 = w.permute(2, 0, 1)                                    # [3, co, c0]
+    bias = a["bias"].to(F64) if a["bias"] is not None else None
+    if a["w_adapt"] is not None:
+        wa = a["w_adapt"].to(F64)
+        skip = torch.einsum("oc,bct->bot", wa, xin) + a["b_adapt"].to(F64)[None, :, None]
+        skip_abs = torch.einsum("oc,bct->bot", wa.abs(), xin.abs()) + a["b_adapt"].to(F64).abs()[None, :, None]
+    else:
+        skip, skip_abs = xin[:, :co], xin[:, :co].abs()
+    gate = a["gate"].to(F64)[:, :co]
+
+    def branch(b):               # gate * conv3(nearest_up(h)) of trunk row b -> [co, T]
+        up = h[b].to(F64).repeat_interleave(f, dim=0)
+        y = _conv3(up, w3, bias).t()
+        ya = _conv3(up.abs(), w3.abs(), None if bias is None else bias.abs()).t()
+        return gate[b][:, None] * y, gate[b].abs()[:, None] * ya
+    v = torch.empty(B, co, T, dtype=F64, device=h.device)
+    vabs = torch.empty_like(v)
+    s = a["cfg_scale"]
+    for b in range(B):
+        yc, yca = branch(b)
+        if s is None:
+            v[b], vabs[b] = skip[b] + yc, skip_abs[b] + yca
+        else:
+            ym, yma = branch(b + B)
+            vc, vm = skip[b] + yc, skip[b] + ym
+            v[b] = vm + (vc - vm) * s
+            vabs[b] = (abs(s) + abs(1 - s)) * skip_abs[b] + abs(s) * yca + abs(1 - s) * yma
+    outs = []
+    if a["v_out"] is not None:
+        outs.append(Val("v_out", arg("v_out"), v, vabs))
+    if a["x_next"] is not None:
+        a0, b0, a1, b1 = a["ab"].to(F64).tolist()
+        xs = xin[:, :co]
+        xn = a1 * (a0 * xs - b0 * v) + b1 * (b0 * xs + a0 * v)
+        xna = (abs(a1 * a0) + abs(b1 * b0)) * xs.abs() + (abs(a1 * b0) + abs(b1 * a0)) * vabs
+        outs.append(Val("x_next", arg("x_next"), xn, xna))
+    return outs
+
+
+def c_narrow_conv(a, ctx):
+    x = a["x"]
+    B, T, C = x.shape
+    G = a["groups"]
+    sc, sh = _gn_coef(a["stats_in"], a["gamma"], a["beta"], G, a["gn_eps"], T, C)
+    act = _silu(x.to(F64) * sc + sh)
+    if a["w_packed"] is not None:          # bf16 [C][3C], k = tap * C + ci
+        w3 = a["w_packed"].to(F64).reshape(C, 3, C).permute(1, 0, 2)
+    else:                                  # fp32 [C][C][3], rounded to bf16 for the tensor cores
+        w3 = a["w"].to(torch.bfloat16).to(F64).permute(2, 0, 1)
+    bias = a["bias"].to(F64) if a["bias"] is not None else None
+    r = torch.stack([_conv3(act[b], w3, bias) for b in range(B)])
+    ra = torch.stack([_conv3(act[b].abs(), w3.abs(), None if bias is None else bias.abs()) for b in range(B)])
+    if a["residual"] is not None:
+        r, ra = r + a["residual"].to(F64), ra + a["residual"].to(F64).abs()
+    ref, absr = r, ra
+    if a["scale_shift"] is not None:
+        ss = a["scale_shift"].to(F64)
+        s, t = ss[:, None, :C], ss[:, None, C:2 * C]
+        xn, std, lnabs = _layer_norm(r, a["ln_eps"])
+        ref = xn * (1 + s) + t
+        # an error e in r moves LN(r) by up to ~2 max|e| / std (the row's own entry, its mean, its variance)
+        absr = (2 * ra.amax(-1, keepdim=True) / std + lnabs) * (1 + s).abs() + t.abs()
+    outs = [Val("y", arg("y"), ref, absr, TAU_BF16_OPERAND)]
+    if a["stats_out"] is not None:
+        outs.append(Stat("stats_out", arg("stats_out"), arg("y"), G))
+    return outs
+
+
+def c_sampler_step(a, ctx):
+    x, v = a["x"].to(F64), a["v"].to(F64)
+    a0, b0, a1, b1 = a["ab"].to(F64).tolist()
+    ref = a1 * (a0 * x - b0 * v) + b1 * (b0 * x + a0 * v)
+    absr = (abs(a1 * a0) + abs(b1 * b0)) * x.abs() + (abs(a1 * b0) + abs(b1 * a0)) * v.abs()
+    return [Val("x_next", arg("x_next"), ref, absr)]
+
+
+def c_step_select(a, ctx):
+    ctrl = a["ctrl"].tolist()
+    div = ctrl[1] if ctrl[1] > 0 else 1
+    n_it = (ctrl[2] if ctrl[2] > 0 else 1) * div
+    it = min(int(a["step"].item()), n_it - 1)
+    n = a["ss_out"].numel()
+    table = ctx.lookup(ctrl[0], (it // div + 1) * n, torch.float32)
+    return [Val("ss_out", arg("ss_out"), table[(it // div) * n:(it // div + 1) * n].reshape(a["ss_out"].shape),
+                exact=True),
+            Val("ab_out", arg("ab_out"), a["ab_table"][it].clone(), exact=True)]
+
+
+def c_step_advance(a, ctx):
+    return [Val("step", arg("step"), a["step"] + 1, exact=True)]
+
+
+# Role of every tensor argument of each checked kind: read, stored (the launch writes it), or
+# accumulated (+=, checked as after - before).  Shadow refuses a launch whose checker returns
+# outputs other than these, or leaves a passed output argument unchecked; `probe=True` also
+# perturbs each read argument and requires some reference to move (an input the restatement
+# ignores is a gap).
+ARGS: Dict[str, Tuple[FrozenSet[str], FrozenSet[str], FrozenSet[str]]] = {k: (frozenset(r), frozenset(st), frozenset(ac)) for k, (r, st, ac) in {
+    "conv_gemm": ({"a", "w", "bias", "residual", "gate", "gn"}, {"out"}, {"stats"}),
+    "gn_silu": ({"x", "stats", "gamma", "beta"}, {"y"}, ()),
+    "gn_stats": ({"x"}, (), {"stats"}),
+    "ln_film": ({"x", "scale_shift"}, {"y", "y2"}, {"stats_out"}),
+    "attention": ({"q", "k", "v"}, {"o", "lse"}, ()),
+    "skinny_linear": ({"x", "w", "bias"}, {"y"}, ()),
+    "time_features": ({"sigma", "freqs"}, {"out"}, ()),
+    "silu_bf16": ({"x"}, {"y"}, ()),
+    "stem_in": ({"x", "w", "bias", "append", "noise", "alpha", "beta"}, {"out"}, {"stats"}),
+    "stem_out": ({"h", "x", "w", "bias", "gate", "append", "w_adapt", "b_adapt", "ab"}, {"v_out", "x_next"}, ()),
+    "narrow_conv": ({"x", "stats_in", "gamma", "beta", "w", "bias", "residual", "scale_shift", "w_packed"},
+                    {"y"}, {"stats_out"}),
+    "sampler_step": ({"x", "v", "ab"}, {"x_next"}, ()),
+    "step_select": ({"step", "ctrl", "ab_table"}, {"ab_out", "ss_out"}, ()),
+    "step_advance": ((), {"step"}, ()),       # step += 1, checked against the snapshot + 1
+}.items()}
+
+# Read arguments the kernel does not read for some argument combinations (the probe skips them):
+# narrow_conv copies the host-packed bf16 image instead of converting `w`, and the conv GEMM's
+# fp32-output epilogue has no residual (adp_conv_gemm refuses one).
+NOT_READ: Dict[str, Callable] = {
+    "narrow_conv": lambda a: {"w"} if a["w_packed"] is not None else set(),
+    "conv_gemm": lambda a: {"residual"} if a["out"].dtype == torch.float32 else set(),
+}
+
+CHECKERS: Dict[str, Callable] = {
+    "conv_gemm": c_conv_gemm, "gn_silu": c_gn_silu, "gn_stats": c_gn_stats, "ln_film": c_ln_film,
+    "attention": c_attention, "skinny_linear": c_skinny_linear, "time_features": c_time_features,
+    "silu_bf16": c_silu_bf16, "stem_in": c_stem_in, "stem_out": c_stem_out, "narrow_conv": c_narrow_conv,
+    "sampler_step": c_sampler_step, "step_select": c_step_select, "step_advance": c_step_advance,
+}
+
+
+# ------------------------------------------------------------------------------ harness
+def _tensors(v):
+    if isinstance(v, torch.Tensor):
+        yield v
+    elif isinstance(v, (tuple, list)):
+        for x in v:
+            yield from _tensors(x)
+
+
+def _key(t):
+    return t.untyped_storage().data_ptr()
+
+
+def _on(storage, t):
+    """t's view over another storage of the same layout (its snapshot)."""
+    return torch.empty(0, dtype=t.dtype, device=t.device).set_(storage, t.storage_offset(), t.shape, t.stride())
+
+
+def _bits(t):
+    return t.view({1: torch.uint8, 2: torch.int16, 4: torch.int32, 8: torch.int64}[t.element_size()])
+
+
+def _flat(storage, dtype, device):
+    n = storage.nbytes() // torch.empty(0, dtype=dtype).element_size()
+    return torch.empty(0, dtype=dtype, device=device).set_(storage, 0, (n,), (1,))
+
+
+def _where(idx, shape):
+    out = []
+    for s in reversed(shape):
+        out.append(idx % s)
+        idx //= s
+    return tuple(reversed(out))
+
+
+class Record:
+    def __init__(self):
+        self.count, self.worst, self.label, self.where = 0, 0.0, "", ""
+
+
+class Shadow:
+    """Context manager: every ops launch of a CHECKERS kind is checked (see the module docstring).
+
+    fake=True: no kernel runs; each launch writes its restatement rounded to the output dtype
+    (statistics: those of the written output).  probe=True: the first launch of each kind and set
+    of passed tensors also runs _probe.  mutate=(kind, fn): after the first launch of that
+    kind where fn(args, outs, snapshot) applies (does not return False), fn damages what it
+    wrote (the checker's self-test)."""
+
+    def __init__(self, fake: bool = False, mutate=None, probe: bool = False):
+        self.fake, self.mutate, self.probe = fake, mutate, probe
+        self.probed = set()
+        self.records: Dict[str, Record] = {}
+        self.n_launch, self.n_checked = 0, 0
+        self.known: Dict[int, torch.Tensor] = {}
+
+    # ---- install
+    def __enter__(self):
+        self._saved = {}
+        for name in launching_functions():
+            self._saved[name] = getattr(ops, name)
+            setattr(ops, name, self._wrap(name, self._saved[name]))
+        return self
+
+    def __exit__(self, *exc):
+        for name, fn in self._saved.items():
+            setattr(ops, name, fn)
+        self.known.clear()
+
+    def lookup(self, ptr, n, dtype):
+        """n elements of `dtype` at device address ptr, from a storage seen in an earlier launch."""
+        for t in self.known.values():
+            st = t.untyped_storage()
+            base = st.data_ptr()
+            if base <= ptr and ptr + n * 4 <= base + st.nbytes():
+                return _flat(st, dtype, t.device)[(ptr - base) // 4:][:n]
+        raise CheckError(f"step_select: no known tensor holds address {ptr:#x}")
+
+    # ---- one launch
+    def _wrap(self, name, real):
+        sig = inspect.signature(real)
+
+        def launch(*args, **kwargs):
+            if name not in CHECKERS:
+                raise CheckError(f"launch {self.n_launch}: {name} has no checker ({UNCHECKED.get(name, '?')})")
+            b = sig.bind(*args, **kwargs)
+            b.apply_defaults()
+            post = dict(b.arguments)
+            idx = self.n_launch
+            self.n_launch += 1
+            label0 = self._label(name, post)
+            for t in _tensors(list(post.values())):
+                self.known[_key(t)] = t
+            if post[next(iter(post))].is_cuda:
+                torch.cuda.synchronize()
+            snaps = {}
+            for t in _tensors(list(post.values())):
+                k = _key(t)
+                if k not in snaps:
+                    snaps[k] = t.untyped_storage().clone()
+
+            def snap(v):
+                if isinstance(v, torch.Tensor):
+                    return _on(snaps[_key(v)], v)
+                if isinstance(v, tuple):
+                    return tuple(snap(x) for x in v)
+                return v
+            pre = {k: snap(v) for k, v in post.items()}
+            outs = CHECKERS[name](pre, self)
+            self._check_roles(idx, name, outs, post)
+            variant = (name, frozenset(n for n, v in post.items() if list(_tensors([v]))))
+            if self.probe and variant not in self.probed:      # once per set of passed tensors
+                self._probe(idx, name, outs, pre)
+                self.probed.add(variant)
+            if self.fake:
+                self._fake_write(outs, pre, post)
+                label = label0
+            else:
+                with ops.trace() as tr:
+                    result = real(*args, **kwargs)
+                label = tr.records[-1]["name"] if tr.records else label0
+                if post[next(iter(post))].is_cuda:
+                    torch.cuda.synchronize()
+            if self.mutate is not None and self.mutate[0] == name:
+                if self.mutate[1](post, outs, pre) is not False:       # False: not applicable here
+                    self.mutate = None
+            self._check(idx, name, label, outs, pre, post, snaps)
+            self.n_checked += 1
+            return None if self.fake else result
+        return launch
+
+    def _check_roles(self, idx, name, outs, post):
+        """The checker's outputs are exactly the output arguments the launch was given."""
+        _, stored, accumulated = ARGS[name]
+        got = {(o.name, isinstance(o, Stat)) for o in outs}
+        want = {(n, False) for n in stored if post.get(n) is not None} | \
+            {(n, True) for n in accumulated if post.get(n) is not None}
+        if got != want:
+            raise CheckError(f"launch {idx}: {name}: checker outputs {sorted(got)}, declared {sorted(want)}")
+
+    def _probe(self, idx, name, outs, pre):
+        """Every tensor the launch reads must move the reference when it changes."""
+        def values(args, os_):
+            return [stats_of(o.src(args), o.groups) if isinstance(o, Stat)
+                    else (o.ref(args)[0] if callable(o.ref) else o.ref) for o in os_]
+        base = values(pre, outs)
+        skip = NOT_READ[name](pre) if name in NOT_READ else set()
+        for n in sorted(ARGS[name][0] - skip):
+            v = pre.get(n)
+            ts = list(_tensors([v]))
+            if not ts or not all(t.is_floating_point() for t in ts):
+                continue                          # absent, or integer control words (step_select)
+
+            def moved(t):
+                return t.clone().mul_(1.25).add_(0.125)
+            args = dict(pre)
+            args[n] = moved(v) if isinstance(v, torch.Tensor) else \
+                tuple(moved(x) if isinstance(x, torch.Tensor) else x for x in v)
+            after = values(args, CHECKERS[name](args, self))
+            if all(torch.equal(a, b) for a, b in zip(base, after)):
+                raise CheckError(f"launch {idx}: {name}: the reference does not depend on `{n}`")
+
+    @staticmethod
+    def _label(name, post):
+        shapes = [tuple(t.shape) for t, _ in zip(_tensors(list(post.values())), range(2))]
+        return f"{name}{shapes}"
+
+    def _fake_write(self, outs, pre, post):
+        for o in outs:
+            if isinstance(o, Stat):
+                continue
+            got = o.view(post)
+            ref = o.ref(post)[0] if callable(o.ref) else o.ref
+            got.copy_(ref.to(got.dtype))
+        for o in outs:                       # statistics of the values just written
+            if isinstance(o, Stat):
+                o.view(post).add_(stats_of(o.src(post), o.groups))
+
+    # ---- comparisons
+    def _fail(self, idx, name, label, msg):
+        raise CheckError(f"launch {idx} ({label}): {name}: {msg}")
+
+    def _note(self, key, ratio, label, where):
+        r = self.records.setdefault(key, Record())
+        r.count += 1
+        if ratio >= r.worst:
+            r.worst, r.label, r.where = ratio, label, where
+
+    def _check(self, idx, name, label, outs, pre, post, snaps):
+        written = {}
+        for o in outs:
+            v = o.view(post)
+            written.setdefault(_key(v), []).append(v)
+        # side effects: read-only storages bitwise unchanged, written ones outside their views
+        for k, st in snaps.items():
+            t = next(t for t in _tensors(list(post.values())) if _key(t) == k)
+            views = written.get(k)
+            if views is None:
+                if not torch.equal(_flat(st, torch.uint8, t.device), _flat(t.untyped_storage(), torch.uint8, t.device)):
+                    argn = next(n for n, v in post.items() if any(_key(x) == k for x in _tensors([v])))
+                    self._fail(idx, name, label, f"read-only argument `{argn}` was modified")
+                continue
+            dt = views[0].dtype
+            before = _bits(_flat(st, dt, t.device))
+            after = _bits(_flat(t.untyped_storage(), dt, t.device))
+            mask = torch.zeros(before.shape, dtype=torch.bool, device=t.device)
+            for v in views:
+                mask.as_strided(v.shape, v.stride(), v.storage_offset()).fill_(True)
+            bad = (before != after) & ~mask
+            if bad.any():
+                i = int(bad.nonzero()[0, 0])
+                self._fail(idx, name, label, f"wrote storage element {i} outside its output view")
+        for o in outs:
+            got = o.view(post)
+            key = f"{name}.{o.name}"
+            if isinstance(o, Stat):
+                self._check_stats(idx, name, label, key, o, got.to(F64) - o.view(pre).to(F64), o.src(post))
+                continue
+            ref, absr = o.ref(post) if callable(o.ref) else (o.ref, o.absref)
+            if o.exact:
+                if not torch.equal(_bits(got.contiguous()), _bits(ref.to(got.dtype).contiguous())):
+                    self._fail(idx, name, label, f"{o.name} differs from the copy it must make")
+                self._note(key, 0.0, label, "")
+                continue
+            g = got.to(F64)
+            err = (g - ref).abs()
+            if got.dtype == torch.bfloat16:
+                bound = BF16_REL * ref.abs() + o.tau * absr
+            else:
+                bound = FP32_REL * ref.abs() + FP32_TAU * absr
+            ratio = torch.where(bound > 0, err / bound.clamp_min(1e-300), torch.where(err > 0, math.inf, 0.0))
+            ratio = torch.where(torch.isnan(g), math.inf, ratio)
+            i = int(ratio.reshape(-1).argmax())
+            worst = float(ratio.reshape(-1)[i])
+            where = _where(i, tuple(ratio.shape))
+            desc = (f"{o.name}{list(where)}: got {float(g.reshape(-1)[i]):.6g}, ref {float(ref.reshape(-1)[i]):.6g}, "
+                    f"bound {float(bound.reshape(-1)[i]):.3g} (err/bound {worst:.3g})")
+            if worst > 1.0:
+                self._fail(idx, name, label, desc)
+            self._note(key, worst, label, f"{list(where)}")
+
+    def _check_stats(self, idx, name, label, key, o, got, src):
+        B, T, C = src.shape
+        G = o.groups
+        ref = stats_of(src, G)
+        yg = src.to(F64).reshape(B, T, G, C // G)
+        scale = torch.stack([yg.abs().sum(dim=(1, 3)), (yg * yg).sum(dim=(1, 3))], dim=-1)
+        err = (got - ref).abs()
+        bound = STATS_TOL * scale
+        ratio = torch.where(bound > 0, err / bound.clamp_min(1e-300), torch.where(err > 0, math.inf, 0.0))
+        i = int(ratio.reshape(-1).argmax())
+        worst = float(ratio.reshape(-1)[i])
+        where = list(_where(i, tuple(ratio.shape)))
+        if worst > 1.0:
+            self._fail(idx, name, label, f"{o.name}{where}: got {float(got.reshape(-1)[i]):.10g}, "
+                                         f"ref {float(ref.reshape(-1)[i]):.10g} (err/bound {worst:.3g})")
+        self._note(key, worst, label, f"{where}")
+        # the variance GroupNorm derives from the slots, against a two-pass fp64 variance
+        n = float(T * (C // G))
+        mean = got[..., 0] / n
+        var = got[..., 1] / n - mean * mean
+        mu = yg.mean(dim=(1, 3), keepdim=True)
+        var2 = ((yg - mu) ** 2).mean(dim=(1, 3))
+        vr = (var - var2).abs() / (VAR_TOL * (var2 + GN_EPS))
+        j = int(vr.reshape(-1).argmax())
+        vworst = float(vr.reshape(-1)[j])
+        vwhere = list(_where(j, tuple(vr.shape)))
+        if vworst > 1.0:
+            self._fail(idx, name, label, f"{o.name} variance {vwhere}: E[x^2]-mean^2 = {float(var.reshape(-1)[j]):.8g}, "
+                                         f"two-pass {float(var2.reshape(-1)[j]):.8g} (err/bound {vworst:.3g})")
+        self._note(key + ".var", vworst, label, f"{vwhere}")
+        # not bounded: the relative error of the variance itself, large only for near-constant groups
+        rel = ((var - var2).abs() / var2.clamp_min(1e-300)).reshape(-1)
+        j = int(rel.argmax())
+        self._note(key + ".var_rel", float(rel[j]), label, f"{list(_where(j, tuple(var2.shape)))} "
+                                                           f"var {float(var2.reshape(-1)[j]):.3g}")
+
+    def table(self) -> str:
+        lines = [f"{'kind.output':28s} {'count':>6s} {'worst err/bound':>16s}  label (where)"]
+        for k in sorted(self.records):
+            r = self.records[k]
+            lines.append(f"{k:28s} {r.count:6d} {r.worst:16.4f}  {r.label} {r.where}")
+        lines.append(f"launches {self.n_launch}, checked {self.n_checked}")
+        return "\n".join(lines)
+
+
+# ---------------------------------------------------------------------------- mutations
+def m_scale_largest(post, outs, pre):
+    """The largest-|ref| element of the first stored output scaled by 1 + 2^-5."""
+    o = next((o for o in outs if isinstance(o, Val)), None)
+    if o is None:
+        return False
+    ref = o.ref(post)[0] if callable(o.ref) else o.ref
+    g = o.view(post)
+    i = int(ref.abs().to(F64).reshape(-1).argmax())
+    idx = _where(i, tuple(g.shape))
+    if g.is_floating_point():
+        g[idx] = (g[idx].to(F64) * (1 + 2 ** -5)).to(g.dtype)
+    else:                                      # the step counter
+        g[idx] += 1
+
+
+def m_stale_tile(post, outs, pre):
+    """The last row tile of the last batch element of the first [B, T, C] output left unwritten."""
+    o = next((o for o in outs if isinstance(o, Val) and not o.exact and o.view(post).dim() == 3), None)
+    if o is None:
+        return False
+    g, old = o.view(post), o.view(pre)
+    g[-1, -ROW_TILE:] = old[-1, -ROW_TILE:]
+
+
+def m_stats_slot(post, outs, pre):
+    """One statistics slot scaled by 1 + 1e-3."""
+    o = next((o for o in outs if isinstance(o, Stat)), None)
+    if o is None:
+        return False
+    g = o.view(post)
+    g[-1, -1, 1] *= 1 + 1e-3
+
+
+def m_outside_view(post, outs, pre):
+    """One element of a written tensor's storage outside the written view changed."""
+    for o in outs:
+        v = o.view(post)
+        flat = _flat(v.untyped_storage(), v.dtype, v.device)
+        mask = torch.zeros(flat.shape, dtype=torch.bool, device=v.device)
+        mask.as_strided(v.shape, v.stride(), v.storage_offset()).fill_(True)
+        free = (~mask).nonzero()
+        if free.numel():
+            i = int(free[-1, 0])
+            flat[i] += 1
+            return None
+    return False
+
+
+def m_readonly(post, outs, pre):
+    """One element of a read-only input changed."""
+    written = {_key(o.view(post)) for o in outs}
+    for v in post.values():
+        for t in _tensors([v]):
+            if _key(t) not in written and t.numel():
+                t[(0,) * t.dim()] += 1
+                return None
+    return False
+
+
+MUTATIONS = {"scale_largest": m_scale_largest, "stale_tile": m_stale_tile, "stats_slot": m_stats_slot,
+             "outside_view": m_outside_view, "readonly": m_readonly}
