@@ -127,6 +127,20 @@ def lib() -> C.CDLL:
         "adp_f32_silu": [vp, vp, C.c_int64, vp],
         "adp_f32_stem_in": [C.POINTER(StemInArgs), vp],
         "adp_f32_stem_out": [C.POINTER(StemOutArgs), vp],
+        "adp_f32_attention_lse": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, f32, vp, vp],
+        "adp_f32_stem_in_train": [C.POINTER(StemInArgs), vp],
+        "adp_f32_stem_out_train": [C.POINTER(StemOutArgs), vp],
+        "adp_f32_wgrad": [C.POINTER(WgradArgs), vp],
+        "adp_f32_gn_silu_bwd": [vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp],
+        "adp_f32_gn_bwd_apply": [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp],
+        "adp_f32_ln_film_bwd": [vp, vp, vp, i32, vp, vp, i32, vp, vp, i32, i32, i32, f32, vp],
+        "adp_f32_colsum": [vp, vp, i32, vp, i32, i32, i32, vp],
+        "adp_f32_skip_gate": [vp, vp, vp, i32, vp, vp, i32, i32, i32, i32, vp],
+        "adp_f32_skip_gate_bwd": [vp, vp, vp, i32, vp, vp, i32, i32, i32, i32, vp],
+        "adp_f32_cond_bwd": [vp, i32, vp, vp, vp, vp, vp, i32, i32, i32, vp],
+        "adp_f32_stem_out_bwd": [C.POINTER(StemOutBwdArgs), vp],
+        "adp_f32_stem_in_bwd": [C.POINTER(StemInBwdArgs), vp],
+        "adp_f32_attention_bwd": [C.POINTER(AttentionBwdArgs), i32, vp],
         "adp_step_select": [vp, vp, vp, vp, vp, C.c_int64, vp],
         "adp_step_advance": [vp, vp],
         "adp_silu_bf16": [vp, vp, C.c_int64, vp],
@@ -166,4 +180,8 @@ EXPORTS = ["adp_version", "adp_last_error", "adp_device_check", "adp_conv_gemm",
            "adp_mel_spectrogram", "adp_to_flat", "adp_to_flat_bwd", "adp_f32_conv_gemm", "adp_f32_gn_stats",
            "adp_f32_gn_silu", "adp_f32_ln_film", "adp_f32_attention", "adp_f32_linear", "adp_f32_silu",
            "adp_f32_stem_in", "adp_f32_stem_out", "adp_step_select", "adp_step_advance",
-           "adp_attention_hd", "adp_attention_bwd_hd", "adp_f32_attention_hd"]
+           "adp_attention_hd", "adp_attention_bwd_hd", "adp_f32_attention_hd", "adp_f32_attention_lse",
+           "adp_f32_stem_in_train", "adp_f32_stem_out_train", "adp_f32_wgrad", "adp_f32_gn_silu_bwd",
+           "adp_f32_gn_bwd_apply", "adp_f32_ln_film_bwd", "adp_f32_colsum", "adp_f32_skip_gate",
+           "adp_f32_skip_gate_bwd", "adp_f32_cond_bwd", "adp_f32_stem_out_bwd", "adp_f32_stem_in_bwd",
+           "adp_f32_attention_bwd"]

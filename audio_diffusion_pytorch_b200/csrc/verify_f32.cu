@@ -157,12 +157,13 @@ __device__ __forceinline__ float ld_nc_volatile(const float* p) {
 // D <= 64 the scaled query and the output accumulator live in registers.  At D = 128 both would
 // not fit: the thread makes one pass over the keys per 64-column half of the output, keeps only
 // that half's accumulator, and re-reads the (L1-resident) query for every key.  Both passes
-// compute the same scores and softmax statistics.
+// compute the same scores and softmax statistics.  lse (training forward, may be NULL): fp32
+// [B][H][Tq] = max + log(sum exp(s - max)) of the scaled scores, for adp_f32_attention_bwd.
 template <int D>
 __global__ void __launch_bounds__(128)
 f32_attention_kernel(const float* __restrict__ q, const float* __restrict__ k, const float* __restrict__ v,
                      float* __restrict__ o, int B, int H, int Tq, int Tk, int ldq, int ldk, int ldv, int ldo,
-                     float scale) {
+                     float scale, float* __restrict__ lse) {
   constexpr bool kQInRegs = D <= 64;
   constexpr int kDO = kQInRegs ? D : 64;   // output columns per pass
   pdl_launch_dependents();
@@ -206,6 +207,7 @@ f32_attention_kernel(const float* __restrict__ q, const float* __restrict__ k, c
       const float inv = 1.f / l;
 #pragma unroll
       for (int d = 0; d < kDO; ++d) orow[d] = acc[d] * inv;
+      if (lse && c0 == 0) lse[i] = mx + logf(l);     // [B][H][Tq] is the loop order
     }
   }
 }
@@ -244,7 +246,8 @@ f32_silu_kernel(const float* __restrict__ x, float* __restrict__ y, int64_t n) {
 }
 
 // Downsample conv of level 0: out[b, to, c] = bias[c] + sum_{ci, j} w[c][ci][j] * in[b, ci, to*f + j],
-// in = cat([x, append]); out fp32 channels-last
+// in = cat([x, append]), x noised to alpha_b*x + beta_b*noise when noise is set (training
+// forward, reference diffusion.py:91); out fp32 channels-last
 __global__ void __launch_bounds__(256) f32_stem_in_kernel(const adp_stem_in_args a) {
   pdl_launch_dependents();
   pdl_wait();
@@ -260,8 +263,14 @@ __global__ void __launch_bounds__(256) f32_stem_in_kernel(const adp_stem_in_args
     for (int ci = 0; ci < cin; ++ci)
       for (int j = 0; j < a.f; ++j) {
         const int64_t tt = static_cast<int64_t>(to) * a.f + j;
-        const float xv = ci < a.cx ? a.x[(static_cast<int64_t>(b) * a.cx + ci) * a.T + tt]
-                                   : a.append[(static_cast<int64_t>(b) * a.ca + (ci - a.cx)) * a.T + tt];
+        float xv;
+        if (ci < a.cx) {
+          const int64_t idx = (static_cast<int64_t>(b) * a.cx + ci) * a.T + tt;
+          xv = a.x[idx];
+          if (a.noise) xv = a.alpha[b] * xv + a.beta[b] * a.noise[idx];
+        } else {
+          xv = a.append[(static_cast<int64_t>(b) * a.ca + (ci - a.cx)) * a.T + tt];
+        }
         acc = fmaf(xv, a.w[(static_cast<int64_t>(c) * cin + ci) * a.f + j], acc);
       }
     out[i] = acc;
@@ -269,7 +278,8 @@ __global__ void __launch_bounds__(256) f32_stem_in_kernel(const adp_stem_in_args
 }
 
 // Level-0 output: v = skip + gate * (conv3(nearest-upsample(h)) + bias), guidance combine, sampler
-// update -- the semantics of stem_out_kernel (stem.cu) with h in fp32
+// update, VDiffusion loss (sum of squared error into loss_sum, dL/dv into dv) -- the semantics of
+// stem_out_kernel (stem.cu) with h in fp32
 __device__ __forceinline__ float f32_stem_branch(const adp_stem_out_args& a, const float* hb, int o, int t) {
   float y = a.bias ? a.bias[o] : 0.f;
   for (int k = 0; k < 3; ++k) {
@@ -288,17 +298,24 @@ __global__ void __launch_bounds__(256) f32_stem_out_kernel(const adp_stem_out_ar
   const int cin = a.cx + a.ca, Tl = a.T / a.f;
   const float* h = static_cast<const float*>(a.h);
   const int64_t total = static_cast<int64_t>(a.B) * a.T;
+  double lsum = 0.0;
   // one thread per (batch, position): every input channel is read before any output channel is
   // written (x_next may alias x)
   for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
        i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
     const int t = static_cast<int>(i % a.T);
     const int b = static_cast<int>(i / a.T);
+    const float al = a.noise ? a.alpha[b] : 1.f, be = a.noise ? a.beta[b] : 0.f;
     float xin[8];
     for (int c = 0; c < 8; ++c) {
       xin[c] = 0.f;
-      if (c < a.cx) xin[c] = a.x[(static_cast<int64_t>(b) * a.cx + c) * a.T + t];
-      else if (c < cin) xin[c] = a.append[(static_cast<int64_t>(b) * a.ca + (c - a.cx)) * a.T + t];
+      if (c < a.cx) {
+        const int64_t idx = (static_cast<int64_t>(b) * a.cx + c) * a.T + t;
+        xin[c] = a.x[idx];
+        if (a.noise) xin[c] = al * xin[c] + be * a.noise[idx];
+      } else if (c < cin) {
+        xin[c] = a.append[(static_cast<int64_t>(b) * a.ca + (c - a.cx)) * a.T + t];
+      }
     }
     for (int o = 0; o < a.co; ++o) {
       float skip;
@@ -321,6 +338,23 @@ __global__ void __launch_bounds__(256) f32_stem_out_kernel(const adp_stem_out_ar
         const float a0 = a.ab[0], b0 = a.ab[1], a1 = a.ab[2], b1 = a.ab[3];
         a.x_next[oidx] = a1 * (a0 * xin[o] - b0 * v) + b1 * (b0 * xin[o] + a0 * v);
       }
+      if (a.loss_sum) {                     // target alpha*noise - beta*x (reference diffusion.py:92,95)
+        const int64_t xidx = (static_cast<int64_t>(b) * a.cx + o) * a.T + t;
+        const float d = v - (al * a.noise[xidx] - be * a.x[xidx]);
+        lsum += static_cast<double>(d) * d;
+        if (a.dv) a.dv[oidx] = 2.f * d / (static_cast<float>(a.B) * a.co * a.T);
+      }
+    }
+  }
+  if (a.loss_sum) {                         // every thread of the block reaches this point
+    __shared__ double s_loss[8];
+    for (int o = 16; o > 0; o >>= 1) lsum += __shfl_xor_sync(0xffffffffu, lsum, o);
+    if ((threadIdx.x & 31) == 0) s_loss[threadIdx.x >> 5] = lsum;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      double tot = 0.0;
+      for (int w = 0; w < (blockDim.x >> 5); ++w) tot += s_loss[w];
+      atomicAdd(a.loss_sum, tot);
     }
   }
 }
@@ -384,6 +418,12 @@ extern "C" int adp_f32_ln_film(const float* x, float* y, float* y2, const float*
 extern "C" int adp_f32_attention_hd(const float* q, const float* k, const float* v, float* o, int B, int H,
                                     int head_dim, int Tq, int Tk, int ldq, int ldk, int ldv, int ldo, float scale,
                                     adp_stream_t stream) {
+  return adp_f32_attention_lse(q, k, v, o, B, H, head_dim, Tq, Tk, ldq, ldk, ldv, ldo, scale, nullptr, stream);
+}
+
+extern "C" int adp_f32_attention_lse(const float* q, const float* k, const float* v, float* o, int B, int H,
+                                     int head_dim, int Tq, int Tk, int ldq, int ldk, int ldv, int ldo, float scale,
+                                     float* lse, adp_stream_t stream) {
   ADP_CHECK(head_dim == 32 || head_dim == 64 || head_dim == 128,
             "adp_f32_attention: head_dim %d not supported (32, 64 or 128)", head_dim);
   ADP_CHECK(q && k && v && o && B > 0 && H > 0 && Tq > 0 && Tk > 0, "adp_f32_attention: bad args");
@@ -396,7 +436,7 @@ extern "C" int adp_f32_attention_hd(const float* q, const float* k, const float*
   auto kern = head_dim == 32 ? f32_attention_kernel<32>
               : head_dim == 128 ? f32_attention_kernel<128> : f32_attention_kernel<64>;
   ADP_CUDA(launch_k(kern, dim3(static_cast<int>(g)), dim3(128), (size_t)0, as_stream(stream), q, k, v, o, B, H,
-                    Tq, Tk, ldq, ldk, ldv, ldo, scale));
+                    Tq, Tk, ldq, ldk, ldv, ldo, scale, lse));
   ADP_LAUNCH_CHECK();
   return 0;
 }
@@ -423,10 +463,17 @@ extern "C" int adp_f32_silu(const float* x, float* y, int64_t n, adp_stream_t st
 }
 
 extern "C" int adp_f32_stem_in(const adp_stem_in_args* args, adp_stream_t stream) {
+  ADP_CHECK(!args || !args->noise, "adp_f32_stem_in: the noised input is adp_f32_stem_in_train");
+  return adp_f32_stem_in_train(args, stream);
+}
+
+extern "C" int adp_f32_stem_in_train(const adp_stem_in_args* args, adp_stream_t stream) {
   ADP_CHECK(args && args->x && args->w && args->out, "adp_f32_stem_in: null pointer");
   const adp_stem_in_args& a = *args;
-  ADP_CHECK(!a.noise && !a.stats, "adp_f32_stem_in: noising / statistics are not part of the verification mode");
-  ADP_CHECK(a.f >= 1 && a.T % a.f == 0 && (a.ca == 0) == (a.append == nullptr), "adp_f32_stem_in: bad args");
+  ADP_CHECK(!a.stats, "adp_f32_stem_in: statistics are a separate adp_f32_gn_stats pass");
+  ADP_CHECK(!a.noise || (a.alpha && a.beta), "adp_f32_stem_in: noise needs alpha/beta");
+  ADP_CHECK(a.B > 0 && a.T > 0 && a.c0 > 0 && a.cx > 0 && a.f >= 1 && a.T % a.f == 0 &&
+            (a.ca == 0) == (a.append == nullptr), "adp_f32_stem_in: bad args");
   ADP_CUDA(launch_k(f32_stem_in_kernel, dim3(f32_grid(static_cast<int64_t>(a.B) * (a.T / a.f) * a.c0)), dim3(256),
                     (size_t)0, as_stream(stream), a));
   ADP_LAUNCH_CHECK();
@@ -434,9 +481,19 @@ extern "C" int adp_f32_stem_in(const adp_stem_in_args* args, adp_stream_t stream
 }
 
 extern "C" int adp_f32_stem_out(const adp_stem_out_args* args, adp_stream_t stream) {
+  ADP_CHECK(!args || (!args->noise && !args->loss_sum && !args->dv),
+            "adp_f32_stem_out: the fused loss is adp_f32_stem_out_train");
+  return adp_f32_stem_out_train(args, stream);
+}
+
+extern "C" int adp_f32_stem_out_train(const adp_stem_out_args* args, adp_stream_t stream) {
   ADP_CHECK(args && args->h && args->x && args->w && args->gate, "adp_f32_stem_out: null pointer");
   const adp_stem_out_args& a = *args;
-  ADP_CHECK(!a.noise && !a.loss_sum && !a.dv, "adp_f32_stem_out: the fused loss is not part of the verification mode");
+  ADP_CHECK(!a.loss_sum || (a.noise && a.alpha && a.beta), "adp_f32_stem_out: loss needs noise/alpha/beta");
+  ADP_CHECK(!a.noise || (a.alpha && a.beta), "adp_f32_stem_out: noise needs alpha/beta");
+  ADP_CHECK(!a.dv || a.loss_sum, "adp_f32_stem_out: dv is part of the loss");
+  ADP_CHECK(!a.loss_sum || (!a.cfg && !a.x_next), "adp_f32_stem_out: the loss excludes guidance / sampler fusion");
+  ADP_CHECK(a.B > 0 && a.T > 0 && a.c0 > 0 && a.co >= 1, "adp_f32_stem_out: bad sizes");
   ADP_CHECK(a.w_adapt || a.cx + a.ca == a.co, "adp_f32_stem_out: identity skip needs cx+ca == co");
   ADP_CHECK(!a.x_next || a.ab, "adp_f32_stem_out: x_next needs ab");
   ADP_CHECK(a.f >= 1 && a.T % a.f == 0 && (a.ca == 0) == (a.append == nullptr), "adp_f32_stem_out: bad args");

@@ -264,7 +264,14 @@ def attention(q: Tensor, k: Tensor, v: Tensor, o: Tensor, heads: int, scale: flo
     Tk = k.shape[1]
     D, tag = head_dim, _hd_tag(head_dim)
     if q.dtype == torch.float32:
-        assert lse is None, "the fp32 verification mode covers inference only"
+        if lse is not None:            # training forward: also the log-sum-exp rows
+            _launch(lambda: _lib.lib().adp_f32_attention_lse(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
+                                                             B, heads, D, Tq, Tk, q.stride(1), k.stride(1),
+                                                             v.stride(1), o.stride(1), scale, lse.data_ptr(),
+                                                             _stream()),
+                    "adp_f32_attention_lse", lambda: (f"f32_attention[B={B} H={heads} Tq={Tq} Tk={Tk}{tag} +lse]",
+                                                      4.0 * B * heads * Tq * Tk * D, 0))
+            return o
         _launch(lambda: _lib.lib().adp_f32_attention_hd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
                                                         B, heads, D, Tq, Tk, q.stride(1), k.stride(1),
                                                         v.stride(1), o.stride(1), scale, _stream()),
@@ -326,10 +333,14 @@ def stem_in(x: Tensor, w: Tensor, bias: Optional[Tensor], out: Tensor, f: int, *
     a.ca = 0 if append is None else append.shape[1]
     a.c0, a.f, a.groups = w.shape[0], f, groups
     if out.dtype == torch.float32:
-        assert noise is None
         a.stats = None
-        _launch(lambda: _lib.lib().adp_f32_stem_in(C.byref(a), _stream()), "adp_f32_stem_in",
-                lambda: (f"f32_stem_in[B={x.shape[0]} T={x.shape[2]} c0={w.shape[0]}]", 0, _nb(x, append, out)))
+        if noise is not None:          # training forward: the VDiffusion noising
+            _launch(lambda: _lib.lib().adp_f32_stem_in_train(C.byref(a), _stream()), "adp_f32_stem_in_train",
+                    lambda: (f"f32_stem_in[B={x.shape[0]} T={x.shape[2]} c0={w.shape[0]} +noise]", 0,
+                             _nb(x, append, noise, out)))
+        else:
+            _launch(lambda: _lib.lib().adp_f32_stem_in(C.byref(a), _stream()), "adp_f32_stem_in",
+                    lambda: (f"f32_stem_in[B={x.shape[0]} T={x.shape[2]} c0={w.shape[0]}]", 0, _nb(x, append, out)))
         if stats is not None:
             gn_stats(out, stats, groups)
         return out
@@ -358,6 +369,11 @@ def stem_out(h: Tensor, x: Tensor, w: Tensor, bias: Optional[Tensor], gate: Tens
     a.c0, a.co, a.f = h.shape[-1], w.shape[0], f
     a.ld_gate = gate.stride(0)
     if h.dtype == torch.float32:
+        if noise is not None or loss_sum is not None or dv is not None:    # training forward
+            _launch(lambda: _lib.lib().adp_f32_stem_out_train(C.byref(a), _stream()), "adp_f32_stem_out_train",
+                    lambda: (f"f32_stem_out[B={x.shape[0]} T={x.shape[2]} c0={h.shape[-1]} +loss]", 0,
+                             _nb(h, x, noise, v_out, dv)))
+            return
         _launch(lambda: _lib.lib().adp_f32_stem_out(C.byref(a), _stream()), "adp_f32_stem_out",
                 lambda: (f"f32_stem_out[B={x.shape[0]} T={x.shape[2]} c0={h.shape[-1]}]", 0, _nb(h, x, v_out)))
         return
@@ -514,6 +530,12 @@ def wgrad(g: Tensor, x: Tensor, dw: Tensor, *, n: int, k: int, off: int = 0, g_c
     a.ldg, a.ldx, a.ldw = g.stride(1), x.stride(1), dw.stride(-2)
     a.g_cols, a.x_cols = g.shape[2], x.shape[2]
     a.g_col0, a.x_col0, a.off = g_col0, x_col0, off
+    if g.dtype == torch.float32:       # fp32 verification mode (csrc/verify_f32_bwd.cu)
+        assert x.dtype == torch.float32
+        _launch(lambda: _lib.lib().adp_f32_wgrad(C.byref(a), _stream()), "adp_f32_wgrad",
+                lambda: (f"f32_wgrad[M={g.shape[0] * g.shape[1]} n={n} k={k}{' x3' if ntaps == 3 else ''}]",
+                         2.0 * g.shape[0] * g.shape[1] * n * k * ntaps, 0))
+        return dw
     _launch(lambda: _lib.lib().adp_wgrad(C.byref(a), _stream()), "adp_wgrad",
             lambda: (f"wgrad[M={g.shape[0] * g.shape[1]} n={n} k={k}{' x3' if ntaps == 3 else ''}]",
                      2.0 * g.shape[0] * g.shape[1] * n * k * ntaps, (g.shape[0] * g.shape[1]) * (n + k) * 2))
@@ -523,6 +545,13 @@ def wgrad(g: Tensor, x: Tensor, dw: Tensor, *, n: int, k: int, off: int = 0, g_c
 def gn_silu_bwd(da: Tensor, x: Tensor, stats: Tensor, gamma: Tensor, beta: Tensor, dxh: Tensor,
                 dgamma: Tensor, dbeta: Tensor, S: Tensor, groups: int, eps: float = 1e-5) -> Tensor:
     B, T, Cc = x.shape
+    if x.dtype == torch.float32:
+        _launch(lambda: _lib.lib().adp_f32_gn_silu_bwd(da.data_ptr(), x.data_ptr(), stats.data_ptr(),
+                                                       gamma.data_ptr(), beta.data_ptr(), dxh.data_ptr(),
+                                                       dgamma.data_ptr(), dbeta.data_ptr(), S.data_ptr(),
+                                                       B, T, Cc, groups, eps, _stream()),
+                "adp_f32_gn_silu_bwd", lambda: (f"f32_gn_silu_bwd[M={B * T} C={Cc}]", 0, _nb(da, x, dxh)))
+        return dxh
     _launch(lambda: _lib.lib().adp_gn_silu_bwd(da.data_ptr(), x.data_ptr(), stats.data_ptr(),
                                                gamma.data_ptr(), beta.data_ptr(), dxh.data_ptr(),
                                                dgamma.data_ptr(), dbeta.data_ptr(), S.data_ptr(),
@@ -535,6 +564,12 @@ def gn_bwd_apply(dxh: Tensor, x: Tensor, stats: Tensor, S: Tensor, dx: Tensor, g
                  dres: Optional[Tensor] = None, colsum: Optional[Tensor] = None,
                  eps: float = 1e-5) -> Tensor:
     B, T, Cc = x.shape
+    if x.dtype == torch.float32:
+        _launch(lambda: _lib.lib().adp_f32_gn_bwd_apply(dxh.data_ptr(), x.data_ptr(), stats.data_ptr(),
+                                                        S.data_ptr(), _p(dres), dx.data_ptr(), _p(colsum),
+                                                        B, T, Cc, groups, eps, _stream()),
+                "adp_f32_gn_bwd_apply", lambda: (f"f32_gn_bwd_apply[M={B * T} C={Cc}]", 0, _nb(dxh, x, dres, dx)))
+        return dx
     _launch(lambda: _lib.lib().adp_gn_bwd_apply(dxh.data_ptr(), x.data_ptr(), stats.data_ptr(),
                                                 S.data_ptr(), _p(dres), dx.data_ptr(), _p(colsum),
                                                 B, T, Cc, groups, eps, _stream()),
@@ -547,6 +582,12 @@ def ln_film_bwd(dy: Tensor, x: Tensor, scale_shift: Optional[Tensor], ss_stride:
                 colsum: Optional[Tensor] = None, dres: Optional[Tensor] = None,
                 eps: float = 1e-6) -> Tensor:
     B, T, Cc = x.shape
+    if x.dtype == torch.float32:
+        _launch(lambda: _lib.lib().adp_f32_ln_film_bwd(dy.data_ptr(), x.data_ptr(), _p(scale_shift),
+                                                       ss_stride, dx.data_ptr(), _p(dss), dss_stride,
+                                                       _p(colsum), _p(dres), B, T, Cc, eps, _stream()),
+                "adp_f32_ln_film_bwd", lambda: (f"f32_ln_film_bwd[M={B * T} C={Cc}]", 0, _nb(dy, x, dx)))
+        return dx
     _launch(lambda: _lib.lib().adp_ln_film_bwd(dy.data_ptr(), x.data_ptr(), _p(scale_shift),
                                                ss_stride, dx.data_ptr(), _p(dss), dss_stride,
                                                _p(colsum), _p(dres), B, T, Cc, eps, _stream()),
@@ -556,6 +597,11 @@ def ln_film_bwd(dy: Tensor, x: Tensor, scale_shift: Optional[Tensor], ss_stride:
 
 def colsum(x: Tensor, out: Tensor, gate: Optional[Tensor] = None) -> Tensor:
     B, T, Cc = x.shape
+    if x.dtype == torch.float32:
+        _launch(lambda: _lib.lib().adp_f32_colsum(x.data_ptr(), _p(gate), 0 if gate is None else gate.stride(0),
+                                                  out.data_ptr(), B, T, Cc, _stream()),
+                "adp_f32_colsum", lambda: (f"f32_colsum[M={B * T} C={Cc}]", 0, _nb(x)))
+        return out
     _launch(lambda: _lib.lib().adp_colsum(x.data_ptr(), _p(gate), 0 if gate is None else gate.stride(0),
                                           out.data_ptr(), B, T, Cc, _stream()),
             "adp_colsum", lambda: (f"colsum[M={B * T} C={Cc}]", 0, _nb(x)))
@@ -565,6 +611,14 @@ def colsum(x: Tensor, out: Tensor, gate: Optional[Tensor] = None) -> Tensor:
 def skip_gate(y: Tensor, skip: Tensor, gate: Tensor, out: Tensor, stats: Optional[Tensor],
               groups: int) -> Tensor:
     B, T, Cc = y.shape
+    if y.dtype == torch.float32:       # the statistics of out are their own pass, as in conv_gemm
+        _launch(lambda: _lib.lib().adp_f32_skip_gate(y.data_ptr(), skip.data_ptr(), gate.data_ptr(),
+                                                     gate.stride(0), out.data_ptr(), None, B, T, Cc, groups,
+                                                     _stream()),
+                "adp_f32_skip_gate", lambda: (f"f32_skip_gate[M={B * T} C={Cc}]", 0, _nb(y, skip, out)))
+        if stats is not None:
+            gn_stats(out, stats, groups)
+        return out
     _launch(lambda: _lib.lib().adp_skip_gate(y.data_ptr(), skip.data_ptr(), gate.data_ptr(),
                                              gate.stride(0), out.data_ptr(), _p(stats), B, T, Cc,
                                              groups, _stream()),
@@ -574,6 +628,12 @@ def skip_gate(y: Tensor, skip: Tensor, gate: Tensor, out: Tensor, stats: Optiona
 
 def skip_gate_bwd(dout: Tensor, y: Tensor, gate: Tensor, dys: Tensor, dgate: Tensor) -> Tensor:
     B, T, Cc = y.shape
+    if y.dtype == torch.float32:
+        _launch(lambda: _lib.lib().adp_f32_skip_gate_bwd(dout.data_ptr(), y.data_ptr(), gate.data_ptr(),
+                                                         gate.stride(0), dys.data_ptr(), dgate.data_ptr(),
+                                                         dgate.stride(0), B, T, Cc, _stream()),
+                "adp_f32_skip_gate_bwd", lambda: (f"f32_skip_gate_bwd[M={B * T} C={Cc}]", 0, _nb(dout, y, dys)))
+        return dys
     _launch(lambda: _lib.lib().adp_skip_gate_bwd(dout.data_ptr(), y.data_ptr(), gate.data_ptr(),
                                                  gate.stride(0), dys.data_ptr(), dgate.data_ptr(),
                                                  dgate.stride(0), B, T, Cc, _stream()),
@@ -584,6 +644,12 @@ def skip_gate_bwd(dout: Tensor, y: Tensor, gate: Tensor, dys: Tensor, dgate: Ten
 def cond_bwd(dss: Tensor, cond: Tensor, w: Tensor, dw: Tensor, dbias: Tensor, dcond: Optional[Tensor],
              N: int) -> None:
     B, K = cond.shape
+    if w.dtype == torch.float32:       # the fp32 verification mode's packed projection
+        _launch(lambda: _lib.lib().adp_f32_cond_bwd(dss.data_ptr(), dss.stride(0), cond.data_ptr(),
+                                                    w.data_ptr(), dw.data_ptr(), dbias.data_ptr(),
+                                                    _p(dcond), B, N, K, _stream()),
+                "adp_f32_cond_bwd", lambda: (f"f32_cond_bwd[B={B} N={N} K={K}]", 4.0 * B * N * K, 0))
+        return
     _launch(lambda: _lib.lib().adp_cond_bwd(dss.data_ptr(), dss.stride(0), cond.data_ptr(),
                                             w.data_ptr(), dw.data_ptr(), dbias.data_ptr(),
                                             _p(dcond), B, N, K, _stream()),
@@ -593,6 +659,7 @@ def cond_bwd(dss: Tensor, cond: Tensor, w: Tensor, dw: Tensor, dbias: Tensor, dc
 def narrow_conv_bwd(dy: Tensor, x: Tensor, stats_in: Tensor, gamma: Tensor, beta: Tensor,
                     w: Tensor, dxh: Tensor, dgamma: Tensor, dbeta: Tensor, S: Tensor, dw: Tensor,
                     dbias: Tensor, groups: int, gn_eps: float = 1e-5) -> Tensor:
+    assert x.dtype == torch.bfloat16, "the fp32 verification mode runs C = 8 ConvBlocks unfused"
     a = NarrowConvBwdArgs()
     a.dy, a.x, a.stats_in = dy.data_ptr(), x.data_ptr(), stats_in.data_ptr()
     a.gamma, a.beta, a.w = gamma.data_ptr(), beta.data_ptr(), w.data_ptr()
@@ -623,6 +690,10 @@ def stem_out_bwd(dv: Tensor, h: Tensor, x: Tensor, w: Tensor, bias: Optional[Ten
     a.ca = 0 if append is None else append.shape[1]
     a.c0, a.co, a.f = h.shape[-1], w.shape[0], f
     a.ld_gate, a.ld_dgate = gate.stride(0), dgate.stride(0)
+    if h.dtype == torch.float32:
+        _launch(lambda: _lib.lib().adp_f32_stem_out_bwd(C.byref(a), _stream()), "adp_f32_stem_out_bwd",
+                lambda: ("f32_stem_out_bwd", 0, _nb(dv, h, x, dh)))
+        return dh
     _launch(lambda: _lib.lib().adp_stem_out_bwd(C.byref(a), _stream()), "adp_stem_out_bwd",
             lambda: ("stem_out_bwd", 0, _nb(dv, h, x, dh)))
     return dh
@@ -640,6 +711,10 @@ def stem_in_bwd(dout: Tensor, x: Tensor, dw: Tensor, dbias: Tensor, f: int, *,
     a.B, a.cx, a.T = x.shape
     a.ca = 0 if append is None else append.shape[1]
     a.c0, a.f = dout.shape[-1], f
+    if dout.dtype == torch.float32:
+        _launch(lambda: _lib.lib().adp_f32_stem_in_bwd(C.byref(a), _stream()), "adp_f32_stem_in_bwd",
+                lambda: ("f32_stem_in_bwd", 0, _nb(dout, x)))
+        return
     _launch(lambda: _lib.lib().adp_stem_in_bwd(C.byref(a), _stream()), "adp_stem_in_bwd",
             lambda: ("stem_in_bwd", 0, _nb(dout, x)))
 
@@ -657,6 +732,11 @@ def attention_bwd(q: Tensor, k: Tensor, v: Tensor, o: Tensor, d_o: Tensor, lse: 
     a.scale = scale
     B, Tq, Tk = a.B, a.Tq, a.Tk
     D, tag = head_dim, _hd_tag(head_dim)
+    if q.dtype == torch.float32:
+        _launch(lambda: _lib.lib().adp_f32_attention_bwd(C.byref(a), D, _stream()), "adp_f32_attention_bwd",
+                lambda: (f"f32_attention_bwd[B={B} H={heads} Tq={Tq} Tk={Tk}{tag}]",
+                         14.0 * B * heads * Tq * Tk * D, 0))
+        return
     _launch(lambda: _lib.lib().adp_attention_bwd_hd(C.byref(a), D, _stream()), "adp_attention_bwd",
             lambda: (f"attention_bwd[B={B} H={heads} Tq={Tq} Tk={Tk}{tag}]", 14.0 * B * heads * Tq * Tk * D,
                      (4 * B * Tq + 4 * B * Tk) * heads * D * 2))

@@ -253,8 +253,8 @@ def resnet_item_bwd(dy: Tensor, x: Tensor, h: Tensor, rr: Tensor, a1: Tensor, a2
     Saved forward tensors: a1 = SiLU(GN1(x)), a2 = SiLU(GN2(h)), GroupNorm statistics x_stats,
     h_stats.  gn1 / gn2 = (gamma, beta); wd1 / wd2 = ops.pack_conv_dgrad packs.  Accumulates the
     parameter gradients gw1 / gw2 ([3, C, C] tap-major), dgn1 / dgn2 = (dgamma, dbeta), db1 / db2;
-    S1 / S2 are the GroupNorm backward sums.  work = (dr, dh, dx, dxh, da) bf16 [B, T, C]
-    buffers.  film = (scale_shift, d scale_shift, row stride, eps) of the ModulationItem, or None
+    S1 / S2 are the GroupNorm backward sums.  work = (dr, dh, dx, dxh, da) activation-dtype
+    [B, T, C] buffers.  film = (scale_shift, d scale_shift, row stride, eps) of the ModulationItem, or None
     without one (dy is then dL/drr).  Returns dx."""
     dr, dh, dx, dxh, da = work
     C = x.shape[-1]
@@ -281,7 +281,7 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
     plan = _TrainPlan()
     G, Fm = net.groups, net.features
     levels = net.levels()
-    bf16 = torch.bfloat16
+    adt = net._act_dtype()         # bf16, or fp32 in the verification mode (B200UNet.verify_fp32)
     loss_mode = mode == "loss"
     heads = net.heads or 0
     D = net.head_features or 64
@@ -289,7 +289,7 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
     att_scale = D ** -0.5
 
     def act(*shape):
-        return torch.empty(*shape, dtype=bf16, device=dev)
+        return torch.empty(*shape, dtype=adt, device=dev)
 
     # ---- static I/O
     cin = net.x_channels + net.append_channels
@@ -299,7 +299,7 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
     plan.alpha = _zeros((B,), dev) if loss_mode else None
     plan.beta = _zeros((B,), dev) if loss_mode else None
     plan.cond = _zeros((B, Fm), dev)                      # SiLU(features), fp32 master
-    plan.cond_bf = torch.zeros(1, B, Fm, dtype=bf16, device=dev)
+    plan.cond_bf = torch.zeros(1, B, Fm, dtype=adt, device=dev)
     plan.loss_sum = torch.zeros(1, dtype=torch.float64, device=dev)
     plan.dv = _zeros((B, net.out_channels, T), dev)
     plan.v = None if loss_mode else _zeros((B, net.out_channels, T), dev)
@@ -307,15 +307,15 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
     plan.dcond = _zeros((B, Fm), dev)
     plan.dxin = _zeros((B, cin, T), dev) if want_dxin else None
     E = net.embedding_features
-    plan.embedding = torch.zeros(B, M, E, dtype=bf16, device=dev) if M else None
-    plan.demb = torch.zeros(B, M, E, dtype=bf16, device=dev) if M else None
-    # InjectChannelsItem context per depth (channels-last bf16, channels zero-padded to 16) + gradient
+    plan.embedding = torch.zeros(B, M, E, dtype=adt, device=dev) if M else None
+    plan.demb = torch.zeros(B, M, E, dtype=adt, device=dev) if M else None
+    # InjectChannelsItem context per depth (channels-last, channels zero-padded to 16) + gradient
     plan.ctx, plan.dctx, t_l = {}, {}, T
     for i, c in enumerate(net.context_channels):
         t_l //= net.factors[i]
         if c > 0:
-            plan.ctx[i] = torch.zeros(B, t_l, ops.round_up(c, 16), dtype=bf16, device=dev)
-            plan.dctx[i] = torch.zeros(B, t_l, ops.round_up(c, 16), dtype=bf16, device=dev)
+            plan.ctx[i] = torch.zeros(B, t_l, ops.round_up(c, 16), dtype=adt, device=dev)
+            plan.dctx[i] = torch.zeros(B, t_l, ops.round_up(c, 16), dtype=adt, device=dev)
 
     # ---- statistics + gradient arenas
     n_items = sum(len(lv.items_down) + len(lv.items_up) for lv in levels)
@@ -323,8 +323,12 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
     plan.fwd.append(lambda: (arena.zero_(), plan.loss_sum.zero_()))
     refreshers: List = []                  # re-pack the dgrad weights in place after a weight update
 
-    def packed_dgrad(make):
-        """make() -> one pack or a tuple of packs, re-made in place by the refreshers."""
+    def packed_dgrad(make_any):
+        """make() -> one pack or a tuple of packs, re-made in place by the refreshers; packed in the
+        activation dtype (the forward packs' B200UNet._compute_packed does the same)."""
+        def make():
+            with ops.pack_dtype(adt):
+                return make_any()
         t = make()
         if isinstance(t, tuple):
             refreshers.append(lambda t=t, make=make: [a.copy_(b) for a, b in zip(t, make())])
@@ -374,7 +378,7 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
     # norm_context affines are folded into each item's to_kv weights)
     en = den = None
     if M:
-        en, den = act(B, M, E), torch.zeros(B, M, E, dtype=bf16, device=dev)
+        en, den = act(B, M, E), torch.zeros(B, M, E, dtype=adt, device=dev)
         plan.fwd.append(lambda: ops.ln_film(plan.embedding, en, None, 0, None, G, net.ATT_LN_EPS))
     # the forward launches; every intermediate the backward reads stays live
     walk = _ForwardWalk(net, P, plan.fwd.append, B, arena, ss_all, keep=True, ctx=plan.ctx,
@@ -458,7 +462,7 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
         dgn2 = (grad_for(r_.gn2.weight), grad_for(r_.gn2.bias))
         db1, db2 = grad_for(r_.conv1.bias), grad_for(r_.conv2.bias)
         dr, dh, dx, dxh = act(B, Tl, C), act(B, Tl, C), act(B, Tl, C), act(B, Tl, C)
-        if C == 8:
+        if res["a1"] is None:      # the forward ran the C = 8 ConvBlocks as adp_narrow_conv
             dw1, dw2 = grad_for(r_.conv1.weight), grad_for(r_.conv2.weight)
             db_scratch = gbuf((C,))
 
@@ -481,6 +485,10 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
             # [tap][co][ci] accumulators of the fused 3-tap wgrad -> PyTorch [co][ci][tap]
             gw1 = grad_for(r_.conv1.weight, (3, C, C), (1, 2, 0))
             gw2 = grad_for(r_.conv2.weight, (3, C, C), (1, 2, 0))
+            if C == 8:
+                # a C = 8 ConvBlock of the fp32 verification mode: the slot of the narrow branch's
+                # bias scratch stays reserved, so every later parameter keeps its arena offset
+                gbuf((C,))
             film = (ss, dss, ss_stride, net.MOD_LN_EPS) if mod else None
 
             def bwd(dy):
@@ -793,9 +801,9 @@ class _UNetFn(torch.autograd.Function):
     def forward(ctx, net: B200UNet, mode: str, x, noise, sigmas, append, cond, embedding, ctx_depths,
                 *rest):
         context, params = rest[:len(ctx_depths)], rest[len(ctx_depths):]
-        if net.verify_fp32:
-            raise NotImplementedError("B200UNet.verify_fp32 covers inference and sampling; run it under "
-                                      "torch.no_grad() (the differentiable program is bf16 only)")
+        if net.verify_fp32 and getattr(net, "_grad_sync", None) is not None:
+            raise NotImplementedError("OverlappedDataParallel does not support B200UNet.verify_fp32; train the "
+                                      "verification mode in one process or under torch DistributedDataParallel")
         B, _, T = x.shape
         M = embedding.shape[1] if (embedding is not None and any(net.cross_attentions)) else 0
         need = ctx.needs_input_grad       # (net, mode, x, noise, sigmas, append, cond, embedding, ...)
@@ -821,7 +829,7 @@ class _UNetFn(torch.autograd.Function):
             plan.beta.copy_(torch.sin(angle))
         if M:
             plan.embedding.copy_(embedding)
-        for d_, c_ in zip(ctx_depths, context):      # [B, ctx, T_d] -> channels-last bf16
+        for d_, c_ in zip(ctx_depths, context):      # [B, ctx, T_d] -> channels-last
             plan.ctx[d_][:, :, : c_.shape[1]].copy_(c_.transpose(1, 2))
         plan.cond.copy_(cond)
         _run(plan, "f", net.use_cuda_graph)

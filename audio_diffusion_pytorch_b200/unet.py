@@ -496,11 +496,13 @@ class B200UNet(nn.Module):
 
     @property
     def verify_fp32(self) -> bool:
-        """fp32 VERIFICATION MODE (inference and sampling): the same launch program, packed-weight
-        layouts and folds, with fp32 storage and fp32 arithmetic on the simple kernels of
-        csrc/verify_f32.cu (the fused thin-level kernels are replaced by their unfused
-        composition).  For checking the program against the reference at rtol 1e-3 / atol 1e-4;
-        ~100x slower than the tensor-core path.  Switching drops every plan and pack."""
+        """fp32 VERIFICATION MODE (inference, sampling and training): the same launch programs,
+        packed-weight layouts and folds -- under autograd the same training program, backward and
+        gradient arena -- with fp32 storage and fp32 arithmetic on the simple kernels of
+        csrc/verify_f32.cu and csrc/verify_f32_bwd.cu (the fused thin-level and C = 8 kernels are
+        replaced by their unfused composition).  For checking the program against the reference at
+        rtol 1e-3 / atol 1e-4; ~100x slower than the tensor-core path.  Not supported under
+        OverlappedDataParallel.  Switching drops every plan and pack."""
         return self._verify_fp32
 
     @verify_fp32.setter
@@ -759,7 +761,9 @@ class B200UNet(nn.Module):
             w_emb = torch.zeros(self.features, kpad, dtype=pd, device=w_all.device)
             w_emb[:, :kdim] = t.to_out.weight.detach().to(pd)
             P["time"] = {"freqs": f32(t.weights), "w_emb": w_emb.contiguous(), "b_emb": f32(t.to_out.bias),
-                         "w_mlp": t.mlp.weight.detach().to(pd).contiguous(),
+                         # a copy also in fp32: an alias would have the in-place re-pack bump the
+                         # version of a weight the time MLP's autograd saved
+                         "w_mlp": t.mlp.weight.detach().to(pd, copy=True).contiguous(),
                          "b_mlp": f32(t.mlp.bias), "kpad": kpad}
         return P
 

@@ -258,7 +258,8 @@ int adp_arv_step(float* chan, const float* v, const float* sig_next, int B, int 
  * the reference at rtol 1e-3 / atol 1e-4.  Same argument meaning as the entry point each one
  * shadows; every activation / weight pointer is fp32; GroupNorm statistics are produced by
  * adp_f32_gn_stats as a separate pass (args->stats, fused GroupNorm, noising and the fused loss
- * must be unset).  ~100x slower than the tensor-core path: never used for measurement. */
+ * must be unset; the training forward's noising and loss are the _train variants below).
+ * ~100x slower than the tensor-core path: never used for measurement. */
 int adp_f32_conv_gemm(const adp_conv_gemm_args* args, adp_stream_t stream);
 int adp_f32_gn_stats(const float* x, double* stats, int B, int T, int C, int groups, adp_stream_t stream);
 int adp_f32_gn_silu(const float* x, float* y, const double* stats, const float* gamma, const float* beta,
@@ -457,6 +458,46 @@ typedef struct adp_stem_in_bwd_args {
   int32_t B, T, cx, ca, c0, f;
 } adp_stem_in_bwd_args;
 int adp_stem_in_bwd(const adp_stem_in_bwd_args* args, adp_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------
+ * The TRAINING program in the fp32 verification mode (training.build_train_plan with verify_fp32):
+ * the forward outputs the training step adds, and one fp32 twin per backward launch kind.  Same
+ * arguments and semantics as the bf16 entry point named in each comment, with every activation and
+ * activation-gradient pointer (bf16 there) fp32; parameter gradients accumulate as there.  GroupNorm
+ * statistics stay separate adp_f32_gn_stats passes.  Sizes are validated before anything is launched. */
+/* adp_f32_attention_hd plus the log-sum-exp rows lse fp32 [B][H][Tq] (adp_attention_hd's lse) */
+int adp_f32_attention_lse(const float* q, const float* k, const float* v, float* o, int B, int H, int head_dim,
+                          int Tq, int Tk, int ldq, int ldk, int ldv, int ldo, float scale, float* lse,
+                          adp_stream_t stream);
+/* adp_f32_stem_in with the VDiffusion noising (args->noise / alpha / beta, as adp_stem_in) */
+int adp_f32_stem_in_train(const adp_stem_in_args* args, adp_stream_t stream);
+/* adp_f32_stem_out with the fused loss: args->noise / alpha / beta, loss_sum (fp64, accumulated),
+ * dv (as adp_stem_out); no guidance or sampler fusion together with the loss */
+int adp_f32_stem_out_train(const adp_stem_out_args* args, adp_stream_t stream);
+int adp_f32_wgrad(const adp_wgrad_args* args, adp_stream_t stream);                 /* adp_wgrad */
+int adp_f32_gn_silu_bwd(const float* da, const float* x, const double* stats, const float* gamma,
+                        const float* beta, float* dxh, float* dgamma, float* dbeta, double* S, int B, int T,
+                        int C, int groups, float eps, adp_stream_t stream);          /* adp_gn_silu_bwd */
+int adp_f32_gn_bwd_apply(const float* dxh, const float* x, const double* stats, const double* S,
+                         const float* dres, float* dx, float* colsum, int B, int T, int C, int groups, float eps,
+                         adp_stream_t stream);                                       /* adp_gn_bwd_apply */
+int adp_f32_ln_film_bwd(const float* dy, const float* x, const float* scale_shift, int ss_stride, float* dx,
+                        float* dss, int dss_stride, float* colsum, const float* dres, int B, int T, int C,
+                        float eps, adp_stream_t stream);                             /* adp_ln_film_bwd */
+int adp_f32_colsum(const float* x, const float* gate, int ld_gate, float* out, int B, int T, int C,
+                   adp_stream_t stream);                                             /* adp_colsum */
+/* adp_skip_gate without its statistics (stats must be NULL) */
+int adp_f32_skip_gate(const float* y, const float* skip, const float* gate, int ld_gate, float* out,
+                      double* stats, int B, int T, int C, int groups, adp_stream_t stream);
+int adp_f32_skip_gate_bwd(const float* dout, const float* y, const float* gate, int ld_gate, float* dys,
+                          float* dgate, int ld_dgate, int B, int T, int C, adp_stream_t stream); /* adp_skip_gate_bwd */
+/* adp_cond_bwd with the projection weights w fp32 [N][K] */
+int adp_f32_cond_bwd(const float* dss, int ld_dss, const float* cond, const float* w, float* dw, float* dbias,
+                     float* dcond, int B, int N, int K, adp_stream_t stream);
+int adp_f32_stem_out_bwd(const adp_stem_out_bwd_args* args, adp_stream_t stream);   /* adp_stem_out_bwd */
+int adp_f32_stem_in_bwd(const adp_stem_in_bwd_args* args, adp_stream_t stream);     /* adp_stem_in_bwd */
+int adp_f32_attention_bwd(const adp_attention_bwd_args* args, int head_dim,
+                          adp_stream_t stream);                                      /* adp_attention_bwd_hd */
 
 #ifdef __cplusplus
 }
