@@ -99,14 +99,15 @@ __device__ __forceinline__ float silu_tanh(float z) {
 // shuffles and lane 0 adds into the warp's OWN shared-memory column.  Each column has a single
 // writer and the columns are summed in warp order, so the statistics do not depend on the
 // order in which warps finish (only the fp64 global reduction across CTAs does).
+// The shuffles sit outside any test of cur_g, and callers derive g from warp-uniform values
+// only: shuffles under a branch that ptxas cannot prove warp-uniform make it serialize the
+// kernel's wgmma instructions (C7520).
 struct WarpStats {
   int cur_g = -1;
   float s = 0.f, q = 0.f;
   __device__ __forceinline__ void flush(float (*slots)[8], int w, int lane) {
-    if (cur_g >= 0) {
-      const float ws = warp_sum(s), wq = warp_sum(q);
-      if (lane == 0) { slots[2 * cur_g][w] += ws; slots[2 * cur_g + 1][w] += wq; }
-    }
+    const float ws = warp_sum(s), wq = warp_sum(q);   // zero while cur_g < 0
+    if (lane == 0 && cur_g >= 0) { slots[2 * cur_g][w] += ws; slots[2 * cur_g + 1][w] += wq; }
     s = 0.f; q = 0.f;
   }
   __device__ __forceinline__ void add(float v, int g, float (*slots)[8], int w, int lane) {
@@ -420,7 +421,7 @@ conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const float2 q_lo = ok_lo ? unpack_bf16(o_lo) : make_float2(0.f, 0.f);
         const float2 q_hi = ok_hi ? unpack_bf16(o_hi) : make_float2(0.f, 0.f);
         if (p.group_shift >= 3) {          // the 8-column block lies in one group: warp-uniform
-          const int g = ch >> p.group_shift;
+          const int g = (ti.ch0 + jb * 8) >> p.group_shift;   // = ch >> shift, without the lane
           acc_st.add(q_lo.x, g, s_part, warp, lane); acc_st.add(q_lo.y, g, s_part, warp, lane);
           acc_st.add(q_hi.x, g, s_part, warp, lane); acc_st.add(q_hi.y, g, s_part, warp, lane);
         } else if (narrow) {

@@ -61,14 +61,13 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   return ok != 0;
 }
 // Bounded wait: a protocol bug must trap (-> CUDA error on the host), never hang the GPU box.
+// No printf here: a device-side printf call on a wait path makes ptxas serialize every wgmma of
+// the calling kernel (C7520, "compiler-inserted WG.AR in divergent path": each HGMMA is
+// followed by a wait for its own completion).
 static __device__ __noinline__ void mbar_wait_slow(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 24)) {
-      printf("adp: mbarrier wait timed out (block %d,%d thread %d)\n", blockIdx.x, blockIdx.y,
-             threadIdx.x);
-      __trap();
-    }
+    if (++spins > (1u << 24)) __trap();
   }
 }
 // fast path: one probe inline (the issue loops run this once per pipeline stage)
