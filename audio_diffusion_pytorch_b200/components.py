@@ -51,8 +51,9 @@ def LTPlugin(net_t: Callable, num_filters: int, window_length: int, stride: int)
     (Conv1d, reflect padding, bias-free) in front of the net and its transposed counterpart behind
     it; the net runs on `in_channels * num_filters` channels at 1/stride of the rate.  The two
     filterbank convolutions are PyTorch modules around the net call; with the CUDA U-Net inside, its
-    stem limits apply to the TRANSFORMED widths (in_channels * num_filters <= 8 inputs,
-    out_channels * num_filters <= 4 outputs) and are asserted by its constructor."""
+    boundary limits apply to the TRANSFORMED widths (in_channels * num_filters <= 64 inputs and
+    outputs, in_channels * num_filters * factors[0] <= 128, channels[0] <= 256; stereo x 32 filters
+    fits) and are asserted by its constructor."""
 
     def Net(dim: int, in_channels: int, out_channels: Optional[int] = None, **kwargs) -> nn.Module:
         assert dim == 1, "the reference builds a ConvTranspose1d decoder: dim must be 1"

@@ -499,6 +499,263 @@ __global__ void __launch_bounds__(256) narrow_conv_kernel(const adp_narrow_conv_
   }
 }
 
+// ------------------------------------------------------------------ wide boundary (stem_in)
+// Boundaries the register-array kernels above cannot hold: (cx+ca)*f up to 128 inputs per output
+// position.  Weights live in smem transposed to [ci][c0] (256 x 128 fp32 = 128 KiB at the corner),
+// the input tile [ci][kWideTP] is staged through smem with coalesced NCW reads, and each thread
+// computes 8 output channels of one position per pass (the warp shares the channel chunk: the
+// weight reads are 16-byte broadcasts).
+constexpr int kWideTP = 64;          // low-rate positions per stem_in tile
+constexpr int kWideMaxIn = 128;      // (cx+ca)*f
+constexpr int kWideMaxCin = 64;      // cx+ca
+constexpr int kWideMaxCo = 64;
+
+__global__ void __launch_bounds__(256) stem_in_wide_kernel(const adp_stem_in_args a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  extern __shared__ __align__(16) float s_dyn[];
+  __shared__ float s_stats[2 * 64];
+  const int cin = a.cx + a.ca, ci_total = cin * a.f;
+  float* s_w = s_dyn;                                   // [ci_total][c0]
+  float* s_b = s_w + ci_total * a.c0;                   // [c0]
+  float* s_in = s_b + a.c0;                             // [ci_total][kWideTP + 1]
+  constexpr int LD = kWideTP + 1;
+  for (int i = threadIdx.x; i < a.c0 * ci_total; i += blockDim.x) {
+    const int o = i / ci_total, ii = i - o * ci_total;
+    s_w[ii * a.c0 + o] = a.w[i];
+  }
+  for (int i = threadIdx.x; i < a.c0; i += blockDim.x) s_b[i] = a.bias ? a.bias[i] : 0.f;
+  if (threadIdx.x < 128) s_stats[threadIdx.x] = 0.f;
+
+  const int b = blockIdx.y;
+  const int lane = threadIdx.x & 31;
+  const int p = threadIdx.x % kWideTP, cg = threadIdx.x / kWideTP;
+  const int To = a.T / a.f;
+  const float al = a.noise ? a.alpha[b] : 1.f, be = a.noise ? a.beta[b] : 0.f;
+  const int gsz = a.stats ? a.c0 / a.groups : 1;
+  GroupStatAcc acc;
+  const int n_tiles = (To + kWideTP - 1) / kWideTP;
+  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const int to0 = tile * kWideTP;
+    __syncthreads();                                    // weights staged / previous tile consumed
+    // (c, tt) with tt contiguous in memory -> s_in[(c*f + j)][p], tt = p*f + j
+    const int span = kWideTP * a.f;
+    for (int i = threadIdx.x; i < cin * span; i += blockDim.x) {
+      const int c = i / span, r = i - c * span, pp = r / a.f, j = r - pp * a.f;
+      const size_t tt = static_cast<size_t>(to0) * a.f + r;
+      float v = 0.f;
+      if (to0 + pp < To) {
+        if (c < a.cx) {
+          const size_t idx = (static_cast<size_t>(b) * a.cx + c) * a.T + tt;
+          v = __ldg(a.x + idx);
+          if (a.noise) v = al * v + be * __ldg(a.noise + idx);   // reference diffusion.py:91
+        } else {
+          v = __ldg(a.append + (static_cast<size_t>(b) * a.ca + (c - a.cx)) * a.T + tt);
+        }
+      }
+      s_in[(c * a.f + j) * LD + pp] = v;
+    }
+    __syncthreads();
+    const int to = to0 + p;
+    const bool ok = to < To;
+    __nv_bfloat16* orow =
+        static_cast<__nv_bfloat16*>(a.out) + (static_cast<size_t>(b) * To + (ok ? to : 0)) * a.c0;
+    for (int ch = cg; ch < a.c0 / 8; ch += 256 / kWideTP) {
+      float v[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[j] = s_b[ch * 8 + j];
+      for (int ii = 0; ii < ci_total; ++ii) {
+        const float xv = s_in[ii * LD + p];
+        const float4 w0 = *reinterpret_cast<const float4*>(s_w + ii * a.c0 + ch * 8);
+        const float4 w1 = *reinterpret_cast<const float4*>(s_w + ii * a.c0 + ch * 8 + 4);
+        v[0] += xv * w0.x; v[1] += xv * w0.y; v[2] += xv * w0.z; v[3] += xv * w0.w;
+        v[4] += xv * w1.x; v[5] += xv * w1.y; v[6] += xv * w1.z; v[7] += xv * w1.w;
+      }
+      uint4 o;
+      o.x = pack_bf16(v[0], v[1]); o.y = pack_bf16(v[2], v[3]);
+      o.z = pack_bf16(v[4], v[5]); o.w = pack_bf16(v[6], v[7]);
+      if (ok) *reinterpret_cast<uint4*>(orow + ch * 8) = o;
+      if (a.stats) {        // statistics of the ROUNDED values the next layer reads
+        const uint32_t ou[4] = {o.x, o.y, o.z, o.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float2 r = unpack_bf16(ou[j]);
+          acc.add(ok ? r.x : 0.f, (ch * 8 + 2 * j) / gsz, s_stats, lane);
+          acc.add(ok ? r.y : 0.f, (ch * 8 + 2 * j + 1) / gsz, s_stats, lane);
+        }
+      }
+    }
+  }
+  if (a.stats) {
+    acc.flush(s_stats, lane);
+    __syncthreads();
+    if (threadIdx.x < 2 * a.groups && s_stats[threadIdx.x] != 0.f)
+      atomicAdd(a.stats + static_cast<size_t>(b) * 2 * a.groups + threadIdx.x,
+                static_cast<double>(s_stats[threadIdx.x]));
+  }
+}
+
+// ----------------------------------------------------------------- wide boundary (stem_out)
+// Up to 64 outputs and 64 block-input channels.  A tile is kWideOP output positions; the conv3 on
+// the nearest-upsampled h runs over c0 in chunks of kWideCK channels (h rows and the [co][3][ck]
+// weight slice staged in smem, 192 KiB of weights at co = 64, c0 = 256 never resident at once).
+// Thread = (position, output parity): up to 32 outputs per thread accumulate in registers, the
+// warp shares its outputs (broadcast weight reads).  The block input cat([x(_noisy), append]) of
+// the whole tile is staged before any store, so x_next may alias x.
+constexpr int kWideOP = 128;
+constexpr int kWideCK = 32;
+constexpr int kWideHL = kWideCK + 4;     // padded h row (16-byte aligned)
+constexpr int kWideOPT = kWideMaxCo / 2; // outputs per thread
+
+__device__ __forceinline__ void stem_out_wide_conv(const adp_stem_out_args& a, const __nv_bfloat16* hb,
+                                                   float* s_h, const float* s_wc, int t0, int q_base,
+                                                   int rows, int c_base, int p, int og,
+                                                   float (&y)[kWideOPT]) {
+  const int Tl = a.T / a.f;
+  const int nck = min(kWideCK, a.c0 - c_base);
+  __syncthreads();                                 // s_h free
+  for (int i = threadIdx.x; i < rows * (kWideCK / 8); i += blockDim.x) {
+    const int r = i / (kWideCK / 8), c8 = (i - r * (kWideCK / 8)) * 8, q = q_base + r;
+    float4 lo = make_float4(0.f, 0.f, 0.f, 0.f), hi = lo;
+    if (q >= 0 && q < Tl && c8 < nck) {
+      const uint4 u = __ldg(reinterpret_cast<const uint4*>(hb + static_cast<size_t>(q) * a.c0 + c_base + c8));
+      const float2 f0 = unpack_bf16(u.x), f1 = unpack_bf16(u.y), f2 = unpack_bf16(u.z), f3 = unpack_bf16(u.w);
+      lo = make_float4(f0.x, f0.y, f1.x, f1.y);
+      hi = make_float4(f2.x, f2.y, f3.x, f3.y);
+    }
+    *reinterpret_cast<float4*>(s_h + r * kWideHL + c8) = lo;
+    *reinterpret_cast<float4*>(s_h + r * kWideHL + c8 + 4) = hi;
+  }
+  __syncthreads();
+  const int t = t0 + p;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const int u = t + k - 1;
+    if (u < 0 || u >= a.T) continue;               // zero padding of the upsampled signal
+    const float* hr = s_h + (u / a.f - q_base) * kWideHL;
+    for (int c4 = 0; c4 < nck; c4 += 4) {
+      const float4 hv = *reinterpret_cast<const float4*>(hr + c4);
+#pragma unroll
+      for (int m = 0; m < kWideOPT; ++m) {
+        const int o = og + 2 * m;
+        if (o < a.co) {
+          const float4 w = *reinterpret_cast<const float4*>(s_wc + (o * 3 + k) * kWideCK + c4);
+          y[m] += (hv.x * w.x + hv.y * w.y) + (hv.z * w.z + hv.w * w.w);
+        }
+      }
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256) stem_out_wide_kernel(const adp_stem_out_args a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  extern __shared__ __align__(16) float s_dyn[];
+  __shared__ double s_loss[8];
+  const int cin = a.cx + a.ca;
+  const int ldg = a.ld_gate > 0 ? a.ld_gate : a.co;
+  const int rows = (kWideOP + 1) / a.f + 2;        // low-rate rows feeding positions t0-1 .. t0+OP
+  float* s_wc = s_dyn;                             // [co][3][CK] weight slice of one c0 chunk
+  float* s_h = s_wc + a.co * 3 * kWideCK;          // [rows][HL]
+  float* s_xin = s_h + rows * kWideHL;             // [cin][OP]
+  float* s_wa = s_xin + cin * kWideOP;             // [co][cin]
+  float* s_ba = s_wa + a.co * cin;                 // [co]
+  if (a.w_adapt)
+    for (int i = threadIdx.x; i < a.co * cin; i += blockDim.x) s_wa[i] = a.w_adapt[i];
+  for (int i = threadIdx.x; i < a.co; i += blockDim.x) s_ba[i] = a.b_adapt ? a.b_adapt[i] : 0.f;
+
+  const int b = blockIdx.y;
+  const int p = threadIdx.x % kWideOP, og = threadIdx.x / kWideOP;
+  const int Tl = a.T / a.f;
+  const float al = a.noise ? a.alpha[b] : 1.f, be = a.noise ? a.beta[b] : 0.f;
+  const __nv_bfloat16* h = static_cast<const __nv_bfloat16*>(a.h);
+  double lsum = 0.0;
+  const int n_tiles = (a.T + kWideOP - 1) / kWideOP;
+  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const int t0 = tile * kWideOP;
+    const int q_base = t0 == 0 ? -1 : (t0 - 1) / a.f;
+    const int t = t0 + p;
+    const bool ok = t < a.T;
+    __syncthreads();                               // previous tile's s_xin consumed
+    for (int i = threadIdx.x; i < cin * kWideOP; i += blockDim.x) {
+      const int c = i / kWideOP, r = i - c * kWideOP, tt = t0 + r;
+      float v = 0.f;
+      if (tt < a.T) {
+        if (c < a.cx) {
+          const size_t idx = (static_cast<size_t>(b) * a.cx + c) * a.T + tt;
+          v = a.x[idx];
+          if (a.noise) v = al * v + be * a.noise[idx];
+        } else {
+          v = a.append[(static_cast<size_t>(b) * a.ca + (c - a.cx)) * a.T + tt];
+        }
+      }
+      s_xin[i] = v;
+    }
+    float y[kWideOPT], ym[kWideOPT];
+#pragma unroll
+    for (int m = 0; m < kWideOPT; ++m) {
+      const int o = og + 2 * m;
+      y[m] = (o < a.co && a.bias) ? a.bias[o] : 0.f;
+      ym[m] = y[m];
+    }
+    for (int c_base = 0; c_base < a.c0; c_base += kWideCK) {
+      const int nck = min(kWideCK, a.c0 - c_base);
+      __syncthreads();                             // s_wc free
+      for (int i = threadIdx.x; i < a.co * 3 * kWideCK; i += blockDim.x) {
+        // PyTorch layout [co][c0][3] -> [co][3][CK], zero beyond the chunk
+        const int o = i / (3 * kWideCK), r = i - o * 3 * kWideCK, k = r / kWideCK, c = r - k * kWideCK;
+        s_wc[i] = c < nck ? a.w[(static_cast<size_t>(o) * a.c0 + c_base + c) * 3 + k] : 0.f;
+      }
+      stem_out_wide_conv(a, h + static_cast<size_t>(b) * Tl * a.c0, s_h, s_wc, t0, q_base, rows, c_base,
+                         p, og, y);
+      if (a.cfg)
+        stem_out_wide_conv(a, h + static_cast<size_t>(b + a.B) * Tl * a.c0, s_h, s_wc, t0, q_base, rows,
+                           c_base, p, og, ym);
+    }
+    if (!ok) continue;
+#pragma unroll
+    for (int m = 0; m < kWideOPT; ++m) {
+      const int o = og + 2 * m;
+      if (o >= a.co) continue;
+      float skip;
+      if (a.w_adapt) {                             // SkipAdapter 1x1 conv (in != out channels)
+        skip = s_ba[o];
+        for (int c = 0; c < cin; ++c) skip += s_xin[c * kWideOP + p] * s_wa[o * cin + c];
+      } else {
+        skip = s_xin[o * kWideOP + p];
+      }
+      float v = skip + a.gate[static_cast<size_t>(b) * ldg + o] * y[m];     // MergeModulate
+      if (a.cfg) {
+        const float vm = skip + a.gate[static_cast<size_t>(b + a.B) * ldg + o] * ym[m];
+        v = vm + (v - vm) * a.cfg_scale;                                   // CFG combine
+      }
+      const size_t oidx = (static_cast<size_t>(b) * a.co + o) * a.T + t;
+      if (a.v_out) a.v_out[oidx] = v;
+      if (a.x_next) {                              // reference diffusion.py:185-187
+        const float a0 = a.ab[0], b0 = a.ab[1], a1 = a.ab[2], b1 = a.ab[3];
+        const float xv = s_xin[o * kWideOP + p];
+        a.x_next[oidx] = a1 * (a0 * xv - b0 * v) + b1 * (b0 * xv + a0 * v);
+      }
+      if (a.loss_sum) {                            // reference diffusion.py:92,95
+        const size_t xidx = (static_cast<size_t>(b) * a.cx + o) * a.T + t;
+        const float d = v - (al * a.noise[xidx] - be * a.x[xidx]);
+        lsum += static_cast<double>(d) * d;
+        if (a.dv) a.dv[oidx] = 2.f * d / (static_cast<float>(a.B) * a.co * a.T);
+      }
+    }
+  }
+  if (a.loss_sum) {
+    for (int o = 16; o > 0; o >>= 1) lsum += __shfl_xor_sync(0xffffffffu, lsum, o);
+    if ((threadIdx.x & 31) == 0) s_loss[threadIdx.x >> 5] = lsum;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      double tot = 0.0;
+      for (int i = 0; i < (blockDim.x >> 5); ++i) tot += s_loss[i];
+      atomicAdd(a.loss_sum, tot);
+    }
+  }
+}
+
 int mid_conv(const adp_narrow_conv_args& a, cudaStream_t stream);   // mid_conv.cu
 
 }  // namespace adp
@@ -508,12 +765,23 @@ using namespace adp;
 extern "C" int adp_stem_in(const adp_stem_in_args* args, adp_stream_t stream) {
   ADP_CHECK(args && args->x && args->w && args->out, "adp_stem_in: null pointer");
   const adp_stem_in_args& a = *args;
-  ADP_CHECK((a.cx + a.ca) * a.f <= kStemMaxIn && a.f >= 1 && a.T % a.f == 0,
-            "adp_stem_in: (cx+ca)*f = %d > %d or T %% f != 0", (a.cx + a.ca) * a.f, kStemMaxIn);
+  const int cin = a.cx + a.ca;
+  ADP_CHECK(cin <= kWideMaxCin, "adp_stem_in: cx+ca = %d > %d", cin, kWideMaxCin);
+  ADP_CHECK(a.f >= 1 && cin * a.f <= kWideMaxIn && a.T % a.f == 0,
+            "adp_stem_in: (cx+ca)*f = %d > %d or T %% f != 0", cin * a.f, kWideMaxIn);
   ADP_CHECK(a.c0 % 8 == 0 && a.c0 <= kStemMaxC0, "adp_stem_in: c0=%d unsupported", a.c0);
   ADP_CHECK((a.ca == 0) == (a.append == nullptr), "adp_stem_in: append / ca mismatch");
   ADP_CHECK(!a.noise || (a.alpha && a.beta), "adp_stem_in: noise needs alpha/beta");
   if (a.stats) ADP_CHECK(a.groups > 0 && a.groups <= 64 && a.c0 % a.groups == 0, "adp_stem_in: groups");
+  if (cin * a.f > kStemMaxIn) {
+    const size_t smem = (static_cast<size_t>(cin) * a.f * (a.c0 + kWideTP + 1) + a.c0) * sizeof(float);
+    static SmemAttrCache smem_cache;
+    ADP_CUDA(ensure_dyn_smem(stem_in_wide_kernel, smem, smem_cache));
+    dim3 grid(persistent_gx(stem_in_wide_kernel, 256, smem, a.B, (a.T / a.f + kWideTP - 1) / kWideTP), a.B);
+    ADP_CUDA(launch_k(stem_in_wide_kernel, grid, dim3(256), smem, as_stream(stream), a));
+    ADP_LAUNCH_CHECK();
+    return 0;
+  }
   const size_t smem = (static_cast<size_t>(a.c0) * (a.cx + a.ca) * a.f + a.c0) * sizeof(float);
   const int n_tiles = (a.T / a.f + 255) / 256;
   if ((a.cx + a.ca) * a.f <= 4) {
@@ -530,14 +798,28 @@ extern "C" int adp_stem_in(const adp_stem_in_args* args, adp_stream_t stream) {
 extern "C" int adp_stem_out(const adp_stem_out_args* args, adp_stream_t stream) {
   ADP_CHECK(args && args->h && args->x && args->w && args->gate, "adp_stem_out: null pointer");
   const adp_stem_out_args& a = *args;
-  ADP_CHECK(a.co >= 1 && a.co <= kStemMaxCo && a.cx + a.ca <= 8 && a.co <= a.cx,
-            "adp_stem_out: co=%d cx=%d ca=%d unsupported", a.co, a.cx, a.ca);
+  const int cin = a.cx + a.ca;
+  ADP_CHECK(a.co >= 1 && a.co <= kWideMaxCo && a.ca >= 0 && cin <= kWideMaxCin && a.co <= a.cx,
+            "adp_stem_out: co=%d cx=%d ca=%d unsupported (co <= cx, co <= %d, cx+ca <= %d)", a.co, a.cx,
+            a.ca, kWideMaxCo, kWideMaxCin);
   ADP_CHECK(a.c0 % 8 == 0 && a.c0 <= kStemMaxC0 && a.f >= 1 && a.T % a.f == 0,
             "adp_stem_out: c0=%d f=%d", a.c0, a.f);
   ADP_CHECK(a.w_adapt || a.cx + a.ca == a.co, "adp_stem_out: identity skip needs cx+ca == co");
   ADP_CHECK((a.ca == 0) == (a.append == nullptr), "adp_stem_out: append / ca mismatch");
   ADP_CHECK(!a.x_next || a.ab, "adp_stem_out: x_next needs ab");
   ADP_CHECK(!a.loss_sum || (a.noise && a.alpha && a.beta), "adp_stem_out: loss needs noise/alpha/beta");
+  if (a.co > kStemMaxCo || cin > 8) {
+    ADP_CHECK(!a.loss_sum || !a.x_next, "adp_stem_out: the loss excludes the sampler fusion");
+    const int rows = (kWideOP + 1) / a.f + 2;
+    const size_t smem = (static_cast<size_t>(a.co) * 3 * kWideCK + static_cast<size_t>(rows) * kWideHL +
+                         static_cast<size_t>(cin) * kWideOP + a.co * cin + a.co) * sizeof(float);
+    static SmemAttrCache smem_cache;
+    ADP_CUDA(ensure_dyn_smem(stem_out_wide_kernel, smem, smem_cache));
+    dim3 grid(persistent_gx(stem_out_wide_kernel, 256, smem, a.B, (a.T + kWideOP - 1) / kWideOP), a.B);
+    ADP_CUDA(launch_k(stem_out_wide_kernel, grid, dim3(256), smem, as_stream(stream), a));
+    ADP_LAUNCH_CHECK();
+    return 0;
+  }
   const size_t smem =
       (static_cast<size_t>(a.co) * 3 * a.c0 + 2 * a.co + a.co * (a.cx + a.ca)) * sizeof(float);
   dim3 grid(persistent_gx(stem_out_kernel, 256, smem, a.B, (a.T + 255) / 256), a.B);

@@ -545,6 +545,295 @@ __global__ void __launch_bounds__(kTB) stem_in_bwd_kernel(const adp_stem_in_bwd_
   }
 }
 
+// ------------------------------------------------------------ wide boundary (stem_out_bwd)
+// Sizes the kernels above do not take: up to 64 outputs, 64 block-input channels, c0 up to 256,
+// any f.  Three kernels, each with a fixed thread -> output mapping and every sum in fp32:
+//   dh    per (low-rate row q, channel c): sum_{o,k} w[o][c][k] D[q][o][k], where
+//         D[q][o][k] = sum of dy over the f upsampled positions fed by row q, shifted by the tap;
+//   param per (output o, channel c) of a slice: G_k = sum_t dvs[t][o] src[t+k-1][c] over a run of
+//         tiles of one batch element, src = nearest-upsampled h (three taps) or the block input
+//         (the SkipAdapter, one tap).  Since dy = dvs * gate[b][o], dw = gate * G and
+//         dgate[b][o] = bias[o] sum_t dvs + sum_{c,k} w[o][c][k] G_k; one atomic per element per block;
+//   dxin  per (channel, position): W_adapt^T dvs (or dvs, identity skip), stored.
+constexpr int kWideQT = 32;      // low-rate rows per dh tile
+constexpr int kWideCKb = 32;     // channels per dh / param slice
+constexpr int kWideOS = 8;       // outputs per param slice
+constexpr int kWidePT = 128;     // positions per param tile
+
+__device__ __forceinline__ float so_wide_dvs(const adp_stem_out_bwd_args& a, float gscale, int b, int o, int t) {
+  return (t >= 0 && t < a.T) ? a.dv[(static_cast<size_t>(b) * a.co + o) * a.T + t] * gscale : 0.f;
+}
+
+__global__ void __launch_bounds__(256) stem_out_bwd_wide_dh_kernel(const adp_stem_out_bwd_args a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  extern __shared__ float s_dyn[];
+  const int n3 = a.co * 3, ld_d = n3 + 1;
+  float* s_w = s_dyn;                              // [co*3][CK]: w[o][c_base + c][k]
+  float* s_d = s_w + n3 * kWideCKb;                // [QT][co*3 + 1]
+  const int b = blockIdx.y, c_base = blockIdx.z * kWideCKb;
+  const int Tl = a.T / a.f;
+  const int ldg = a.ld_gate > 0 ? a.ld_gate : a.co;
+  const float gscale = a.gscale ? a.gscale[0] : 1.f;
+  for (int i = threadIdx.x; i < n3 * kWideCKb; i += blockDim.x) {
+    const int ok3 = i / kWideCKb, c = i - ok3 * kWideCKb, o = ok3 / 3, k = ok3 - o * 3;
+    s_w[i] = c_base + c < a.c0 ? a.w[(static_cast<size_t>(o) * a.c0 + c_base + c) * 3 + k] : 0.f;
+  }
+  const int c = threadIdx.x & 31, rg = threadIdx.x >> 5;
+  const int n_tiles = (Tl + kWideQT - 1) / kWideQT;
+  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const int q0 = tile * kWideQT;
+    __syncthreads();
+    // D[r][o][k]: tap k of output t reads upsampled position u = t + k - 1, so row q collects
+    // dy[t] for t in [q f - k + 1, q f + f - k + 1)
+    for (int i = threadIdx.x; i < kWideQT * a.co; i += blockDim.x) {
+      const int o = i / kWideQT, r = i - o * kWideQT, q = q0 + r;
+      float s0 = 0.f, s1 = 0.f, s2 = 0.f;
+      if (q < Tl) {
+        const int u0 = q * a.f;
+        float mid = 0.f;                                               // t in [u0+1, u0+f-1)
+        for (int u = u0 + 1; u < u0 + a.f - 1; ++u) mid += so_wide_dvs(a, gscale, b, o, u);
+        const float first = so_wide_dvs(a, gscale, b, o, u0);
+        const float last = a.f > 1 ? so_wide_dvs(a, gscale, b, o, u0 + a.f - 1) : 0.f;
+        s1 = first + mid + last;                                       // t in [u0, u0+f)
+        s0 = mid + last + so_wide_dvs(a, gscale, b, o, u0 + a.f);      // t in [u0+1, u0+f]
+        s2 = so_wide_dvs(a, gscale, b, o, u0 - 1) + (a.f > 1 ? first + mid : 0.f);   // [u0-1, u0+f-1)
+        const float g = a.gate[static_cast<size_t>(b) * ldg + o];
+        s0 *= g; s1 *= g; s2 *= g;
+      }
+      float* d = s_d + r * ld_d + o * 3;
+      d[0] = s0; d[1] = s1; d[2] = s2;
+    }
+    __syncthreads();
+    if (c_base + c < a.c0) {
+      float acc[kWideQT / 8];
+#pragma unroll
+      for (int i = 0; i < kWideQT / 8; ++i) acc[i] = 0.f;
+      for (int j = 0; j < n3; ++j) {
+        const float w = s_w[j * kWideCKb + c];
+#pragma unroll
+        for (int i = 0; i < kWideQT / 8; ++i) acc[i] += w * s_d[(rg + 8 * i) * ld_d + j];
+      }
+      __nv_bfloat16* dh = static_cast<__nv_bfloat16*>(a.dh);
+#pragma unroll
+      for (int i = 0; i < kWideQT / 8; ++i) {
+        const int q = q0 + rg + 8 * i;
+        if (q < Tl) dh[(static_cast<size_t>(b) * Tl + q) * a.c0 + c_base + c] = __float2bfloat16_rn(acc[i]);
+      }
+    }
+  }
+}
+
+// blockIdx.z = (o slice) * (h chunks + adapter chunks) + chunk
+__global__ void __launch_bounds__(256) stem_out_bwd_wide_param_kernel(const adp_stem_out_bwd_args a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  extern __shared__ float s_dyn[];
+  const int cin = a.cx + a.ca;
+  const int n_hc = (a.c0 + kWideCKb - 1) / kWideCKb;
+  const int n_chunks = n_hc + (a.w_adapt ? (cin + kWideCKb - 1) / kWideCKb : 0);
+  const int os = blockIdx.z / n_chunks, chunk = blockIdx.z - os * n_chunks;
+  const bool on_h = chunk < n_hc;                  // else: SkipAdapter slice on the block input
+  const int c_base = (on_h ? chunk : chunk - n_hc) * kWideCKb;
+  const int nc = on_h ? a.c0 : cin;
+  const int f = on_h ? a.f : 1;
+  const int rows = (kWidePT + 1) / f + 2;
+  float* s_dvs = s_dyn;                            // [OS][PT]
+  float* s_src = s_dvs + kWideOS * kWidePT;        // [rows][CK + 1]
+  constexpr int LS = kWideCKb + 1;
+  const int b = blockIdx.y;
+  const int Tl = a.T / a.f;
+  const float gscale = a.gscale ? a.gscale[0] : 1.f;
+  const float al = a.noise ? a.alpha[b] : 1.f, be = a.noise ? a.beta[b] : 0.f;
+  const int c = threadIdx.x & 31, ol = threadIdx.x >> 5, o = os * kWideOS + ol;
+  const int n_tiles = (a.T + kWidePT - 1) / kWidePT;
+  float g0 = 0.f, g1 = 0.f, g2 = 0.f, sdv = 0.f;
+  const __nv_bfloat16* hb = static_cast<const __nv_bfloat16*>(a.h) + static_cast<size_t>(b) * Tl * a.c0;
+  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const int t0 = tile * kWidePT;
+    const int q_base = t0 == 0 ? -1 : (t0 - 1) / f;
+    __syncthreads();
+    for (int i = threadIdx.x; i < kWideOS * kWidePT; i += blockDim.x) {
+      const int oo = os * kWideOS + i / kWidePT, t = t0 + i % kWidePT;
+      s_dvs[i] = oo < a.co ? so_wide_dvs(a, gscale, b, oo, t) : 0.f;
+    }
+    if (on_h) {
+      for (int i = threadIdx.x; i < rows * kWideCKb; i += blockDim.x) {
+        const int r = i / kWideCKb, cc = i - r * kWideCKb, q = q_base + r;
+        s_src[r * LS + cc] = (q >= 0 && q < Tl && c_base + cc < nc)
+            ? __bfloat162float(hb[static_cast<size_t>(q) * a.c0 + c_base + cc]) : 0.f;
+      }
+    } else {                                       // rows are positions t0-1 .. t0+PT, channel-major reads
+      for (int i = threadIdx.x; i < rows * kWideCKb; i += blockDim.x) {
+        const int cc = i / rows, r = i - cc * rows, t = q_base + r, ch = c_base + cc;
+        float v = 0.f;
+        if (t >= 0 && t < a.T && ch < cin) {
+          if (ch < a.cx) {
+            const size_t idx = (static_cast<size_t>(b) * a.cx + ch) * a.T + t;
+            v = a.x[idx];
+            if (a.noise) v = al * v + be * a.noise[idx];
+          } else {
+            v = a.append[(static_cast<size_t>(b) * a.ca + (ch - a.cx)) * a.T + t];
+          }
+        }
+        s_src[r * LS + cc] = v;
+      }
+    }
+    __syncthreads();
+    const int nvalid = min(kWidePT, a.T - t0);
+    if (on_h) {
+      // sliding window over the upsampled positions u = t-1, t, t+1
+      auto src = [&](int u) { return (u >= 0 && u < a.T) ? s_src[(u / f - q_base) * LS + c] : 0.f; };
+      float hm = src(t0 - 1), h0 = src(t0);
+      for (int i = 0; i < nvalid; ++i) {
+        const float hp = src(t0 + i + 1);
+        const float d = s_dvs[ol * kWidePT + i];
+        g0 += d * hm; g1 += d * h0; g2 += d * hp; sdv += d;
+        hm = h0; h0 = hp;
+      }
+    } else {
+      for (int i = 0; i < nvalid; ++i) {
+        const float d = s_dvs[ol * kWidePT + i];
+        g1 += d * s_src[(i + 1) * LS + c]; sdv += d;
+      }
+    }
+  }
+  const int ldg = a.ld_gate > 0 ? a.ld_gate : a.co;
+  const int ch = c_base + c;
+  float part = 0.f;                                // this lane's share of dgate[b][o]
+  if (o < a.co && ch < nc) {
+    if (on_h) {
+      const float gt = a.gate[static_cast<size_t>(b) * ldg + o];
+      float* dw = a.dw + (static_cast<size_t>(o) * a.c0 + ch) * 3;
+      atomicAdd(dw + 0, gt * g0); atomicAdd(dw + 1, gt * g1); atomicAdd(dw + 2, gt * g2);
+      const float* w = a.w + (static_cast<size_t>(o) * a.c0 + ch) * 3;
+      part = w[0] * g0 + w[1] * g1 + w[2] * g2;
+      if (chunk == 0 && c == 0) {
+        part += (a.bias ? a.bias[o] : 0.f) * sdv;
+        atomicAdd(a.dbias + o, gt * sdv);
+      }
+    } else {
+      atomicAdd(a.dw_adapt + o * cin + ch, g1);
+      if (chunk == n_hc && c == 0) atomicAdd(a.db_adapt + o, sdv);
+    }
+  }
+  if (on_h) {
+    part = warp_sum(part);                         // the warp is one output o
+    if (c == 0 && o < a.co) atomicAdd(a.dgate + static_cast<size_t>(b) * a.ld_dgate + o, part);
+  }
+}
+
+__global__ void __launch_bounds__(256) stem_out_bwd_wide_dxin_kernel(const adp_stem_out_bwd_args a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int cin = a.cx + a.ca;
+  const float gscale = a.gscale ? a.gscale[0] : 1.f;
+  const size_t total = static_cast<size_t>(a.B) * cin * a.T;
+  for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const int t = static_cast<int>(i % a.T);
+    const int ch = static_cast<int>((i / a.T) % cin);
+    const int b = static_cast<int>(i / (static_cast<size_t>(a.T) * cin));
+    float acc = 0.f;
+    if (a.w_adapt) {
+      for (int o = 0; o < a.co; ++o) acc += so_wide_dvs(a, gscale, b, o, t) * __ldg(a.w_adapt + o * cin + ch);
+    } else if (ch < a.co) {
+      acc = so_wide_dvs(a, gscale, b, ch, t);
+    }
+    a.dxin[i] = acc;
+  }
+}
+
+// ------------------------------------------------------------- wide boundary (stem_in_bwd)
+// dW[o][ii] = sum_to dout[to][o] in[to][ii] (ii = c*f + j < 128, o < 256): blocks own a 32 x 32
+// slice (blockIdx.z), thread = (o, 4 inputs), registers across the tiles of a run, one atomic per
+// element per block.  dxin: block per tile of kWideQT low-rate rows, dout rows staged in smem.
+__global__ void __launch_bounds__(256) stem_in_bwd_wide_param_kernel(const adp_stem_in_bwd_args a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  __shared__ float s_g[kWidePT][kWideCKb + 1];     // dout [to][o slice]
+  __shared__ float s_in[kWidePT][kWideCKb + 1];    // input [to][ii slice]
+  const int cin = a.cx + a.ca, ci_total = cin * a.f, To = a.T / a.f;
+  const int n_ic = (ci_total + kWideCKb - 1) / kWideCKb;
+  const int oc = blockIdx.z / n_ic, ic = blockIdx.z - oc * n_ic;
+  const int o = oc * kWideCKb + (threadIdx.x & 31), ig = threadIdx.x >> 5;
+  const int b = blockIdx.y;
+  const float al = a.noise ? a.alpha[b] : 1.f, be = a.noise ? a.beta[b] : 0.f;
+  const __nv_bfloat16* gb = static_cast<const __nv_bfloat16*>(a.dout) + static_cast<size_t>(b) * To * a.c0;
+  float acc[4] = {0.f, 0.f, 0.f, 0.f}, gsum = 0.f;
+  const int n_tiles = (To + kWidePT - 1) / kWidePT;
+  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const int to0 = tile * kWidePT;
+    __syncthreads();
+    for (int i = threadIdx.x; i < kWidePT * kWideCKb; i += blockDim.x) {
+      const int r = i / kWideCKb, cc = i - r * kWideCKb, to = to0 + r, oo = oc * kWideCKb + cc;
+      s_g[r][cc] = (to < To && oo < a.c0) ? __bfloat162float(gb[static_cast<size_t>(to) * a.c0 + oo]) : 0.f;
+    }
+    for (int i = threadIdx.x; i < kWidePT * kWideCKb; i += blockDim.x) {
+      const int cc = i / kWidePT, r = i - cc * kWidePT, ii = ic * kWideCKb + cc, to = to0 + r;
+      float v = 0.f;
+      if (to < To && ii < ci_total) {              // input ii = c*f + j at position to*f + j
+        const int ch = ii / a.f;
+        const size_t tt = static_cast<size_t>(to) * a.f + (ii - ch * a.f);
+        if (ch < a.cx) {
+          const size_t idx = (static_cast<size_t>(b) * a.cx + ch) * a.T + tt;
+          v = a.x[idx];
+          if (a.noise) v = al * v + be * a.noise[idx];
+        } else {
+          v = a.append[(static_cast<size_t>(b) * a.ca + (ch - a.cx)) * a.T + tt];
+        }
+      }
+      s_in[r][cc] = v;
+    }
+    __syncthreads();
+    const int nvalid = min(kWidePT, To - to0);
+    for (int r = 0; r < nvalid; ++r) {
+      const float g = s_g[r][threadIdx.x & 31];
+      gsum += g;
+#pragma unroll
+      for (int m = 0; m < 4; ++m) acc[m] += g * s_in[r][ig + 8 * m];
+    }
+  }
+  if (o < a.c0) {
+#pragma unroll
+    for (int m = 0; m < 4; ++m) {
+      const int ii = ic * kWideCKb + ig + 8 * m;
+      if (ii < ci_total) atomicAdd(a.dw + static_cast<size_t>(o) * ci_total + ii, acc[m]);
+    }
+    if (ic == 0 && ig == 0) atomicAdd(a.dbias + o, gsum);
+  }
+}
+
+__global__ void __launch_bounds__(256) stem_in_bwd_wide_dxin_kernel(const adp_stem_in_bwd_args a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  extern __shared__ float s_dyn[];                 // dout rows [QT][c0 + 1]
+  const int cin = a.cx + a.ca, ci_total = cin * a.f, To = a.T / a.f, ld = a.c0 + 1;
+  const int b = blockIdx.y;
+  const __nv_bfloat16* gb = static_cast<const __nv_bfloat16*>(a.dout) + static_cast<size_t>(b) * To * a.c0;
+  const int n_tiles = (To + kWideQT - 1) / kWideQT;
+  const int span = kWideQT * a.f;
+  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const int to0 = tile * kWideQT;
+    __syncthreads();
+    for (int i = threadIdx.x; i < kWideQT * a.c0; i += blockDim.x) {
+      const int r = i / a.c0, o = i - r * a.c0, to = to0 + r;
+      s_dyn[r * ld + o] = to < To ? __bfloat162float(gb[static_cast<size_t>(to) * a.c0 + o]) : 0.f;
+    }
+    __syncthreads();
+    // dxin[b][c][to*f + j] += sum_o dout[to][o] w[o][c*f + j], positions contiguous across threads
+    for (int i = threadIdx.x; i < cin * span; i += blockDim.x) {
+      const int ch = i / span, rr = i - ch * span, r = rr / a.f, j = rr - r * a.f;
+      if (to0 + r >= To) continue;
+      const float* wp = a.w + ch * a.f + j;
+      const float* g = s_dyn + r * ld;
+      float acc = 0.f;
+      for (int o = 0; o < a.c0; ++o) acc += g[o] * __ldg(wp + static_cast<size_t>(o) * ci_total);
+      a.dxin[(static_cast<size_t>(b) * cin + ch) * a.T + static_cast<size_t>(to0) * a.f + rr] += acc;
+    }
+  }
+}
+
 }  // namespace adp
 
 using namespace adp;
@@ -564,12 +853,47 @@ extern "C" int adp_stem_out_bwd(const adp_stem_out_bwd_args* args, adp_stream_t 
   ADP_CHECK(args && args->dv && args->h && args->x && args->w && args->gate && args->dh && args->dw &&
             args->dbias && args->dgate, "adp_stem_out_bwd: null pointer");
   const adp_stem_out_bwd_args& a = *args;
-  ADP_CHECK(a.co >= 1 && a.co <= kSoMaxCo && a.c0 % 8 == 0 && a.c0 <= kSoMaxC0 && a.cx + a.ca <= 8,
-            "adp_stem_out_bwd: co=%d c0=%d unsupported", a.co, a.c0);
-  ADP_CHECK(a.f >= 1 && kTB % a.f == 0 && a.T % a.f == 0, "adp_stem_out_bwd: f=%d", a.f);
+  const int cin = a.cx + a.ca;
+  ADP_CHECK(a.co >= 1 && a.co <= 64 && a.co <= a.cx && a.ca >= 0 && cin <= 64 && a.c0 % 8 == 0 &&
+            a.c0 >= 8 && a.c0 <= 256,
+            "adp_stem_out_bwd: co=%d cx=%d ca=%d c0=%d unsupported (co <= cx, co <= 64, cx+ca <= 64, c0 <= 256)",
+            a.co, a.cx, a.ca, a.c0);
+  ADP_CHECK(a.f >= 1 && a.T % a.f == 0, "adp_stem_out_bwd: f=%d", a.f);
   ADP_CHECK(!a.w_adapt || (a.dw_adapt && a.db_adapt), "adp_stem_out_bwd: adapter grads missing");
   ADP_CHECK((a.ca == 0) == (a.append == nullptr), "adp_stem_out_bwd: append / ca mismatch");
-  const int cin = a.cx + a.ca, rows_h = kTB / a.f + 2;
+  if (a.co > kSoMaxCo || a.c0 > kSoMaxC0 || cin > 8 || kTB % a.f != 0 ||
+      a.co * a.c0 * 3 + 3 * a.co + a.co * cin > kSoItems * kTB) {
+    ADP_CHECK(a.w_adapt || cin == a.co, "adp_stem_out_bwd: identity skip needs cx+ca == co");
+    ADP_CHECK(a.ld_dgate >= a.co && (a.ld_gate == 0 || a.ld_gate >= a.co), "adp_stem_out_bwd: gate pitches");
+    cudaStream_t s = as_stream(stream);
+    const int Tl = a.T / a.f;
+    const int n_cz = (a.c0 + kWideCKb - 1) / kWideCKb;
+    const size_t smem_dh = (static_cast<size_t>(a.co) * 3 * kWideCKb + kWideQT * (a.co * 3 + 1)) * sizeof(float);
+    static SmemAttrCache dh_cache;
+    ADP_CUDA(ensure_dyn_smem(stem_out_bwd_wide_dh_kernel, smem_dh, dh_cache));
+    int gx = (num_sms() * 4 + a.B * n_cz - 1) / (a.B * n_cz);
+    gx = max(1, min(gx, (Tl + kWideQT - 1) / kWideQT));
+    ADP_CUDA(launch_k(stem_out_bwd_wide_dh_kernel, dim3(gx, a.B, n_cz), dim3(256), smem_dh, s, a));
+    const int n_chunks = n_cz + (a.w_adapt ? (cin + kWideCKb - 1) / kWideCKb : 0);
+    const int nz = ((a.co + kWideOS - 1) / kWideOS) * n_chunks;
+    const int f_rows = a.w_adapt ? 1 : a.f;        // adapter slices stage positions (f = 1)
+    const size_t smem_p = (static_cast<size_t>(kWideOS) * kWidePT +
+                           static_cast<size_t>((kWidePT + 1) / f_rows + 2) * (kWideCKb + 1)) * sizeof(float);
+    static SmemAttrCache p_cache;
+    ADP_CUDA(ensure_dyn_smem(stem_out_bwd_wide_param_kernel, smem_p, p_cache));
+    gx = (num_sms() * 4 + a.B * nz - 1) / (a.B * nz);
+    gx = max(1, min(gx, (a.T + kWidePT - 1) / kWidePT));
+    ADP_CUDA(launch_k(stem_out_bwd_wide_param_kernel, dim3(gx, a.B, nz), dim3(256), smem_p, s, a));
+    if (a.dxin) {
+      const size_t n = static_cast<size_t>(a.B) * cin * a.T;
+      const size_t cap = static_cast<size_t>(num_sms()) * 16;
+      const int g = static_cast<int>((n + 255) / 256 < cap ? (n + 255) / 256 : cap);
+      ADP_CUDA(launch_k(stem_out_bwd_wide_dxin_kernel, dim3(g), dim3(256), (size_t)0, s, a));
+    }
+    ADP_LAUNCH_CHECK();
+    return 0;
+  }
+  const int rows_h = kTB / a.f + 2;
   const size_t smem = (static_cast<size_t>(a.co) * 3 * a.c0 + static_cast<size_t>(rows_h) * a.c0 +
                        static_cast<size_t>(kTB + 2) * a.co + static_cast<size_t>(kTB) * a.co +
                        static_cast<size_t>(kTB) * cin) * sizeof(float);
@@ -584,10 +908,29 @@ extern "C" int adp_stem_out_bwd(const adp_stem_out_bwd_args* args, adp_stream_t 
 extern "C" int adp_stem_in_bwd(const adp_stem_in_bwd_args* args, adp_stream_t stream) {
   ADP_CHECK(args && args->dout && args->x && args->dw && args->dbias, "adp_stem_in_bwd: null pointer");
   const adp_stem_in_bwd_args& a = *args;
-  ADP_CHECK((a.cx + a.ca) * a.f <= 32 && a.c0 % 8 == 0 && a.c0 <= 64 && a.T % a.f == 0,
-            "adp_stem_in_bwd: unsupported sizes");
+  const int cin = a.cx + a.ca;
+  ADP_CHECK(a.f >= 1 && a.ca >= 0 && cin <= 64 && cin * a.f <= 128 && a.c0 % 8 == 0 && a.c0 >= 8 &&
+            a.c0 <= 256 && a.T % a.f == 0,
+            "adp_stem_in_bwd: cx+ca=%d f=%d c0=%d unsupported (cx+ca <= 64, (cx+ca)*f <= 128, c0 <= 256)",
+            cin, a.f, a.c0);
   ADP_CHECK((a.ca == 0) == (a.append == nullptr), "adp_stem_in_bwd: append / ca mismatch");
   ADP_CHECK(!a.dxin || a.w, "adp_stem_in_bwd: dxin needs the conv weights");
+  if (cin * a.f > 32 || a.c0 > 64) {
+    cudaStream_t s = as_stream(stream);
+    const int To = a.T / a.f;
+    const int nz = ((a.c0 + kWideCKb - 1) / kWideCKb) * ((cin * a.f + kWideCKb - 1) / kWideCKb);
+    int gx = (num_sms() * 4 + a.B * nz - 1) / (a.B * nz);
+    gx = max(1, min(gx, (To + kWidePT - 1) / kWidePT));
+    ADP_CUDA(launch_k(stem_in_bwd_wide_param_kernel, dim3(gx, a.B, nz), dim3(256), (size_t)0, s, a));
+    if (a.dxin) {
+      const size_t smem = static_cast<size_t>(kWideQT) * (a.c0 + 1) * sizeof(float);
+      gx = (num_sms() * 4 + a.B - 1) / a.B;
+      gx = max(1, min(gx, (To + kWideQT - 1) / kWideQT));
+      ADP_CUDA(launch_k(stem_in_bwd_wide_dxin_kernel, dim3(gx, a.B), dim3(256), smem, s, a));
+    }
+    ADP_LAUNCH_CHECK();
+    return 0;
+  }
   const size_t smem = (static_cast<size_t>(kTB) * (a.cx + a.ca) * a.f + static_cast<size_t>(kTB) * a.c0) * sizeof(float);
   static SmemAttrCache smem_cache;
   ADP_CUDA(ensure_dyn_smem(stem_in_bwd_kernel, smem, smem_cache));

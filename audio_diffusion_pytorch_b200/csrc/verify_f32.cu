@@ -291,6 +291,8 @@ __device__ __forceinline__ float f32_stem_branch(const adp_stem_out_args& a, con
   return y;
 }
 
+constexpr int kF32StemMaxCin = 64;   // cx + ca (the block input held per position)
+
 __global__ void __launch_bounds__(256) f32_stem_out_kernel(const adp_stem_out_args a) {
   pdl_launch_dependents();
   pdl_wait();
@@ -306,8 +308,8 @@ __global__ void __launch_bounds__(256) f32_stem_out_kernel(const adp_stem_out_ar
     const int t = static_cast<int>(i % a.T);
     const int b = static_cast<int>(i / a.T);
     const float al = a.noise ? a.alpha[b] : 1.f, be = a.noise ? a.beta[b] : 0.f;
-    float xin[8];
-    for (int c = 0; c < 8; ++c) {
+    float xin[kF32StemMaxCin];
+    for (int c = 0; c < kF32StemMaxCin; ++c) {
       xin[c] = 0.f;
       if (c < a.cx) {
         const int64_t idx = (static_cast<int64_t>(b) * a.cx + c) * a.T + t;
@@ -497,7 +499,8 @@ extern "C" int adp_f32_stem_out_train(const adp_stem_out_args* args, adp_stream_
   ADP_CHECK(a.w_adapt || a.cx + a.ca == a.co, "adp_f32_stem_out: identity skip needs cx+ca == co");
   ADP_CHECK(!a.x_next || a.ab, "adp_f32_stem_out: x_next needs ab");
   ADP_CHECK(a.f >= 1 && a.T % a.f == 0 && (a.ca == 0) == (a.append == nullptr), "adp_f32_stem_out: bad args");
-  ADP_CHECK(a.cx + a.ca <= 8 && a.co <= a.cx, "adp_f32_stem_out: in <= 8 channels, out <= x channels");
+  ADP_CHECK(a.cx + a.ca <= kF32StemMaxCin && a.co <= a.cx,
+            "adp_f32_stem_out: in <= %d channels, out <= x channels", kF32StemMaxCin);
   ADP_CUDA(launch_k(f32_stem_out_kernel, dim3(f32_grid(static_cast<int64_t>(a.B) * a.T)), dim3(256),
                     (size_t)0, as_stream(stream), a));
   ADP_LAUNCH_CHECK();

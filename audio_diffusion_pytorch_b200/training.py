@@ -567,7 +567,7 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
             # branches (B200UNet._compute_packed): they produce the gradients of the FOLDED
             # weights, unfolded below (a few hundred numbers) into merge / up / adapter gradients
             Co, Ci = lv.out_ch, lv.in_ch
-            gate, dgate = torch.ones(B, 8, device=dev), gbuf((B, 8))
+            gate, dgate = torch.ones(B, max(8, Co), device=dev), gbuf((B, max(8, Co)))
             dw_up, db_up = gbuf((Co, C, 3)), gbuf((Co,))
             dwa, dba = gbuf((Co, Ci)), gbuf((Co,))
 

@@ -397,6 +397,9 @@ class B200UNet(nn.Module):
     ATT_LN_EPS = 1e-5  # nn.LayerNorm default (a_unet Attention norms)
     MOD_LN_EPS = 1e-6  # a_unet Modulation LayerNorm
     HEAD_DIMS = (32, 64, 128)   # attention_features the attention kernels are built for
+    MAX_BOUNDARY = 64           # in_channels (x + appended) and out_channels of the stem kernels
+    MAX_STEM_IN = 128           # in_channels * factors[0]: inputs of one stem_in output position
+    MAX_C0 = 256                # channels[0]
 
     def __init__(self, dim: int, in_channels: int, channels: Sequence[int],
                  factors: Sequence[int], items: Sequence[int],
@@ -455,7 +458,20 @@ class B200UNet(nn.Module):
         # which holds at most 8 groups (csrc/conv_gemm.cu kMaxGroups)
         assert 1 <= resnet_groups <= 8, \
             f"resnet_groups={resnet_groups}: the conv GEMM's fused GroupNorm statistics support at most 8 groups"
-        assert self.out_channels <= 4 and self.in_channels <= 8, "stem kernels: in<=8, out<=4 channels"
+        # the level-0 stem kernels (csrc/stem.cu, stem_bwd.cu) hold the whole boundary of a position
+        assert self.in_channels <= self.MAX_BOUNDARY, \
+            f"in_channels={self.in_channels} (x plus appended channels): the stem kernels support at most " \
+            f"{self.MAX_BOUNDARY} input channels"
+        assert self.out_channels <= self.MAX_BOUNDARY, \
+            f"out_channels={self.out_channels}: the stem kernels support at most {self.MAX_BOUNDARY} output channels"
+        assert self.out_channels <= self.x_channels, \
+            f"out_channels={self.out_channels} exceeds the {self.x_channels} channels of x (the identity skip " \
+            f"and the sampler update need out_channels <= x channels)"
+        assert self.in_channels * factors[0] <= self.MAX_STEM_IN, \
+            f"in_channels * factors[0] = {self.in_channels * factors[0]}: the stem_in conv supports at most " \
+            f"{self.MAX_STEM_IN} inputs per output position"
+        assert channels[0] <= self.MAX_C0, \
+            f"channels[0]={channels[0]}: the stem kernels support a level 0 at most {self.MAX_C0} wide"
 
         # registration order mirrors a_unet: time plugin, cfg plugin, then the recursive blocks
         self.time = TimeParams(modulation_features) if use_time_conditioning else None
@@ -917,7 +933,8 @@ class B200UNet(nn.Module):
 
         h0, _ = run_level(0, None, T)
         lv0, L0 = levels[0], P["levels"][0]
-        gate0 = ss_all[:, L0["gate_off"]:] if self.use_modulation else torch.ones(Bh, 8, device=dev)
+        gate0 = (ss_all[:, L0["gate_off"]:] if self.use_modulation
+                 else torch.ones(Bh, max(8, self.out_channels), device=dev))
 
         def final():
             kw = dict(append=plan.append, w_adapt=L0.get("adapt_w"), b_adapt=L0.get("adapt_b"),

@@ -144,7 +144,11 @@ int adp_time_features(const float* sigma, const float* freqs, float* out, int32_
  * adp_stem_in: level-0 DownsampleItem Conv1d(cx+ca -> c0, k=s=f) on cat([x, append],1)
  * (reference components.py:175 AppendChannelsPlugin + a_unet Downsample), optionally on the
  * VDiffusion-noised input x_noisy = alpha_b*x + beta_b*noise (reference diffusion.py:91).
- * Emits the GroupNorm statistics of its output. */
+ * Emits the GroupNorm statistics of its output.
+ * Limits of the stem entry points (adp_stem_in / _out / _in_bwd / _out_bwd; their adp_f32_ twins take
+ * at least the same sizes): cx+ca <= 64, (cx+ca)*f <= 128, c0 <= 256 and a multiple of 8, co <= 64 and co <= cx; sizes the
+ * narrow kernels take ((cx+ca)*f <= 32, co <= 4, cx+ca <= 8; backward c0 <= 64) run on them, the rest
+ * of the envelope on the wide kernels.  Out-of-envelope sizes are refused before any launch. */
 typedef struct adp_stem_in_args {
   const float* x;       /* fp32 [B][cx][T]                          */
   const float* append;  /* fp32 [B][ca][T] or NULL                  */
