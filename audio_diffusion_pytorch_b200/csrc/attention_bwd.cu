@@ -38,21 +38,6 @@ struct AttnBwdParams {
   float scale, scale_log2;
 };
 
-__device__ __forceinline__ void ldsm4(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void ldsm4t(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
-      "{%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 __device__ __forceinline__ float ex2f(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -78,20 +63,20 @@ __device__ __forceinline__ void load_tile(__nv_bfloat16* dst, const __nv_bfloat1
 template <int LD>
 __device__ __forceinline__ void frag_a(const __nv_bfloat16* tile, int r0, int kc, int lane, uint32_t (&a)[4]) {
   const int row = r0 + (lane & 7) + ((lane >> 3) & 1) * 8, col = kc + (lane >> 4) * 8;
-  ldsm4(smem_u32(tile + row * LD + col), a);
+  ldmatrix_x4(smem_u32(tile + row * LD + col), a);
 }
 // B fragments of TWO n-tiles (n0..n0+15) x k (kc..kc+15) from a tile stored [n][k] (k contiguous):
 // r[0],r[1] = (b0,b1) of n-tile n0, r[2],r[3] = n-tile n0+8
 template <int LD>
 __device__ __forceinline__ void frag_b_nk(const __nv_bfloat16* tile, int n0, int kc, int lane, uint32_t (&r)[4]) {
   const int row = n0 + (lane & 7) + (lane >> 4) * 8, col = kc + ((lane >> 3) & 1) * 8;
-  ldsm4(smem_u32(tile + row * LD + col), r);
+  ldmatrix_x4(smem_u32(tile + row * LD + col), r);
 }
 // same, from a tile stored [k][n] (n contiguous): transposing load
 template <int LD>
 __device__ __forceinline__ void frag_b_kn(const __nv_bfloat16* tile, int n0, int kc, int lane, uint32_t (&r)[4]) {
   const int row = kc + (lane & 7) + ((lane >> 3) & 1) * 8, col = n0 + (lane >> 4) * 8;
-  ldsm4t(smem_u32(tile + row * LD + col), r);
+  ldmatrix_x4_trans(smem_u32(tile + row * LD + col), r);
 }
 
 // ------------------------------------------------------------------------------- delta
@@ -185,10 +170,10 @@ attn_dkv_kernel(const AttnBwdParams p) {
         uint32_t bq[4], bd[4];
         frag_b_nk<kLd>(q_s, n2 * 16, ks * 16, lane, bq);
         frag_b_nk<kLd>(do_s, n2 * 16, ks * 16, lane, bd);
-        mma16816(s[2 * n2], ka, bq[0], bq[1]);
-        mma16816(s[2 * n2 + 1], ka, bq[2], bq[3]);
-        mma16816(dp[2 * n2], va, bd[0], bd[1]);
-        mma16816(dp[2 * n2 + 1], va, bd[2], bd[3]);
+        mma_16816(s[2 * n2], ka, bq[0], bq[1]);
+        mma_16816(s[2 * n2 + 1], ka, bq[2], bq[3]);
+        mma_16816(dp[2 * n2], va, bd[0], bd[1]);
+        mma_16816(dp[2 * n2 + 1], va, bd[2], bd[3]);
       }
     }
     // P^T and dS^T as bf16 A fragments (k = queries)
@@ -215,10 +200,10 @@ attn_dkv_kernel(const AttnBwdParams p) {
         uint32_t bd[4], bq[4];
         frag_b_kn<kLd>(do_s, n2 * 16, ks * 16, lane, bd);
         frag_b_kn<kLd>(q_s, n2 * 16, ks * 16, lane, bq);
-        mma16816(dv[2 * n2], pa[ks], bd[0], bd[1]);
-        mma16816(dv[2 * n2 + 1], pa[ks], bd[2], bd[3]);
-        mma16816(dk[2 * n2], dsa[ks], bq[0], bq[1]);
-        mma16816(dk[2 * n2 + 1], dsa[ks], bq[2], bq[3]);
+        mma_16816(dv[2 * n2], pa[ks], bd[0], bd[1]);
+        mma_16816(dv[2 * n2 + 1], pa[ks], bd[2], bd[3]);
+        mma_16816(dk[2 * n2], dsa[ks], bq[0], bq[1]);
+        mma_16816(dk[2 * n2 + 1], dsa[ks], bq[2], bq[3]);
       }
     }
   }
@@ -291,10 +276,10 @@ attn_dq_kernel(const AttnBwdParams p) {
         uint32_t bk[4], bv[4];
         frag_b_nk<kLd>(k_s, n2 * 16, ks * 16, lane, bk);
         frag_b_nk<kLd>(v_s, n2 * 16, ks * 16, lane, bv);
-        mma16816(s[2 * n2], qa, bk[0], bk[1]);
-        mma16816(s[2 * n2 + 1], qa, bk[2], bk[3]);
-        mma16816(dp[2 * n2], da, bv[0], bv[1]);
-        mma16816(dp[2 * n2 + 1], da, bv[2], bv[3]);
+        mma_16816(s[2 * n2], qa, bk[0], bk[1]);
+        mma_16816(s[2 * n2 + 1], qa, bk[2], bk[3]);
+        mma_16816(dp[2 * n2], da, bv[0], bv[1]);
+        mma_16816(dp[2 * n2 + 1], da, bv[2], bv[3]);
       }
     }
     uint32_t dsa[kBT / 16][4];
@@ -317,8 +302,8 @@ attn_dq_kernel(const AttnBwdParams p) {
       for (int n2 = 0; n2 < D / 16; ++n2) {
         uint32_t bk[4];
         frag_b_kn<kLd>(k_s, n2 * 16, ks * 16, lane, bk);
-        mma16816(dq[2 * n2], dsa[ks], bk[0], bk[1]);
-        mma16816(dq[2 * n2 + 1], dsa[ks], bk[2], bk[3]);
+        mma_16816(dq[2 * n2], dsa[ks], bk[0], bk[1]);
+        mma_16816(dq[2 * n2 + 1], dsa[ks], bk[2], bk[3]);
       }
     }
   }

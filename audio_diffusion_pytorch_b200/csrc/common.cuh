@@ -75,4 +75,32 @@ inline cudaError_t launch_k(Kern kernel, dim3 grid, dim3 block, size_t smem, cud
 // streaming multiprocessors of the current device (grid sizing of persistent / capped grids)
 int num_sms();
 
+// grid.x of a persistent (tile-looping) kernel launched as grid(gx, B): exactly one wave of
+// resident blocks (a grid larger than occupancy * SMs would run a second, mostly empty wave)
+template <typename K>
+inline int one_wave_gx(K kernel, int threads, size_t smem, int B, int n_tiles) {
+  int occ = 1;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, threads, smem) != cudaSuccess || occ < 1)
+    occ = 1;
+  int gx = (occ * num_sms()) / B;
+  if (gx < 1) gx = 1;
+  if (gx > n_tiles) gx = n_tiles;
+  return gx;
+}
+
+// grid.x of a tile loop launched as grid(gx, B, z): about 4 blocks per SM in total
+inline int blocks_per_batch(int n_tiles, int B, int z = 1) {
+  int gx = (num_sms() * 4 + B * z - 1) / (B * z);
+  if (gx > n_tiles) gx = n_tiles;
+  return gx < 1 ? 1 : gx;
+}
+
+// 1-D grid-stride launch over n items: one item per thread, at most 16 blocks per SM
+inline int capped_grid(int64_t n, int threads) {
+  int64_t g = (n + threads - 1) / threads;
+  if (g < 1) g = 1;
+  if (g > num_sms() * 16) g = num_sms() * 16;
+  return static_cast<int>(g);
+}
+
 }  // namespace adp

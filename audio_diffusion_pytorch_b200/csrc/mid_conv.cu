@@ -19,19 +19,6 @@
 
 namespace adp {
 
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0,
-                                               uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
-      "{%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
 // NTH = threads per block.  256 threads x 2 blocks / SM or 128 threads x 4 blocks / SM (half-size
 // tiles): the same 16 warps per SM, but four independent barrier-separated phase streams instead
 // of two (selected by g_mid_threads, adp_debug_set(8, ..)).
@@ -225,19 +212,19 @@ __global__ void __launch_bounds__(NTH, 512 / NTH) mid_conv_kernel(const adp_narr
         for (int mb = 0; mb < MB; ++mb) {
           const int r0 = warp * RPW + mb * 16;
           // matrices: (rows 0-7, k 0-7) (rows 8-15, k 0-7) (rows 0-7, k 8-15) (rows 8-15, k 8-15)
-          ldsm_x4(x_base + static_cast<uint32_t>(r0 + (lane & 7) + ((lane >> 3) & 1) * 8 + tap) * RS +
+          ldmatrix_x4(x_base + static_cast<uint32_t>(r0 + (lane & 7) + ((lane >> 3) & 1) * 8 + tap) * RS +
                       (c16 * 16 + ((lane >> 4) & 1) * 8) * 2, af[mb]);
         }
 #pragma unroll
         for (int np = 0; np < NT / 2; ++np) {
           uint32_t bf[4];
           // matrices: (n 0-7, k 0-7) (n 0-7, k 8-15) (n 8-15, k 0-7) (n 8-15, k 8-15)
-          ldsm_x4(w_base + static_cast<uint32_t>(np * 16 + (lane & 7) + ((lane >> 4) & 1) * 8) * WS +
+          ldmatrix_x4(w_base + static_cast<uint32_t>(np * 16 + (lane & 7) + ((lane >> 4) & 1) * 8) * WS +
                       (tap * C + c16 * 16 + ((lane >> 3) & 1) * 8) * 2, bf);
 #pragma unroll
           for (int mb = 0; mb < MB; ++mb) {
-            mma_bf16_16816(acc[mb][2 * np], af[mb], bf[0], bf[1]);
-            mma_bf16_16816(acc[mb][2 * np + 1], af[mb], bf[2], bf[3]);
+            mma_16816(acc[mb][2 * np], af[mb], bf[0], bf[1]);
+            mma_16816(acc[mb][2 * np + 1], af[mb], bf[2], bf[3]);
           }
         }
       }
@@ -313,8 +300,7 @@ __global__ void __launch_bounds__(NTH, 512 / NTH) mid_conv_kernel(const adp_narr
       }
     }
     __syncthreads();
-    if (tid < 2 * a.groups && s_stats[tid] != 0.f)
-      atomicAdd(a.stats_out + static_cast<size_t>(b) * 2 * a.groups + tid, static_cast<double>(s_stats[tid]));
+    flush_group_stats(s_stats, a.stats_out, b, a.groups);
   }
 }
 
@@ -326,15 +312,7 @@ static int launch_mid(const adp_narrow_conv_args& a, cudaStream_t stream) {
   using Cfg = MidCfg<C, NTH>;
   static SmemAttrCache smem_cache;
   ADP_CUDA(ensure_dyn_smem(mid_conv_kernel<C, NTH>, (size_t)Cfg::SMEM, smem_cache));
-  int occ = 1;
-  const int sms = num_sms();
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, mid_conv_kernel<C, NTH>, NTH, Cfg::SMEM) != cudaSuccess ||
-      occ < 1)
-    occ = 1;
-  const int n_tiles = (a.T + Cfg::TB - 1) / Cfg::TB;
-  int gx = (occ * sms) / a.B;               // one wave of persistent blocks
-  if (gx < 1) gx = 1;
-  if (gx > n_tiles) gx = n_tiles;
+  const int gx = one_wave_gx(mid_conv_kernel<C, NTH>, NTH, (size_t)Cfg::SMEM, a.B, (a.T + Cfg::TB - 1) / Cfg::TB);
   ADP_CUDA(launch_k(mid_conv_kernel<C, NTH>, dim3(gx, a.B), dim3(NTH), (size_t)Cfg::SMEM, stream, a));
   return 0;
 }

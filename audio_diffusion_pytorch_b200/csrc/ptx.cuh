@@ -205,6 +205,29 @@ template <> struct Wgmma<256> {
   }
 };
 
+// ----------------------------------------------------------------- mma.sync (warp-level)
+// ldmatrix: 8x8 b16 matrices from shared memory; lane l supplies the row address of matrix l / 8.
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
+}
+__device__ __forceinline__ void ldmatrix_x2(uint32_t addr, uint32_t (&r)[2]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x2.shared.b16 {%0,%1}, [%2];"
+               : "=r"(r[0]), "=r"(r[1]) : "r"(addr));
+}
+__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
+}
+// D += A * B, m16n8k16, bf16 x bf16 -> fp32: A four .b32 of bf16 pairs, B two
+__device__ __forceinline__ void mma_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
+      "{%0,%1,%2,%3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
 // ------------------------------------------------------------------------- descriptors
 // wgmma shared-memory matrix descriptor (sm_90): start>>4 [0,14) | LBO>>4 [16,30) |
 // SBO>>4 [32,46) | base_offset [49,52) | layout [62,64).  The swizzle is a function of the
@@ -301,5 +324,13 @@ struct GroupStatAcc {
     s += v; q += v * v;
   }
 };
+
+// The block's shared-memory bins s_stats[2 * groups] -> the fp64 statistics of batch element b
+// (one atomic per non-zero bin).  After a __syncthreads that follows the last bin update.
+__device__ __forceinline__ void flush_group_stats(const float* s_stats, double* stats, int b, int groups) {
+  const int tid = threadIdx.x;
+  if (tid < 2 * groups && s_stats[tid] != 0.f)
+    atomicAdd(stats + static_cast<size_t>(b) * 2 * groups + tid, static_cast<double>(s_stats[tid]));
+}
 
 }  // namespace adp

@@ -2,28 +2,9 @@
 //   adp_stem_in     fp32 [B][C][T] (+append, +VDiffusion noising) -> k=s=f conv -> bf16 NWC
 //   adp_stem_out    bf16 NWC -> nearest-up f + conv3 -> skip/gate -> v (+CFG, +sampler step, +loss)
 //   adp_narrow_conv C == 8 ConvBlock: GN+SiLU -> conv3 (+residual) (+LayerNorm/FiLM) (+stats)
-#include "common.cuh"
-#include "ptx.cuh"
+#include "stem.cuh"
 
 namespace adp {
-
-// grid.x of a persistent (tile-looping) kernel launched as grid(gx, B): exactly one wave of
-// resident blocks (a grid larger than occupancy * SMs would run a second, mostly empty wave)
-template <typename K>
-static int persistent_gx(K kernel, int threads, size_t smem, int B, int n_tiles) {
-  int occ = 1;
-  const int sms = num_sms();
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, threads, smem) != cudaSuccess || occ < 1)
-    occ = 1;
-  int gx = (occ * sms) / B;
-  if (gx < 1) gx = 1;
-  if (gx > n_tiles) gx = n_tiles;
-  return gx;
-}
-
-constexpr int kStemMaxIn = 32;   // (cx+ca)*f
-constexpr int kStemMaxC0 = 256;
-constexpr int kStemMaxCo = 4;
 
 // Per-thread (sum, sum of squares) of an 8-channel row -> block reduction through a transposed
 // smem scratch (conflict-free, 16 LDS + 10 shuffles per thread) -> fp64 GroupNorm bins.
@@ -84,15 +65,7 @@ __global__ void __launch_bounds__(256) stem_in_kernel(const adp_stem_in_args a) 
     for (int i = 0; i < MAXIN; ++i) {
       if (i < ci_total) {
         const int c = i / a.f, j = i - c * a.f;
-        const size_t tt = static_cast<size_t>(to) * a.f + j;
-        if (c < a.cx) {
-          const size_t idx = (static_cast<size_t>(b) * a.cx + c) * a.T + tt;
-          float v = __ldg(a.x + idx);
-          if (a.noise) v = al * v + be * __ldg(a.noise + idx);   // reference diffusion.py:91
-          in[i] = v;
-        } else {
-          in[i] = __ldg(a.append + (static_cast<size_t>(b) * a.ca + (c - a.cx)) * a.T + tt);
-        }
+        in[i] = block_input<true>(a, b, c, static_cast<size_t>(to) * a.f + j, al, be);
       }
     }
   };
@@ -150,9 +123,7 @@ __global__ void __launch_bounds__(256) stem_in_kernel(const adp_stem_in_args a) 
   } else if (a.stats) {
     acc.flush(s_stats, lane);
     __syncthreads();
-    if (threadIdx.x < 2 * a.groups && s_stats[threadIdx.x] != 0.f)
-      atomicAdd(a.stats + static_cast<size_t>(b) * 2 * a.groups + threadIdx.x,
-                static_cast<double>(s_stats[threadIdx.x]));
+    flush_group_stats(s_stats, a.stats, b, a.groups);
   }
 }
 
@@ -160,14 +131,12 @@ __global__ void __launch_bounds__(256) stem_in_kernel(const adp_stem_in_args a) 
 // conv3 on the nearest-upsampled h for one output position; w in smem as [co][k][c0]
 __device__ __forceinline__ void stem_out_conv(const __nv_bfloat16* __restrict__ hb, int T, int f,
                                               int c0, int co_n, int t, const float* s_w,
-                                              float (&y)[kStemMaxCo]) {
-  const int Tl = T / f;
+                                              float (&y)[kStemOutNarrowCo]) {
 #pragma unroll
   for (int k = 0; k < 3; ++k) {
     const int idx = t + k - 1;
     if (idx < 0 || idx >= T) continue;       // zero padding of the upsampled signal
     const int q = f == 1 ? idx : idx / f;    // nearest-neighbour source row
-    (void)Tl;
     const uint4* row = reinterpret_cast<const uint4*>(hb + static_cast<size_t>(q) * c0);
     for (int c8 = 0; c8 < c0; c8 += 8) {
       const uint4 u = __ldg(row + (c8 >> 3));
@@ -179,7 +148,7 @@ __device__ __forceinline__ void stem_out_conv(const __nv_bfloat16* __restrict__ 
         hv[2 * j] = f2.x; hv[2 * j + 1] = f2.y;
       }
 #pragma unroll
-      for (int o = 0; o < kStemMaxCo; ++o) {
+      for (int o = 0; o < kStemOutNarrowCo; ++o) {
         if (o < co_n) {
           // two 16-byte broadcast reads (c0 % 8 == 0 keeps them aligned) instead of eight scalar
           const float4 w0 = *reinterpret_cast<const float4*>(s_w + (o * 3 + k) * c0 + c8);
@@ -195,9 +164,7 @@ __device__ __forceinline__ void stem_out_conv(const __nv_bfloat16* __restrict__ 
 __global__ void __launch_bounds__(256, 3) stem_out_kernel(const adp_stem_out_args a) {
   pdl_launch_dependents();
   pdl_wait();
-  const int ldg = a.ld_gate > 0 ? a.ld_gate : a.co;
   extern __shared__ __align__(16) float s_w[];   // conv w [co][3][c0], bias[co], adapt w [co][cin], adapt b[co]
-  __shared__ double s_loss[8];
   const int cin = a.cx + a.ca;
   float* s_b = s_w + a.co * 3 * a.c0;
   float* s_wa = s_b + a.co;
@@ -223,78 +190,33 @@ __global__ void __launch_bounds__(256, 3) stem_out_kernel(const adp_stem_out_arg
   // persistent blocks (grid-stride over positions): the smem weight prologue is paid once and
   // several independent positions per thread are in flight
   for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < a.T; t += gridDim.x * blockDim.x) {
-    // block input at this position (the U-Net skip): cat([x(_noisy), append])
-    float xin[8];
-    float xraw[kStemMaxCo], nraw[kStemMaxCo];
+    float xin[kStemOutNarrowCin];        // block input at this position (the U-Net skip)
 #pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      xin[c] = 0.f;
-      if (c < a.cx) {
-        const size_t idx = (static_cast<size_t>(b) * a.cx + c) * a.T + t;
-        float v = a.x[idx];
-        if (c < kStemMaxCo) { xraw[c] = v; nraw[c] = 0.f; }
-        if (a.noise) {
-          const float nv = a.noise[idx];
-          if (c < kStemMaxCo) nraw[c] = nv;
-          v = al * v + be * nv;
-        }
-        xin[c] = v;
-      } else if (c < cin) {
-        xin[c] = a.append[(static_cast<size_t>(b) * a.ca + (c - a.cx)) * a.T + t];
-      }
-    }
-    float y[kStemMaxCo], ym[kStemMaxCo];
+    for (int c = 0; c < kStemOutNarrowCin; ++c) xin[c] = c < cin ? block_input(a, b, c, t, al, be) : 0.f;
+    float y[kStemOutNarrowCo], ym[kStemOutNarrowCo];
 #pragma unroll
-    for (int o = 0; o < kStemMaxCo; ++o) { y[o] = o < a.co ? s_b[o] : 0.f; ym[o] = y[o]; }
+    for (int o = 0; o < kStemOutNarrowCo; ++o) { y[o] = o < a.co ? s_b[o] : 0.f; ym[o] = y[o]; }
     const __nv_bfloat16* h = static_cast<const __nv_bfloat16*>(a.h);
     stem_out_conv(h + static_cast<size_t>(b) * Tl * a.c0, a.T, a.f, a.c0, a.co, t, s_w, y);
     if (a.cfg)
       stem_out_conv(h + static_cast<size_t>(b + a.B) * Tl * a.c0, a.T, a.f, a.c0, a.co, t, s_w, ym);
 #pragma unroll
-    for (int o = 0; o < kStemMaxCo; ++o) {
+    for (int o = 0; o < kStemOutNarrowCo; ++o) {
       if (o < a.co) {
         float skip;
         if (a.w_adapt) {                       // SkipAdapter 1x1 conv (in != out channels)
           skip = s_ba[o];
 #pragma unroll
-          for (int c = 0; c < 8; ++c)
+          for (int c = 0; c < kStemOutNarrowCin; ++c)
             if (c < cin) skip += xin[c] * s_wa[o * cin + c];
         } else {
           skip = xin[o];
         }
-        float v = skip + a.gate[static_cast<size_t>(b) * ldg + o] * y[o];   // MergeModulate
-        if (a.cfg) {
-          const float vm = skip + a.gate[static_cast<size_t>(b + a.B) * ldg + o] * ym[o];
-          v = vm + (v - vm) * a.cfg_scale;                                   // CFG combine
-        }
-        const size_t oidx = (static_cast<size_t>(b) * a.co + o) * a.T + t;
-        if (a.v_out) a.v_out[oidx] = v;
-        if (a.x_next) {                       // reference diffusion.py:185-187
-          const float a0 = a.ab[0], b0 = a.ab[1], a1 = a.ab[2], b1 = a.ab[3];
-          const float xv = xin[o];
-          const float x_pred = a0 * xv - b0 * v;
-          const float n_pred = b0 * xv + a0 * v;
-          a.x_next[oidx] = a1 * x_pred + b1 * n_pred;
-        }
-        if (a.loss_sum) {                     // reference diffusion.py:92,95
-          const float vt = al * nraw[o] - be * xraw[o];
-          const float d = v - vt;
-          lsum += static_cast<double>(d) * d;
-          if (a.dv) a.dv[oidx] = 2.f * d / (static_cast<float>(a.B) * a.co * a.T);
-        }
+        stem_out_finish(a, b, o, t, skip, y[o], ym[o], xin[o], al, be, lsum);
       }
     }
   }
-  if (a.loss_sum) {
-    for (int o = 16; o > 0; o >>= 1) lsum += __shfl_xor_sync(0xffffffffu, lsum, o);
-    if ((threadIdx.x & 31) == 0) s_loss[threadIdx.x >> 5] = lsum;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      double tot = 0.0;
-      for (int i = 0; i < (blockDim.x >> 5); ++i) tot += s_loss[i];
-      atomicAdd(a.loss_sum, tot);
-    }
-  }
+  if (a.loss_sum) block_loss_flush(lsum, a.loss_sum);
 }
 
 // -------------------------------------------------------------------------- narrow_conv
@@ -311,23 +233,6 @@ __global__ void __launch_bounds__(256, 3) stem_out_kernel(const adp_stem_out_arg
 //     buffered (one __syncthreads per tile).
 //   * Epilogue in the accumulator layout (a quad owns one row): bias, residual, LayerNorm+FiLM
 //     via two quad shuffles, 128-byte coalesced stores, per-channel statistics in registers.
-__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void ldmatrix_x2(uint32_t addr, uint32_t (&r)[2]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x2.shared.b16 {%0,%1}, [%2];"
-               : "=r"(r[0]), "=r"(r[1]) : "r"(addr));
-}
-__device__ __forceinline__ void mma_16816(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2,
-                                          uint32_t a3, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
-      "{%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-
 template <int C>
 __global__ void __launch_bounds__(256) narrow_conv_kernel(const adp_narrow_conv_args a) {
   static_assert(C == 8, "narrow_conv is written for 8 channels (one 16-byte row)");
@@ -444,8 +349,9 @@ __global__ void __launch_bounds__(256) narrow_conv_kernel(const adp_narrow_conv_
       ldmatrix_x4(base + static_cast<uint32_t>(r0 + (lane & 7) + ((lane >> 3) & 1) * 8 + (lane >> 4)) * 16, af);
       ldmatrix_x2(base + static_cast<uint32_t>(r0 + (lane & 7) + ((lane >> 3) & 1) * 8 + 2) * 16, a2);
       float d[4] = {bias0, bias1, bias0, bias1};
-      mma_16816(d, af[0], af[1], af[2], af[3], bw[0], bw[1]);
-      mma_16816(d, a2[0], a2[1], 0u, 0u, bw[2], 0u);
+      const uint32_t at2[4] = {a2[0], a2[1], 0u, 0u};   // tap 2: k 16..23, 24..31 zero
+      mma_16816(d, af, bw[0], bw[1]);
+      mma_16816(d, at2, bw[2], 0u);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {                     // rows g and g + 8 of the block
         const int t = t0 + r0 + g + h * 8;
@@ -500,15 +406,12 @@ __global__ void __launch_bounds__(256) narrow_conv_kernel(const adp_narrow_conv_
 }
 
 // ------------------------------------------------------------------ wide boundary (stem_in)
-// Boundaries the register-array kernels above cannot hold: (cx+ca)*f up to 128 inputs per output
-// position.  Weights live in smem transposed to [ci][c0] (256 x 128 fp32 = 128 KiB at the corner),
+// Every size of the envelope the register-array kernel above does not take: (cx+ca)*f up to 128
+// inputs per output position.  Weights live in smem transposed to [ci][c0] (256 x 128 fp32 = 128 KiB at the corner),
 // the input tile [ci][kWideTP] is staged through smem with coalesced NCW reads, and each thread
 // computes 8 output channels of one position per pass (the warp shares the channel chunk: the
 // weight reads are 16-byte broadcasts).
 constexpr int kWideTP = 64;          // low-rate positions per stem_in tile
-constexpr int kWideMaxIn = 128;      // (cx+ca)*f
-constexpr int kWideMaxCin = 64;      // cx+ca
-constexpr int kWideMaxCo = 64;
 
 __global__ void __launch_bounds__(256) stem_in_wide_kernel(const adp_stem_in_args a) {
   pdl_launch_dependents();
@@ -544,15 +447,7 @@ __global__ void __launch_bounds__(256) stem_in_wide_kernel(const adp_stem_in_arg
       const int c = i / span, r = i - c * span, pp = r / a.f, j = r - pp * a.f;
       const size_t tt = static_cast<size_t>(to0) * a.f + r;
       float v = 0.f;
-      if (to0 + pp < To) {
-        if (c < a.cx) {
-          const size_t idx = (static_cast<size_t>(b) * a.cx + c) * a.T + tt;
-          v = __ldg(a.x + idx);
-          if (a.noise) v = al * v + be * __ldg(a.noise + idx);   // reference diffusion.py:91
-        } else {
-          v = __ldg(a.append + (static_cast<size_t>(b) * a.ca + (c - a.cx)) * a.T + tt);
-        }
-      }
+      if (to0 + pp < To) v = block_input<true>(a, b, c, tt, al, be);
       s_in[(c * a.f + j) * LD + pp] = v;
     }
     __syncthreads();
@@ -589,9 +484,7 @@ __global__ void __launch_bounds__(256) stem_in_wide_kernel(const adp_stem_in_arg
   if (a.stats) {
     acc.flush(s_stats, lane);
     __syncthreads();
-    if (threadIdx.x < 2 * a.groups && s_stats[threadIdx.x] != 0.f)
-      atomicAdd(a.stats + static_cast<size_t>(b) * 2 * a.groups + threadIdx.x,
-                static_cast<double>(s_stats[threadIdx.x]));
+    flush_group_stats(s_stats, a.stats, b, a.groups);
   }
 }
 
@@ -605,7 +498,7 @@ __global__ void __launch_bounds__(256) stem_in_wide_kernel(const adp_stem_in_arg
 constexpr int kWideOP = 128;
 constexpr int kWideCK = 32;
 constexpr int kWideHL = kWideCK + 4;     // padded h row (16-byte aligned)
-constexpr int kWideOPT = kWideMaxCo / 2; // outputs per thread
+constexpr int kWideOPT = kStemMaxCo / 2; // outputs per thread
 
 __device__ __forceinline__ void stem_out_wide_conv(const adp_stem_out_args& a, const __nv_bfloat16* hb,
                                                    float* s_h, const float* s_wc, int t0, int q_base,
@@ -651,9 +544,7 @@ __global__ void __launch_bounds__(256) stem_out_wide_kernel(const adp_stem_out_a
   pdl_launch_dependents();
   pdl_wait();
   extern __shared__ __align__(16) float s_dyn[];
-  __shared__ double s_loss[8];
   const int cin = a.cx + a.ca;
-  const int ldg = a.ld_gate > 0 ? a.ld_gate : a.co;
   const int rows = (kWideOP + 1) / a.f + 2;        // low-rate rows feeding positions t0-1 .. t0+OP
   float* s_wc = s_dyn;                             // [co][3][CK] weight slice of one c0 chunk
   float* s_h = s_wc + a.co * 3 * kWideCK;          // [rows][HL]
@@ -679,17 +570,7 @@ __global__ void __launch_bounds__(256) stem_out_wide_kernel(const adp_stem_out_a
     __syncthreads();                               // previous tile's s_xin consumed
     for (int i = threadIdx.x; i < cin * kWideOP; i += blockDim.x) {
       const int c = i / kWideOP, r = i - c * kWideOP, tt = t0 + r;
-      float v = 0.f;
-      if (tt < a.T) {
-        if (c < a.cx) {
-          const size_t idx = (static_cast<size_t>(b) * a.cx + c) * a.T + tt;
-          v = a.x[idx];
-          if (a.noise) v = al * v + be * a.noise[idx];
-        } else {
-          v = a.append[(static_cast<size_t>(b) * a.ca + (c - a.cx)) * a.T + tt];
-        }
-      }
-      s_xin[i] = v;
+      s_xin[i] = tt < a.T ? block_input(a, b, c, tt, al, be) : 0.f;
     }
     float y[kWideOPT], ym[kWideOPT];
 #pragma unroll
@@ -724,36 +605,10 @@ __global__ void __launch_bounds__(256) stem_out_wide_kernel(const adp_stem_out_a
       } else {
         skip = s_xin[o * kWideOP + p];
       }
-      float v = skip + a.gate[static_cast<size_t>(b) * ldg + o] * y[m];     // MergeModulate
-      if (a.cfg) {
-        const float vm = skip + a.gate[static_cast<size_t>(b + a.B) * ldg + o] * ym[m];
-        v = vm + (v - vm) * a.cfg_scale;                                   // CFG combine
-      }
-      const size_t oidx = (static_cast<size_t>(b) * a.co + o) * a.T + t;
-      if (a.v_out) a.v_out[oidx] = v;
-      if (a.x_next) {                              // reference diffusion.py:185-187
-        const float a0 = a.ab[0], b0 = a.ab[1], a1 = a.ab[2], b1 = a.ab[3];
-        const float xv = s_xin[o * kWideOP + p];
-        a.x_next[oidx] = a1 * (a0 * xv - b0 * v) + b1 * (b0 * xv + a0 * v);
-      }
-      if (a.loss_sum) {                            // reference diffusion.py:92,95
-        const size_t xidx = (static_cast<size_t>(b) * a.cx + o) * a.T + t;
-        const float d = v - (al * a.noise[xidx] - be * a.x[xidx]);
-        lsum += static_cast<double>(d) * d;
-        if (a.dv) a.dv[oidx] = 2.f * d / (static_cast<float>(a.B) * a.co * a.T);
-      }
+      stem_out_finish(a, b, o, t, skip, y[m], ym[m], s_xin[o * kWideOP + p], al, be, lsum);
     }
   }
-  if (a.loss_sum) {
-    for (int o = 16; o > 0; o >>= 1) lsum += __shfl_xor_sync(0xffffffffu, lsum, o);
-    if ((threadIdx.x & 31) == 0) s_loss[threadIdx.x >> 5] = lsum;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      double tot = 0.0;
-      for (int i = 0; i < (blockDim.x >> 5); ++i) tot += s_loss[i];
-      atomicAdd(a.loss_sum, tot);
-    }
-  }
+  if (a.loss_sum) block_loss_flush(lsum, a.loss_sum);
 }
 
 int mid_conv(const adp_narrow_conv_args& a, cudaStream_t stream);   // mid_conv.cu
@@ -765,31 +620,22 @@ using namespace adp;
 extern "C" int adp_stem_in(const adp_stem_in_args* args, adp_stream_t stream) {
   ADP_CHECK(args && args->x && args->w && args->out, "adp_stem_in: null pointer");
   const adp_stem_in_args& a = *args;
-  const int cin = a.cx + a.ca;
-  ADP_CHECK(cin <= kWideMaxCin, "adp_stem_in: cx+ca = %d > %d", cin, kWideMaxCin);
-  ADP_CHECK(a.f >= 1 && cin * a.f <= kWideMaxIn && a.T % a.f == 0,
-            "adp_stem_in: (cx+ca)*f = %d > %d or T %% f != 0", cin * a.f, kWideMaxIn);
-  ADP_CHECK(a.c0 % 8 == 0 && a.c0 <= kStemMaxC0, "adp_stem_in: c0=%d unsupported", a.c0);
+  if (int e = check_stem_envelope("adp_stem_in", a.cx, a.ca, a.c0, a.f, a.T, 1)) return e;
   ADP_CHECK((a.ca == 0) == (a.append == nullptr), "adp_stem_in: append / ca mismatch");
   ADP_CHECK(!a.noise || (a.alpha && a.beta), "adp_stem_in: noise needs alpha/beta");
   if (a.stats) ADP_CHECK(a.groups > 0 && a.groups <= 64 && a.c0 % a.groups == 0, "adp_stem_in: groups");
-  if (cin * a.f > kStemMaxIn) {
-    const size_t smem = (static_cast<size_t>(cin) * a.f * (a.c0 + kWideTP + 1) + a.c0) * sizeof(float);
+  const int ci_total = (a.cx + a.ca) * a.f;
+  if (stem_in_narrow(a)) {
+    const size_t smem = (static_cast<size_t>(a.c0) * ci_total + a.c0) * sizeof(float);
+    auto kernel = ci_total <= 4 ? stem_in_kernel<4> : stem_in_kernel<kStemInNarrowIn>;
+    dim3 grid(one_wave_gx(kernel, 256, smem, a.B, (a.T / a.f + 255) / 256), a.B);
+    ADP_CUDA(launch_k(kernel, grid, dim3(256), smem, as_stream(stream), a));
+  } else {
+    const size_t smem = (static_cast<size_t>(ci_total) * (a.c0 + kWideTP + 1) + a.c0) * sizeof(float);
     static SmemAttrCache smem_cache;
     ADP_CUDA(ensure_dyn_smem(stem_in_wide_kernel, smem, smem_cache));
-    dim3 grid(persistent_gx(stem_in_wide_kernel, 256, smem, a.B, (a.T / a.f + kWideTP - 1) / kWideTP), a.B);
+    dim3 grid(one_wave_gx(stem_in_wide_kernel, 256, smem, a.B, (a.T / a.f + kWideTP - 1) / kWideTP), a.B);
     ADP_CUDA(launch_k(stem_in_wide_kernel, grid, dim3(256), smem, as_stream(stream), a));
-    ADP_LAUNCH_CHECK();
-    return 0;
-  }
-  const size_t smem = (static_cast<size_t>(a.c0) * (a.cx + a.ca) * a.f + a.c0) * sizeof(float);
-  const int n_tiles = (a.T / a.f + 255) / 256;
-  if ((a.cx + a.ca) * a.f <= 4) {
-    dim3 grid(persistent_gx(stem_in_kernel<4>, 256, smem, a.B, n_tiles), a.B);
-    ADP_CUDA(launch_k(stem_in_kernel<4>, grid, dim3(256), smem, as_stream(stream), a));
-  } else {
-    dim3 grid(persistent_gx(stem_in_kernel<kStemMaxIn>, 256, smem, a.B, n_tiles), a.B);
-    ADP_CUDA(launch_k(stem_in_kernel<kStemMaxIn>, grid, dim3(256), smem, as_stream(stream), a));
   }
   ADP_LAUNCH_CHECK();
   return 0;
@@ -798,32 +644,26 @@ extern "C" int adp_stem_in(const adp_stem_in_args* args, adp_stream_t stream) {
 extern "C" int adp_stem_out(const adp_stem_out_args* args, adp_stream_t stream) {
   ADP_CHECK(args && args->h && args->x && args->w && args->gate, "adp_stem_out: null pointer");
   const adp_stem_out_args& a = *args;
+  if (int e = check_stem_envelope("adp_stem_out", a.cx, a.ca, a.c0, a.f, a.T, a.co)) return e;
   const int cin = a.cx + a.ca;
-  ADP_CHECK(a.co >= 1 && a.co <= kWideMaxCo && a.ca >= 0 && cin <= kWideMaxCin && a.co <= a.cx,
-            "adp_stem_out: co=%d cx=%d ca=%d unsupported (co <= cx, co <= %d, cx+ca <= %d)", a.co, a.cx,
-            a.ca, kWideMaxCo, kWideMaxCin);
-  ADP_CHECK(a.c0 % 8 == 0 && a.c0 <= kStemMaxC0 && a.f >= 1 && a.T % a.f == 0,
-            "adp_stem_out: c0=%d f=%d", a.c0, a.f);
-  ADP_CHECK(a.w_adapt || a.cx + a.ca == a.co, "adp_stem_out: identity skip needs cx+ca == co");
+  ADP_CHECK(a.w_adapt || cin == a.co, "adp_stem_out: identity skip needs cx+ca == co");
   ADP_CHECK((a.ca == 0) == (a.append == nullptr), "adp_stem_out: append / ca mismatch");
   ADP_CHECK(!a.x_next || a.ab, "adp_stem_out: x_next needs ab");
   ADP_CHECK(!a.loss_sum || (a.noise && a.alpha && a.beta), "adp_stem_out: loss needs noise/alpha/beta");
-  if (a.co > kStemMaxCo || cin > 8) {
-    ADP_CHECK(!a.loss_sum || !a.x_next, "adp_stem_out: the loss excludes the sampler fusion");
+  ADP_CHECK(!a.loss_sum || !a.x_next, "adp_stem_out: the loss excludes the sampler fusion");
+  if (stem_out_narrow(a)) {
+    const size_t smem = (static_cast<size_t>(a.co) * 3 * a.c0 + 2 * a.co + a.co * cin) * sizeof(float);
+    dim3 grid(one_wave_gx(stem_out_kernel, 256, smem, a.B, (a.T + 255) / 256), a.B);
+    ADP_CUDA(launch_k(stem_out_kernel, grid, dim3(256), smem, as_stream(stream), a));
+  } else {
     const int rows = (kWideOP + 1) / a.f + 2;
     const size_t smem = (static_cast<size_t>(a.co) * 3 * kWideCK + static_cast<size_t>(rows) * kWideHL +
                          static_cast<size_t>(cin) * kWideOP + a.co * cin + a.co) * sizeof(float);
     static SmemAttrCache smem_cache;
     ADP_CUDA(ensure_dyn_smem(stem_out_wide_kernel, smem, smem_cache));
-    dim3 grid(persistent_gx(stem_out_wide_kernel, 256, smem, a.B, (a.T + kWideOP - 1) / kWideOP), a.B);
+    dim3 grid(one_wave_gx(stem_out_wide_kernel, 256, smem, a.B, (a.T + kWideOP - 1) / kWideOP), a.B);
     ADP_CUDA(launch_k(stem_out_wide_kernel, grid, dim3(256), smem, as_stream(stream), a));
-    ADP_LAUNCH_CHECK();
-    return 0;
   }
-  const size_t smem =
-      (static_cast<size_t>(a.co) * 3 * a.c0 + 2 * a.co + a.co * (a.cx + a.ca)) * sizeof(float);
-  dim3 grid(persistent_gx(stem_out_kernel, 256, smem, a.B, (a.T + 255) / 256), a.B);
-  ADP_CUDA(launch_k(stem_out_kernel, grid, dim3(256), smem, as_stream(stream), a));
   ADP_LAUNCH_CHECK();
   return 0;
 }
@@ -843,7 +683,7 @@ extern "C" int adp_narrow_conv(const adp_narrow_conv_args* args, adp_stream_t st
     return 0;
   }
   // persistent blocks: one wave of resident blocks shares the tiles of each batch element
-  dim3 grid(persistent_gx(narrow_conv_kernel<8>, 256, 0, a.B, (a.T + 255) / 256), a.B);
+  dim3 grid(one_wave_gx(narrow_conv_kernel<8>, 256, 0, a.B, (a.T + 255) / 256), a.B);
   ADP_CUDA(launch_k(narrow_conv_kernel<8>, grid, dim3(256), (size_t)0, as_stream(stream), a));
   ADP_LAUNCH_CHECK();
   return 0;

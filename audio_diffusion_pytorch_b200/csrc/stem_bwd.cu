@@ -2,19 +2,11 @@
 // Pattern: stage the tile's activations and output gradients in shared memory, then
 //   (1) one thread per position for the data gradient, (2) one thread per parameter for the
 //   weight gradient (a 256-step dot product out of smem), one atomic per parameter per CTA.
-#include "common.cuh"
-#include "ptx.cuh"
+#include "stem.cuh"
 
 namespace adp {
 
 constexpr int kTB = 256;
-
-// blocks per batch element for the persistent tile loops: ~4 blocks per SM in total
-static int persistent_blocks(int n_tiles, int B) {
-  int g = (num_sms() * 4 + B - 1) / B;
-  if (g > n_tiles) g = n_tiles;
-  return g < 1 ? 1 : g;
-}
 
 // ---------------------------------------------------------------------- narrow_conv_bwd
 // forward: y = conv3(a) + bias, a = silu(xhat*gamma + beta), C == 8.  Given dy:
@@ -134,7 +126,6 @@ narrow_conv_bwd_kernel(const adp_narrow_conv_bwd_args a) {
       }
     }
   }
-  // (2) weight gradient: thread j < 3*C*C owns dw[co][ci][k]; threads after that own dbias[co]
   // (2) weight gradient: thread = (position p of a 64-position pass, output-channel pair cg); its
   // 2 x C x 3 dw elements and 2 dbias elements live in registers across all tiles of the block
   const int nvalid = min(kTB, a.T - t0);
@@ -205,8 +196,6 @@ narrow_conv_bwd_kernel(const adp_narrow_conv_bwd_args a) {
 }
 
 // ------------------------------------------------------------------------- stem_out_bwd
-constexpr int kSoMaxC0 = 64;
-constexpr int kSoMaxCo = 4;
 constexpr int kSoItems = 4;      // parameter-gradient elements per thread (co*c0*3 + ... <= 1024)
 __global__ void __launch_bounds__(kTB) stem_out_bwd_kernel(const adp_stem_out_bwd_args a) {
   pdl_launch_dependents();
@@ -271,13 +260,7 @@ __global__ void __launch_bounds__(kTB) stem_out_bwd_kernel(const adp_stem_out_bw
     const int r = i / cin, c = i - r * cin, t = t0 + r;
     float v = 0.f;
     if (t < a.T) {
-      if (c < a.cx) {
-        const size_t idx = (static_cast<size_t>(b) * a.cx + c) * a.T + t;
-        v = a.x[idx];
-        if (a.noise) v = al * v + be * a.noise[idx];
-      } else {
-        v = a.append[(static_cast<size_t>(b) * a.ca + (c - a.cx)) * a.T + t];
-      }
+      v = block_input(a, b, c, t, al, be);
     }
     s_xin[i] = v;
   }
@@ -490,16 +473,7 @@ __global__ void __launch_bounds__(kTB) stem_in_bwd_kernel(const adp_stem_in_bwd_
   for (int i = threadIdx.x; i < kTB * ci_total; i += kTB) {
     const int r = i / ci_total, ii = i - r * ci_total, c = ii / a.f, j = ii - c * a.f, to = to0 + r;
     float v = 0.f;
-    if (to < To) {
-      const size_t tt = static_cast<size_t>(to) * a.f + j;
-      if (c < a.cx) {
-        const size_t idx = (static_cast<size_t>(b) * a.cx + c) * a.T + tt;
-        v = a.x[idx];
-        if (a.noise) v = al * v + be * a.noise[idx];
-      } else {
-        v = a.append[(static_cast<size_t>(b) * a.ca + (c - a.cx)) * a.T + tt];
-      }
-    }
+    if (to < To) v = block_input(a, b, c, static_cast<size_t>(to) * a.f + j, al, be);
     s_in[i] = v;
   }
   const __nv_bfloat16* gb = static_cast<const __nv_bfloat16*>(a.dout) + static_cast<size_t>(b) * To * a.c0;
@@ -546,8 +520,9 @@ __global__ void __launch_bounds__(kTB) stem_in_bwd_kernel(const adp_stem_in_bwd_
 }
 
 // ------------------------------------------------------------ wide boundary (stem_out_bwd)
-// Sizes the kernels above do not take: up to 64 outputs, 64 block-input channels, c0 up to 256,
-// any f.  Three kernels, each with a fixed thread -> output mapping and every sum in fp32:
+// Every size of the envelope the narrow kernels above do not take (up to 64 outputs, 64 block-input
+// channels, c0 up to 256, any f).  Three kernels, each with a fixed thread -> output mapping and
+// every sum in fp32:
 //   dh    per (low-rate row q, channel c): sum_{o,k} w[o][c][k] D[q][o][k], where
 //         D[q][o][k] = sum of dy over the f upsampled positions fed by row q, shifted by the tap;
 //   param per (output o, channel c) of a slice: G_k = sum_t dvs[t][o] src[t+k-1][c] over a run of
@@ -667,15 +642,7 @@ __global__ void __launch_bounds__(256) stem_out_bwd_wide_param_kernel(const adp_
       for (int i = threadIdx.x; i < rows * kWideCKb; i += blockDim.x) {
         const int cc = i / rows, r = i - cc * rows, t = q_base + r, ch = c_base + cc;
         float v = 0.f;
-        if (t >= 0 && t < a.T && ch < cin) {
-          if (ch < a.cx) {
-            const size_t idx = (static_cast<size_t>(b) * a.cx + ch) * a.T + t;
-            v = a.x[idx];
-            if (a.noise) v = al * v + be * a.noise[idx];
-          } else {
-            v = a.append[(static_cast<size_t>(b) * a.ca + (ch - a.cx)) * a.T + t];
-          }
-        }
+        if (t >= 0 && t < a.T && ch < cin) v = block_input(a, b, ch, t, al, be);
         s_src[r * LS + cc] = v;
       }
     }
@@ -774,14 +741,7 @@ __global__ void __launch_bounds__(256) stem_in_bwd_wide_param_kernel(const adp_s
       float v = 0.f;
       if (to < To && ii < ci_total) {              // input ii = c*f + j at position to*f + j
         const int ch = ii / a.f;
-        const size_t tt = static_cast<size_t>(to) * a.f + (ii - ch * a.f);
-        if (ch < a.cx) {
-          const size_t idx = (static_cast<size_t>(b) * a.cx + ch) * a.T + tt;
-          v = a.x[idx];
-          if (a.noise) v = al * v + be * a.noise[idx];
-        } else {
-          v = a.append[(static_cast<size_t>(b) * a.ca + (ch - a.cx)) * a.T + tt];
-        }
+        v = block_input(a, b, ch, static_cast<size_t>(to) * a.f + (ii - ch * a.f), al, be);
       }
       s_in[r][cc] = v;
     }
@@ -844,7 +804,7 @@ extern "C" int adp_narrow_conv_bwd(const adp_narrow_conv_bwd_args* args, adp_str
             "adp_narrow_conv_bwd: null pointer");
   const adp_narrow_conv_bwd_args& a = *args;
   ADP_CHECK(a.C == 8 && a.groups > 0 && a.C % a.groups == 0, "adp_narrow_conv_bwd: C=%d groups=%d", a.C, a.groups);
-  dim3 grid(persistent_blocks((a.T + kTB - 1) / kTB, a.B), a.B);
+  dim3 grid(blocks_per_batch((a.T + kTB - 1) / kTB, a.B), a.B);
   ADP_CUDA(launch_k(narrow_conv_bwd_kernel<8>, grid, dim3(kTB), (size_t)0, as_stream(stream), a));
   return 0;
 }
@@ -853,88 +813,70 @@ extern "C" int adp_stem_out_bwd(const adp_stem_out_bwd_args* args, adp_stream_t 
   ADP_CHECK(args && args->dv && args->h && args->x && args->w && args->gate && args->dh && args->dw &&
             args->dbias && args->dgate, "adp_stem_out_bwd: null pointer");
   const adp_stem_out_bwd_args& a = *args;
+  if (int e = check_stem_envelope("adp_stem_out_bwd", a.cx, a.ca, a.c0, a.f, a.T, a.co)) return e;
   const int cin = a.cx + a.ca;
-  ADP_CHECK(a.co >= 1 && a.co <= 64 && a.co <= a.cx && a.ca >= 0 && cin <= 64 && a.c0 % 8 == 0 &&
-            a.c0 >= 8 && a.c0 <= 256,
-            "adp_stem_out_bwd: co=%d cx=%d ca=%d c0=%d unsupported (co <= cx, co <= 64, cx+ca <= 64, c0 <= 256)",
-            a.co, a.cx, a.ca, a.c0);
-  ADP_CHECK(a.f >= 1 && a.T % a.f == 0, "adp_stem_out_bwd: f=%d", a.f);
   ADP_CHECK(!a.w_adapt || (a.dw_adapt && a.db_adapt), "adp_stem_out_bwd: adapter grads missing");
   ADP_CHECK((a.ca == 0) == (a.append == nullptr), "adp_stem_out_bwd: append / ca mismatch");
-  if (a.co > kSoMaxCo || a.c0 > kSoMaxC0 || cin > 8 || kTB % a.f != 0 ||
-      a.co * a.c0 * 3 + 3 * a.co + a.co * cin > kSoItems * kTB) {
-    ADP_CHECK(a.w_adapt || cin == a.co, "adp_stem_out_bwd: identity skip needs cx+ca == co");
-    ADP_CHECK(a.ld_dgate >= a.co && (a.ld_gate == 0 || a.ld_gate >= a.co), "adp_stem_out_bwd: gate pitches");
-    cudaStream_t s = as_stream(stream);
-    const int Tl = a.T / a.f;
-    const int n_cz = (a.c0 + kWideCKb - 1) / kWideCKb;
-    const size_t smem_dh = (static_cast<size_t>(a.co) * 3 * kWideCKb + kWideQT * (a.co * 3 + 1)) * sizeof(float);
-    static SmemAttrCache dh_cache;
-    ADP_CUDA(ensure_dyn_smem(stem_out_bwd_wide_dh_kernel, smem_dh, dh_cache));
-    int gx = (num_sms() * 4 + a.B * n_cz - 1) / (a.B * n_cz);
-    gx = max(1, min(gx, (Tl + kWideQT - 1) / kWideQT));
-    ADP_CUDA(launch_k(stem_out_bwd_wide_dh_kernel, dim3(gx, a.B, n_cz), dim3(256), smem_dh, s, a));
-    const int n_chunks = n_cz + (a.w_adapt ? (cin + kWideCKb - 1) / kWideCKb : 0);
-    const int nz = ((a.co + kWideOS - 1) / kWideOS) * n_chunks;
-    const int f_rows = a.w_adapt ? 1 : a.f;        // adapter slices stage positions (f = 1)
-    const size_t smem_p = (static_cast<size_t>(kWideOS) * kWidePT +
-                           static_cast<size_t>((kWidePT + 1) / f_rows + 2) * (kWideCKb + 1)) * sizeof(float);
-    static SmemAttrCache p_cache;
-    ADP_CUDA(ensure_dyn_smem(stem_out_bwd_wide_param_kernel, smem_p, p_cache));
-    gx = (num_sms() * 4 + a.B * nz - 1) / (a.B * nz);
-    gx = max(1, min(gx, (a.T + kWidePT - 1) / kWidePT));
-    ADP_CUDA(launch_k(stem_out_bwd_wide_param_kernel, dim3(gx, a.B, nz), dim3(256), smem_p, s, a));
-    if (a.dxin) {
-      const size_t n = static_cast<size_t>(a.B) * cin * a.T;
-      const size_t cap = static_cast<size_t>(num_sms()) * 16;
-      const int g = static_cast<int>((n + 255) / 256 < cap ? (n + 255) / 256 : cap);
-      ADP_CUDA(launch_k(stem_out_bwd_wide_dxin_kernel, dim3(g), dim3(256), (size_t)0, s, a));
-    }
-    ADP_LAUNCH_CHECK();
+  ADP_CHECK(a.w_adapt || cin == a.co, "adp_stem_out_bwd: identity skip needs cx+ca == co");
+  ADP_CHECK(a.ld_dgate >= a.co && (a.ld_gate == 0 || a.ld_gate >= a.co), "adp_stem_out_bwd: gate pitches");
+  cudaStream_t s = as_stream(stream);
+  if (stem_out_bwd_narrow(a)) {
+    const size_t smem = (static_cast<size_t>(a.co) * 3 * a.c0 + static_cast<size_t>(kTB / a.f + 2) * a.c0 +
+                         static_cast<size_t>(kTB + 2) * a.co + static_cast<size_t>(kTB) * a.co +
+                         static_cast<size_t>(kTB) * cin) * sizeof(float);
+    static SmemAttrCache smem_cache;
+    ADP_CUDA(ensure_dyn_smem(stem_out_bwd_kernel, smem, smem_cache));
+    dim3 grid(blocks_per_batch((a.T + kTB - 1) / kTB, a.B), a.B);
+    ADP_CUDA(launch_k(stem_out_bwd_kernel, grid, dim3(kTB), smem, s, a));
     return 0;
   }
-  const int rows_h = kTB / a.f + 2;
-  const size_t smem = (static_cast<size_t>(a.co) * 3 * a.c0 + static_cast<size_t>(rows_h) * a.c0 +
-                       static_cast<size_t>(kTB + 2) * a.co + static_cast<size_t>(kTB) * a.co +
-                       static_cast<size_t>(kTB) * cin) * sizeof(float);
-  static SmemAttrCache smem_cache;
-  ADP_CUDA(ensure_dyn_smem(stem_out_bwd_kernel, smem, smem_cache));
-  ADP_CHECK(a.co * a.c0 * 3 + 3 * a.co + a.co * cin <= kSoItems * kTB, "adp_stem_out_bwd: too many parameters");
-  dim3 grid(persistent_blocks((a.T + kTB - 1) / kTB, a.B), a.B);
-  ADP_CUDA(launch_k(stem_out_bwd_kernel, grid, dim3(kTB), smem, as_stream(stream), a));
+  const int Tl = a.T / a.f;
+  const int n_cz = (a.c0 + kWideCKb - 1) / kWideCKb;
+  const size_t smem_dh = (static_cast<size_t>(a.co) * 3 * kWideCKb + kWideQT * (a.co * 3 + 1)) * sizeof(float);
+  static SmemAttrCache dh_cache;
+  ADP_CUDA(ensure_dyn_smem(stem_out_bwd_wide_dh_kernel, smem_dh, dh_cache));
+  ADP_CUDA(launch_k(stem_out_bwd_wide_dh_kernel, dim3(blocks_per_batch((Tl + kWideQT - 1) / kWideQT, a.B, n_cz), a.B, n_cz),
+                    dim3(256), smem_dh, s, a));
+  const int n_chunks = n_cz + (a.w_adapt ? (cin + kWideCKb - 1) / kWideCKb : 0);
+  const int nz = ((a.co + kWideOS - 1) / kWideOS) * n_chunks;
+  const int f_rows = a.w_adapt ? 1 : a.f;        // adapter slices stage positions (f = 1)
+  const size_t smem_p = (static_cast<size_t>(kWideOS) * kWidePT +
+                         static_cast<size_t>((kWidePT + 1) / f_rows + 2) * (kWideCKb + 1)) * sizeof(float);
+  static SmemAttrCache p_cache;
+  ADP_CUDA(ensure_dyn_smem(stem_out_bwd_wide_param_kernel, smem_p, p_cache));
+  ADP_CUDA(launch_k(stem_out_bwd_wide_param_kernel, dim3(blocks_per_batch((a.T + kWidePT - 1) / kWidePT, a.B, nz), a.B, nz),
+                    dim3(256), smem_p, s, a));
+  if (a.dxin)
+    ADP_CUDA(launch_k(stem_out_bwd_wide_dxin_kernel, dim3(capped_grid(static_cast<int64_t>(a.B) * cin * a.T, 256)),
+                      dim3(256), (size_t)0, s, a));
+  ADP_LAUNCH_CHECK();
   return 0;
 }
 
 extern "C" int adp_stem_in_bwd(const adp_stem_in_bwd_args* args, adp_stream_t stream) {
   ADP_CHECK(args && args->dout && args->x && args->dw && args->dbias, "adp_stem_in_bwd: null pointer");
   const adp_stem_in_bwd_args& a = *args;
-  const int cin = a.cx + a.ca;
-  ADP_CHECK(a.f >= 1 && a.ca >= 0 && cin <= 64 && cin * a.f <= 128 && a.c0 % 8 == 0 && a.c0 >= 8 &&
-            a.c0 <= 256 && a.T % a.f == 0,
-            "adp_stem_in_bwd: cx+ca=%d f=%d c0=%d unsupported (cx+ca <= 64, (cx+ca)*f <= 128, c0 <= 256)",
-            cin, a.f, a.c0);
+  if (int e = check_stem_envelope("adp_stem_in_bwd", a.cx, a.ca, a.c0, a.f, a.T, 1)) return e;
   ADP_CHECK((a.ca == 0) == (a.append == nullptr), "adp_stem_in_bwd: append / ca mismatch");
   ADP_CHECK(!a.dxin || a.w, "adp_stem_in_bwd: dxin needs the conv weights");
-  if (cin * a.f > 32 || a.c0 > 64) {
-    cudaStream_t s = as_stream(stream);
-    const int To = a.T / a.f;
-    const int nz = ((a.c0 + kWideCKb - 1) / kWideCKb) * ((cin * a.f + kWideCKb - 1) / kWideCKb);
-    int gx = (num_sms() * 4 + a.B * nz - 1) / (a.B * nz);
-    gx = max(1, min(gx, (To + kWidePT - 1) / kWidePT));
-    ADP_CUDA(launch_k(stem_in_bwd_wide_param_kernel, dim3(gx, a.B, nz), dim3(256), (size_t)0, s, a));
-    if (a.dxin) {
-      const size_t smem = static_cast<size_t>(kWideQT) * (a.c0 + 1) * sizeof(float);
-      gx = (num_sms() * 4 + a.B - 1) / a.B;
-      gx = max(1, min(gx, (To + kWideQT - 1) / kWideQT));
-      ADP_CUDA(launch_k(stem_in_bwd_wide_dxin_kernel, dim3(gx, a.B), dim3(256), smem, s, a));
-    }
-    ADP_LAUNCH_CHECK();
+  cudaStream_t s = as_stream(stream);
+  const int ci_total = (a.cx + a.ca) * a.f, To = a.T / a.f;
+  if (stem_in_bwd_narrow(a)) {
+    const size_t smem = (static_cast<size_t>(kTB) * ci_total + static_cast<size_t>(kTB) * a.c0) * sizeof(float);
+    static SmemAttrCache smem_cache;
+    ADP_CUDA(ensure_dyn_smem(stem_in_bwd_kernel, smem, smem_cache));
+    ADP_CUDA(launch_k(stem_in_bwd_kernel, dim3(blocks_per_batch((To + kTB - 1) / kTB, a.B), a.B), dim3(kTB), smem,
+                      s, a));
     return 0;
   }
-  const size_t smem = (static_cast<size_t>(kTB) * (a.cx + a.ca) * a.f + static_cast<size_t>(kTB) * a.c0) * sizeof(float);
-  static SmemAttrCache smem_cache;
-  ADP_CUDA(ensure_dyn_smem(stem_in_bwd_kernel, smem, smem_cache));
-  dim3 grid(persistent_blocks((a.T / a.f + kTB - 1) / kTB, a.B), a.B);
-  ADP_CUDA(launch_k(stem_in_bwd_kernel, grid, dim3(kTB), smem, as_stream(stream), a));
+  const int nz = ((a.c0 + kWideCKb - 1) / kWideCKb) * ((ci_total + kWideCKb - 1) / kWideCKb);
+  ADP_CUDA(launch_k(stem_in_bwd_wide_param_kernel, dim3(blocks_per_batch((To + kWidePT - 1) / kWidePT, a.B, nz), a.B, nz),
+                    dim3(256), (size_t)0, s, a));
+  if (a.dxin) {
+    const size_t smem = static_cast<size_t>(kWideQT) * (a.c0 + 1) * sizeof(float);
+    ADP_CUDA(launch_k(stem_in_bwd_wide_dxin_kernel, dim3(blocks_per_batch((To + kWideQT - 1) / kWideQT, a.B), a.B),
+                      dim3(256), smem, s, a));
+  }
+  ADP_LAUNCH_CHECK();
   return 0;
 }

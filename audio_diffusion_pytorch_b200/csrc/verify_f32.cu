@@ -6,8 +6,7 @@
 // the reference at fp32 tolerance (rtol 1e-3 / atol 1e-4), which the bf16 storage of the fast
 // path cannot show.  Not a performance path: far slower than the tensor-core kernels.
 // Entry points mirror their bf16 counterparts argument for argument (a/w/out/residual/h are fp32).
-#include "common.cuh"
-#include "ptx.cuh"
+#include "stem.cuh"
 
 namespace adp {
 
@@ -259,20 +258,12 @@ __global__ void __launch_bounds__(256) f32_stem_in_kernel(const adp_stem_in_args
     const int c = static_cast<int>(i % a.c0);
     const int to = static_cast<int>((i / a.c0) % To);
     const int b = static_cast<int>(i / (static_cast<int64_t>(a.c0) * To));
+    const float al = a.noise ? a.alpha[b] : 1.f, be = a.noise ? a.beta[b] : 0.f;
     float acc = a.bias ? a.bias[c] : 0.f;
     for (int ci = 0; ci < cin; ++ci)
-      for (int j = 0; j < a.f; ++j) {
-        const int64_t tt = static_cast<int64_t>(to) * a.f + j;
-        float xv;
-        if (ci < a.cx) {
-          const int64_t idx = (static_cast<int64_t>(b) * a.cx + ci) * a.T + tt;
-          xv = a.x[idx];
-          if (a.noise) xv = a.alpha[b] * xv + a.beta[b] * a.noise[idx];
-        } else {
-          xv = a.append[(static_cast<int64_t>(b) * a.ca + (ci - a.cx)) * a.T + tt];
-        }
-        acc = fmaf(xv, a.w[(static_cast<int64_t>(c) * cin + ci) * a.f + j], acc);
-      }
+      for (int j = 0; j < a.f; ++j)
+        acc = fmaf(block_input(a, b, ci, static_cast<size_t>(to) * a.f + j, al, be),
+                   a.w[(static_cast<int64_t>(c) * cin + ci) * a.f + j], acc);
     out[i] = acc;
   }
 }
@@ -291,12 +282,9 @@ __device__ __forceinline__ float f32_stem_branch(const adp_stem_out_args& a, con
   return y;
 }
 
-constexpr int kF32StemMaxCin = 64;   // cx + ca (the block input held per position)
-
 __global__ void __launch_bounds__(256) f32_stem_out_kernel(const adp_stem_out_args a) {
   pdl_launch_dependents();
   pdl_wait();
-  const int ldg = a.ld_gate > 0 ? a.ld_gate : a.co;
   const int cin = a.cx + a.ca, Tl = a.T / a.f;
   const float* h = static_cast<const float*>(a.h);
   const int64_t total = static_cast<int64_t>(a.B) * a.T;
@@ -308,17 +296,8 @@ __global__ void __launch_bounds__(256) f32_stem_out_kernel(const adp_stem_out_ar
     const int t = static_cast<int>(i % a.T);
     const int b = static_cast<int>(i / a.T);
     const float al = a.noise ? a.alpha[b] : 1.f, be = a.noise ? a.beta[b] : 0.f;
-    float xin[kF32StemMaxCin];
-    for (int c = 0; c < kF32StemMaxCin; ++c) {
-      xin[c] = 0.f;
-      if (c < a.cx) {
-        const int64_t idx = (static_cast<int64_t>(b) * a.cx + c) * a.T + t;
-        xin[c] = a.x[idx];
-        if (a.noise) xin[c] = al * xin[c] + be * a.noise[idx];
-      } else if (c < cin) {
-        xin[c] = a.append[(static_cast<int64_t>(b) * a.ca + (c - a.cx)) * a.T + t];
-      }
-    }
+    float xin[kStemMaxCin];
+    for (int c = 0; c < kStemMaxCin; ++c) xin[c] = c < cin ? block_input(a, b, c, t, al, be) : 0.f;
     for (int o = 0; o < a.co; ++o) {
       float skip;
       if (a.w_adapt) {
@@ -327,45 +306,12 @@ __global__ void __launch_bounds__(256) f32_stem_out_kernel(const adp_stem_out_ar
       } else {
         skip = xin[o];
       }
-      float v = skip + a.gate[static_cast<int64_t>(b) * ldg + o] *
-                           f32_stem_branch(a, h + static_cast<int64_t>(b) * Tl * a.c0, o, t);
-      if (a.cfg) {
-        const float vm = skip + a.gate[static_cast<int64_t>(b + a.B) * ldg + o] *
-                                    f32_stem_branch(a, h + static_cast<int64_t>(b + a.B) * Tl * a.c0, o, t);
-        v = vm + (v - vm) * a.cfg_scale;
-      }
-      const int64_t oidx = (static_cast<int64_t>(b) * a.co + o) * a.T + t;
-      if (a.v_out) a.v_out[oidx] = v;
-      if (a.x_next) {
-        const float a0 = a.ab[0], b0 = a.ab[1], a1 = a.ab[2], b1 = a.ab[3];
-        a.x_next[oidx] = a1 * (a0 * xin[o] - b0 * v) + b1 * (b0 * xin[o] + a0 * v);
-      }
-      if (a.loss_sum) {                     // target alpha*noise - beta*x (reference diffusion.py:92,95)
-        const int64_t xidx = (static_cast<int64_t>(b) * a.cx + o) * a.T + t;
-        const float d = v - (al * a.noise[xidx] - be * a.x[xidx]);
-        lsum += static_cast<double>(d) * d;
-        if (a.dv) a.dv[oidx] = 2.f * d / (static_cast<float>(a.B) * a.co * a.T);
-      }
+      const float y = f32_stem_branch(a, h + static_cast<int64_t>(b) * Tl * a.c0, o, t);
+      const float ym = a.cfg ? f32_stem_branch(a, h + static_cast<int64_t>(b + a.B) * Tl * a.c0, o, t) : 0.f;
+      stem_out_finish(a, b, o, t, skip, y, ym, xin[o], al, be, lsum);
     }
   }
-  if (a.loss_sum) {                         // every thread of the block reaches this point
-    __shared__ double s_loss[8];
-    for (int o = 16; o > 0; o >>= 1) lsum += __shfl_xor_sync(0xffffffffu, lsum, o);
-    if ((threadIdx.x & 31) == 0) s_loss[threadIdx.x >> 5] = lsum;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      double tot = 0.0;
-      for (int w = 0; w < (blockDim.x >> 5); ++w) tot += s_loss[w];
-      atomicAdd(a.loss_sum, tot);
-    }
-  }
-}
-
-static int f32_grid(int64_t n) {
-  int64_t g = (n + 255) / 256;
-  if (g < 1) g = 1;
-  if (g > num_sms() * 16) g = num_sms() * 16;
-  return static_cast<int>(g);
+  if (a.loss_sum) block_loss_flush(lsum, a.loss_sum);   // every thread of the block reaches this point
 }
 
 }  // namespace adp
@@ -379,7 +325,7 @@ extern "C" int adp_f32_conv_gemm(const adp_conv_gemm_args* args, adp_stream_t st
   ADP_CHECK(!a.stats && !a.gn_stats, "adp_f32_conv_gemm: statistics / fused GroupNorm are separate passes");
   ADP_CHECK(a.up_factor <= 1 || a.phases == a.up_factor, "adp_f32_conv_gemm: phases != up_factor");
   ADP_CHECK(a.up_factor > 1 || (a.ntaps >= 1 && a.ntaps <= 3 && a.phases == 1), "adp_f32_conv_gemm: taps");
-  ADP_CUDA(launch_k(f32_conv_gemm_kernel, dim3(f32_grid(static_cast<int64_t>(a.B) * a.T * a.phases * a.n_valid)),
+  ADP_CUDA(launch_k(f32_conv_gemm_kernel, dim3(capped_grid(static_cast<int64_t>(a.B) * a.T * a.phases * a.n_valid, 256)),
                     dim3(256), (size_t)0, as_stream(stream), a));
   ADP_LAUNCH_CHECK();
   return 0;
@@ -389,7 +335,7 @@ extern "C" int adp_f32_gn_stats(const float* x, double* stats, int B, int T, int
                                 adp_stream_t stream) {
   ADP_CHECK(x && stats && B > 0 && B <= 65535 && T > 0 && C > 0 && groups > 0 && groups <= 64 && C % groups == 0,
             "adp_f32_gn_stats: bad args");
-  int gx = f32_grid(static_cast<int64_t>(T) * C);
+  int gx = capped_grid(static_cast<int64_t>(T) * C, 256);
   if (gx > num_sms() * 4) gx = num_sms() * 4;
   ADP_CUDA(launch_k(f32_gn_stats_kernel, dim3(gx, B), dim3(256), (size_t)0, as_stream(stream), x, stats, T, C,
                     groups));
@@ -402,7 +348,7 @@ extern "C" int adp_f32_gn_silu(const float* x, float* y, const double* stats, co
                                adp_stream_t stream) {
   ADP_CHECK(x && y && stats && gamma && beta && B > 0 && T > 0 && C > 0 && groups > 0 && C % groups == 0,
             "adp_f32_gn_silu: bad args");
-  ADP_CUDA(launch_k(f32_gn_silu_kernel, dim3(f32_grid(static_cast<int64_t>(B) * T * C)), dim3(256), (size_t)0,
+  ADP_CUDA(launch_k(f32_gn_silu_kernel, dim3(capped_grid(static_cast<int64_t>(B) * T * C, 256)), dim3(256), (size_t)0,
                     as_stream(stream), x, y, stats, gamma, beta, B, T, C, groups, eps));
   ADP_LAUNCH_CHECK();
   return 0;
@@ -411,7 +357,7 @@ extern "C" int adp_f32_gn_silu(const float* x, float* y, const double* stats, co
 extern "C" int adp_f32_ln_film(const float* x, float* y, float* y2, const float* scale_shift, int ss_stride,
                                int B, int T, int C, float eps, float eps2, adp_stream_t stream) {
   ADP_CHECK(x && y && B > 0 && T > 0 && C > 0, "adp_f32_ln_film: bad args");
-  ADP_CUDA(launch_k(f32_ln_film_kernel, dim3(f32_grid(static_cast<int64_t>(B) * T * 32)), dim3(256), (size_t)0,
+  ADP_CUDA(launch_k(f32_ln_film_kernel, dim3(capped_grid(static_cast<int64_t>(B) * T * 32, 256)), dim3(256), (size_t)0,
                     as_stream(stream), x, y, y2, scale_shift, ss_stride, B, T, C, eps, eps2));
   ADP_LAUNCH_CHECK();
   return 0;
@@ -432,12 +378,10 @@ extern "C" int adp_f32_attention_lse(const float* q, const float* k, const float
   const int64_t w = static_cast<int64_t>(H) * head_dim;
   ADP_CHECK(ldq >= w && ldk >= w && ldv >= w && ldo >= w,
             "adp_f32_attention: row pitches must be >= heads*head_dim (%d*%d)", H, head_dim);
-  int64_t n = static_cast<int64_t>(B) * H * Tq;
-  int64_t g = (n + 127) / 128;
-  if (g > num_sms() * 16) g = num_sms() * 16;
+  const int g = capped_grid(static_cast<int64_t>(B) * H * Tq, 128);
   auto kern = head_dim == 32 ? f32_attention_kernel<32>
               : head_dim == 128 ? f32_attention_kernel<128> : f32_attention_kernel<64>;
-  ADP_CUDA(launch_k(kern, dim3(static_cast<int>(g)), dim3(128), (size_t)0, as_stream(stream), q, k, v, o, B, H,
+  ADP_CUDA(launch_k(kern, dim3(g), dim3(128), (size_t)0, as_stream(stream), q, k, v, o, B, H,
                     Tq, Tk, ldq, ldk, ldv, ldo, scale, lse));
   ADP_LAUNCH_CHECK();
   return 0;
@@ -451,7 +395,7 @@ extern "C" int adp_f32_attention(const float* q, const float* k, const float* v,
 extern "C" int adp_f32_linear(const float* x, const float* w, const float* bias, float* y, int B, int K, int N,
                               int ldx, int ldw, int ldy, int in_act, int out_act, adp_stream_t stream) {
   ADP_CHECK(x && w && y && B > 0 && K > 0 && N > 0, "adp_f32_linear: bad args");
-  ADP_CUDA(launch_k(f32_linear_kernel, dim3(f32_grid(static_cast<int64_t>(B) * N)), dim3(256), (size_t)0,
+  ADP_CUDA(launch_k(f32_linear_kernel, dim3(capped_grid(static_cast<int64_t>(B) * N, 256)), dim3(256), (size_t)0,
                     as_stream(stream), x, w, bias, y, B, K, N, ldx, ldw, ldy, in_act, out_act));
   ADP_LAUNCH_CHECK();
   return 0;
@@ -459,7 +403,7 @@ extern "C" int adp_f32_linear(const float* x, const float* w, const float* bias,
 
 extern "C" int adp_f32_silu(const float* x, float* y, int64_t n, adp_stream_t stream) {
   ADP_CHECK(x && y && n > 0, "adp_f32_silu: bad args");
-  ADP_CUDA(launch_k(f32_silu_kernel, dim3(f32_grid(n)), dim3(256), (size_t)0, as_stream(stream), x, y, n));
+  ADP_CUDA(launch_k(f32_silu_kernel, dim3(capped_grid(n, 256)), dim3(256), (size_t)0, as_stream(stream), x, y, n));
   ADP_LAUNCH_CHECK();
   return 0;
 }
@@ -476,7 +420,7 @@ extern "C" int adp_f32_stem_in_train(const adp_stem_in_args* args, adp_stream_t 
   ADP_CHECK(!a.noise || (a.alpha && a.beta), "adp_f32_stem_in: noise needs alpha/beta");
   ADP_CHECK(a.B > 0 && a.T > 0 && a.c0 > 0 && a.cx > 0 && a.f >= 1 && a.T % a.f == 0 &&
             (a.ca == 0) == (a.append == nullptr), "adp_f32_stem_in: bad args");
-  ADP_CUDA(launch_k(f32_stem_in_kernel, dim3(f32_grid(static_cast<int64_t>(a.B) * (a.T / a.f) * a.c0)), dim3(256),
+  ADP_CUDA(launch_k(f32_stem_in_kernel, dim3(capped_grid(static_cast<int64_t>(a.B) * (a.T / a.f) * a.c0, 256)), dim3(256),
                     (size_t)0, as_stream(stream), a));
   ADP_LAUNCH_CHECK();
   return 0;
@@ -499,9 +443,9 @@ extern "C" int adp_f32_stem_out_train(const adp_stem_out_args* args, adp_stream_
   ADP_CHECK(a.w_adapt || a.cx + a.ca == a.co, "adp_f32_stem_out: identity skip needs cx+ca == co");
   ADP_CHECK(!a.x_next || a.ab, "adp_f32_stem_out: x_next needs ab");
   ADP_CHECK(a.f >= 1 && a.T % a.f == 0 && (a.ca == 0) == (a.append == nullptr), "adp_f32_stem_out: bad args");
-  ADP_CHECK(a.cx + a.ca <= kF32StemMaxCin && a.co <= a.cx,
-            "adp_f32_stem_out: in <= %d channels, out <= x channels", kF32StemMaxCin);
-  ADP_CUDA(launch_k(f32_stem_out_kernel, dim3(f32_grid(static_cast<int64_t>(a.B) * a.T)), dim3(256),
+  ADP_CHECK(a.cx + a.ca <= kStemMaxCin && a.co <= a.cx,
+            "adp_f32_stem_out: in <= %d channels, out <= x channels", kStemMaxCin);
+  ADP_CUDA(launch_k(f32_stem_out_kernel, dim3(capped_grid(static_cast<int64_t>(a.B) * a.T, 256)), dim3(256),
                     (size_t)0, as_stream(stream), a));
   ADP_LAUNCH_CHECK();
   return 0;

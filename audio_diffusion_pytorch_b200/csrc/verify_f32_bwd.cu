@@ -5,8 +5,7 @@
 // summed over the batch, a GroupNorm group summed over its channels), as in the bf16 kernels.
 // Entry points take the arguments of the bf16 entry point they shadow, every activation pointer
 // fp32.  Not a performance path.
-#include "common.cuh"
-#include "ptx.cuh"
+#include "stem.cuh"
 
 namespace adp {
 namespace {
@@ -276,15 +275,6 @@ __device__ __forceinline__ float so_dy(const adp_stem_out_bwd_args& a, int b, in
   const int ldg = a.ld_gate > 0 ? a.ld_gate : a.co;
   return so_dvs(a, b, o, t) * a.gate[static_cast<int64_t>(b) * ldg + o];
 }
-__device__ __forceinline__ float so_xin(const adp_stem_out_bwd_args& a, int b, int c, int t) {
-  if (c < a.cx) {
-    const int64_t idx = (static_cast<int64_t>(b) * a.cx + c) * a.T + t;
-    float v = a.x[idx];
-    if (a.noise) v = a.alpha[b] * v + a.beta[b] * a.noise[idx];
-    return v;
-  }
-  return a.append[(static_cast<int64_t>(b) * a.ca + (c - a.cx)) * a.T + t];
-}
 
 // dh[b][q][c] = sum over the upsampled positions u fed by row q and taps k of dy[t = u-k+1] w[o][c][k]
 __global__ void __launch_bounds__(256) f32_stem_out_bwd_dh_kernel(const adp_stem_out_bwd_args a) {
@@ -349,8 +339,10 @@ __global__ void __launch_bounds__(256) f32_stem_out_bwd_param_kernel(const adp_s
       a.dgate[static_cast<int64_t>(b) * a.ld_dgate + o] += acc;
     } else if (item < n_w + a.co + n_g + n_ad) {        // dw_adapt[o][c]
       const int r = item - n_w - a.co - n_g, o = r / cin, c = r - o * cin;
-      for (int b = 0; b < a.B; ++b)
-        for (int t = 0; t < a.T; ++t) acc = fmaf(so_dvs(a, b, o, t), so_xin(a, b, c, t), acc);
+      for (int b = 0; b < a.B; ++b) {
+        const float al = a.noise ? a.alpha[b] : 1.f, be = a.noise ? a.beta[b] : 0.f;
+        for (int t = 0; t < a.T; ++t) acc = fmaf(so_dvs(a, b, o, t), block_input(a, b, c, t, al, be), acc);
+      }
       a.dw_adapt[r] += acc;
     } else {                                            // db_adapt[o]
       const int o = item - n_w - a.co - n_g - n_ad;
@@ -382,16 +374,6 @@ __global__ void __launch_bounds__(256) f32_stem_out_bwd_dxin_kernel(const adp_st
 
 // ------------------------------------------------------------------------- stem_in backward
 // forward (f32_stem_in_kernel): out[b,to,o] = bias[o] + sum_{c,j} w[o][c][j] xin[b,c,to*f+j]
-__device__ __forceinline__ float si_xin(const adp_stem_in_bwd_args& a, int b, int c, int64_t t) {
-  if (c < a.cx) {
-    const int64_t idx = (static_cast<int64_t>(b) * a.cx + c) * a.T + t;
-    float v = a.x[idx];
-    if (a.noise) v = a.alpha[b] * v + a.beta[b] * a.noise[idx];
-    return v;
-  }
-  return a.append[(static_cast<int64_t>(b) * a.ca + (c - a.cx)) * a.T + t];
-}
-
 __global__ void __launch_bounds__(256) f32_stem_in_bwd_param_kernel(const adp_stem_in_bwd_args a) {
   pdl_launch_dependents();
   pdl_wait();
@@ -403,10 +385,12 @@ __global__ void __launch_bounds__(256) f32_stem_in_bwd_param_kernel(const adp_st
     float acc = 0.f;
     if (item < n_w) {                                   // dw[o][c][j]
       const int o = item / ci_total, r = item - o * ci_total, c = r / a.f, j = r - c * a.f;
-      for (int b = 0; b < a.B; ++b)
+      for (int b = 0; b < a.B; ++b) {
+        const float al = a.noise ? a.alpha[b] : 1.f, be = a.noise ? a.beta[b] : 0.f;
         for (int to = 0; to < To; ++to)
           acc = fmaf(g[(static_cast<int64_t>(b) * To + to) * a.c0 + o],
-                     si_xin(a, b, c, static_cast<int64_t>(to) * a.f + j), acc);
+                     block_input(a, b, c, static_cast<size_t>(to) * a.f + j, al, be), acc);
+      }
       a.dw[item] += acc;
     } else {
       const int o = item - n_w;
@@ -546,13 +530,6 @@ __global__ void __launch_bounds__(128) f32_attention_dkdv_kernel(const adp_atten
   }
 }
 
-int grid_for(int64_t n, int threads) {
-  int64_t g = (n + threads - 1) / threads;
-  if (g < 1) g = 1;
-  if (g > num_sms() * 16) g = num_sms() * 16;
-  return static_cast<int>(g);
-}
-
 }  // namespace
 }  // namespace adp
 
@@ -567,7 +544,7 @@ extern "C" int adp_f32_wgrad(const adp_wgrad_args* args, adp_stream_t stream) {
   ADP_CHECK(a.ntaps == 0 || a.ntaps == 1 || a.ntaps == 3, "adp_f32_wgrad: ntaps must be 1 or 3");
   ADP_CHECK(a.ntaps != 3 || a.tap_stride >= (long long)a.n * a.ldw, "adp_f32_wgrad: tap_stride smaller than one dW slab");
   const int64_t n = static_cast<int64_t>(a.ntaps == 3 ? 3 : 1) * a.n * a.k;
-  ADP_CUDA(launch_k(f32_wgrad_kernel, dim3(grid_for(n, 256)), dim3(256), (size_t)0, as_stream(stream), a));
+  ADP_CUDA(launch_k(f32_wgrad_kernel, dim3(capped_grid(n, 256)), dim3(256), (size_t)0, as_stream(stream), a));
   ADP_LAUNCH_CHECK();
   return 0;
 }
@@ -578,7 +555,7 @@ extern "C" int adp_f32_gn_silu_bwd(const float* da, const float* x, const double
   ADP_CHECK(da && x && stats && gamma && beta && dxh && dgamma && dbeta && S, "adp_f32_gn_silu_bwd: null");
   ADP_CHECK(B > 0 && T > 0 && C > 0 && groups > 0 && C % groups == 0, "adp_f32_gn_silu_bwd: C=%d groups=%d",
             C, groups);
-  ADP_CUDA(launch_k(f32_gn_silu_bwd_kernel, dim3(grid_for(static_cast<int64_t>(B) * C, 256)), dim3(256),
+  ADP_CUDA(launch_k(f32_gn_silu_bwd_kernel, dim3(capped_grid(static_cast<int64_t>(B) * C, 256)), dim3(256),
                     (size_t)0, as_stream(stream), da, x, stats, gamma, beta, dxh, dgamma, dbeta, S, B, T, C,
                     groups, eps));
   ADP_LAUNCH_CHECK();
@@ -591,7 +568,7 @@ extern "C" int adp_f32_gn_bwd_apply(const float* dxh, const float* x, const doub
   ADP_CHECK(dxh && x && stats && S && dx, "adp_f32_gn_bwd_apply: null");
   ADP_CHECK(B > 0 && T > 0 && C > 0 && groups > 0 && C % groups == 0, "adp_f32_gn_bwd_apply: C=%d groups=%d",
             C, groups);
-  ADP_CUDA(launch_k(f32_gn_bwd_apply_kernel, dim3(grid_for(static_cast<int64_t>(B) * C, 256)), dim3(256),
+  ADP_CUDA(launch_k(f32_gn_bwd_apply_kernel, dim3(capped_grid(static_cast<int64_t>(B) * C, 256)), dim3(256),
                     (size_t)0, as_stream(stream), dxh, x, stats, S, dres, dx, colsum, B, T, C, groups, eps));
   ADP_LAUNCH_CHECK();
   return 0;
@@ -605,7 +582,7 @@ extern "C" int adp_f32_ln_film_bwd(const float* dy, const float* x, const float*
   ADP_CHECK(!scale_shift || ss_stride >= 2 * C, "adp_f32_ln_film_bwd: ss_stride %d < 2C", ss_stride);
   ADP_CHECK(!dss || dss_stride >= 2 * C, "adp_f32_ln_film_bwd: dss_stride %d < 2C", dss_stride);
   const int64_t warps = static_cast<int64_t>(B) * ((C + 31) / 32);
-  ADP_CUDA(launch_k(f32_ln_film_bwd_kernel, dim3(grid_for(warps * 32, 256)), dim3(256), (size_t)0,
+  ADP_CUDA(launch_k(f32_ln_film_bwd_kernel, dim3(capped_grid(warps * 32, 256)), dim3(256), (size_t)0,
                     as_stream(stream), dy, x, scale_shift, ss_stride, dx, dss, dss_stride, colsum, dres, B, T, C,
                     eps));
   ADP_LAUNCH_CHECK();
@@ -616,7 +593,7 @@ extern "C" int adp_f32_colsum(const float* x, const float* gate, int ld_gate, fl
                               adp_stream_t stream) {
   ADP_CHECK(x && out && B > 0 && T > 0 && C > 0, "adp_f32_colsum: bad args");
   ADP_CHECK(!gate || ld_gate >= C, "adp_f32_colsum: ld_gate %d < C", ld_gate);
-  ADP_CUDA(launch_k(f32_colsum_kernel, dim3(grid_for(C, 256)), dim3(256), (size_t)0, as_stream(stream), x, gate,
+  ADP_CUDA(launch_k(f32_colsum_kernel, dim3(capped_grid(C, 256)), dim3(256), (size_t)0, as_stream(stream), x, gate,
                     ld_gate, out, B, T, C));
   ADP_LAUNCH_CHECK();
   return 0;
@@ -627,7 +604,7 @@ extern "C" int adp_f32_skip_gate(const float* y, const float* skip, const float*
   (void)groups;
   ADP_CHECK(y && skip && gate && out && B > 0 && T > 0 && C > 0 && ld_gate >= C, "adp_f32_skip_gate: bad args");
   ADP_CHECK(!stats, "adp_f32_skip_gate: statistics are a separate adp_f32_gn_stats pass");
-  ADP_CUDA(launch_k(f32_skip_gate_kernel, dim3(grid_for(static_cast<int64_t>(B) * T * C, 256)), dim3(256),
+  ADP_CUDA(launch_k(f32_skip_gate_kernel, dim3(capped_grid(static_cast<int64_t>(B) * T * C, 256)), dim3(256),
                     (size_t)0, as_stream(stream), y, skip, gate, ld_gate, out, B, T, C));
   ADP_LAUNCH_CHECK();
   return 0;
@@ -637,7 +614,7 @@ extern "C" int adp_f32_skip_gate_bwd(const float* dout, const float* y, const fl
                                      float* dgate, int ld_dgate, int B, int T, int C, adp_stream_t stream) {
   ADP_CHECK(dout && y && gate && dys && dgate && B > 0 && T > 0 && C > 0 && ld_gate >= C && ld_dgate >= C,
             "adp_f32_skip_gate_bwd: bad args");
-  ADP_CUDA(launch_k(f32_skip_gate_bwd_kernel, dim3(grid_for(static_cast<int64_t>(B) * C, 256)), dim3(256),
+  ADP_CUDA(launch_k(f32_skip_gate_bwd_kernel, dim3(capped_grid(static_cast<int64_t>(B) * C, 256)), dim3(256),
                     (size_t)0, as_stream(stream), dout, y, gate, ld_gate, dys, dgate, ld_dgate, B, T, C));
   ADP_LAUNCH_CHECK();
   return 0;
@@ -648,10 +625,10 @@ extern "C" int adp_f32_cond_bwd(const float* dss, int ld_dss, const float* cond,
   ADP_CHECK(dss && cond && w && dw && dbias, "adp_f32_cond_bwd: null");   // dcond may be NULL
   ADP_CHECK(B >= 1 && N >= 1 && K >= 1 && ld_dss >= N, "adp_f32_cond_bwd: B=%d N=%d K=%d", B, N, K);
   cudaStream_t s = as_stream(stream);
-  ADP_CUDA(launch_k(f32_cond_bwd_w_kernel, dim3(grid_for(static_cast<int64_t>(N) * K, 256)), dim3(256), (size_t)0,
+  ADP_CUDA(launch_k(f32_cond_bwd_w_kernel, dim3(capped_grid(static_cast<int64_t>(N) * K, 256)), dim3(256), (size_t)0,
                     s, dss, ld_dss, cond, dw, dbias, B, N, K));
   if (dcond)
-    ADP_CUDA(launch_k(f32_cond_bwd_x_kernel, dim3(grid_for(static_cast<int64_t>(B) * K, 256)), dim3(256),
+    ADP_CUDA(launch_k(f32_cond_bwd_x_kernel, dim3(capped_grid(static_cast<int64_t>(B) * K, 256)), dim3(256),
                       (size_t)0, s, dss, ld_dss, w, dcond, B, N, K));
   ADP_LAUNCH_CHECK();
   return 0;
@@ -671,11 +648,11 @@ extern "C" int adp_f32_stem_out_bwd(const adp_stem_out_bwd_args* args, adp_strea
   cudaStream_t s = as_stream(stream);
   const int cin = a.cx + a.ca;
   const int n_items = a.co * a.c0 * 3 + a.co + a.B * a.co + (a.w_adapt ? a.co * cin + a.co : 0);
-  ADP_CUDA(launch_k(f32_stem_out_bwd_dh_kernel, dim3(grid_for(static_cast<int64_t>(a.B) * (a.T / a.f) * a.c0, 256)),
+  ADP_CUDA(launch_k(f32_stem_out_bwd_dh_kernel, dim3(capped_grid(static_cast<int64_t>(a.B) * (a.T / a.f) * a.c0, 256)),
                     dim3(256), (size_t)0, s, a));
-  ADP_CUDA(launch_k(f32_stem_out_bwd_param_kernel, dim3(grid_for(n_items, 256)), dim3(256), (size_t)0, s, a));
+  ADP_CUDA(launch_k(f32_stem_out_bwd_param_kernel, dim3(capped_grid(n_items, 256)), dim3(256), (size_t)0, s, a));
   if (a.dxin)
-    ADP_CUDA(launch_k(f32_stem_out_bwd_dxin_kernel, dim3(grid_for(static_cast<int64_t>(a.B) * cin * a.T, 256)),
+    ADP_CUDA(launch_k(f32_stem_out_bwd_dxin_kernel, dim3(capped_grid(static_cast<int64_t>(a.B) * cin * a.T, 256)),
                       dim3(256), (size_t)0, s, a));
   ADP_LAUNCH_CHECK();
   return 0;
@@ -691,10 +668,10 @@ extern "C" int adp_f32_stem_in_bwd(const adp_stem_in_bwd_args* args, adp_stream_
   ADP_CHECK(!a.dxin || a.w, "adp_f32_stem_in_bwd: dxin needs the conv weights");
   cudaStream_t s = as_stream(stream);
   const int cin = a.cx + a.ca;
-  ADP_CUDA(launch_k(f32_stem_in_bwd_param_kernel, dim3(grid_for(a.c0 * cin * a.f + a.c0, 256)), dim3(256),
+  ADP_CUDA(launch_k(f32_stem_in_bwd_param_kernel, dim3(capped_grid(a.c0 * cin * a.f + a.c0, 256)), dim3(256),
                     (size_t)0, s, a));
   if (a.dxin)
-    ADP_CUDA(launch_k(f32_stem_in_bwd_dxin_kernel, dim3(grid_for(static_cast<int64_t>(a.B) * cin * a.T, 256)),
+    ADP_CUDA(launch_k(f32_stem_in_bwd_dxin_kernel, dim3(capped_grid(static_cast<int64_t>(a.B) * cin * a.T, 256)),
                       dim3(256), (size_t)0, s, a));
   ADP_LAUNCH_CHECK();
   return 0;
@@ -713,13 +690,13 @@ extern "C" int adp_f32_attention_bwd(const adp_attention_bwd_args* args, int hea
             a.lddv >= w, "adp_f32_attention_bwd: row pitches must be >= heads*head_dim (%d*%d)", a.H, head_dim);
   cudaStream_t s = as_stream(stream);
   const int64_t nq = static_cast<int64_t>(a.B) * a.H * a.Tq, nk = static_cast<int64_t>(a.B) * a.H * a.Tk;
-  ADP_CUDA(launch_k(f32_attention_delta_kernel, dim3(grid_for(nq, 256)), dim3(256), (size_t)0, s, a, head_dim));
+  ADP_CUDA(launch_k(f32_attention_delta_kernel, dim3(capped_grid(nq, 256)), dim3(256), (size_t)0, s, a, head_dim));
   auto dq = head_dim == 32 ? f32_attention_dq_kernel<32>
             : head_dim == 128 ? f32_attention_dq_kernel<128> : f32_attention_dq_kernel<64>;
   auto dkdv = head_dim == 32 ? f32_attention_dkdv_kernel<32>
               : head_dim == 128 ? f32_attention_dkdv_kernel<128> : f32_attention_dkdv_kernel<64>;
-  ADP_CUDA(launch_k(dq, dim3(grid_for(nq, 128)), dim3(128), (size_t)0, s, a));
-  ADP_CUDA(launch_k(dkdv, dim3(grid_for(nk, 128)), dim3(128), (size_t)0, s, a));
+  ADP_CUDA(launch_k(dq, dim3(capped_grid(nq, 128)), dim3(128), (size_t)0, s, a));
+  ADP_CUDA(launch_k(dkdv, dim3(capped_grid(nk, 128)), dim3(128), (size_t)0, s, a));
   ADP_LAUNCH_CHECK();
   return 0;
 }

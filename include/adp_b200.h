@@ -146,9 +146,14 @@ int adp_time_features(const float* sigma, const float* freqs, float* out, int32_
  * VDiffusion-noised input x_noisy = alpha_b*x + beta_b*noise (reference diffusion.py:91).
  * Emits the GroupNorm statistics of its output.
  * Limits of the stem entry points (adp_stem_in / _out / _in_bwd / _out_bwd; their adp_f32_ twins take
- * at least the same sizes): cx+ca <= 64, (cx+ca)*f <= 128, c0 <= 256 and a multiple of 8, co <= 64 and co <= cx; sizes the
- * narrow kernels take ((cx+ca)*f <= 32, co <= 4, cx+ca <= 8; backward c0 <= 64) run on them, the rest
- * of the envelope on the wide kernels.  Out-of-envelope sizes are refused before any launch. */
+ * at least the same sizes): cx+ca <= 64, (cx+ca)*f <= 128, T a multiple of f, c0 <= 256 and a
+ * multiple of 8, co <= 64 and co <= cx.  Out-of-envelope sizes are refused before any launch.
+ * Inside the envelope, sizes the narrow kernels take run on them and the rest on the wide kernels:
+ *   adp_stem_in       (cx+ca)*f <= 32
+ *   adp_stem_out      co <= 4 and cx+ca <= 8
+ *   adp_stem_out_bwd  co <= 4, cx+ca <= 8, c0 <= 64, f dividing 256 and
+ *                     co*c0*3 + 3*co + co*(cx+ca) <= 1024 parameter gradients
+ *   adp_stem_in_bwd   (cx+ca)*f <= 32 and c0 <= 64 */
 typedef struct adp_stem_in_args {
   const float* x;       /* fp32 [B][cx][T]                          */
   const float* append;  /* fp32 [B][ca][T] or NULL                  */
@@ -170,7 +175,7 @@ int adp_stem_in(const adp_stem_in_args* args, adp_stream_t stream);
  *     h holds 2B rows: conditional then masked),
  *   - the VSampler update (reference diffusion.py:185-187) writing x_next,
  *   - the VDiffusion loss partial sums of (v - (alpha*noise - beta*x))^2 (diffusion.py:92-95)
- *     and d(loss)/dv. */
+ *     and d(loss)/dv (not together with x_next). */
 typedef struct adp_stem_out_args {
   const void* h;        /* bf16 [Bh][T/f][c0], Bh = B (or 2B with cfg) */
   const float* x;       /* fp32 [B][cx][T]   (block input, the skip) */

@@ -216,7 +216,7 @@ def test_narrow_conv_backward_groups(ops, groups):
     _narrow_conv_backward(ops, groups)
 
 
-@pytest.mark.parametrize("cx,ca,co,c0,f", [(2, 0, 2, 8, 1), (2, 2, 2, 8, 1), (1, 1, 1, 32, 4)])
+@pytest.mark.parametrize("cx,ca,co,c0,f", [(2, 0, 2, 8, 1), (2, 2, 2, 8, 1), (1, 1, 1, 32, 4), (4, 4, 4, 8, 1)])
 def test_stem_backward(ops, cx, ca, co, c0, f):
     B, T = 2, 1024
     cin = cx + ca
