@@ -24,7 +24,9 @@
 namespace adp {
 
 // diagnostic switches (adp_debug_set): [2] 1 = weights are not written by the preceding kernels
-// (fetch them before griddepcontrol.wait); [3] CTAs/SM override; [5] KC override; [6] PDL
+// (fetch them before griddepcontrol.wait); [3] CTAs/SM override; [5] KC override; [6] PDL;
+// [7] 1 = every BN <= 64 tile without the A transform takes the narrow-statistics variant,
+// whether or not its groups need it (compares that variant with the unserialized one)
 int g_debug[8] = {0, 0, 0, 0, 0, 0, 0, 0};
 
 constexpr int kBM = 128;
@@ -155,10 +157,15 @@ struct NarrowStats {
   }
 };
 
-template <int BN, int SW, bool XF>
+// NARROW: per-lane statistics registers (NarrowStats) for power-of-two groups narrower than 8
+// channels.  They fit only in BN <= 64 tiles without the A transform, and only launches whose
+// groups need them take this variant: ptxas serializes its wgmma instructions (C7520), which
+// the variant without them does not.
+template <int BN, int SW, bool XF, bool NARROW>
 __global__ void __launch_bounds__(kGemmThreads, BN <= 32 ? 3 : (BN <= 64 ? 2 : 1))
 conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
                   const Gemm2Params p) {
+  static_assert(!NARROW || (BN <= 64 && !XF), "narrow statistics registers: BN <= 64 without XF");
   constexpr int BK = SW / 2;
   constexpr int NACC = BN / 2;                    // accumulator registers per consumer thread
   constexpr uint32_t kWTapBytes = BN * SW;        // bytes one W box writes
@@ -250,10 +257,9 @@ conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // fragment rows r0 and r0 + 8
   const int cq = 2 * (lane & 3);               // fragment column offset inside each 8-column block
   const bool do_stats = p.stats != nullptr;
-  // narrow power-of-two groups keep per-lane registers only where they fit without spills
-  // (BN <= 64, no A-operand transform); other tiles take the per-block path of other group sizes
-  constexpr bool kNarrowRegs = BN <= 64 && !XF;
-  const bool narrow = kNarrowRegs && p.group_shift >= 0 && p.group_shift < 3;
+  // narrow power-of-two groups keep per-lane registers in the NARROW variant; other tiles take
+  // the per-block path of other group sizes
+  const bool narrow = NARROW && p.group_shift >= 0 && p.group_shift < 3;
   WarpStats acc_st;
   NarrowStats nar_st;
   int cur_b = -1, coef_b = -1;
@@ -457,10 +463,10 @@ conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (do_stats && cur_b >= 0) publish_stats(cur_b);
 }
 
-template <int BN, int SW, bool XF>
+template <int BN, int SW, bool XF, bool NARROW>
 static int launch_gemm2(const adp_conv_gemm_args& a, cudaStream_t stream) {
   constexpr int BK = SW / 2;
-  auto kernel = conv_gemm2_kernel<BN, SW, XF>;
+  auto kernel = conv_gemm2_kernel<BN, SW, XF, NARROW>;
   const int tiles_per_batch = (a.T + kBM - 1) / kBM;
   const bool up = a.up_factor > 1;
   const int max_taps = up ? 2 : a.ntaps;
@@ -578,19 +584,22 @@ template <int SW>
 static int dispatch_bn2(const adp_conv_gemm_args& a, int bn, cudaStream_t s) {
   if (a.gn_stats) {
     switch (bn) {
-      case 16: return launch_gemm2<16, SW, true>(a, s);
-      case 32: return launch_gemm2<32, SW, true>(a, s);
-      case 64: return launch_gemm2<64, SW, true>(a, s);
-      case 128: return launch_gemm2<128, SW, true>(a, s);
-      case 256: return launch_gemm2<256, SW, true>(a, s);
+      case 16: return launch_gemm2<16, SW, true, false>(a, s);
+      case 32: return launch_gemm2<32, SW, true, false>(a, s);
+      case 64: return launch_gemm2<64, SW, true, false>(a, s);
+      case 128: return launch_gemm2<128, SW, true, false>(a, s);
+      case 256: return launch_gemm2<256, SW, true, false>(a, s);
     }
   }
+  // GroupNorm groups of 1, 2 or 4 channels need the per-lane statistics registers
+  const int group_size = a.stats ? a.n_valid / a.groups : 0;
+  const bool narrow = group_size == 1 || group_size == 2 || group_size == 4 || g_debug[7] != 0;
   switch (bn) {
-    case 16: return launch_gemm2<16, SW, false>(a, s);
-    case 32: return launch_gemm2<32, SW, false>(a, s);
-    case 64: return launch_gemm2<64, SW, false>(a, s);
-    case 128: return launch_gemm2<128, SW, false>(a, s);
-    case 256: return launch_gemm2<256, SW, false>(a, s);
+    case 16: return narrow ? launch_gemm2<16, SW, false, true>(a, s) : launch_gemm2<16, SW, false, false>(a, s);
+    case 32: return narrow ? launch_gemm2<32, SW, false, true>(a, s) : launch_gemm2<32, SW, false, false>(a, s);
+    case 64: return narrow ? launch_gemm2<64, SW, false, true>(a, s) : launch_gemm2<64, SW, false, false>(a, s);
+    case 128: return launch_gemm2<128, SW, false, false>(a, s);
+    case 256: return launch_gemm2<256, SW, false, false>(a, s);
   }
   return set_error("adp_conv_gemm: unsupported N tile %d", bn);
 }
@@ -651,13 +660,19 @@ extern "C" int adp_conv_gemm(const adp_conv_gemm_args* args, adp_stream_t stream
               "adp_conv_gemm: groups=%d n_valid=%d (fused statistics handle <= %d groups)",
               a.groups, a.n_valid, kMaxGroups);
   }
-  // N tile: persistent CTAs take care of SM fill; prefer 128 (W traffic dominates either way
-  // and two accumulator buffers of 128 columns leave room for 2 CTAs/SM on short-K shapes)
+  // N tile: persistent CTAs take care of SM fill.  Tiles with a long reduction (taps * c_in >
+  // 1024) prefer 128 columns: each A box then feeds twice the MMAs.  Shorter ones prefer 64,
+  // which gives the persistent grid twice the tiles and more CTAs per SM where the ring allows
+  // (measured in isolation on H100, cfg2 shapes: the L3 / L4 convs run 18-27 % and the q|k|v
+  // projections of L5-L8 2-10 % faster at 64 than at 128; the k=3 convs with c_in >= 512 run
+  // 4-8 % slower at 64).  The XF tiles keep 128 (not measured at 64).
   int bn = a.block_n;
   if (bn == 0) {
     const long m_tiles = (long)a.B * ((a.T + kBM - 1) / kBM);
+    const int k_per_tile = (a.up_factor > 1 ? 2 : a.ntaps) * a.c_in;
+    const int widest = !a.gn_stats && k_per_tile <= 1024 ? 64 : 128;
     bn = 16;
-    for (int cand = 128; cand >= 16; cand >>= 1) {
+    for (int cand = widest; cand >= 16; cand >>= 1) {
       if (a.n_pad % cand) continue;
       const long tiles = m_tiles * (a.phases * a.n_pad / cand);
       if (tiles >= 96 || cand <= 64) { bn = cand; break; }
