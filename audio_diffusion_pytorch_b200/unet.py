@@ -18,6 +18,7 @@ from typing import Callable, Dict, List, Optional, Sequence, Tuple
 import torch
 import torch.nn.functional as F
 from torch import Tensor, nn
+from torch.optim.optimizer import register_optimizer_step_post_hook
 
 from . import _lib, ops
 
@@ -575,7 +576,12 @@ class B200UNet(nn.Module):
             dst.copy_(src)
 
     def _version(self) -> int:
-        return sum(p._version for p in self.parameters())
+        """Moves whenever a parameter may have changed in place: the tensors' version counters, plus
+        the number of optimizer steps taken in the process.  Fused optimizers (`fused=True`) update
+        the parameters through one multi-tensor kernel that bumps no version counter; without the
+        second term the packs, and with them the whole forward and backward, stayed at the weights
+        from before the step."""
+        return sum(p._version for p in self.parameters()) + _OPTIMIZER_STEPS[0]
 
     def _storage_signature(self):
         return tuple((p.data_ptr(), p.dtype) for p in self.parameters())
@@ -1228,6 +1234,17 @@ def _arv_loop(self, current: Tensor, sigmas: Tensor, progress=None, **kwargs) ->
 
 
 B200UNet.arv_loop = torch.no_grad()(_arv_loop)
+
+
+_OPTIMIZER_STEPS = [0]
+
+
+def _count_optimizer_step(optimizer, args, kwargs) -> None:
+    _OPTIMIZER_STEPS[0] += 1
+
+
+# every torch.optim step in the process: a step of an unrelated optimizer costs one in-place re-pack
+register_optimizer_step_post_hook(_count_optimizer_step)
 
 
 def _copy_tree(dst, src) -> None:

@@ -21,13 +21,24 @@ values: conv of |a| with |w|, P |V|, ...):
                    variance (GroupNorm normalises by sqrt(var + 1e-5); the plain relative error
                    of the variance is recorded as `.var_rel`, unbounded: a single-pass variance
                    of a near-constant group, var << mean^2, keeps only a few digits)
+    accumulators   (Acc: fp32 parameter / conditioning gradients, fp64 sums) the launch's own
+                   contribution, after - before, against the fp64 sum of its terms:
+                   fp32  err <= 1e-5 |ref| + 2^-14 absref + 2^-23 (|before| + |after|)
+                   fp64  err <= 1e-4 absref      (GroupNorm backward sums, the loss sum)
+                   absref = the same sum over absolute terms; the GroupNorm backward sums are taken
+                   over dxh as stored, as statistics are over the stored output
+    attention lse  the fp32 bound + 2^-9 (LSE_FLOOR: the row sum is taken over P rounded to bf16)
     copies         bitwise
 Every launch also checks that read-only arguments are bitwise unchanged and that no byte of a
-written tensor's storage outside the written view changed.
+written tensor's storage outside the written view changed -- the rest of the gradient arena
+included, every accumulator being a view of that one storage.
 
-Checked kinds are the launches of the inference and sampling programs; the training backward
-and the vocoder / sampler front-end launches are listed in UNCHECKED, and a program that reaches
-one of them under Shadow fails instead of passing unchecked.
+Checked kinds are the launches of the inference, sampling and training programs (forward, fused
+loss and backward; tau = 2^-8 also for attention_bwd, which rounds P and dS to bf16) and
+fir_resample, whose output is the tensor it returns.  The vocoder front-end (to_flat, to_flat_bwd,
+mel_spectrogram) and the inpainting / autoregressive sampler steps (inpaint_blend, arv_step) are
+listed in UNCHECKED, and a program that reaches one of them under Shadow fails instead of passing
+unchecked.
 """
 import inspect
 import math
@@ -45,21 +56,18 @@ FP32_REL, FP32_TAU = 1e-5, 2.0 ** -14
 STATS_TOL = 1e-4
 VAR_TOL = 1e-3
 GN_EPS = 1e-5                    # every statistics slot feeds a GroupNorm: it divides by sqrt(var + eps)
+# attention's lse is log of the row sum of P AS ROUNDED TO bf16 for the P V GEMM (the sum that
+# normalises o): every term carries a relative rounding of up to 2^-9, so does the sum, and its log
+# moves by up to 2^-9 in absolute terms.  attention_bwd rounds the P it recomputes from lse to bf16 too.
+LSE_FLOOR = 2.0 ** -9
+ACC_EPS = 2.0 ** -23              # an fp32 accumulator's own rounding, per unit of |before| + |after|
+SIDE_CHUNK = 1 << 28              # bytes compared at a time by the side-effect check
 ROW_TILE = 64                    # rows left stale by the mutation: half the conv GEMM's 128-row M tile
 
 UNCHECKED = {
-    # training backward (training.py's plans)
-    "wgrad": "training backward", "gn_silu_bwd": "training backward",
-    "gn_bwd_apply": "training backward", "ln_film_bwd": "training backward",
-    "colsum": "training backward", "skip_gate_bwd": "training backward",
-    "cond_bwd": "training backward", "narrow_conv_bwd": "training backward",
-    "stem_out_bwd": "training backward", "stem_in_bwd": "training backward",
-    "attention_bwd": "training backward", "ln_fold_bwd": "training backward",
-    "to_flat_bwd": "training backward",
-    # inference launches outside the sampling programs of UNetV0
-    "skip_gate": "keep=True plans and use_modulation=False nets only",
-    "fir_resample": "vocoder / upsampler front-end", "mel_spectrogram": "vocoder front-end",
-    "to_flat": "vocoder front-end", "inpaint_blend": "VInpainter loop", "arv_step": "ARVSampler loop",
+    # the vocoder front-end (cfg5) and the two sampler loops outside VSampler
+    "to_flat": "vocoder front-end", "to_flat_bwd": "vocoder front-end (training)",
+    "mel_spectrogram": "vocoder front-end", "inpaint_blend": "VInpainter loop", "arv_step": "ARVSampler loop",
 }
 
 
@@ -81,9 +89,9 @@ class Val:
     """A stored output: `view(args)` is the written view; ref / absref fp64 of its shape (or a
     callable(post args) -> (ref, absref) when the reference reads another output of the launch)."""
 
-    def __init__(self, name, view, ref, absref=None, tau=TAU_FP32_ACC, exact=False):
+    def __init__(self, name, view, ref, absref=None, tau=TAU_FP32_ACC, exact=False, floor=0.0):
         self.name, self.view, self.ref, self.absref, self.tau, self.exact = name, view, ref, absref, tau, exact
-        self.acc = False
+        self.acc, self.floor = False, floor      # floor: an absolute term of the bound (see LSE_FLOOR)
 
 
 class Stat:
@@ -94,8 +102,23 @@ class Stat:
         self.acc = True
 
 
+class Acc:
+    """An accumulator the launch adds to (+=): fp32 parameter / conditioning gradients, or fp64 sums.
+    Checked as after - before against ref, the launch's own contribution (fp64; absref = the same sum
+    over absolute terms), or a callable(post args) -> (ref, absref) when the contribution is defined
+    on another output of the launch as stored (the GroupNorm backward sums of the rounded dxh)."""
+
+    def __init__(self, name, view, ref, absref=None):
+        self.name, self.view, self.ref, self.absref = name, view, ref, absref
+        self.acc, self.exact = True, False
+
+
 def arg(name):
     return lambda a: a[name]
+
+
+def cols(name, n):
+    return lambda a: a[name][..., :n]
 
 
 def stats_of(y: torch.Tensor, groups: int) -> torch.Tensor:
@@ -255,7 +278,7 @@ def c_attention(a, ctx):
             lse_abs[b] = S.abs().amax(-1)
     outs = [Val("o", lambda p: p["o"][..., :mid], ref, absr, TAU_BF16_OPERAND)]
     if lse is not None:
-        outs.append(Val("lse", arg("lse"), lse, lse_abs))
+        outs.append(Val("lse", arg("lse"), lse, lse_abs, floor=LSE_FLOOR))
     return outs
 
 
@@ -317,8 +340,6 @@ def c_stem_in(a, ctx):
 
 
 def c_stem_out(a, ctx):
-    if a["loss_sum"] is not None or a["dv"] is not None:
-        raise NotImplementedError("stem_out's training loss outputs are not checked here")
     h, f = a["h"], a["f"]
     xin = _stem_input(a)
     B, _, T = xin.shape
@@ -360,6 +381,16 @@ def c_stem_out(a, ctx):
         xn = a1 * (a0 * xs - b0 * v) + b1 * (b0 * xs + a0 * v)
         xna = (abs(a1 * a0) + abs(b1 * b0)) * xs.abs() + (abs(a1 * b0) + abs(b1 * a0)) * vabs
         outs.append(Val("x_next", arg("x_next"), xn, xna))
+    if a["loss_sum"] is not None:      # VDiffusion: sum (v - (alpha noise - beta x))^2, dv = 2 (v - target) / numel
+        al, be = a["alpha"].to(F64)[:, None, None], a["beta"].to(F64)[:, None, None]
+        nz, x0 = a["noise"].to(F64), a["x"].to(F64)
+        d = v - (al * nz - be * x0)
+        dabs = vabs + (al * nz).abs() + (be * x0).abs()
+        # an error e of v within its fp32 bound moves d^2 by 2 |d| e: carried at the same weight
+        outs.append(Acc("loss_sum", arg("loss_sum"), (d * d).sum().reshape(1),
+                        ((d * d).sum() + (FP32_TAU / STATS_TOL) * (2 * d.abs() * dabs).sum()).reshape(1)))
+        if a["dv"] is not None:
+            outs.append(Val("dv", arg("dv"), 2 * d / d.numel(), 2 * dabs / d.numel()))
     return outs
 
 
@@ -416,6 +447,301 @@ def c_step_advance(a, ctx):
     return [Val("step", arg("step"), a["step"] + 1, exact=True)]
 
 
+# ------------------------------------------------------------- training launch kinds
+def _shift(t, off):
+    """t[:, i] <- t[:, i + off] along dim 1, zeros outside."""
+    if off == 0:
+        return t
+    z = t.new_zeros(t.shape[0], abs(off), *t.shape[2:])
+    return torch.cat([t[:, off:], z], 1) if off > 0 else torch.cat([z, t[:, :off]], 1)
+
+
+def _gn_xhat(x, stats, groups, eps):
+    """(xhat, rstd [B, 1, C]) of GroupNorm from the statistics slots (arithmetic of _gn_coef)."""
+    B, T, C = x.shape
+    one = torch.ones(C, dtype=F64, device=x.device)
+    sc, sh = _gn_coef(stats, one, torch.zeros_like(one), groups, eps, T, C)     # rstd, -mean rstd
+    return x.to(F64) * sc + sh, sc
+
+
+def _dsilu(z):
+    sg = torch.sigmoid(z)
+    return sg * (1 + z * (1 - sg))
+
+
+DSILU_MAX = 1.1                  # max |SiLU'|
+
+
+def _group_sums(t, groups):
+    B, T, C = t.shape
+    return t.reshape(B, T, groups, C // groups).sum(dim=(1, 3))
+
+
+def _gn_S(xh, groups):
+    """The GroupNorm backward sums S[b, g] = (sum dxh, sum dxh xhat) of dxh AS STORED."""
+    def ref(p):
+        d = p["dxh"].to(F64)
+        return (torch.stack([_group_sums(d, groups), _group_sums(d * xh, groups)], -1),
+                torch.stack([_group_sums(d.abs(), groups), _group_sums((d * xh).abs(), groups)], -1))
+    return ref
+
+
+def c_wgrad(a, ctx):
+    g, x, n, k = a["g"], a["x"], a["n"], a["k"]
+    assert g.dtype == torch.bfloat16, "the fp32 verification mode is not checked here"
+    G = g[..., a["g_col0"]:a["g_col0"] + n].to(F64).reshape(-1, n)
+    X = x[..., a["x_col0"]:a["x_col0"] + k].to(F64)
+    taps = 3 if a["ntaps"] == 3 else 1
+    ref = [G.t() @ _shift(X, a["off"] + j).reshape(-1, k) for j in range(taps)]
+    absr = [G.abs().t() @ _shift(X.abs(), a["off"] + j).reshape(-1, k) for j in range(taps)]
+    if taps == 3:
+        return [Acc("dw", lambda p: p["dw"][:, :n, :k], torch.stack(ref), torch.stack(absr))]
+    return [Acc("dw", lambda p: p["dw"][:n, :k], ref[0], absr[0])]
+
+
+def c_gn_silu_bwd(a, ctx):
+    x, G = a["x"], a["groups"]
+    xh, _ = _gn_xhat(x, a["stats"], G, a["eps"])
+    ga, da = a["gamma"].to(F64), a["da"].to(F64)
+    dz = da * _dsilu(xh * ga + a["beta"].to(F64))
+    return [Val("dxh", arg("dxh"), dz * ga, DSILU_MAX * (da * ga).abs()),
+            Acc("dgamma", arg("dgamma"), (dz * xh).sum((0, 1)), (dz * xh).abs().sum((0, 1))),
+            Acc("dbeta", arg("dbeta"), dz.sum((0, 1)), dz.abs().sum((0, 1))),
+            Acc("S", arg("S"), _gn_S(xh, G))]
+
+
+def c_gn_bwd_apply(a, ctx):
+    x, G = a["x"], a["groups"]
+    B, T, C = x.shape
+    xh, rstd = _gn_xhat(x, a["stats"], G, a["eps"])
+    c = (a["S"].to(F64) / float(T * (C // G))).repeat_interleave(C // G, dim=1)[:, None]     # [B, 1, C, 2]
+    d = a["dxh"].to(F64)
+    ref = rstd * (d - c[..., 0] - xh * c[..., 1])
+    absr = rstd.abs() * (d.abs() + c[..., 0].abs() + (xh * c[..., 1]).abs())
+    if a["dres"] is not None:
+        ref, absr = ref + a["dres"].to(F64), absr + a["dres"].to(F64).abs()
+    outs = [Val("dx", arg("dx"), ref, absr)]
+    if a["colsum"] is not None:        # the kernel sums the values before they are rounded to bf16
+        outs.append(Acc("colsum", cols("colsum", C), ref.sum((0, 1)), absr.sum((0, 1))))
+    return outs
+
+
+def c_ln_film_bwd(a, ctx):
+    x = a["x"]
+    B, T, C = x.shape
+    xh, std, _ = _layer_norm(x.to(F64), a["eps"])
+    dy = a["dy"].to(F64)
+    f = 1 + a["scale_shift"].to(F64)[:, None, :C] if a["scale_shift"] is not None else 1.0
+    g = dy * f
+    m1, m2 = g.mean(-1, keepdim=True), (g * xh).mean(-1, keepdim=True)
+    ref = (g - m1 - xh * m2) / std
+    absr = (g.abs() + g.abs().mean(-1, keepdim=True) + xh.abs() * (g * xh).abs().mean(-1, keepdim=True)) / std
+    if a["dres"] is not None:
+        ref, absr = ref + a["dres"].to(F64), absr + a["dres"].to(F64).abs()
+    outs = [Val("dx", arg("dx"), ref, absr)]
+    if a["dss"] is not None:
+        outs.append(Acc("dss", cols("dss", 2 * C), torch.cat([(dy * xh).sum(1), dy.sum(1)], -1),
+                        torch.cat([(dy * xh).abs().sum(1), dy.abs().sum(1)], -1)))
+    if a["colsum"] is not None:
+        outs.append(Acc("colsum", cols("colsum", C), ref.sum((0, 1)), absr.sum((0, 1))))
+    return outs
+
+
+def c_colsum(a, ctx):
+    x = a["x"].to(F64)
+    C = x.shape[-1]
+    if a["gate"] is not None:
+        x = x * a["gate"].to(F64)[:, None, :C]
+    return [Acc("out", cols("out", C), x.sum((0, 1)), x.abs().sum((0, 1)))]
+
+
+def c_skip_gate(a, ctx):
+    y, skip = a["y"].to(F64), a["skip"].to(F64)
+    gy = a["gate"].to(F64)[:, None, :y.shape[-1]] * y
+    outs = [Val("out", arg("out"), skip + gy, skip.abs() + gy.abs())]
+    if a["stats"] is not None:
+        outs.append(Stat("stats", arg("stats"), arg("out"), a["groups"]))
+    return outs
+
+
+def c_skip_gate_bwd(a, ctx):
+    d, y = a["dout"].to(F64), a["y"].to(F64)
+    C = y.shape[-1]
+    ref = a["gate"].to(F64)[:, None, :C] * d
+    return [Val("dys", arg("dys"), ref, ref.abs()),
+            Acc("dgate", cols("dgate", C), (d * y).sum(1), (d * y).abs().sum(1))]
+
+
+def c_cond_bwd(a, ctx):
+    N = a["N"]
+    d, c, W = a["dss"][:, :N].to(F64), a["cond"].to(F64), a["w"][:N].to(F64)
+    outs = [Val("dw", lambda p: p["dw"][:N], d.t() @ c, d.abs().t() @ c.abs()),
+            Val("dbias", lambda p: p["dbias"][:N], d.sum(0), d.abs().sum(0))]
+    if a["dcond"] is not None:
+        outs.append(Acc("dcond", arg("dcond"), d @ W, d.abs() @ W.abs()))
+    return outs
+
+
+def _conv3_t(dy, w3):
+    """Transpose of _conv3 over [B, T, Co]: da[t] = sum_k dy[t - (k - 1)] @ w3[k]  (w3 [3, Co, Ci])."""
+    return sum(_shift(dy, 1 - k) @ w3[k] for k in range(3))
+
+
+def c_narrow_conv_bwd(a, ctx):
+    x, G = a["x"], a["groups"]
+    xh, _ = _gn_xhat(x, a["stats_in"], G, a["gn_eps"])
+    ga = a["gamma"].to(F64)
+    z = xh * ga + a["beta"].to(F64)
+    act, dy = _silu(z), a["dy"].to(F64)
+    w3 = a["w"].to(F64).permute(2, 0, 1)                        # [3, co, ci]
+    da, da_abs = _conv3_t(dy, w3), _conv3_t(dy.abs(), w3.abs())
+    dz = da * _dsilu(z)
+    C = x.shape[-1]
+    dw = torch.stack([dy.reshape(-1, C).t() @ _shift(act, k - 1).reshape(-1, C) for k in range(3)], -1)
+    dwa = torch.stack([dy.abs().reshape(-1, C).t() @ _shift(act.abs(), k - 1).reshape(-1, C) for k in range(3)], -1)
+    # the sums of dz inherit the error of da (fp32 dot products of 3 C terms): its absref, not |dz|
+    dza = DSILU_MAX * da_abs
+    return [Val("dxh", arg("dxh"), dz * ga, dza * ga.abs()),
+            Acc("dgamma", arg("dgamma"), (dz * xh).sum((0, 1)), (dza * xh.abs()).sum((0, 1))),
+            Acc("dbeta", arg("dbeta"), dz.sum((0, 1)), dza.sum((0, 1))),
+            Acc("S", arg("S"), _gn_S(xh, G)),
+            Acc("dw", arg("dw"), dw, dwa),
+            Acc("dbias", arg("dbias"), dy.sum((0, 1)), dy.abs().sum((0, 1)))]
+
+
+def c_stem_out_bwd(a, ctx):
+    h, f = a["h"], a["f"]
+    B, Tl, c0 = h.shape
+    w = a["w"].to(F64)
+    co = w.shape[0]
+    w3 = w.permute(2, 0, 1)                                     # [3, co, c0]
+    gs = a["gscale"].to(F64)[0] if a["gscale"] is not None else 1.0
+    dvs = (a["dv"].to(F64) * gs).transpose(1, 2)                # [B, T, co]
+    gate = a["gate"].to(F64)[:, None, :co]
+    dy = dvs * gate
+    up = h.to(F64).repeat_interleave(f, dim=1)                  # nearest upsampling [B, T, c0]
+    dup, dupa = _conv3_t(dy, w3), _conv3_t(dy.abs(), w3.abs())
+    bias = a["bias"].to(F64) if a["bias"] is not None else None
+    y = torch.stack([_conv3(up[b], w3, bias) for b in range(B)])
+    ya = torch.stack([_conv3(up[b].abs(), w3.abs(), None if bias is None else bias.abs()) for b in range(B)])
+    T = up.shape[1]
+    dw = torch.stack([dy.reshape(-1, co).t() @ _shift(up, k - 1).reshape(-1, c0) for k in range(3)], -1)
+    dwa = torch.stack([dy.abs().reshape(-1, co).t() @ _shift(up.abs(), k - 1).reshape(-1, c0) for k in range(3)], -1)
+    outs = [Val("dh", arg("dh"), dup.reshape(B, Tl, f, c0).sum(2), dupa.reshape(B, Tl, f, c0).sum(2)),
+            Acc("dw", arg("dw"), dw, dwa),
+            Acc("dbias", cols("dbias", co), dy.sum((0, 1)), dy.abs().sum((0, 1))),
+            Acc("dgate", cols("dgate", co), (dvs * y).sum(1), (dvs.abs() * ya).sum(1))]
+    xin = None
+    if a["w_adapt"] is not None:
+        xin = _stem_input(a).transpose(1, 2)                    # [B, T, cin]
+        cin = xin.shape[-1]
+        outs += [Acc("dw_adapt", arg("dw_adapt"), dvs.reshape(-1, co).t() @ xin.reshape(-1, cin),
+                     dvs.abs().reshape(-1, co).t() @ xin.abs().reshape(-1, cin)),
+                 Acc("db_adapt", arg("db_adapt"), dvs.sum((0, 1)), dvs.abs().sum((0, 1)))]
+    if a["dxin"] is not None:          # through the skip path only, stored
+        cin = a["dxin"].shape[1]
+        if a["w_adapt"] is not None:
+            wa = a["w_adapt"].to(F64)
+            ref, absr = dvs @ wa, dvs.abs() @ wa.abs()
+        else:
+            ref = torch.cat([dvs, dvs.new_zeros(B, T, cin - co)], -1)
+            absr = ref.abs()
+        outs.append(Val("dxin", arg("dxin"), ref.transpose(1, 2), absr.transpose(1, 2)))
+    return outs
+
+
+def c_stem_in_bwd(a, ctx):
+    f = a["f"]
+    xin, d = _stem_input(a), a["dout"].to(F64)
+    B, cin, T = xin.shape
+    c0 = d.shape[-1]
+    xr = xin.reshape(B, cin, T // f, f).permute(0, 2, 1, 3).reshape(-1, cin * f)
+    d2 = d.reshape(-1, c0)
+    outs = [Acc("dw", arg("dw"), (d2.t() @ xr).reshape(c0, cin, f), (d2.abs().t() @ xr.abs()).reshape(c0, cin, f)),
+            Acc("dbias", arg("dbias"), d2.sum(0), d2.abs().sum(0))]
+    if a["dxin"] is not None:
+        Wm = a["w"].to(F64).reshape(c0, cin * f)
+
+        def back(t):
+            return t.reshape(B, T // f, cin, f).permute(0, 2, 1, 3).reshape(B, cin, T)
+        outs.append(Acc("dxin", arg("dxin"), back(d2 @ Wm), back(d2.abs() @ Wm.abs())))
+    return outs
+
+
+def c_attention_bwd(a, ctx):
+    q, k, v = a["q"], a["k"], a["v"]
+    H, D, scale = a["heads"], a["head_dim"], a["scale"]
+    B, Tq, Tk, mid = q.shape[0], q.shape[1], k.shape[1], H * D
+    dev = q.device
+    r = {n: torch.empty(B, t, mid, dtype=F64, device=dev) for n, t in
+         (("dq", Tq), ("dk", Tk), ("dv", Tk), ("dqa", Tq), ("dka", Tk), ("dva", Tk))}
+    delta = torch.empty(B, H, Tq, dtype=F64, device=dev)
+    delta_abs = torch.empty_like(delta)
+
+    def heads(t, b, n):
+        return t[b, :, :mid].to(F64).reshape(n, H, D).transpose(0, 1)
+
+    def rows(t, n):
+        return t.transpose(0, 1).reshape(n, mid)
+    for b in range(B):
+        Q, K, V = heads(q, b, Tq), heads(k, b, Tk), heads(v, b, Tk)
+        O, dO = heads(a["o"], b, Tq), heads(a["d_o"], b, Tq)
+        P = torch.exp((Q @ K.transpose(1, 2)) * scale - a["lse"][b].to(F64)[..., None])
+        dl, dla = (dO * O).sum(-1), (dO * O).abs().sum(-1)
+        dS = P * (dO @ V.transpose(1, 2) - dl[..., None])
+        dSa = P * (dO.abs() @ V.abs().transpose(1, 2) + dla[..., None])
+        delta[b], delta_abs[b] = dl, dla
+        r["dv"][b], r["dva"][b] = rows(P.transpose(1, 2) @ dO, Tk), rows(P.transpose(1, 2) @ dO.abs(), Tk)
+        r["dq"][b], r["dqa"][b] = rows(dS @ K * scale, Tq), rows(dSa @ K.abs() * scale, Tq)
+        r["dk"][b], r["dka"][b] = rows(dS.transpose(1, 2) @ Q * scale, Tk), rows(dSa.transpose(1, 2) @ Q.abs() * scale, Tk)
+    # P and dS are rounded to bf16 for the second GEMMs
+    def delta_view(p):       # a flat workspace sized for the largest item: this launch's rows come first
+        return p["delta"].reshape(-1)[:B * H * Tq].view(B, H, Tq)
+    return [Val("delta", delta_view, delta, delta_abs),
+            Val("dq", cols("dq", mid), r["dq"], r["dqa"], TAU_BF16_OPERAND),
+            Val("dk", cols("dk", mid), r["dk"], r["dka"], TAU_BF16_OPERAND),
+            Val("dv", cols("dv", mid), r["dv"], r["dva"], TAU_BF16_OPERAND)]
+
+
+def c_ln_fold_bwd(a, ctx):
+    W, g, b = a["w"].to(F64), a["g"].to(F64), a["b"].to(F64)
+    N, C = W.shape
+    dwf, dbf = a["dwf"][:N, :C].to(F64), a["dbf"][:N].to(F64)
+    return [Val("dw", arg("dw"), dwf * g + dbf[:, None] * b, (dwf * g).abs() + (dbf[:, None] * b).abs()),
+            Acc("dg", arg("dg"), (dwf * W).sum(0), (dwf * W).abs().sum(0)),
+            Acc("db", arg("db"), W.t() @ dbf, W.abs().t() @ dbf.abs())]
+
+
+def _fir_result(a):
+    """The tensor fir_resample allocates and returns."""
+    n = a["t_out"] if a["adjoint_of"] is None else a["adjoint_of"]
+    return torch.empty(a["x"].shape[0], n, dtype=torch.float32, device=a["x"].device)
+
+
+def c_fir_resample(a, ctx):
+    """y[r, i fo + p] = sum_k xpad[r, i fi + k] bank[p, k], xpad[j] = x[j - half]; or its transpose."""
+    x, bank = a["x"].to(F64), a["bank"].to(F64)
+    fi, fo, half, t_out = a["factor_in"], a["factor_out"], a["half"], a["t_out"]
+    taps = bank.shape[1]
+    rows = x.shape[0]
+    frames = -(-t_out // fo)
+    span = (frames - 1) * fi + taps
+
+    def forward(xs, bk):
+        t = xs.shape[1]
+        xp = torch.cat([xs.new_zeros(rows, half), xs, xs.new_zeros(rows, max(0, span - half - t))], 1)[:, :span]
+        return (xp.unfold(1, taps, fi) @ bk.t()).reshape(rows, frames * fo)[:, :t_out]
+
+    def adjoint(dy, bk):
+        t = a["adjoint_of"]
+        d = torch.cat([dy, dy.new_zeros(rows, frames * fo - t_out)], 1).reshape(rows, frames, fo) @ bk
+        idx = (torch.arange(frames, device=x.device)[:, None] * fi + torch.arange(taps, device=x.device)).reshape(-1)
+        xp = dy.new_zeros(rows, max(span, half + t)).index_add_(1, idx, d.reshape(rows, -1))
+        return xp[:, half:half + t]
+    op = forward if a["adjoint_of"] is None else adjoint
+    return [Val("_result", arg("_result"), op(x, bank), op(x.abs(), bank.abs()))]
+
+
 # Role of every tensor argument of each checked kind: read, stored (the launch writes it), or
 # accumulated (+=, checked as after - before).  Shadow refuses a launch whose checker returns
 # outputs other than these, or leaves a passed output argument unchecked; `probe=True` also
@@ -431,20 +757,46 @@ ARGS: Dict[str, Tuple[FrozenSet[str], FrozenSet[str], FrozenSet[str]]] = {k: (fr
     "time_features": ({"sigma", "freqs"}, {"out"}, ()),
     "silu_bf16": ({"x"}, {"y"}, ()),
     "stem_in": ({"x", "w", "bias", "append", "noise", "alpha", "beta"}, {"out"}, {"stats"}),
-    "stem_out": ({"h", "x", "w", "bias", "gate", "append", "w_adapt", "b_adapt", "ab"}, {"v_out", "x_next"}, ()),
+    "stem_out": ({"h", "x", "w", "bias", "gate", "append", "w_adapt", "b_adapt", "ab", "noise", "alpha", "beta"},
+                 {"v_out", "x_next", "dv"}, {"loss_sum"}),
     "narrow_conv": ({"x", "stats_in", "gamma", "beta", "w", "bias", "residual", "scale_shift", "w_packed"},
                     {"y"}, {"stats_out"}),
     "sampler_step": ({"x", "v", "ab"}, {"x_next"}, ()),
     "step_select": ({"step", "ctrl", "ab_table"}, {"ab_out", "ss_out"}, ()),
     "step_advance": ((), {"step"}, ()),       # step += 1, checked against the snapshot + 1
+    # training (training.py's plans): the third set holds fp32 / fp64 accumulators (Acc) and statistics
+    "wgrad": ({"g", "x"}, (), {"dw"}),
+    "gn_silu_bwd": ({"da", "x", "stats", "gamma", "beta"}, {"dxh"}, {"dgamma", "dbeta", "S"}),
+    "gn_bwd_apply": ({"dxh", "x", "stats", "S", "dres"}, {"dx"}, {"colsum"}),
+    "ln_film_bwd": ({"dy", "x", "scale_shift", "dres"}, {"dx"}, {"dss", "colsum"}),
+    "colsum": ({"x", "gate"}, (), {"out"}),
+    "skip_gate": ({"y", "skip", "gate"}, {"out"}, {"stats"}),
+    "skip_gate_bwd": ({"dout", "y", "gate"}, {"dys"}, {"dgate"}),
+    "cond_bwd": ({"dss", "cond", "w"}, {"dw", "dbias"}, {"dcond"}),
+    "narrow_conv_bwd": ({"dy", "x", "stats_in", "gamma", "beta", "w"}, {"dxh"},
+                        {"dgamma", "dbeta", "S", "dw", "dbias"}),
+    "stem_out_bwd": ({"dv", "h", "x", "w", "bias", "gate", "gscale", "append", "noise", "alpha", "beta", "w_adapt"},
+                     {"dh", "dxin"}, {"dw", "dbias", "dgate", "dw_adapt", "db_adapt"}),
+    "stem_in_bwd": ({"dout", "x", "append", "noise", "alpha", "beta", "w"}, (), {"dw", "dbias", "dxin"}),
+    "attention_bwd": ({"q", "k", "v", "o", "d_o", "lse"}, {"delta", "dq", "dk", "dv"}, ()),
+    "ln_fold_bwd": ({"w", "g", "b", "dwf", "dbf"}, {"dw"}, {"dg", "db"}),
+    "fir_resample": ({"x", "bank"}, {"_result"}, ()),      # the output is the tensor the launch returns
 }.items()}
+
+# Kinds whose output is the tensor the launch allocates and returns (`_result` in the roles above).
+RESULT: Dict[str, Callable] = {"fir_resample": _fir_result}
 
 # Read arguments the kernel does not read for some argument combinations (the probe skips them):
 # narrow_conv copies the host-packed bf16 image instead of converting `w`, and the conv GEMM's
 # fp32-output epilogue has no residual (adp_conv_gemm refuses one).
+# stem_out_bwd reads the block input only for the SkipAdapter's weight gradient, and stem_in_bwd
+# the weight only for dxin; stem_out reads x un-noised only for the loss target.
 NOT_READ: Dict[str, Callable] = {
     "narrow_conv": lambda a: {"w"} if a["w_packed"] is not None else set(),
     "conv_gemm": lambda a: {"residual"} if a["out"].dtype == torch.float32 else set(),
+    "stem_out_bwd": lambda a: {"x", "append", "noise", "alpha", "beta"} if a["w_adapt"] is None else set(),
+    "stem_in_bwd": lambda a: {"w"} if a["dxin"] is None else set(),
+    "cond_bwd": lambda a: {"w"} if a["dcond"] is None else set(),     # the weights serve dcond only
 }
 
 CHECKERS: Dict[str, Callable] = {
@@ -452,6 +804,10 @@ CHECKERS: Dict[str, Callable] = {
     "attention": c_attention, "skinny_linear": c_skinny_linear, "time_features": c_time_features,
     "silu_bf16": c_silu_bf16, "stem_in": c_stem_in, "stem_out": c_stem_out, "narrow_conv": c_narrow_conv,
     "sampler_step": c_sampler_step, "step_select": c_step_select, "step_advance": c_step_advance,
+    "wgrad": c_wgrad, "gn_silu_bwd": c_gn_silu_bwd, "gn_bwd_apply": c_gn_bwd_apply, "ln_film_bwd": c_ln_film_bwd,
+    "colsum": c_colsum, "skip_gate": c_skip_gate, "skip_gate_bwd": c_skip_gate_bwd, "cond_bwd": c_cond_bwd,
+    "narrow_conv_bwd": c_narrow_conv_bwd, "stem_out_bwd": c_stem_out_bwd, "stem_in_bwd": c_stem_in_bwd,
+    "attention_bwd": c_attention_bwd, "ln_fold_bwd": c_ln_fold_bwd, "fir_resample": c_fir_resample,
 }
 
 
@@ -509,6 +865,7 @@ class Shadow:
         self.probed = set()
         self.records: Dict[str, Record] = {}
         self.n_launch, self.n_checked = 0, 0
+        self.labels = set()                      # trace labels of the launches seen (shapes included)
         self.known: Dict[int, torch.Tensor] = {}
 
     # ---- install
@@ -570,6 +927,9 @@ class Shadow:
                 self._probe(idx, name, outs, pre)
                 self.probed.add(variant)
             if self.fake:
+                result = None
+                if name in RESULT:
+                    result = post["_result"] = RESULT[name](post)
                 self._fake_write(outs, pre, post)
                 label = label0
             else:
@@ -578,19 +938,23 @@ class Shadow:
                 label = tr.records[-1]["name"] if tr.records else label0
                 if post[next(iter(post))].is_cuda:
                     torch.cuda.synchronize()
+                if name in RESULT:
+                    post["_result"] = result
             if self.mutate is not None and self.mutate[0] == name:
                 if self.mutate[1](post, outs, pre) is not False:       # False: not applicable here
                     self.mutate = None
+            self.labels.add(label)
             self._check(idx, name, label, outs, pre, post, snaps)
+            snaps.clear()            # `snap` refers to itself: without this the snapshots wait for the cycle collector
             self.n_checked += 1
-            return None if self.fake else result
+            return result
         return launch
 
     def _check_roles(self, idx, name, outs, post):
         """The checker's outputs are exactly the output arguments the launch was given."""
         _, stored, accumulated = ARGS[name]
-        got = {(o.name, isinstance(o, Stat)) for o in outs}
-        want = {(n, False) for n in stored if post.get(n) is not None} | \
+        got = {(o.name, o.acc) for o in outs}
+        want = {(n, False) for n in stored if post.get(n) is not None or n == "_result"} | \
             {(n, True) for n in accumulated if post.get(n) is not None}
         if got != want:
             raise CheckError(f"launch {idx}: {name}: checker outputs {sorted(got)}, declared {sorted(want)}")
@@ -624,14 +988,15 @@ class Shadow:
 
     def _fake_write(self, outs, pre, post):
         for o in outs:
-            if isinstance(o, Stat):
-                continue
-            got = o.view(post)
-            ref = o.ref(post)[0] if callable(o.ref) else o.ref
-            got.copy_(ref.to(got.dtype))
-        for o in outs:                       # statistics of the values just written
+            if isinstance(o, Val) or (isinstance(o, Acc) and not callable(o.ref)):
+                got = o.view(post)
+                ref = o.ref(post)[0] if callable(o.ref) else o.ref
+                got.add_(ref.to(got.dtype)) if o.acc else got.copy_(ref.to(got.dtype))
+        for o in outs:                       # statistics / sums of the values just written
             if isinstance(o, Stat):
                 o.view(post).add_(stats_of(o.src(post), o.groups))
+            elif isinstance(o, Acc) and callable(o.ref):
+                o.view(post).add_(o.ref(post)[0].to(o.view(post).dtype))
 
     # ---- comparisons
     def _fail(self, idx, name, label, msg):
@@ -644,29 +1009,6 @@ class Shadow:
             r.worst, r.label, r.where = ratio, label, where
 
     def _check(self, idx, name, label, outs, pre, post, snaps):
-        written = {}
-        for o in outs:
-            v = o.view(post)
-            written.setdefault(_key(v), []).append(v)
-        # side effects: read-only storages bitwise unchanged, written ones outside their views
-        for k, st in snaps.items():
-            t = next(t for t in _tensors(list(post.values())) if _key(t) == k)
-            views = written.get(k)
-            if views is None:
-                if not torch.equal(_flat(st, torch.uint8, t.device), _flat(t.untyped_storage(), torch.uint8, t.device)):
-                    argn = next(n for n, v in post.items() if any(_key(x) == k for x in _tensors([v])))
-                    self._fail(idx, name, label, f"read-only argument `{argn}` was modified")
-                continue
-            dt = views[0].dtype
-            before = _bits(_flat(st, dt, t.device))
-            after = _bits(_flat(t.untyped_storage(), dt, t.device))
-            mask = torch.zeros(before.shape, dtype=torch.bool, device=t.device)
-            for v in views:
-                mask.as_strided(v.shape, v.stride(), v.storage_offset()).fill_(True)
-            bad = (before != after) & ~mask
-            if bad.any():
-                i = int(bad.nonzero()[0, 0])
-                self._fail(idx, name, label, f"wrote storage element {i} outside its output view")
         for o in outs:
             got = o.view(post)
             key = f"{name}.{o.name}"
@@ -680,21 +1022,55 @@ class Shadow:
                 self._note(key, 0.0, label, "")
                 continue
             g = got.to(F64)
-            err = (g - ref).abs()
-            if got.dtype == torch.bfloat16:
-                bound = BF16_REL * ref.abs() + o.tau * absr
+            if isinstance(o, Acc):                    # the launch's own contribution
+                before = o.view(pre).to(F64)
+                val = g - before
+                if got.dtype == torch.float64:
+                    bound = STATS_TOL * absr
+                else:                                 # + the rounding of the two fp32 values subtracted
+                    bound = FP32_REL * ref.abs() + FP32_TAU * absr + ACC_EPS * (before.abs() + g.abs())
             else:
-                bound = FP32_REL * ref.abs() + FP32_TAU * absr
+                val = g
+                if got.dtype == torch.bfloat16:
+                    bound = BF16_REL * ref.abs() + o.tau * absr
+                else:
+                    bound = FP32_REL * ref.abs() + FP32_TAU * absr + o.floor
+            err = (val - ref).abs()
             ratio = torch.where(bound > 0, err / bound.clamp_min(1e-300), torch.where(err > 0, math.inf, 0.0))
             ratio = torch.where(torch.isnan(g), math.inf, ratio)
             i = int(ratio.reshape(-1).argmax())
             worst = float(ratio.reshape(-1)[i])
             where = _where(i, tuple(ratio.shape))
-            desc = (f"{o.name}{list(where)}: got {float(g.reshape(-1)[i]):.6g}, ref {float(ref.reshape(-1)[i]):.6g}, "
+            desc = (f"{o.name}{list(where)}: {'added' if o.acc else 'got'} {float(val.reshape(-1)[i]):.6g}, "
+                    f"ref {float(ref.reshape(-1)[i]):.6g}, "
                     f"bound {float(bound.reshape(-1)[i]):.3g} (err/bound {worst:.3g})")
             if worst > 1.0:
                 self._fail(idx, name, label, desc)
             self._note(key, worst, label, f"{list(where)}")
+        self._check_side_effects(idx, name, label, outs, post, snaps)
+
+    def _check_side_effects(self, idx, name, label, outs, post, snaps):
+        """Read-only storages are bitwise unchanged, written ones outside their written views: the
+        written views are copied into the snapshot, which must then equal the live storage byte for
+        byte (in chunks: the gradient arena and the activation arena are one storage each)."""
+        written = {}
+        for o in outs:
+            v = o.view(post)
+            written.setdefault(_key(v), []).append(v)
+        for k, st in snaps.items():
+            t = next(t for t in _tensors(list(post.values())) if _key(t) == k)
+            for v in written.get(k, ()):
+                _on(st, v).copy_(v)
+            before, after = _flat(st, torch.uint8, t.device), _flat(t.untyped_storage(), torch.uint8, t.device)
+            for lo in range(0, before.numel(), SIDE_CHUNK):
+                bb, aa = before[lo:lo + SIDE_CHUNK], after[lo:lo + SIDE_CHUNK]
+                if torch.equal(bb, aa):
+                    continue
+                if k not in written:
+                    argn = next(n for n, v in post.items() if any(_key(x) == k for x in _tensors([v])))
+                    self._fail(idx, name, label, f"read-only argument `{argn}` was modified")
+                i = lo + int((bb != aa).nonzero()[0, 0])
+                self._fail(idx, name, label, f"wrote byte {i} of a storage outside its output view")
 
     def _check_stats(self, idx, name, label, key, o, got, src):
         B, T, C = src.shape
@@ -775,6 +1151,33 @@ def m_stats_slot(post, outs, pre):
     g[-1, -1, 1] *= 1 + 1e-3
 
 
+def _first_acc(outs, post, pre):
+    for o in outs:
+        if isinstance(o, Acc) and bool((o.view(pre) != 0).any()):
+            return o
+    return None
+
+
+def m_acc_stored(post, outs, pre):
+    """An accumulator with a non-zero value before the launch stored to instead of added to
+    (what wgrad's single-split configuration once did)."""
+    o = _first_acc(outs, post, pre)
+    if o is None:
+        return False
+    o.view(post).sub_(o.view(pre))
+
+
+def m_acc_lost_split(post, outs, pre):
+    """The largest element of an accumulator's contribution short of 2^-5 of itself (a lost split)."""
+    o = next((o for o in outs if isinstance(o, Acc)), None)
+    if o is None:
+        return False
+    g, old = o.view(post), o.view(pre)
+    ref = o.ref(post)[0] if callable(o.ref) else o.ref
+    idx = _where(int(ref.abs().reshape(-1).argmax()), tuple(g.shape))
+    g[idx] = (old[idx].to(F64) + (g[idx].to(F64) - old[idx].to(F64)) * (1 - 2 ** -5)).to(g.dtype)
+
+
 def m_outside_view(post, outs, pre):
     """One element of a written tensor's storage outside the written view changed."""
     for o in outs:
@@ -802,4 +1205,5 @@ def m_readonly(post, outs, pre):
 
 
 MUTATIONS = {"scale_largest": m_scale_largest, "stale_tile": m_stale_tile, "stats_slot": m_stats_slot,
-             "outside_view": m_outside_view, "readonly": m_readonly}
+             "outside_view": m_outside_view, "readonly": m_readonly, "acc_stored": m_acc_stored,
+             "acc_lost_split": m_acc_lost_split}

@@ -294,3 +294,19 @@ def test_polyphase_bank_geometry(fi, fo):
     from audio_diffusion_pytorch_b200.utils import _polyphase_bank
     bank, half = _polyphase_bank(fi, fo, 0.99, 6, torch.float32, "cpu")
     assert bank.shape == (fo, 1, 2 * half + fi)
+
+
+def test_a_fused_optimizer_step_moves_the_pack_version():
+    """`fused=True` optimizers update the parameters without bumping their version counters: the
+    packs must still be refreshed after the step."""
+    from audio_diffusion_pytorch_b200.unet import UNetV0
+    torch.manual_seed(0)
+    net = UNetV0(dim=1, in_channels=2, channels=[8, 32], factors=[1, 4], items=[1, 1])
+    for fused in (True, False):
+        opt = torch.optim.AdamW(net.parameters(), lr=1e-2, fused=fused)
+        for p in net.parameters():
+            p.grad = torch.ones_like(p)
+        before, w0 = net._version(), net.net.down.weight.detach().clone()
+        opt.step()
+        assert not torch.equal(w0, net.net.down.weight.detach())
+        assert net._version() != before, f"fused={fused}: the optimizer step left the pack version unchanged"

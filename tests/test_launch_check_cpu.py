@@ -1,7 +1,7 @@
 """The per-launch checker of tests/launch_check.py, without a GPU.
 
-  * coverage: the checkers are exactly the launch kinds of the recorded inference, sampling and
-    conditioning programs (plus the generic sampler step); every other launching function of `ops`
+  * coverage: the checkers are exactly the launch kinds of the recorded inference, sampling,
+    conditioning and training programs (plus the generic sampler step and the resampler); every other launching function of `ops`
     is listed as unchecked, and every tensor argument of a checked kind in those programs has
     exactly one declared role;
   * probes: changing any input a launch reads must move its reference;
@@ -46,11 +46,14 @@ def test_checker_table_matches_ops():
     assert set(LAUNCHES) <= fns
     assert {"fir_resample", "mel_spectrogram", "to_flat", "to_flat_bwd", "sampler_step", "inpaint_blend",
             "arv_step"} <= fns
-    inference = {launch[0] for launch in _fixture_launches()}
-    # the generic VSampler step (a net that is not a B200UNet) is the one checked kind outside them
-    assert set(lc.CHECKERS) == inference | {"sampler_step"}
+    recorded = {launch[0] for launch in _fixture_launches(inference_only=False)}
+    assert {launch[0] for launch in _fixture_launches()} < recorded
+    # outside the recorded programs: the generic VSampler step (a net that is not a B200UNet) and the
+    # upsampler's resampling of the clip (host tensors, as recorded, take the tensor-op route)
+    assert set(lc.CHECKERS) == recorded | {"sampler_step", "fir_resample"}
     assert set(lc.ARGS) == set(lc.CHECKERS)
     assert set(lc.UNCHECKED) == fns - set(lc.CHECKERS)
+    assert set(lc.UNCHECKED) == {"to_flat", "to_flat_bwd", "mel_spectrogram", "inpaint_blend", "arv_step"}
 
 
 def _tensor_args(v):
@@ -60,11 +63,11 @@ def _tensor_args(v):
 
 
 def test_every_tensor_argument_is_classified():
-    """Each tensor argument of a checked kind in the recorded programs is declared as read, stored
-    or accumulated, in exactly one of the three (the declarations are enforced at run time:
+    """Each tensor argument of a checked kind in the recorded inference and training programs is
+    declared as read, stored or accumulated (statistics, fp32 / fp64 accumulators), in exactly one of the three (the declarations are enforced at run time:
     Shadow._check_roles and the probes of the program tests below)."""
     seen = {}
-    for launch in _fixture_launches():
+    for launch in _fixture_launches(inference_only=False):
         seen.setdefault(launch[0], set()).update(k for k, v in launch[1:] if _tensor_args(v))
     for name, names in seen.items():
         read, stored, acc = lc.ARGS[name]
