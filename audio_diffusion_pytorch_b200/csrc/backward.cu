@@ -11,7 +11,9 @@
 
 namespace adp {
 
-constexpr int kBwMaxC = 1024;
+// Widest row of the streaming kernels below.  Their per-channel arrays live in dynamic shared
+// memory sized by C (gn_silu_bwd: six of them, 48 KB at C = 2048).
+constexpr int kBwMaxC = 2048;
 
 __device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
   const float2 a = unpack_bf16(u.x), b = unpack_bf16(u.y), c = unpack_bf16(u.z), d = unpack_bf16(u.w);
@@ -27,6 +29,10 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
 // SAME channels: fold their partial sums with shuffles so that one lane per channel touches the
 // block's shared-memory bins (at C = 32 the unfolded version sent 64 threads to every bin and
 // the kernel ran far below HBM bandwidth).
+// Their per-thread stride is the largest multiple of vpr the grid's threads reach (threads past it
+// sit out; the host launches at least vpr threads): a stride rounded UP would skip the vectors
+// between the last thread and the stride whenever the thread count is not a multiple of vpr.
+__device__ __forceinline__ size_t chan_stride(size_t nthreads, int vpr) { return nthreads / vpr * vpr; }
 __device__ __forceinline__ bool fold_ok(int vpr) { return vpr < 32 && (32 % vpr) == 0; }
 __device__ __forceinline__ float fold_lanes(float v, int vpr) {
   for (int o = vpr; o < 32; o <<= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -60,9 +66,13 @@ gn_silu_bwd_kernel(const uint4* __restrict__ da, const uint4* __restrict__ x,
                    int T, int C, int groups, float eps) {
   pdl_launch_dependents();
   pdl_wait();
-  __shared__ float s_mean[kBwMaxC], s_rstd[kBwMaxC];
-  __shared__ float s_dg[kBwMaxC], s_db[kBwMaxC];
-  __shared__ float s_s1[kBwMaxC], s_s2[kBwMaxC];      // per-channel sums of dxh, dxh*xhat
+  extern __shared__ __align__(16) float s_bw[];     // 6 x C
+  float* s_mean = s_bw;
+  float* s_rstd = s_bw + C;
+  float* s_dg = s_bw + 2 * C;
+  float* s_db = s_bw + 3 * C;
+  float* s_s1 = s_bw + 4 * C;                        // per-channel sums of dxh, dxh*xhat
+  float* s_s2 = s_bw + 5 * C;
   const int b = blockIdx.y;
   gn_coeffs(stats, b, T, C, groups, eps, s_mean, s_rstd);
   for (int c = threadIdx.x; c < C; c += blockDim.x) { s_dg[c] = 0.f; s_db[c] = 0.f; s_s1[c] = 0.f; s_s2[c] = 0.f; }
@@ -76,7 +86,7 @@ gn_silu_bwd_kernel(const uint4* __restrict__ da, const uint4* __restrict__ x,
   // per-thread stride is a multiple of vectors-per-row: the thread's 8 channels never change
   const size_t tid = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   const size_t nthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
-  const size_t stride = (nthreads + vpr - 1) / vpr * vpr;
+  const size_t stride = chan_stride(nthreads, vpr);
   const int c0 = static_cast<int>(tid % vpr) << 3;
   float g8[8], b8[8], m8[8], r8[8];
 #pragma unroll
@@ -86,7 +96,7 @@ gn_silu_bwd_kernel(const uint4* __restrict__ da, const uint4* __restrict__ x,
   float adg[8], adb[8], as1[8], as2[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) { adg[j] = 0.f; adb[j] = 0.f; as1[j] = 0.f; as2[j] = 0.f; }
-  for (size_t i = tid; i < nvec; i += stride) {
+  for (size_t i = tid; tid < stride && i < nvec; i += stride) {
     float fa[8], fx[8], o[8];
     unpack8(__ldg(dab + i), fa);
     unpack8(__ldg(xb + i), fx);
@@ -150,8 +160,12 @@ gn_bwd_apply_kernel(const uint4* __restrict__ dxh, const uint4* __restrict__ x,
                     float* __restrict__ colsum, int T, int C, int groups, float eps) {
   pdl_launch_dependents();
   pdl_wait();
-  __shared__ float s_mean[kBwMaxC], s_rstd[kBwMaxC], s_c1[kBwMaxC], s_c2[kBwMaxC];
-  __shared__ float s_cs[kBwMaxC];
+  extern __shared__ __align__(16) float s_bw[];     // 5 x C
+  float* s_mean = s_bw;
+  float* s_rstd = s_bw + C;
+  float* s_c1 = s_bw + 2 * C;
+  float* s_c2 = s_bw + 3 * C;
+  float* s_cs = s_bw + 4 * C;
   const int b = blockIdx.y;
   gn_coeffs(stats, b, T, C, groups, eps, s_mean, s_rstd);
   const int gsz = C / groups;
@@ -168,12 +182,12 @@ gn_bwd_apply_kernel(const uint4* __restrict__ dxh, const uint4* __restrict__ x,
   const size_t boff = static_cast<size_t>(b) * nvec;
   const size_t tid = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   const size_t nthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
-  const size_t stride = (nthreads + vpr - 1) / vpr * vpr;
+  const size_t stride = chan_stride(nthreads, vpr);
   const int c0 = static_cast<int>(tid % vpr) << 3;
   float acs[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) acs[j] = 0.f;
-  for (size_t i = tid; i < nvec; i += stride) {
+  for (size_t i = tid; tid < stride && i < nvec; i += stride) {
     float fd[8], fx[8], fr[8], o[8];
     unpack8(__ldg(dxh + boff + i), fd);
     unpack8(__ldg(x + boff + i), fx);
@@ -209,7 +223,11 @@ gn_bwd_apply_kernel(const uint4* __restrict__ dxh, const uint4* __restrict__ x,
 // ----------------------------------------------------------------------- ln_film_bwd
 // y = xhat*(1+s) + t per row.  dx = rstd*(g - mean(g) - xhat*mean(g*xhat)), g = dy*(1+s);
 // dss[b, c] += sum_t dy*xhat, dss[b, C+c] += sum_t dy;  optional colsum[c] += sum dx.
-template <int VPL>
+// Row layout as ln_film (ln_row_layout; TAIL masks the vectors past the row end).  Up to 4 vectors
+// per lane the per-channel sums stay in registers over all rows of a lane; wider rows (C > 1024)
+// would need 3 x 64 more registers than a thread has, so each row adds its terms to shared
+// memory, laid out [channel % 8][channel / 8] so that the 32 lanes of a warp hit 32 banks.
+template <int VPL, bool TAIL>
 __global__ void __launch_bounds__(256)
 ln_film_bwd_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x,
                    const float* __restrict__ ss, int ss_stride, uint4* __restrict__ dx,
@@ -217,20 +235,25 @@ ln_film_bwd_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x,
                    const uint4* __restrict__ dres, int T, int C, int lpr, float eps) {
   pdl_launch_dependents();
   pdl_wait();
-  __shared__ __align__(16) float s_fs[kBwMaxC];
-  __shared__ float s_ds[kBwMaxC], s_dt[kBwMaxC], s_cs[kBwMaxC];
+  constexpr bool REG = VPL <= 4;
+  constexpr int kRowC = REG ? 1024 : kBwMaxC;
+  __shared__ __align__(16) float s_fs[kRowC];
+  __shared__ float s_ds[kRowC], s_dt[kRowC], s_cs[kRowC];
   const int b = blockIdx.y;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int rpw = 32 / lpr, sub = lane / lpr, l = lane - sub * lpr;
   const int vpr = C >> 3;
+#define live(it) (!TAIL || (it) * lpr + l < vpr)
+#define acc_at(c) (REG ? (c) : ((c) & 7) * (kBwMaxC / 8) + ((c) >> 3))
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     s_fs[c] = ss ? 1.f + ss[static_cast<size_t>(b) * ss_stride + c] : 1.f;
-    s_ds[c] = 0.f; s_dt[c] = 0.f; s_cs[c] = 0.f;
+    s_ds[acc_at(c)] = 0.f; s_dt[acc_at(c)] = 0.f; s_cs[acc_at(c)] = 0.f;
   }
   __syncthreads();
-  float ads[VPL][8], adt[VPL][8], acs[VPL][8];
+  constexpr int NA = REG ? VPL : 1;
+  float ads[NA][8], adt[NA][8], acs[NA][8];
 #pragma unroll
-  for (int it = 0; it < VPL; ++it)
+  for (int it = 0; it < NA; ++it)
 #pragma unroll
     for (int j = 0; j < 8; ++j) { ads[it][j] = 0.f; adt[it][j] = 0.f; acs[it][j] = 0.f; }
   const size_t boff = static_cast<size_t>(b) * T * vpr;
@@ -244,7 +267,7 @@ ln_film_bwd_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x,
 #pragma unroll
     for (int it = 0; it < VPL; ++it) {
       uint4 ux = make_uint4(0, 0, 0, 0), ud = make_uint4(0, 0, 0, 0);
-      if (ok) {
+      if (ok && live(it)) {
         ux = __ldg(x + boff + static_cast<size_t>(row) * vpr + it * lpr + l);
         ud = __ldg(dy + boff + static_cast<size_t>(row) * vpr + it * lpr + l);
       }
@@ -258,13 +281,16 @@ ln_film_bwd_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x,
     float sq = 0.f;
 #pragma unroll
     for (int it = 0; it < VPL; ++it)
+      if (live(it)) {
 #pragma unroll
-      for (int j = 0; j < 8; ++j) { const float d = vx[it][j] - mean; sq += d * d; }
+        for (int j = 0; j < 8; ++j) { const float d = vx[it][j] - mean; sq += d * d; }
+      }
     for (int o = lpr >> 1; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
     const float rstd = rsqrtf(sq * inv_c + eps);
     float m1 = 0.f, m2 = 0.f;
 #pragma unroll
     for (int it = 0; it < VPL; ++it) {
+      if (!live(it)) continue;
       const int c = (it * lpr + l) << 3;
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
@@ -273,7 +299,12 @@ ln_film_bwd_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x,
         const float g = vd[it][j] * s_fs[c + j];
         vg[it][j] = g;
         m1 += g; m2 += g * xh;
-        if (ok) { ads[it][j] += vd[it][j] * xh; adt[it][j] += vd[it][j]; }
+        if constexpr (REG) {
+          if (ok) { ads[it][j] += vd[it][j] * xh; adt[it][j] += vd[it][j]; }
+        } else if (ok) {
+          atomicAdd(&s_ds[acc_at(c + j)], vd[it][j] * xh);
+          atomicAdd(&s_dt[acc_at(c + j)], vd[it][j]);
+        }
       }
     }
     for (int o = lpr >> 1; o > 0; o >>= 1) {
@@ -283,6 +314,7 @@ ln_film_bwd_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x,
     m1 *= inv_c; m2 *= inv_c;
 #pragma unroll
     for (int it = 0; it < VPL; ++it) {
+      if (!live(it)) continue;
       float o[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) o[j] = rstd * (vg[it][j] - m1 - vx[it][j] * m2);
@@ -298,51 +330,64 @@ ln_film_bwd_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x,
         if (colsum) {
           float orr[8];
           unpack8(ov, orr);
+          if constexpr (REG) {
 #pragma unroll
-          for (int j = 0; j < 8; ++j) acs[it][j] += o[j];
+            for (int j = 0; j < 8; ++j) acs[it][j] += o[j];
+          } else {
+            const int c = (it * lpr + l) << 3;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) atomicAdd(&s_cs[acc_at(c + j)], o[j]);
+          }
         }
       }
     }
   }
-  // lanes l, l+lpr, ... hold the same channels: fold, then one smem atomic per channel
-#pragma unroll
-  for (int it = 0; it < VPL; ++it)
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-      for (int o = lpr; o < 32; o <<= 1) {
-        ads[it][j] += __shfl_xor_sync(0xffffffffu, ads[it][j], o);
-        adt[it][j] += __shfl_xor_sync(0xffffffffu, adt[it][j], o);
-        acs[it][j] += __shfl_xor_sync(0xffffffffu, acs[it][j], o);
-      }
-  if (sub == 0) {
+  if constexpr (REG) {
+    // lanes l, l+lpr, ... hold the same channels: fold, then one smem atomic per channel
 #pragma unroll
     for (int it = 0; it < VPL; ++it)
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int c = ((it * lpr + l) << 3) + j;
-        atomicAdd(&s_ds[c], ads[it][j]);
-        atomicAdd(&s_dt[c], adt[it][j]);
-        atomicAdd(&s_cs[c], acs[it][j]);
+      for (int j = 0; j < 8; ++j)
+        for (int o = lpr; o < 32; o <<= 1) {
+          ads[it][j] += __shfl_xor_sync(0xffffffffu, ads[it][j], o);
+          adt[it][j] += __shfl_xor_sync(0xffffffffu, adt[it][j], o);
+          acs[it][j] += __shfl_xor_sync(0xffffffffu, acs[it][j], o);
+        }
+    if (sub == 0) {
+#pragma unroll
+      for (int it = 0; it < VPL; ++it) {
+        if (!live(it)) continue;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int c = ((it * lpr + l) << 3) + j;
+          atomicAdd(&s_ds[c], ads[it][j]);
+          atomicAdd(&s_dt[c], adt[it][j]);
+          atomicAdd(&s_cs[c], acs[it][j]);
+        }
       }
+    }
   }
   __syncthreads();
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     if (dss) {
-      atomicAdd(dss + static_cast<size_t>(b) * dss_stride + c, s_ds[c]);
-      atomicAdd(dss + static_cast<size_t>(b) * dss_stride + C + c, s_dt[c]);
+      atomicAdd(dss + static_cast<size_t>(b) * dss_stride + c, s_ds[acc_at(c)]);
+      atomicAdd(dss + static_cast<size_t>(b) * dss_stride + C + c, s_dt[acc_at(c)]);
     }
-    if (colsum) atomicAdd(colsum + c, s_cs[c]);
+    if (colsum) atomicAdd(colsum + c, s_cs[acc_at(c)]);
   }
+#undef acc_at
+#undef live
 }
 
 // ---------------------------------------------------------------------------- colsum
-constexpr int kColsumMaxC = 2048;     // fused q|k|v gradient rows are 3*512 wide
+constexpr int kColsumMaxC = 3 * 2048;     // fused q|k|v gradient rows are 3 * heads * D wide
 __global__ void __launch_bounds__(256)
 colsum_kernel(const uint4* __restrict__ x, const float* __restrict__ gate, int ld_gate,
               float* __restrict__ out, int T, int C) {
   pdl_launch_dependents();
   pdl_wait();
-  __shared__ float s_cs[kColsumMaxC];
+  extern __shared__ __align__(16) float s_bw[];     // C
+  float* s_cs = s_bw;
   const int b = blockIdx.y;
   for (int c = threadIdx.x; c < C; c += blockDim.x) s_cs[c] = 0.f;
   __syncthreads();
@@ -350,12 +395,12 @@ colsum_kernel(const uint4* __restrict__ x, const float* __restrict__ gate, int l
   const size_t nvec = static_cast<size_t>(T) * vpr;
   const size_t tid = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   const size_t nthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
-  const size_t stride = (nthreads + vpr - 1) / vpr * vpr;
+  const size_t stride = chan_stride(nthreads, vpr);
   const int c0 = static_cast<int>(tid % vpr) << 3;
   float acc[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) acc[j] = 0.f;
-  for (size_t i = tid; i < nvec; i += stride) {
+  for (size_t i = tid; tid < stride && i < nvec; i += stride) {
     float f[8];
     unpack8(__ldg(x + static_cast<size_t>(b) * nvec + i), f);
 #pragma unroll
@@ -382,20 +427,24 @@ skip_gate_kernel(const uint4* __restrict__ y, const uint4* __restrict__ skip,
                  double* __restrict__ stats, int T, int C, int groups) {
   pdl_launch_dependents();
   pdl_wait();
-  __shared__ float s_s1[kBwMaxC], s_s2[kBwMaxC];      // per-channel sum / sum of squares of out
+  extern __shared__ __align__(16) float s_bw[];     // 2 x C: per-channel sum / sum of squares of out
+  float* s_s1 = s_bw;
+  float* s_s2 = s_bw + C;
   const int b = blockIdx.y;
-  for (int c = threadIdx.x; c < C; c += blockDim.x) { s_s1[c] = 0.f; s_s2[c] = 0.f; }
+  if (stats) {                                     // no shared memory without statistics
+    for (int c = threadIdx.x; c < C; c += blockDim.x) { s_s1[c] = 0.f; s_s2[c] = 0.f; }
+  }
   __syncthreads();
   const int vpr = C >> 3, gsz = groups > 0 ? C / groups : C;
   const size_t nvec = static_cast<size_t>(T) * vpr, boff = static_cast<size_t>(b) * nvec;
   const size_t tid = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   const size_t nthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
-  const size_t stride = (nthreads + vpr - 1) / vpr * vpr;
+  const size_t stride = chan_stride(nthreads, vpr);
   const int c0 = static_cast<int>(tid % vpr) << 3;
   float g8[8], s1[8], s2[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) { g8[j] = gate[static_cast<size_t>(b) * ld_gate + c0 + j]; s1[j] = 0.f; s2[j] = 0.f; }
-  for (size_t i = tid; i < nvec; i += stride) {
+  for (size_t i = tid; tid < stride && i < nvec; i += stride) {
     float fy[8], fs[8], o[8];
     unpack8(__ldg(y + boff + i), fy);
     unpack8(__ldg(skip + boff + i), fs);
@@ -439,7 +488,8 @@ skip_gate_bwd_kernel(const uint4* __restrict__ dout, const uint4* __restrict__ y
                      float* __restrict__ dgate, int ld_dgate, int T, int C) {
   pdl_launch_dependents();
   pdl_wait();
-  __shared__ float s_dg[kBwMaxC];
+  extern __shared__ __align__(16) float s_bw[];     // C
+  float* s_dg = s_bw;
   const int b = blockIdx.y;
   for (int c = threadIdx.x; c < C; c += blockDim.x) s_dg[c] = 0.f;
   __syncthreads();
@@ -447,12 +497,12 @@ skip_gate_bwd_kernel(const uint4* __restrict__ dout, const uint4* __restrict__ y
   const size_t nvec = static_cast<size_t>(T) * vpr, boff = static_cast<size_t>(b) * nvec;
   const size_t tid = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   const size_t nthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
-  const size_t stride = (nthreads + vpr - 1) / vpr * vpr;
+  const size_t stride = chan_stride(nthreads, vpr);
   const int c0 = static_cast<int>(tid % vpr) << 3;
   float g8[8], adg[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) { g8[j] = gate[static_cast<size_t>(b) * ld_gate + c0 + j]; adg[j] = 0.f; }
-  for (size_t i = tid; i < nvec; i += stride) {
+  for (size_t i = tid; tid < stride && i < nvec; i += stride) {
     float fd[8], fy[8], o[8];
     unpack8(__ldg(dout + boff + i), fd);
     unpack8(__ldg(y + boff + i), fy);
@@ -542,11 +592,13 @@ cond_bwd_kernel(const float* __restrict__ dss, int ld_dss, const float* __restri
   }
 }
 
-static int grid_for(size_t nvec, int B) {
+static int grid_for(size_t nvec, int B, int vpr) {
   // every block ends in 2C global atomics: a few hundred blocks in total, each streaming many rows
   size_t g = (nvec + 256 * 4 - 1) / (256 * 4);
   const size_t cap = num_sms() * 3 / (B < 8 ? B : 8) + 1;
   if (g > cap) g = cap;
+  const size_t least = (static_cast<size_t>(vpr) + 255) / 256;     // every channel vector has a thread
+  if (g < least) g = least;
   if (g < 1) g = 1;
   return static_cast<int>(g);
 }
@@ -562,8 +614,11 @@ extern "C" int adp_gn_silu_bwd(const void* da, const void* x, const double* stat
   ADP_CHECK(da && x && stats && gamma && beta && dxh && dgamma && dbeta && S, "adp_gn_silu_bwd: null");
   ADP_CHECK(C % 8 == 0 && C <= kBwMaxC && groups > 0 && groups <= 64 && C % groups == 0,
             "adp_gn_silu_bwd: C=%d groups=%d", C, groups);
-  dim3 grid(grid_for(static_cast<size_t>(T) * (C / 8), B), B);
-  ADP_CUDA(launch_k(gn_silu_bwd_kernel, grid, dim3(256), (size_t)0, as_stream(stream),
+  dim3 grid(grid_for(static_cast<size_t>(T) * (C / 8), B, C / 8), B);
+  const size_t smem = 6 * static_cast<size_t>(C) * sizeof(float);
+  static SmemAttrCache smem_cache;
+  ADP_CUDA(ensure_dyn_smem(gn_silu_bwd_kernel, smem, smem_cache));
+  ADP_CUDA(launch_k(gn_silu_bwd_kernel, grid, dim3(256), smem, as_stream(stream),
                     static_cast<const uint4*>(da), static_cast<const uint4*>(x), stats, gamma, beta,
                     static_cast<uint4*>(dxh), dgamma, dbeta, S, (int)T, (int)C, (int)groups, eps));
   return 0;
@@ -575,8 +630,11 @@ extern "C" int adp_gn_bwd_apply(const void* dxh, const void* x, const double* st
                                 adp_stream_t stream) {
   ADP_CHECK(dxh && x && stats && S && dx, "adp_gn_bwd_apply: null");
   ADP_CHECK(C % 8 == 0 && C <= kBwMaxC && groups > 0 && C % groups == 0, "adp_gn_bwd_apply: C=%d", C);
-  dim3 grid(grid_for(static_cast<size_t>(T) * (C / 8), B), B);
-  ADP_CUDA(launch_k(gn_bwd_apply_kernel, grid, dim3(256), (size_t)0, as_stream(stream),
+  dim3 grid(grid_for(static_cast<size_t>(T) * (C / 8), B, C / 8), B);
+  const size_t smem = 5 * static_cast<size_t>(C) * sizeof(float);
+  static SmemAttrCache smem_cache;
+  ADP_CUDA(ensure_dyn_smem(gn_bwd_apply_kernel, smem, smem_cache));
+  ADP_CUDA(launch_k(gn_bwd_apply_kernel, grid, dim3(256), smem, as_stream(stream),
                     static_cast<const uint4*>(dxh), static_cast<const uint4*>(x), stats, S,
                     static_cast<const uint4*>(dres), static_cast<uint4*>(dx), colsum, (int)T,
                     (int)C, (int)groups, eps));
@@ -588,16 +646,10 @@ extern "C" int adp_ln_film_bwd(const void* dy, const void* x, const float* scale
                                float* colsum, const void* dres, int32_t B, int32_t T, int32_t C,
                                float eps, adp_stream_t stream) {
   ADP_CHECK(dy && x && dx, "adp_ln_film_bwd: null");
-  ADP_CHECK(C % 8 == 0 && C <= kBwMaxC, "adp_ln_film_bwd: C=%d", C);
-  const int vpr = C / 8;
+  ADP_CHECK(C > 0 && C % 8 == 0 && C <= kBwMaxC, "adp_ln_film_bwd: C=%d must be a multiple of 8 and <= %d",
+            C, kBwMaxC);
   int lpr, vpl;
-  if (vpr <= 32) {
-    ADP_CHECK((vpr & (vpr - 1)) == 0, "adp_ln_film_bwd: C/8=%d must be a power of two", vpr);
-    lpr = vpr; vpl = 1;
-  } else {
-    ADP_CHECK(vpr % 32 == 0 && vpr / 32 <= 4, "adp_ln_film_bwd: C=%d unsupported", C);
-    lpr = 32; vpl = vpr / 32;
-  }
+  const bool tail = ln_row_layout(C, &lpr, &vpl);
   const int rows_per_block = 8 * (32 / lpr);
   // few rows (deep levels): one pass per warp so that every SM gets a block; many rows: persistent
   // blocks (each ends in 3C global atomics)
@@ -611,22 +663,30 @@ extern "C" int adp_ln_film_bwd(const void* dy, const void* x, const float* scale
   uint4* pdx = static_cast<uint4*>(dx);
   cudaStream_t s = as_stream(stream);
 #define ADP_LNB(VPL)                                                                              \
-  ADP_CUDA(launch_k(ln_film_bwd_kernel<VPL>, grid, dim3(256), (size_t)0, s, pdy, px, scale_shift, \
-                    (int)ss_stride, pdx, dss, (int)dss_stride, colsum,                            \
-                    static_cast<const uint4*>(dres), (int)T, (int)C, (int)lpr, eps))
-  if (vpl == 1) ADP_LNB(1);
-  else if (vpl == 2) ADP_LNB(2);
-  else if (vpl == 3) ADP_LNB(3);
-  else ADP_LNB(4);
+  if (tail) ADP_CUDA(launch_k(ln_film_bwd_kernel<VPL, true>, grid, dim3(256), (size_t)0, s, LNB_ARGS)); \
+  else ADP_CUDA(launch_k(ln_film_bwd_kernel<VPL, false>, grid, dim3(256), (size_t)0, s, LNB_ARGS))
+#define LNB_ARGS pdy, px, scale_shift, (int)ss_stride, pdx, dss, (int)dss_stride, colsum, \
+                 static_cast<const uint4*>(dres), (int)T, (int)C, (int)lpr, eps
+  switch (vpl) {
+    case 1: ADP_LNB(1); break;  case 2: ADP_LNB(2); break;
+    case 3: ADP_LNB(3); break;  case 4: ADP_LNB(4); break;
+    case 5: ADP_LNB(5); break;  case 6: ADP_LNB(6); break;
+    case 7: ADP_LNB(7); break;  default: ADP_LNB(8); break;
+  }
+#undef LNB_ARGS
 #undef ADP_LNB
   return 0;
 }
 
 extern "C" int adp_colsum(const void* x, const float* gate, int32_t ld_gate, float* out, int32_t B,
                           int32_t T, int32_t C, adp_stream_t stream) {
-  ADP_CHECK(x && out && C % 8 == 0 && C <= kColsumMaxC, "adp_colsum: bad args (C=%d)", C);
-  dim3 grid(grid_for(static_cast<size_t>(T) * (C / 8), B), B);
-  ADP_CUDA(launch_k(colsum_kernel, grid, dim3(256), (size_t)0, as_stream(stream),
+  ADP_CHECK(x && out && C > 0 && C % 8 == 0 && C <= kColsumMaxC, "adp_colsum: bad args (C=%d, at most %d)",
+            C, kColsumMaxC);
+  dim3 grid(grid_for(static_cast<size_t>(T) * (C / 8), B, C / 8), B);
+  const size_t smem = static_cast<size_t>(C) * sizeof(float);
+  static SmemAttrCache smem_cache;
+  ADP_CUDA(ensure_dyn_smem(colsum_kernel, smem, smem_cache));
+  ADP_CUDA(launch_k(colsum_kernel, grid, dim3(256), smem, as_stream(stream),
                     static_cast<const uint4*>(x), gate, (int)ld_gate, out, (int)T, (int)C));
   return 0;
 }
@@ -635,9 +695,13 @@ extern "C" int adp_skip_gate(const void* y, const void* skip, const float* gate,
                              void* out, double* stats, int32_t B, int32_t T, int32_t C,
                              int32_t groups, adp_stream_t stream) {
   ADP_CHECK(y && skip && gate && out && C % 8 == 0, "adp_skip_gate: bad args");
-  ADP_CHECK(!stats || (groups > 0 && groups <= 64 && C % groups == 0 && C <= kBwMaxC), "adp_skip_gate: groups");
-  dim3 grid(grid_for(static_cast<size_t>(T) * (C / 8), B), B);
-  ADP_CUDA(launch_k(skip_gate_kernel, grid, dim3(256), (size_t)0, as_stream(stream),
+  ADP_CHECK(!stats || (groups > 0 && groups <= 64 && C % groups == 0 && C <= kBwMaxC),
+            "adp_skip_gate: C=%d groups=%d (statistics need C <= %d)", C, groups, kBwMaxC);
+  dim3 grid(grid_for(static_cast<size_t>(T) * (C / 8), B, C / 8), B);
+  const size_t smem = stats ? 2 * static_cast<size_t>(C) * sizeof(float) : 0;
+  static SmemAttrCache smem_cache;
+  ADP_CUDA(ensure_dyn_smem(skip_gate_kernel, smem, smem_cache));
+  ADP_CUDA(launch_k(skip_gate_kernel, grid, dim3(256), smem, as_stream(stream),
                     static_cast<const uint4*>(y), static_cast<const uint4*>(skip), gate,
                     (int)ld_gate, static_cast<uint4*>(out), stats, (int)T, (int)C, (int)groups));
   return 0;
@@ -647,8 +711,11 @@ extern "C" int adp_skip_gate_bwd(const void* dout, const void* y, const float* g
                                  int32_t ld_gate, void* dys, float* dgate, int32_t ld_dgate,
                                  int32_t B, int32_t T, int32_t C, adp_stream_t stream) {
   ADP_CHECK(dout && y && gate && dys && dgate && C % 8 == 0 && C <= kBwMaxC, "adp_skip_gate_bwd: bad args");
-  dim3 grid(grid_for(static_cast<size_t>(T) * (C / 8), B), B);
-  ADP_CUDA(launch_k(skip_gate_bwd_kernel, grid, dim3(256), (size_t)0, as_stream(stream),
+  dim3 grid(grid_for(static_cast<size_t>(T) * (C / 8), B, C / 8), B);
+  const size_t smem = static_cast<size_t>(C) * sizeof(float);
+  static SmemAttrCache smem_cache;
+  ADP_CUDA(ensure_dyn_smem(skip_gate_bwd_kernel, smem, smem_cache));
+  ADP_CUDA(launch_k(skip_gate_bwd_kernel, grid, dim3(256), smem, as_stream(stream),
                     static_cast<const uint4*>(dout), static_cast<const uint4*>(y), gate,
                     (int)ld_gate, static_cast<uint4*>(dys), dgate, (int)ld_dgate, (int)T, (int)C));
   return 0;

@@ -95,6 +95,22 @@ inline int blocks_per_batch(int n_tiles, int B, int z = 1) {
   return gx < 1 ? 1 : gx;
 }
 
+// Row layout of the LayerNorm row kernels (ln_film, ln_film_bwd), C a multiple of 8: the C/8
+// vectors of a row spread over lpr lanes, vpl vectors per lane, lpr a power of two.  Up to 32
+// vectors: one per lane on the next power of two of lanes; more: 32 lanes, ceil(C/256) vectors
+// each.  Returns true when lpr * vpl > C/8, i.e. the kernel masks the vectors past the row end.
+inline bool ln_row_layout(int C, int* lpr, int* vpl) {
+  const int vpr = C / 8;
+  if (vpr <= 32) {
+    int p = 1;
+    while (p < vpr) p <<= 1;
+    *lpr = p; *vpl = 1;
+  } else {
+    *lpr = 32; *vpl = (vpr + 31) / 32;
+  }
+  return *lpr * *vpl != vpr;
+}
+
 // 1-D grid-stride launch over n items: one item per thread, at most 16 blocks per SM
 inline int capped_grid(int64_t n, int threads) {
   int64_t g = (n + threads - 1) / threads;

@@ -167,17 +167,27 @@ gn_stats_kernel(const uint4* __restrict__ x, double* __restrict__ stats, int T, 
 // --------------------------------------------------------------------------- ln_film
 // One row = C channels = C/8 vectors spread over LPR lanes (VPL vectors per lane); UNR
 // independent row groups per warp iteration keep several 16-byte loads in flight per lane.
-constexpr int kMaxLnC = 1024;
-template <int VPL, bool PER_CH, int UNR>
+// LPR is a power of two (the shuffle reductions); when LPR * VPL exceeds C/8 (TAIL), the
+// vectors it * LPR + l >= C/8 are masked: they load nothing, store nothing and add nothing.
+// Statistics (STATS): LN_GROUP  every vector lies inside one group (group size a multiple of 8);
+//                     LN_PER_CH per-channel sums, group taken per element at the end (VPL <= 2:
+//                               group sizes below 8 need C < 512 at the 64 groups allowed);
+//                     LN_SPLIT  group size >= 8 but not a multiple of 8: a vector holds the tail
+//                               of one group and the head of the next, summed separately.
+constexpr int kMaxLnC = kMaxC;
+enum { LN_GROUP = 0, LN_PER_CH = 1, LN_SPLIT = 2 };
+template <int VPL, int STATS, int UNR, bool TAIL>
 __global__ void __launch_bounds__(256)
 ln_film_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, const float* __restrict__ ss,
                int ss_stride, double* __restrict__ stats, int T, int C, int lpr, int groups,
                float eps, uint4* __restrict__ y2, float eps2) {
+  static_assert(STATS != LN_PER_CH || VPL <= 2, "per-channel statistics hold 8 sums per vector");
   pdl_launch_dependents();
   pdl_wait();
+  constexpr int kFilmC = VPL <= 4 ? 1024 : kMaxLnC;   // rows of up to 4 x 32 vectors: 1024 channels
   __shared__ float s_acc[2 * 64];
-  __shared__ __align__(16) float s_fs[kMaxLnC];
-  __shared__ __align__(16) float s_ft[kMaxLnC];
+  __shared__ __align__(16) float s_fs[kFilmC];
+  __shared__ __align__(16) float s_ft[kFilmC];
   const int b = blockIdx.y;
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
@@ -188,11 +198,18 @@ ln_film_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, const float* 
   const int gsz = groups > 0 ? C / groups : C;
   const bool do_stats = stats != nullptr;
   if (threadIdx.x < 128) s_acc[threadIdx.x] = 0.f;
+#define live(it) (!TAIL || (it) * lpr + l < vpr)
 
-  constexpr int NACC = PER_CH ? 8 : VPL;
+  constexpr int NACC = STATS == LN_PER_CH ? 8 * VPL : STATS == LN_SPLIT ? 2 * VPL : VPL;
   float as[NACC], aq[NACC];
 #pragma unroll
   for (int j = 0; j < NACC; ++j) { as[j] = 0.f; aq[j] = 0.f; }
+  // LN_SPLIT: channels [0, head[it]) of vector it belong to its first group, the rest to the next
+  int head[STATS == LN_SPLIT ? VPL : 1];
+  if constexpr (STATS == LN_SPLIT) {
+#pragma unroll
+    for (int it = 0; it < VPL; ++it) head[it] = gsz - (((it * lpr + l) << 3) % gsz);
+  }
 
   const uint4* xb = x + static_cast<size_t>(b) * T * vpr;
   uint4* yb = y + static_cast<size_t>(b) * T * vpr;
@@ -206,7 +223,7 @@ ln_film_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, const float* 
 #pragma unroll
       for (int it = 0; it < VPL; ++it) {
         dst[un][it] = make_uint4(0, 0, 0, 0);
-        if (row < T) dst[un][it] = __ldg(xb + static_cast<size_t>(row) * vpr + it * lpr + l);
+        if (row < T && live(it)) dst[un][it] = __ldg(xb + static_cast<size_t>(row) * vpr + it * lpr + l);
       }
     }
   };
@@ -244,12 +261,15 @@ ln_film_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, const float* 
       float sq = 0.f;
 #pragma unroll
       for (int it = 0; it < VPL; ++it)
+        if (live(it)) {
 #pragma unroll
-        for (int j = 0; j < 8; ++j) { const float d = v[it][j] - mean; sq += d * d; }
+          for (int j = 0; j < 8; ++j) { const float d = v[it][j] - mean; sq += d * d; }
+        }
       for (int o = lpr >> 1; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
       const float rstd = rsqrtf(sq * inv_c + eps);
 #pragma unroll
       for (int it = 0; it < VPL; ++it) {
+        if (!live(it)) continue;       // v[it] stays 0: nothing for the second LayerNorm's mean
         const int c = (it * lpr + l) << 3;
         const float4 f0 = *reinterpret_cast<const float4*>(&s_fs[c]);
         const float4 f1 = *reinterpret_cast<const float4*>(&s_fs[c + 4]);
@@ -271,9 +291,16 @@ ln_film_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, const float* 
         if (ok) {
           yb[static_cast<size_t>(row) * vpr + it * lpr + l] = make_uint4(o4[0], o4[1], o4[2], o4[3]);
           if (do_stats) {
-            if constexpr (PER_CH) {
+            if constexpr (STATS == LN_PER_CH) {
 #pragma unroll
-              for (int j = 0; j < 8; ++j) { as[j] += r[j]; aq[j] += r[j] * r[j]; }
+              for (int j = 0; j < 8; ++j) { as[8 * it + j] += r[j]; aq[8 * it + j] += r[j] * r[j]; }
+            } else if constexpr (STATS == LN_SPLIT) {
+#pragma unroll
+              for (int j = 0; j < 8; ++j) {
+                const bool first = j < head[it];
+                as[2 * it] += first ? r[j] : 0.f; aq[2 * it] += first ? r[j] * r[j] : 0.f;
+                as[2 * it + 1] += first ? 0.f : r[j]; aq[2 * it + 1] += first ? 0.f : r[j] * r[j];
+              }
             } else {
 #pragma unroll
               for (int j = 0; j < 8; ++j) { as[it] += r[j]; aq[it] += r[j] * r[j]; }
@@ -292,13 +319,16 @@ ln_film_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, const float* 
         float sq2 = 0.f;
 #pragma unroll
         for (int it = 0; it < VPL; ++it)
+          if (live(it)) {
 #pragma unroll
-          for (int j = 0; j < 8; ++j) { const float d = v[it][j] - mean2; sq2 += d * d; }
+            for (int j = 0; j < 8; ++j) { const float d = v[it][j] - mean2; sq2 += d * d; }
+          }
         for (int o = lpr >> 1; o > 0; o >>= 1) sq2 += __shfl_xor_sync(0xffffffffu, sq2, o);
         const float rstd2 = rsqrtf(sq2 * inv_c + eps2);
         if (ok) {
 #pragma unroll
           for (int it = 0; it < VPL; ++it) {
+            if (!live(it)) continue;
             uint4 o;
             o.x = pack_bf16((v[it][0] - mean2) * rstd2, (v[it][1] - mean2) * rstd2);
             o.y = pack_bf16((v[it][2] - mean2) * rstd2, (v[it][3] - mean2) * rstd2);
@@ -323,16 +353,32 @@ ln_film_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, const float* 
         aq[j] += __shfl_xor_sync(0xffffffffu, aq[j], o);
       }
     if (sub == 0) {
-      if constexpr (PER_CH) {
+      if constexpr (STATS == LN_PER_CH) {
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const int g = ((l << 3) + j) / gsz;
-          atomicAdd(&s_acc[2 * g], as[j]);
-          atomicAdd(&s_acc[2 * g + 1], aq[j]);
+        for (int it = 0; it < VPL; ++it) {
+          if (!live(it)) continue;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const int g = (((it * lpr + l) << 3) + j) / gsz;
+            atomicAdd(&s_acc[2 * g], as[8 * it + j]);
+            atomicAdd(&s_acc[2 * g + 1], aq[8 * it + j]);
+          }
+        }
+      } else if constexpr (STATS == LN_SPLIT) {
+#pragma unroll
+        for (int it = 0; it < VPL; ++it) {
+          if (!live(it)) continue;
+          const int g = ((it * lpr + l) << 3) / gsz;
+          atomicAdd(&s_acc[2 * g], as[2 * it]);
+          atomicAdd(&s_acc[2 * g + 1], aq[2 * it]);
+          if (head[it] < 8) {
+            atomicAdd(&s_acc[2 * g + 2], as[2 * it + 1]);
+            atomicAdd(&s_acc[2 * g + 3], aq[2 * it + 1]);
+          }
         }
       }
     }
-    if constexpr (!PER_CH) {
+    if constexpr (STATS == LN_GROUP) {
       // gsz/8 consecutive lanes of a row hold channels of the SAME group: reduce them with
       // shuffles so that one lane per (warp, group) touches the 2*groups shared bins (at
       // C = 1024 the per-lane version queued 16 lanes on every bin and tripled the kernel time)
@@ -348,7 +394,8 @@ ln_film_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, const float* 
             sq += __shfl_xor_sync(0xffffffffu, sq, o);
           }
         }
-        if (sub == 0 && (!tree || (l & (span - 1)) == 0)) {
+        // a masked lane is never the first of its span (lanes are masked from the top)
+        if (sub == 0 && live(it) && (!tree || (l & (span - 1)) == 0)) {
           const int g = ((it * lpr + l) << 3) / gsz;
           atomicAdd(&s_acc[2 * g], sa);
           atomicAdd(&s_acc[2 * g + 1], sq);
@@ -604,25 +651,17 @@ extern "C" int adp_ln_film_dual(const void* x, void* y, void* y2, const float* s
                                 int32_t C, int32_t groups, float eps, float eps2,
                                 adp_stream_t stream) {
   ADP_CHECK(x && y, "adp_ln_film: null pointer");
-  ADP_CHECK(C % 8 == 0, "adp_ln_film: C=%d must be a multiple of 8", C);
-  const int vpr = C / 8;
+  ADP_CHECK(C > 0 && C % 8 == 0 && C <= kMaxLnC, "adp_ln_film: C=%d must be a multiple of 8 and <= %d",
+            C, kMaxLnC);
   int lpr, vpl;
-  if (vpr <= 32) {
-    ADP_CHECK((vpr & (vpr - 1)) == 0, "adp_ln_film: C/8=%d must be a power of two (<=32)", vpr);
-    lpr = vpr; vpl = 1;
-  } else {
-    ADP_CHECK(vpr % 32 == 0 && vpr / 32 <= 4, "adp_ln_film: C=%d unsupported (need C%%256==0, "
-              "C<=1024)", C);
-    lpr = 32; vpl = vpr / 32;
-  }
-  bool per_ch = false;
+  const bool tail = ln_row_layout(C, &lpr, &vpl);
+  int mode = LN_GROUP;
   if (stats_out) {
     ADP_CHECK(groups > 0 && groups <= 64 && C % groups == 0, "adp_ln_film: groups=%d", groups);
     const int gsz = C / groups;
-    per_ch = gsz < 8;
-    ADP_CHECK(per_ch ? (vpl == 1) : (gsz % 8 == 0), "adp_ln_film: group size %d unsupported", gsz);
+    // gsz < 8 with at most 64 groups: C < 512, at most 2 vectors per lane
+    mode = gsz % 8 == 0 ? LN_GROUP : (vpl == 1 || gsz < 8) ? LN_PER_CH : LN_SPLIT;
   }
-  ADP_CHECK(C <= kMaxLnC, "adp_ln_film: C=%d > %d", C, kMaxLnC);
   const int unr = vpl <= 2 ? 2 : 1;
   const int rows_per_block = 8 * (32 / lpr) * unr;
   // deep levels have few rows: one pass per warp (all SMs busy) instead of two
@@ -631,15 +670,29 @@ extern "C" int adp_ln_film_dual(const void* x, void* y, void* y2, const float* s
   const uint4* xi = static_cast<const uint4*>(x);
   uint4* yo = static_cast<uint4*>(y);
   cudaStream_t s = as_stream(stream);
-#define ADP_LN(VPL, PC)                                                                         \
-  ADP_CUDA(launch_k(ln_film_kernel<VPL, PC, (VPL <= 2 ? 2 : 1)>, grid, dim3(256), (size_t)0, s, \
-                    xi, yo, scale_shift, (int)ss_stride, stats_out, (int)T, (int)C, (int)lpr,   \
+#define ADP_LN(VPL, M, TL)                                                                          \
+  ADP_CUDA(launch_k(ln_film_kernel<VPL, M, (VPL <= 2 ? 2 : 1), TL>, grid, dim3(256), (size_t)0, s,  \
+                    xi, yo, scale_shift, (int)ss_stride, stats_out, (int)T, (int)C, (int)lpr,       \
                     (int)groups, eps, static_cast<uint4*>(y2), eps2))
-  if (per_ch) ADP_LN(1, true);
-  else if (vpl == 1) ADP_LN(1, false);
-  else if (vpl == 2) ADP_LN(2, false);
-  else if (vpl == 3) ADP_LN(3, false);
-  else ADP_LN(4, false);
+#define ADP_LN_VPL(M, TL)                                                                           \
+  switch (vpl) {                                                                                    \
+    case 2: ADP_LN(2, M, TL); break;  case 3: ADP_LN(3, M, TL); break;                              \
+    case 4: ADP_LN(4, M, TL); break;  case 5: ADP_LN(5, M, TL); break;                              \
+    case 6: ADP_LN(6, M, TL); break;  case 7: ADP_LN(7, M, TL); break;                              \
+    default: ADP_LN(8, M, TL); break;                                                               \
+  }
+  if (mode == LN_PER_CH && vpl == 1) {
+    if (tail) ADP_LN(1, LN_PER_CH, true); else ADP_LN(1, LN_PER_CH, false);
+  } else if (mode == LN_PER_CH) {
+    if (tail) ADP_LN(2, LN_PER_CH, true); else ADP_LN(2, LN_PER_CH, false);
+  } else if (vpl == 1) {
+    if (tail) ADP_LN(1, LN_GROUP, true); else ADP_LN(1, LN_GROUP, false);
+  } else if (mode == LN_SPLIT) {
+    if (tail) { ADP_LN_VPL(LN_SPLIT, true) } else { ADP_LN_VPL(LN_SPLIT, false) }
+  } else {
+    if (tail) { ADP_LN_VPL(LN_GROUP, true) } else { ADP_LN_VPL(LN_GROUP, false) }
+  }
+#undef ADP_LN_VPL
 #undef ADP_LN
   ADP_LAUNCH_CHECK();
   return 0;

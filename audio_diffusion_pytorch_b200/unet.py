@@ -265,7 +265,7 @@ class _ForwardWalk:
             rs = None if mod else y_stats
             if narrow:
                 add(lambda: ops.narrow_conv(h, r, h_stats, g2, be2, w2, ip["b2"], G, residual=x, stats_out=rs))
-            elif net.fuse_groupnorm and not self.keep:
+            elif net.fuse_groupnorm and not self.keep and C <= net.MAX_FUSED_GN_C:
                 # ConvBlock = ONE kernel: GroupNorm+SiLU applied to the smem A tile
                 add(lambda: ops.conv_gemm(x, ip["w1"], h, c_in=C, n_valid=C, taps=(-1, 0, 1), bias=ip["b1"],
                                           stats=h_stats, groups=G, gn=(x_stats, g1, be1, G, net.GN_EPS)))
@@ -401,6 +401,13 @@ class B200UNet(nn.Module):
     MAX_BOUNDARY = 64           # in_channels (x + appended) and out_channels of the stem kernels
     MAX_STEM_IN = 128           # in_channels * factors[0]: inputs of one stem_in output position
     MAX_C0 = 256                # channels[0]
+    # channels[i] (8 or a multiple of 16), attention_heads * attention_features and
+    # embedding_features: the LayerNorm, GroupNorm-backward and bias-gradient row kernels hold a
+    # row of at most this many channels (csrc/rowwise.cu kMaxLnC, csrc/backward.cu kBwMaxC)
+    MAX_WIDTH = 2048
+    # widest level whose ConvBlocks fuse_groupnorm applies to: the conv GEMM's GroupNorm A transform
+    # keeps the coefficients of at most this many input channels (csrc/conv_gemm.cu s_coef)
+    MAX_FUSED_GN_C = 1024
 
     def __init__(self, dim: int, in_channels: int, channels: Sequence[int],
                  factors: Sequence[int], items: Sequence[int],
@@ -473,6 +480,20 @@ class B200UNet(nn.Module):
             f"{self.MAX_STEM_IN} inputs per output position"
         assert channels[0] <= self.MAX_C0, \
             f"channels[0]={channels[0]}: the stem kernels support a level 0 at most {self.MAX_C0} wide"
+        for i, c in enumerate(self.channels):
+            # the conv GEMM's K step is 16 channels; an 8-wide level runs on its own kernels
+            assert c == 8 or c % 16 == 0, \
+                f"channels[{i}]={c}: levels are 8 channels wide or a multiple of 16"
+            assert c <= self.MAX_WIDTH, \
+                f"channels[{i}]={c}: the row kernels support levels at most {self.MAX_WIDTH} wide"
+        if any(attentions) or any(cross_attentions):
+            assert attention_heads * attention_features <= self.MAX_WIDTH, \
+                f"attention_heads * attention_features = {attention_heads * attention_features}: the row " \
+                f"kernels support an attention width of at most {self.MAX_WIDTH}"
+        if exists(embedding_features) and (any(cross_attentions) or use_embedding_cfg):
+            assert embedding_features % 8 == 0 and embedding_features <= self.MAX_WIDTH, \
+                f"embedding_features={embedding_features}: the embedding LayerNorm supports a multiple of 8 " \
+                f"up to {self.MAX_WIDTH}"
 
         # registration order mirrors a_unet: time plugin, cfg plugin, then the recursive blocks
         self.time = TimeParams(modulation_features) if use_time_conditioning else None
@@ -501,7 +522,8 @@ class B200UNet(nn.Module):
         self.use_cuda_graph = True
         # GroupNorm+SiLU applied to the A tile inside the conv GEMM (adp_conv_gemm gn_*).
         # Bit-compatible with the two-kernel path, but every N tile repeats the transform of
-        # its A rows, so it only pays for N <= BN.  Off by default.
+        # its A rows, so it only pays for N <= BN.  Off by default.  Levels wider than
+        # MAX_FUSED_GN_C keep the two-kernel path under this flag.
         self.fuse_groupnorm = False
         # C = 32 / 64 ConvBlocks as ONE fused kernel (GroupNorm+SiLU -> conv3 -> +res -> LN/FiLM ->
         # statistics, csrc/mid_conv.cu) instead of three: those levels are HBM-bound
