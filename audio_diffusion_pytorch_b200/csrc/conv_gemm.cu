@@ -10,13 +10,16 @@
 //   W: packed weights [N][taps*C_in] -> K-major operand.
 //   A pipeline stage = KC chunks x {A box, one W box per tap} behind ONE full/empty mbarrier
 //      pair, so the issue loops pay one barrier round trip per KC*taps*4 MMAs.
-//   D: fp32 in registers.  Two consumer warpgroups own 64 tile rows each (m64nBNk16 per
+//   D: fp32 in registers.  Each consumer warpgroup owns 64 tile rows (m64nBNk16 per
 //      warpgroup); one MMA stage stays in flight while the next is issued.
-// Persistent: each CTA owns a contiguous range of tiles (n fastest).  Warp roles (288 threads):
-// warps 0-7 the two consumer warpgroups (MMA issue + epilogue straight from the accumulator
-// registers), warp 8 the TMA producer, which keeps filling the ring while the consumers drain
-// a tile.  GroupNorm partial sums of the output are reduced per warp into per-warp shared-memory
-// slots (per-lane registers for groups narrower than 8 channels); one global reduction per batch
+//   BM = 256 rows (four consumer warpgroups, BN = 64) loads each W slice half as often per FLOP
+//      as BM = 128; its A chunk is two boxes of 128 + span rows at rows 0 and 128 (a box holds at
+//      most 256 rows), whose span shared rows are written twice with the same data.
+// Persistent: each CTA owns a contiguous range of tiles (n fastest).  Warp roles: warps
+// 0..BM/16-1 the consumer warpgroups (MMA issue + epilogue straight from the accumulator
+// registers), warp BM/16 the TMA producer, which keeps filling the ring while the consumers
+// drain a tile (288 threads at BM = 128, 544 at BM = 256).  GroupNorm partial sums of the
+// output are reduced per warp into per-warp shared-memory slots (per-lane registers for groups narrower than 8 channels); one global reduction per batch
 // change.
 #include "common.cuh"
 #include "ptx.cuh"
@@ -25,15 +28,14 @@ namespace adp {
 
 // diagnostic switches (adp_debug_set): [2] 1 = weights are not written by the preceding kernels
 // (fetch them before griddepcontrol.wait); [3] CTAs/SM override; [5] KC override; [6] PDL;
-// [7] 1 = every BN <= 64 tile without the A transform takes the narrow-statistics variant,
-// whether or not its groups need it (compares that variant with the unserialized one)
+// [4] tile rows: 0 = the tile plan, 128 = 128-row tiles only, 256 = 256-row tiles (an error
+// where the kernel has none); [7] 1 = every BN <= 64 tile without the A transform takes the
+// narrow-statistics variant, whether or not its groups need it (compares that variant with the
+// unserialized one)
 int g_debug[8] = {0, 0, 0, 0, 0, 0, 0, 0};
 
-constexpr int kBM = 128;
 constexpr int kMaxStages = 8;
 constexpr int kMaxGroups = 8;      // GroupNorm groups handled by the fused statistics
-constexpr int kConsumers = 256;    // two warpgroups
-constexpr int kGemmThreads = kConsumers + 32;
 constexpr int kSmemPerSM = 228 * 1024;
 constexpr int kSmemPerBlock = 227 * 1024;
 
@@ -67,12 +69,13 @@ struct TileInfo {
   int b, t0, n0, phase, ch0, ntaps, min_off;
 };
 
+template <int BM>
 __device__ __forceinline__ TileInfo tile_info(const Gemm2Params& p, int tile, int BN) {
   TileInfo ti;
   const int m_tile = tile / p.n_tiles_n;
   const int n_tile = tile - m_tile * p.n_tiles_n;
   ti.b = m_tile / p.tiles_per_batch;
-  ti.t0 = (m_tile - ti.b * p.tiles_per_batch) * kBM;
+  ti.t0 = (m_tile - ti.b * p.tiles_per_batch) * BM;
   ti.n0 = n_tile * BN;
   ti.phase = ti.n0 / p.n_pad;
   ti.ch0 = ti.n0 - ti.phase * p.n_pad;
@@ -107,12 +110,14 @@ __device__ __forceinline__ float silu_tanh(float z) {
 struct WarpStats {
   int cur_g = -1;
   float s = 0.f, q = 0.f;
-  __device__ __forceinline__ void flush(float (*slots)[8], int w, int lane) {
+  template <int NW>
+  __device__ __forceinline__ void flush(float (*slots)[NW], int w, int lane) {
     const float ws = warp_sum(s), wq = warp_sum(q);   // zero while cur_g < 0
     if (lane == 0 && cur_g >= 0) { slots[2 * cur_g][w] += ws; slots[2 * cur_g + 1][w] += wq; }
     s = 0.f; q = 0.f;
   }
-  __device__ __forceinline__ void add(float v, int g, float (*slots)[8], int w, int lane) {
+  template <int NW>
+  __device__ __forceinline__ void add(float v, int g, float (*slots)[NW], int w, int lane) {
     if (g != cur_g) { flush(slots, w, lane); cur_g = g; }
     s += v; q += v * v;
   }
@@ -130,7 +135,8 @@ struct NarrowStats {
   int ch0 = -1;
   float s[4] = {0.f, 0.f, 0.f, 0.f}, q[4] = {0.f, 0.f, 0.f, 0.f};
   __device__ __forceinline__ void add(int k, float v) { s[k] += v; q[k] += v * v; }
-  __device__ __forceinline__ void flush(float (*slots)[8], int w, int lane, int shift, int groups) {
+  template <int NW>
+  __device__ __forceinline__ void flush(float (*slots)[NW], int w, int lane, int shift, int groups) {
     if (ch0 >= 0) {
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
@@ -161,17 +167,26 @@ struct NarrowStats {
 // channels.  They fit only in BN <= 64 tiles without the A transform, and only launches whose
 // groups need them take this variant: ptxas serializes its wgmma instructions (C7520), which
 // the variant without them does not.
-template <int BN, int SW, bool XF, bool NARROW>
-__global__ void __launch_bounds__(kGemmThreads, BN <= 32 ? 3 : (BN <= 64 ? 2 : 1))
+// BM = 256 runs BN = 64 only: each quarter of the register file serves 5 of its 17 warps, which
+// caps a thread at 96 registers, and the BN = 128 tile (64 accumulators) spills there.  The A
+// transform and the narrow statistics stay 128-row.
+template <int BM> constexpr int gemm_threads() { return 2 * BM + 32; }
+
+template <int BM, int BN, int SW, bool XF, bool NARROW>
+__global__ void __launch_bounds__(gemm_threads<BM>(), BM == 256 ? 1 : (BN <= 32 ? 3 : (BN <= 64 ? 2 : 1)))
 conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
                   const Gemm2Params p) {
   static_assert(!NARROW || (BN <= 64 && !XF), "narrow statistics registers: BN <= 64 without XF");
+  static_assert(BM == 128 || (BM == 256 && BN == 64 && !XF && !NARROW),
+                "256-row tiles: BN = 64, without the A transform or the narrow statistics");
   constexpr int BK = SW / 2;
   constexpr int NACC = BN / 2;                    // accumulator registers per consumer thread
+  constexpr int kConsumers = 2 * BM;              // BM / 64 warpgroups
+  constexpr int kConsumerWarps = BM / 16;         // the producer is warp kConsumerWarps
   constexpr uint32_t kWTapBytes = BN * SW;        // bytes one W box writes
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t full_bar[kMaxStages], empty_bar[kMaxStages];
-  __shared__ float s_part[2 * kMaxGroups][8];     // (sum, sumsq) per group of the current batch, per consumer warp
+  __shared__ float s_part[2 * kMaxGroups][kConsumerWarps];   // (sum, sumsq) per group of the current batch, per consumer warp
   __shared__ __align__(16) float s_coef[XF ? 2 * 1024 : 4];   // (a, d) per input channel of the current batch
 
   pdl_launch_dependents();
@@ -184,9 +199,9 @@ conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   int tile_end = tile_begin + p.tiles_per_cta;
   if (tile_end > p.total_tiles) tile_end = p.total_tiles;
 
-  if (threadIdx.x < 2 * kMaxGroups * 8) (&s_part[0][0])[threadIdx.x] = 0.f;
-  if (warp == 8 && lane == 0) {
-    for (int s = 0; s < p.n_stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
+  if (threadIdx.x < 2 * kMaxGroups * kConsumerWarps) (&s_part[0][0])[threadIdx.x] = 0.f;
+  if (warp == kConsumerWarps && lane == 0) {
+    for (int s = 0; s < p.n_stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumerWarps); }
     fence_mbar_init();
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmW);
@@ -198,9 +213,9 @@ conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   // host only while it captures an inference graph): the producer puts the weight boxes of the
   // first ring stages in flight BEFORE waiting, taking the first-load latency off the
   // critical path of the many short GEMMs that follow an elementwise kernel.
-  if (warp == 8) {
+  if (warp == kConsumerWarps) {
     // ---------------------------------------------------------------------- TMA producer
-    const uint32_t a_bytes = static_cast<uint32_t>(p.a_rows) * SW;
+    const uint32_t a_bytes = static_cast<uint32_t>(BM / 128) * p.a_rows * SW;   // A boxes per chunk
     const int total_it = (tile_end - tile_begin) * p.k_stages;
     int early = 0;
     if (p.early_w) {
@@ -208,7 +223,7 @@ conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       if (elect_one()) {
         int tile = tile_begin, ks = 0;
         for (int it = 0; it < early; ++it) {          // stage `it` of the (still empty) ring
-          const TileInfo ti = tile_info(p, tile, BN);
+          const TileInfo ti = tile_info<BM>(p, tile, BN);
           uint8_t* st = ring + it * p.stage_bytes;
           mbar_arrive_expect_tx(&full_bar[it], static_cast<uint32_t>(p.kc) * (a_bytes + ti.ntaps * kWTapBytes));
           for (int c = 0; c < p.kc; ++c) {
@@ -226,7 +241,7 @@ conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     int s = 0, it = 0;
     uint32_t ph = 0;
     for (int tile = tile_begin; tile < tile_end; ++tile) {
-      const TileInfo ti = tile_info(p, tile, BN);
+      const TileInfo ti = tile_info<BM>(p, tile, BN);
       const uint32_t tx = static_cast<uint32_t>(p.kc) * (a_bytes + ti.ntaps * kWTapBytes);
       for (int ks = 0; ks < p.k_stages; ++ks, ++it) {
         const bool armed = it < early;                 // barrier armed + weights already issued
@@ -237,6 +252,8 @@ conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           for (int c = 0; c < p.kc; ++c) {
             const int k0 = (ks * p.kc + c) * BK;
             tma_load_3d(st + c * p.a_sub_bytes, &tmA, &full_bar[s], k0, ti.t0 + ti.min_off, ti.b);
+            if constexpr (BM == 256)
+              tma_load_3d(st + c * p.a_sub_bytes + 128 * SW, &tmA, &full_bar[s], k0, ti.t0 + ti.min_off + 128, ti.b);
             if (armed) continue;
             uint8_t* wdst = st + p.kc * p.a_sub_bytes + c * p.max_taps * p.w_sub_bytes;
             for (int tap = 0; tap < ti.ntaps; ++tap)
@@ -252,7 +269,7 @@ conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
   // ------------------------------------------------------------------------------ consumers
   pdl_wait();
-  const int tid = threadIdx.x;                 // 0..255
+  const int tid = threadIdx.x;                 // 0..kConsumers-1
   const int wg = tid >> 7;                     // warpgroup: tile rows [64*wg, 64*wg + 64)
   const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // fragment rows r0 and r0 + 8
   const int cq = 2 * (lane & 3);               // fragment column offset inside each 8-column block
@@ -264,7 +281,7 @@ conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   NarrowStats nar_st;
   int cur_b = -1, coef_b = -1;
 
-  auto publish_stats = [&](int b_done) {       // all 256 consumer threads
+  auto publish_stats = [&](int b_done) {       // all consumer threads
     acc_st.flush(s_part, warp, lane);
     acc_st.cur_g = -1;
     if (narrow) nar_st.flush(s_part, warp, lane, p.group_shift, p.groups);
@@ -272,7 +289,7 @@ conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     if (tid < 2 * p.groups) {
       float tot = 0.f;
 #pragma unroll
-      for (int w = 0; w < 8; ++w) { tot += s_part[tid][w]; s_part[tid][w] = 0.f; }
+      for (int w = 0; w < kConsumerWarps; ++w) { tot += s_part[tid][w]; s_part[tid][w] = 0.f; }
       if (tot != 0.f) atomicAdd(p.stats + static_cast<size_t>(b_done) * 2 * p.groups + tid, static_cast<double>(tot));
     }
     named_bar_sync(1, kConsumers);
@@ -288,7 +305,7 @@ conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   int s = 0;
   uint32_t ph = 0;
   for (int tile = tile_begin; tile < tile_end; ++tile) {
-    const TileInfo ti = tile_info(p, tile, BN);
+    const TileInfo ti = tile_info<BM>(p, tile, BN);
     if constexpr (XF) {
       if (ti.b != coef_b) {     // (a, d) of every input channel for this batch element, once
         named_bar_sync(1, kConsumers);          // previous batch's coefficients no longer in use
@@ -463,19 +480,20 @@ conv_gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (do_stats && cur_b >= 0) publish_stats(cur_b);
 }
 
-template <int BN, int SW, bool XF, bool NARROW>
+template <int BM, int BN, int SW, bool XF, bool NARROW>
 static int launch_gemm2(const adp_conv_gemm_args& a, cudaStream_t stream) {
   constexpr int BK = SW / 2;
-  auto kernel = conv_gemm2_kernel<BN, SW, XF, NARROW>;
-  const int tiles_per_batch = (a.T + kBM - 1) / kBM;
+  constexpr int kThreads = gemm_threads<BM>();
+  auto kernel = conv_gemm2_kernel<BM, BN, SW, XF, NARROW>;
+  const int tiles_per_batch = (a.T + BM - 1) / BM;
   const bool up = a.up_factor > 1;
   const int max_taps = up ? 2 : a.ntaps;
   const int span = up ? 1 : a.ntaps - 1;
-  const int a_rows = kBM + span;
+  const int a_rows = 128 + span;            // rows per A box
   const int k_chunks = a.c_in / BK;
 
   Gemm2Params p;
-  p.a_sub_bytes = (a_rows * SW + 1023) / 1024 * 1024;
+  p.a_sub_bytes = ((BM + span) * SW + 1023) / 1024 * 1024;
   p.w_sub_bytes = (BN * SW + 1023) / 1024 * 1024;
   p.max_taps = max_taps;
   const int chunk_bytes = p.a_sub_bytes + max_taps * p.w_sub_bytes;
@@ -484,7 +502,8 @@ static int launch_gemm2(const adp_conv_gemm_args& a, cudaStream_t stream) {
   // when 2-3 CTAs share an SM; long-K tiles want deep rings of fat stages instead.
   const int w_iters = k_chunks * max_taps;
   int occ = 1;
-  if (BN <= 64 && w_iters <= 8) occ = 3;
+  if (BM == 256) occ = 1;
+  else if (BN <= 64 && w_iters <= 8) occ = 3;
   else if (BN <= 128 && w_iters <= 12) occ = 2;
   if (XF && occ > (BN <= 64 ? 2 : 1)) occ = BN <= 64 ? 2 : 1;
   if (g_debug[3] > 0) occ = g_debug[3];
@@ -534,7 +553,7 @@ static int launch_gemm2(const adp_conv_gemm_args& a, cudaStream_t stream) {
   static SmemAttrCache smem_cache;
   ADP_CUDA(ensure_dyn_smem(kernel, smem, smem_cache));
   int occ_hw = 1;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_hw, kernel, kGemmThreads, smem) != cudaSuccess ||
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_hw, kernel, kThreads, smem) != cudaSuccess ||
       occ_hw < 1)
     occ_hw = 1;
   if (occ > occ_hw) occ = occ_hw;
@@ -575,33 +594,43 @@ static int launch_gemm2(const adp_conv_gemm_args& a, cudaStream_t stream) {
   int grid = p.total_tiles < slots ? p.total_tiles : slots;
   p.tiles_per_cta = (p.total_tiles + grid - 1) / grid;
   grid = (p.total_tiles + p.tiles_per_cta - 1) / p.tiles_per_cta;
-  ADP_CUDA(launch_k(kernel, dim3(grid), dim3(kGemmThreads), smem, stream, tmA, tmW, p));
+  ADP_CUDA(launch_k(kernel, dim3(grid), dim3(kThreads), smem, stream, tmA, tmW, p));
   ADP_LAUNCH_CHECK();
   return 0;
+}
+
+// GroupNorm groups of 1, 2 or 4 channels need the per-lane statistics registers
+static bool needs_narrow(const adp_conv_gemm_args& a) {
+  const int group_size = a.stats ? a.n_valid / a.groups : 0;
+  return group_size == 1 || group_size == 2 || group_size == 4 || g_debug[7] != 0;
 }
 
 template <int SW>
 static int dispatch_bn2(const adp_conv_gemm_args& a, int bn, cudaStream_t s) {
   if (a.gn_stats) {
     switch (bn) {
-      case 16: return launch_gemm2<16, SW, true, false>(a, s);
-      case 32: return launch_gemm2<32, SW, true, false>(a, s);
-      case 64: return launch_gemm2<64, SW, true, false>(a, s);
-      case 128: return launch_gemm2<128, SW, true, false>(a, s);
-      case 256: return launch_gemm2<256, SW, true, false>(a, s);
+      case 16: return launch_gemm2<128, 16, SW, true, false>(a, s);
+      case 32: return launch_gemm2<128, 32, SW, true, false>(a, s);
+      case 64: return launch_gemm2<128, 64, SW, true, false>(a, s);
+      case 128: return launch_gemm2<128, 128, SW, true, false>(a, s);
+      case 256: return launch_gemm2<128, 256, SW, true, false>(a, s);
     }
   }
-  // GroupNorm groups of 1, 2 or 4 channels need the per-lane statistics registers
-  const int group_size = a.stats ? a.n_valid / a.groups : 0;
-  const bool narrow = group_size == 1 || group_size == 2 || group_size == 4 || g_debug[7] != 0;
+  const bool narrow = needs_narrow(a);
   switch (bn) {
-    case 16: return narrow ? launch_gemm2<16, SW, false, true>(a, s) : launch_gemm2<16, SW, false, false>(a, s);
-    case 32: return narrow ? launch_gemm2<32, SW, false, true>(a, s) : launch_gemm2<32, SW, false, false>(a, s);
-    case 64: return narrow ? launch_gemm2<64, SW, false, true>(a, s) : launch_gemm2<64, SW, false, false>(a, s);
-    case 128: return launch_gemm2<128, SW, false, false>(a, s);
-    case 256: return launch_gemm2<256, SW, false, false>(a, s);
+    case 16: return narrow ? launch_gemm2<128, 16, SW, false, true>(a, s) : launch_gemm2<128, 16, SW, false, false>(a, s);
+    case 32: return narrow ? launch_gemm2<128, 32, SW, false, true>(a, s) : launch_gemm2<128, 32, SW, false, false>(a, s);
+    case 64: return narrow ? launch_gemm2<128, 64, SW, false, true>(a, s) : launch_gemm2<128, 64, SW, false, false>(a, s);
+    case 128: return launch_gemm2<128, 128, SW, false, false>(a, s);
+    case 256: return launch_gemm2<128, 256, SW, false, false>(a, s);
   }
   return set_error("adp_conv_gemm: unsupported N tile %d", bn);
+}
+
+// 256-row tiles exist for 64-channel chunks (SW = 128) and BN = 64, without the A transform or
+// the narrow statistics, and at T >= 256 (tiles never span batch elements)
+static bool has_256_rows(const adp_conv_gemm_args& a) {
+  return a.n_pad % 64 == 0 && a.c_in % 64 == 0 && !a.gn_stats && !needs_narrow(a) && a.T >= 256;
 }
 
 }  // namespace adp
@@ -615,6 +644,8 @@ extern "C" int adp_debug_set(int key, int value) {
     return 0;
   }
   if (key < 0 || key >= 8) return adp::set_error("adp_debug_set: bad key %d", key);
+  if (key == 4 && value != 0 && value != 128 && value != 256)
+    return adp::set_error("adp_debug_set: key 4 takes 0, 128 or 256");
   adp::g_debug[key] = value;
   if (key == 6) adp::g_pdl = value;
   return 0;
@@ -660,7 +691,7 @@ extern "C" int adp_conv_gemm(const adp_conv_gemm_args* args, adp_stream_t stream
               "adp_conv_gemm: groups=%d n_valid=%d (fused statistics handle <= %d groups)",
               a.groups, a.n_valid, kMaxGroups);
   }
-  // N tile: persistent CTAs take care of SM fill.  Tiles with a long reduction (taps * c_in >
+  // Tile plan.  N tile of the 128-row tiles: persistent CTAs take care of SM fill.  Tiles with a long reduction (taps * c_in >
   // 1024) prefer 128 columns: each A box then feeds twice the MMAs.  Shorter ones prefer 64,
   // which gives the persistent grid twice the tiles and more CTAs per SM where the ring allows
   // (measured in isolation on H100, cfg2 shapes: the L3 / L4 convs run 18-27 % and the q|k|v
@@ -668,7 +699,7 @@ extern "C" int adp_conv_gemm(const adp_conv_gemm_args* args, adp_stream_t stream
   // 4-8 % slower at 64).  The XF tiles keep 128 (not measured at 64).
   int bn = a.block_n;
   if (bn == 0) {
-    const long m_tiles = (long)a.B * ((a.T + kBM - 1) / kBM);
+    const long m_tiles = (long)a.B * ((a.T + 127) / 128);
     const int k_per_tile = (a.up_factor > 1 ? 2 : a.ntaps) * a.c_in;
     const int widest = !a.gn_stats && k_per_tile <= 1024 ? 64 : 128;
     bn = 16;
@@ -678,8 +709,23 @@ extern "C" int adp_conv_gemm(const adp_conv_gemm_args* args, adp_stream_t stream
       if (tiles >= 96 || cand <= 64) { bn = cand; break; }
     }
   }
+  // 256 x 64 replaces 128 x 128 where it exists: the same MMAs per tile and the same tile
+  // count, with 256 + span A rows and 64 weight rows per tap loaded per tile instead of
+  // 128 + span and 128 (measured on H100, DESIGN.md section 8: the k=3 convs with
+  // c_in >= 512 run 7-23 % faster).  The 128 x 64 tiles stay: 256 x 64 halves their weight
+  // loads too, but the k=1 projections ran 5-44 % slower on it.  An explicit N tile keeps 128
+  // rows unless adp_debug_set(4, 256) asks for 256.
+  bool rows256 = false;
+  if (g_debug[4] == 256) {
+    ADP_CHECK(has_256_rows(a) && (a.block_n == 0 || a.block_n == 64),
+              "adp_conv_gemm: no 256-row tile for block_n=%d c_in=%d T=%d", a.block_n, a.c_in, a.T);
+    rows256 = true;
+  } else if (a.block_n == 0 && g_debug[4] != 128) {
+    rows256 = bn == 128 && has_256_rows(a);
+  }
   ADP_CHECK(a.n_pad % bn == 0, "adp_conv_gemm: N tile %d does not divide n_pad %d", bn, a.n_pad);
   cudaStream_t s = as_stream(stream);
+  if (rows256) return launch_gemm2<256, 64, 128, false, false>(a, s);
   if (a.c_in % 64 == 0) return dispatch_bn2<128>(a, bn, s);
   if (a.c_in % 32 == 0) return dispatch_bn2<64>(a, bn, s);
   return dispatch_bn2<32>(a, bn, s);
