@@ -340,7 +340,11 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
     finals: List = []                      # closures turning packed grads into PyTorch layout
     # one flat fp32 arena for every gradient accumulator: a single memset per backward
     n_param = sum(p.numel() for p in net.parameters())
-    flat = torch.zeros(int(1.25 * n_param) + 64 * (4 * n_param // 1000 + 4096), device=dev)
+    # the repeated attention items of a level (counts > 1) each add a projection-gradient scratch
+    # smaller than their parameters on top of their gradients
+    n_extra = sum(p.numel() for lv in levels for it in (*lv.items_down, *lv.items_up)
+                  for am in (it.attentions()[1:] + it.crosses()[1:]) for p in am.parameters())
+    flat = torch.zeros(int(1.25 * n_param) + n_extra + 64 * (4 * n_param // 1000 + 4096), device=dev)
     cursor = [0]
 
     specs: Dict[int, tuple] = {}           # id(param) -> (arena start, numel, view shape, permutation)
@@ -449,8 +453,8 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
                 return dx
         return bwd
 
-    # ---- backward of one [ResnetItem, ModulationItem, InjectChannelsItem?, AttentionItem?,
-    # CrossAttentionItem?] from the tensors of the walk's forward
+    # ---- backward of one [ResnetItem, ModulationItem, InjectChannelsItem?] + AttentionItems +
+    # CrossAttentionItems from the tensors of the walk's forward
     def item_backward(rec, ip: Dict, im, C: int, Tl: int, li: int):
         res, inj, atts = rec
         r_ = im.resnet
@@ -509,9 +513,10 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
             # d context is summed over the items of this depth (in place through the residual)
             chain.append(lambda d_out: inject_bwd(d_out, inj["x"], ctxb, dctxb, wd_x, wd_c, gw_inj, db_inj, dyi,
                                                   n_ctx))
-        kinds = [(kind, am) for kind, am in (("att", im.attention), ("cross", im.cross)) if am is not None]
-        for a, (kind, am) in zip(atts, kinds):
-            chain.append(attention_backward(a, am, kind == "cross", Tl, C))
+        # every AttentionItem, then every CrossAttentionItem (the walk's order); run in reverse
+        ams = [(False, am) for am in im.attentions()] + [(True, am) for am in im.crosses()]
+        for a, (cross, am) in zip(atts, ams):
+            chain.append(attention_backward(a, am, cross, Tl, C))
 
         def item_bwd(dy):
             for fn in reversed(chain):

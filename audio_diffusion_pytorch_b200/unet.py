@@ -67,10 +67,13 @@ class AttentionParams(nn.Module):
 
 
 class ItemParams(nn.Module):
-    """One repetition of [ResnetItem, ModulationItem, InjectChannelsItem?, AttentionItem?,
-    CrossAttentionItem?] (reference components.py:89-95)."""
+    """One repetition of [ResnetItem, ModulationItem?, InjectChannelsItem?] + [AttentionItem] * att
+    + [CrossAttentionItem] * cross (reference components.py:89-95).  The first attention and
+    cross-attention are `attention` / `cross`; further ones follow each in `extra_attention` /
+    `extra_cross`, registered only when a count exceeds 1 (a net with counts <= 1 keeps the
+    state_dict keys it always had)."""
 
-    def __init__(self, channels: int, groups: int, features: int, att: bool, cross: bool,
+    def __init__(self, channels: int, groups: int, features: int, att: int, cross: int,
                  head_features: Optional[int], heads: Optional[int],
                  embedding_features: Optional[int], context: int = 0, modulation: bool = True):
         super().__init__()
@@ -78,9 +81,25 @@ class ItemParams(nn.Module):
         self.modulation = ModulationParams(channels, features) if modulation else None
         # a_unet InjectChannelsItem: Conv1d(C + ctx -> C, k=1) over cat([x, channels[depth]]), + x
         self.inject = nn.Conv1d(channels + context, channels, 1) if context > 0 else None
-        self.attention = AttentionParams(channels, head_features, heads) if att else None
+        self.attention = AttentionParams(channels, head_features, heads) if att > 0 else None
+        if att > 1:
+            self.extra_attention = nn.ModuleList(
+                [AttentionParams(channels, head_features, heads) for _ in range(att - 1)])
         self.cross = (AttentionParams(channels, head_features, heads, embedding_features)
-                      if cross else None)
+                      if cross > 0 else None)
+        if cross > 1:
+            self.extra_cross = nn.ModuleList(
+                [AttentionParams(channels, head_features, heads, embedding_features) for _ in range(cross - 1)])
+
+    def attentions(self) -> List[AttentionParams]:
+        """The item's AttentionItems in a_unet order."""
+        first = [self.attention] if self.attention is not None else []
+        return first + list(getattr(self, "extra_attention", []))
+
+    def crosses(self) -> List[AttentionParams]:
+        """The item's CrossAttentionItems in a_unet order (after every AttentionItem)."""
+        first = [self.cross] if self.cross is not None else []
+        return first + list(getattr(self, "extra_cross", []))
 
 
 class LevelParams(nn.Module):
@@ -214,23 +233,25 @@ class _ForwardWalk:
         return x, x_stats, recs
 
     def item(self, x: Tensor, x_stats: Tensor, ip: Dict, C: int, Tl: int, li: int, want_stats: bool):
-        """[ResnetItem, ModulationItem?, InjectChannelsItem?, AttentionItem?, CrossAttentionItem?];
-        returns (output, its statistics, (resnet record, inject record or None, attention records))."""
-        has_att, has_cross, has_inj = "att" in ip, "cross" in ip, "inj" in ip
-        y_stats = self.new_stats() if (want_stats and not (has_att or has_cross or has_inj)) else None
-        res = self._resnet(x, x_stats, ip, C, Tl, y_stats, (has_att or has_cross) and not has_inj)
+        """[ResnetItem, ModulationItem?, InjectChannelsItem?] + AttentionItems + CrossAttentionItems;
+        returns (output, its statistics, (resnet record, inject record or None, attention records)).
+        Only the item's last launch writes the statistics of the next GroupNorm; the first attention
+        reads the pre-norm of the Modulation pass, every later one runs its own LayerNorm."""
+        chain = [(False, ap) for ap in ip.get("att", [])] + [(True, ap) for ap in ip.get("cross", [])]
+        has_inj = "inj" in ip
+        y_stats = self.new_stats() if (want_stats and not (chain or has_inj)) else None
+        res = self._resnet(x, x_stats, ip, C, Tl, y_stats, bool(chain) and not has_inj)
         x, x_stats, xn = res["y"], y_stats, res["xn"]
         inj = None
         if has_inj:
-            x_stats = self.new_stats() if (want_stats and not (has_att or has_cross)) else None
+            x_stats = self.new_stats() if (want_stats and not chain) else None
             inj = self._inject(x, ip["inj"], C, Tl, li, x_stats)
             x = inj["y"]
         atts = []
-        for kind in ("att", "cross"):
-            if kind in ip:
-                x_stats = self.new_stats() if (want_stats and (kind == "cross" or not has_cross)) else None
-                atts.append(self._attention(x, xn, ip[kind], kind == "cross", C, Tl, x_stats))
-                x, xn = atts[-1]["y"], None
+        for j, (cross, ap) in enumerate(chain):
+            x_stats = self.new_stats() if (want_stats and j == len(chain) - 1) else None
+            atts.append(self._attention(x, xn, ap, cross, C, Tl, x_stats))
+            x, xn = atts[-1]["y"], None
         return x, x_stats, (res, inj, atts)
 
     def _resnet(self, x: Tensor, x_stats: Tensor, ip: Dict, C: int, Tl: int, y_stats: Optional[Tensor],
@@ -429,6 +450,9 @@ class B200UNet(nn.Module):
         context_channels = default(context_channels, [0] * n)
         xs = (channels, factors, items, attentions, cross_attentions, context_channels)
         assert all(len(x) == n for x in xs)                       # reference components.py:61
+        # a_unet repeats each item as `[Item] * count`: True is one item, 0 / False / negative none
+        attentions = [max(0, int(a)) for a in attentions]
+        cross_attentions = [max(0, int(a)) for a in cross_attentions]
         assert dim == 1, "the CUDA path implements the 1-D (waveform) U-Net"
         if use_embedding_cfg:                                     # components.py:66-68
             assert exists(embedding_max_length), "use_embedding_cfg requires embedding_max_length"
@@ -507,7 +531,7 @@ class B200UNet(nn.Module):
             out_ch = self.out_channels if i == 0 else in_ch
             return LevelParams(in_ch, out_ch, channels[i], factors[i], items[i], build(i + 1),
                                groups=resnet_groups, features=modulation_features,
-                               att=bool(attentions[i]), cross=bool(cross_attentions[i]),
+                               att=attentions[i], cross=cross_attentions[i],
                                head_features=attention_features, heads=attention_heads,
                                embedding_features=embedding_features, context=context_channels[i],
                                modulation=use_modulation)
@@ -740,10 +764,12 @@ class B200UNet(nn.Module):
                 wc[:, :ctx] = wi[:, C_:]
                 d["inj"] = {"w_x": ops.pack_linear(wi[:, :C_]), "w_c": ops.pack_linear(wc),
                             "b": f32(it.inject.bias)}
+            # one pack per attention item, in order; each cross-attention projects the context
+            # through its own K|V weights (its norm_context affine folded in)
             if it.attention is not None:
-                d["att"] = pack_att(it.attention, True)
+                d["att"] = [pack_att(a, True) for a in it.attentions()]
             if it.cross is not None:
-                d["cross"] = pack_att(it.cross, False)
+                d["cross"] = [pack_att(a, False) for a in it.crosses()]
             return d
 
         P["levels"] = []
