@@ -28,17 +28,19 @@ values: conv of |a| with |w|, P |V|, ...):
                    absref = the same sum over absolute terms; the GroupNorm backward sums are taken
                    over dxh as stored, as statistics are over the stored output
     attention lse  the fp32 bound + 2^-9 (LSE_FLOOR: the row sum is taken over P rounded to bf16)
-    copies         bitwise
+    log mel        the fp32 bound b of the linear value carried through log(max(., 1e-5)): b divided
+                   by max(ref - b, 1e-5), + 1e-5 |ref| of the log
+    copies         bitwise (the step selector's rows, arv_step's sigma channel, and inpaint_blend's
+                   positions outside the mask, which hold the sampler's value)
 Every launch also checks that read-only arguments are bitwise unchanged and that no byte of a
 written tensor's storage outside the written view changed -- the rest of the gradient arena
 included, every accumulator being a view of that one storage.
 
-Checked kinds are the launches of the inference, sampling and training programs (forward, fused
-loss and backward; tau = 2^-8 also for attention_bwd, which rounds P and dS to bf16) and
-fir_resample, whose output is the tensor it returns.  The vocoder front-end (to_flat, to_flat_bwd,
-mel_spectrogram) and the inpainting / autoregressive sampler steps (inpaint_blend, arv_step) are
-listed in UNCHECKED, and a program that reaches one of them under Shadow fails instead of passing
-unchecked.
+Checked kinds are every launching function of `ops` (UNCHECKED is empty): the launches of the
+inference, sampling and training programs (forward, fused loss and backward; tau = 2^-8 also for
+attention_bwd, which rounds P and dS to bf16); the tensors fir_resample, mel_spectrogram, to_flat
+and to_flat_bwd allocate and return (RESULT); and the in-place sampler steps of VSampler's generic
+loop (sampler_step), VInpainter (inpaint_blend) and ARVSampler (arv_step).
 """
 import inspect
 import math
@@ -64,11 +66,7 @@ ACC_EPS = 2.0 ** -23              # an fp32 accumulator's own rounding, per unit
 SIDE_CHUNK = 1 << 28              # bytes compared at a time by the side-effect check
 ROW_TILE = 64                    # rows left stale by the mutation: half the conv GEMM's 128-row M tile
 
-UNCHECKED = {
-    # the vocoder front-end (cfg5) and the two sampler loops outside VSampler
-    "to_flat": "vocoder front-end", "to_flat_bwd": "vocoder front-end (training)",
-    "mel_spectrogram": "vocoder front-end", "inpaint_blend": "VInpainter loop", "arv_step": "ARVSampler loop",
-}
+UNCHECKED: Dict[str, str] = {}          # launching functions of `ops` without a checker: none
 
 
 class CheckError(AssertionError):
@@ -87,11 +85,16 @@ def launching_functions() -> List[str]:
 # ------------------------------------------------------------------------------ outputs
 class Val:
     """A stored output: `view(args)` is the written view; ref / absref fp64 of its shape (or a
-    callable(post args) -> (ref, absref) when the reference reads another output of the launch)."""
+    callable(post args) -> (ref, absref) when the reference reads another output of the launch).
+    keep: a bool mask of the view's positions the launch must leave bitwise unchanged (an in-place
+    update of part of a tensor).  of: the argument the view belongs to (default: name), when one
+    argument has several outputs."""
 
-    def __init__(self, name, view, ref, absref=None, tau=TAU_FP32_ACC, exact=False, floor=0.0):
+    def __init__(self, name, view, ref, absref=None, tau=TAU_FP32_ACC, exact=False, floor=0.0, keep=None,
+                 of=None):
         self.name, self.view, self.ref, self.absref, self.tau, self.exact = name, view, ref, absref, tau, exact
         self.acc, self.floor = False, floor      # floor: an absolute term of the bound (see LSE_FLOOR)
+        self.keep, self.of = keep, of or name
 
 
 class Stat:
@@ -99,7 +102,7 @@ class Stat:
 
     def __init__(self, name, view, src, groups):
         self.name, self.view, self.src, self.groups = name, view, src, groups
-        self.acc = True
+        self.acc, self.of = True, name
 
 
 class Acc:
@@ -110,7 +113,7 @@ class Acc:
 
     def __init__(self, name, view, ref, absref=None):
         self.name, self.view, self.ref, self.absref = name, view, ref, absref
-        self.acc, self.exact = True, False
+        self.acc, self.exact, self.of, self.keep = True, False, name, None
 
 
 def arg(name):
@@ -713,9 +716,8 @@ def c_ln_fold_bwd(a, ctx):
 
 
 def _fir_result(a):
-    """The tensor fir_resample allocates and returns."""
     n = a["t_out"] if a["adjoint_of"] is None else a["adjoint_of"]
-    return torch.empty(a["x"].shape[0], n, dtype=torch.float32, device=a["x"].device)
+    return {"_result": (a["x"].shape[0], n)}
 
 
 def c_fir_resample(a, ctx):
@@ -740,6 +742,133 @@ def c_fir_resample(a, ctx):
         return xp[:, half:half + t]
     op = forward if a["adjoint_of"] is None else adjoint
     return [Val("_result", arg("_result"), op(x, bank), op(x.abs(), bank.abs()))]
+
+
+# ---------------------------------------------------- vocoder front-end and sampler steps
+# Keyword options of these restatements state an alternative operation (a padding, a frame order, a
+# batch stride): the kind-specific mutations below write it over the output, so the checker must
+# tell the two apart.
+def _mel_result(a):
+    rows, t = a["wave"].shape
+    frames = 1 + (t + 2 * a["pad"] - a["n_fft"]) // a["hop"]
+    return {"mel": (rows, a["fb"].shape[1], frames)}
+
+
+def _frames(wave, n_fft, hop, pad, frames, symmetric=False):
+    """[rows, frames, n_fft]: frame f is padded[f hop : f hop + n_fft] of the row padded by `pad` on
+    both sides, by reflection (F.pad mode="reflect": the edge sample is not repeated) or, with
+    symmetric=True, by mirroring (the edge sample repeated)."""
+    t = wave.shape[1]
+    j = torch.arange(frames, device=wave.device)[:, None] * hop + torch.arange(n_fft, device=wave.device) - pad
+    if symmetric:
+        j = torch.where(j < 0, -j - 1, torch.where(j >= t, 2 * t - 1 - j, j))
+    else:
+        j = torch.where(j < 0, -j, torch.where(j >= t, 2 * (t - 1) - j, j))
+    return wave[:, j]
+
+
+def c_mel_spectrogram(a, ctx, symmetric=False, swap_pairs=False):
+    """mel[r, m, f] = sum_k fb[k, m] |rfft(window frame_f)[k]|, then log(max(., 1e-5)) if apply_log.
+    absref = sum_k |fb[k, m]| sum_n |window_n frame_f[n]|, which bounds every |X_k| (triangle
+    inequality); a float FFT's error is ~log2(N) 2^-24 of it."""
+    wave, window, fb = a["wave"].to(F64), a["window"].to(F64), a["fb"].to(F64)
+    n_fft, hop, pad = a["n_fft"], a["hop"], a["pad"]
+    rows, n_mels, frames = _mel_result(a)["mel"]
+    fr = _frames(wave, n_fft, hop, pad, frames, symmetric) * window
+    mel = (torch.fft.rfft(fr, dim=-1).abs() @ fb).transpose(1, 2)              # [rows, n_mels, frames]
+    absr = (fr.abs().sum(-1)[:, None, :] * fb.abs().sum(0)[None, :, None])
+    if swap_pairs:                     # the two frames of each FFT pair exchanged (2p <-> 2p + 1)
+        f = torch.arange(frames, device=wave.device)
+        f = torch.where((f ^ 1) < frames, f ^ 1, f)
+        mel, absr = mel[..., f], absr[..., f]
+    if not a["apply_log"]:
+        return [Val("mel", arg("mel"), mel, absr)]
+    # an error within b of the linear value moves log(max(., 1e-5)) by at most b / max(ref - b, 1e-5)
+    # (the clamped log's Lipschitz constant on [ref - b, ref + b]); 1e-5 |log| is the log's own rounding
+    b = FP32_REL * mel.abs() + FP32_TAU * absr
+    return [Val("mel", arg("mel"), torch.log(mel.clamp_min(1e-5)), b / (mel - b).clamp_min(1e-5) / FP32_TAU)]
+
+
+def _to_flat_result(a):
+    B, _, frames = a["spec"].shape
+    return {"out": (B, (frames - 1) * a["hop"] - 2 * a["pad"] + a["w"].shape[1])}
+
+
+def _overlap_add(spec, w, hop, start, t_out):
+    """out[b, t] = sum_c sum_j spec[b, c, j] w[c, t + start - j hop] (0 <= t + start - j hop < win)."""
+    B, _, frames = spec.shape
+    win = w.shape[1]
+    cols = torch.einsum("bcj,ck->bjk", spec, w)                                 # frame j's window
+    at = (torch.arange(frames, device=spec.device)[:, None] * hop + torch.arange(win, device=spec.device)).reshape(-1)
+    full = cols.new_zeros(B, (frames - 1) * hop + win).index_add_(1, at, cols.reshape(B, -1))
+    return full[:, start:start + t_out]
+
+
+def c_to_flat(a, ctx, shift=0):
+    """The bias-free ConvTranspose1d(C -> 1, kernel win, stride hop, padding pad); shift=1: the output
+    one sample late."""
+    spec, w, hop, pad = a["spec"].to(F64), a["w"].to(F64), a["hop"], a["pad"]
+    t_out = _to_flat_result(a)["out"][1]
+    return [Val("out", arg("out"), _overlap_add(spec, w, hop, pad - shift, t_out),
+                _overlap_add(spec.abs(), w.abs(), hop, pad - shift, t_out))]
+
+
+def _to_flat_bwd_result(a):
+    return {"dspec": tuple(a["spec"].shape) if a["need_dspec"] else None,
+            "dw": tuple(a["w"].shape) if a["need_dw"] else None}
+
+
+def c_to_flat_bwd(a, ctx, dw_rows=None):
+    """dspec[b, c, j] = sum_k w[c, k] dout[b, j hop + k - pad] and dw[c, k] = sum_b sum_j spec[b, c, j]
+    dout[b, j hop + k - pad] (dout zero outside [0, t_out)); both are tensors the launch allocates and
+    returns (dw zeroed inside ops.to_flat_bwd: stored, not accumulated).  dw_rows: dw over the first
+    rows only (a lost batch row)."""
+    spec, w, dout, hop, pad = a["spec"].to(F64), a["w"].to(F64), a["dout"].to(F64), a["hop"], a["pad"]
+    B, win = dout.shape[0], w.shape[1]
+    z = dout.new_zeros(B, pad)
+    d = torch.cat([z, dout, z], 1).unfold(1, win, hop)                        # [B, frames, win]
+    outs = []
+    if a["need_dspec"]:
+        outs.append(Val("dspec", arg("dspec"), torch.einsum("bjk,ck->bcj", d, w),
+                        torch.einsum("bjk,ck->bcj", d.abs(), w.abs())))
+    if a["need_dw"]:
+        n = B if dw_rows is None else dw_rows
+        outs.append(Val("dw", arg("dw"), torch.einsum("bcj,bjk->ck", spec[:n], d[:n]),
+                        torch.einsum("bcj,bjk->ck", spec[:n].abs(), d[:n].abs())))
+    return outs
+
+
+def c_inpaint_blend(a, ctx, level=2):
+    """x <- ab[2] source + ab[3] noise where mask, in place; elsewhere x keeps the sampler's value, bit
+    for bit.  level=0: blended to the level the step started from (ab[0], ab[1])."""
+    x, keep = a["x"], a["mask_u8"] == 0
+    al, be = (float(c) for c in a["ab"].to(F64)[level:level + 2])
+    src, nz = a["source"].to(F64), a["noise"].to(F64)
+    ref = torch.where(keep, x.to(F64), al * src + be * nz)
+    absr = torch.where(keep, 0.0, abs(al) * src.abs() + abs(be) * nz.abs())
+    return [Val("x", arg("x"), ref, absr, keep=keep)]
+
+
+def c_arv_step(a, ctx, advance_sigma=True, v_batch_stride=None):
+    """In place on chan [B, C+1, T] = (x | sigma_0), with a = cos(sigma pi / 2), b = sin(sigma pi / 2):
+    x <- a_1 (a_0 x - b_0 v) + b_1 (b_0 x + a_0 v), sigma_1 = sig_next [B, T] (bitwise) into channel C.
+    v_batch_stride: v [B, C, T] read with another batch stride (zero past its end)."""
+    chan, sig1 = a["chan"].to(F64), a["sig_next"].to(F64)
+    B, C1, T = chan.shape
+    C = C1 - 1
+    v = a["v"].to(F64)
+    if v_batch_stride is not None:
+        flat = torch.cat([v.reshape(-1), v.new_zeros(B * v_batch_stride)])
+        at = (torch.arange(B, device=v.device)[:, None, None] * v_batch_stride +
+              torch.arange(C, device=v.device)[:, None] * T + torch.arange(T, device=v.device))
+        v = flat[at]
+    x, s0, s1 = chan[:, :C], chan[:, C:], sig1.reshape(B, 1, T)
+    a0, b0, a1, b1 = torch.cos(s0 * math.pi / 2), torch.sin(s0 * math.pi / 2), \
+        torch.cos(s1 * math.pi / 2), torch.sin(s1 * math.pi / 2)
+    ref = a1 * (a0 * x - b0 * v) + b1 * (b0 * x + a0 * v)
+    absr = ((a1 * a0).abs() + (b1 * b0).abs()) * x.abs() + ((a1 * b0).abs() + (b1 * a0).abs()) * v.abs()
+    return [Val("chan", lambda p: p["chan"][:, :C], ref, absr),
+            Val("chan.sigma", lambda p: p["chan"][:, C], (s1 if advance_sigma else s0)[:, 0], exact=True, of="chan")]
 
 
 # Role of every tensor argument of each checked kind: read, stored (the launch writes it), or
@@ -781,10 +910,20 @@ ARGS: Dict[str, Tuple[FrozenSet[str], FrozenSet[str], FrozenSet[str]]] = {k: (fr
     "attention_bwd": ({"q", "k", "v", "o", "d_o", "lse"}, {"delta", "dq", "dk", "dv"}, ()),
     "ln_fold_bwd": ({"w", "g", "b", "dwf", "dbf"}, {"dw"}, {"dg", "db"}),
     "fir_resample": ({"x", "bank"}, {"_result"}, ()),      # the output is the tensor the launch returns
+    # the vocoder front-end: outputs are tensors the launch returns (RESULT)
+    "mel_spectrogram": ({"wave", "window", "fb", "band"}, {"mel"}, ()),
+    "to_flat": ({"spec", "w"}, {"out"}, ()),
+    "to_flat_bwd": ({"spec", "w", "dout"}, {"dspec", "dw"}, ()),
+    # the sampler steps of VInpainter and ARVSampler, in place (x / chan are read too)
+    "inpaint_blend": ({"source", "noise", "mask_u8", "ab"}, {"x"}, ()),
+    "arv_step": ({"v", "sig_next"}, {"chan"}, ()),
 }.items()}
 
-# Kinds whose output is the tensor the launch allocates and returns (`_result` in the roles above).
-RESULT: Dict[str, Callable] = {"fir_resample": _fir_result}
+# Kinds whose outputs are tensors the launch allocates and returns: RESULT[kind](args) gives
+# {name: fp32 shape, or None for an output the launch does not make}, in the order of the returned
+# tuple (one name: the returned tensor itself).  The names are the stored roles above.
+RESULT: Dict[str, Callable] = {"fir_resample": _fir_result, "mel_spectrogram": _mel_result,
+                               "to_flat": _to_flat_result, "to_flat_bwd": _to_flat_bwd_result}
 
 # Read arguments the kernel does not read for some argument combinations (the probe skips them):
 # narrow_conv copies the host-packed bf16 image instead of converting `w`, and the conv GEMM's
@@ -797,6 +936,8 @@ NOT_READ: Dict[str, Callable] = {
     "stem_out_bwd": lambda a: {"x", "append", "noise", "alpha", "beta"} if a["w_adapt"] is None else set(),
     "stem_in_bwd": lambda a: {"w"} if a["dxin"] is None else set(),
     "cond_bwd": lambda a: {"w"} if a["dcond"] is None else set(),     # the weights serve dcond only
+    # to_flat_bwd: the spectrogram serves dw only, the weights dspec only
+    "to_flat_bwd": lambda a: ({"spec"} if not a["need_dw"] else set()) | ({"w"} if not a["need_dspec"] else set()),
 }
 
 CHECKERS: Dict[str, Callable] = {
@@ -808,6 +949,8 @@ CHECKERS: Dict[str, Callable] = {
     "colsum": c_colsum, "skip_gate": c_skip_gate, "skip_gate_bwd": c_skip_gate_bwd, "cond_bwd": c_cond_bwd,
     "narrow_conv_bwd": c_narrow_conv_bwd, "stem_out_bwd": c_stem_out_bwd, "stem_in_bwd": c_stem_in_bwd,
     "attention_bwd": c_attention_bwd, "ln_fold_bwd": c_ln_fold_bwd, "fir_resample": c_fir_resample,
+    "mel_spectrogram": c_mel_spectrogram, "to_flat": c_to_flat, "to_flat_bwd": c_to_flat_bwd,
+    "inpaint_blend": c_inpaint_blend, "arv_step": c_arv_step,
 }
 
 
@@ -921,15 +1064,19 @@ class Shadow:
                 return v
             pre = {k: snap(v) for k, v in post.items()}
             outs = CHECKERS[name](pre, self)
-            self._check_roles(idx, name, outs, post)
-            variant = (name, frozenset(n for n, v in post.items() if list(_tensors([v]))))
-            if self.probe and variant not in self.probed:      # once per set of passed tensors
+            made = RESULT[name](pre) if name in RESULT else {}
+            self._check_roles(idx, name, outs, post, made)
+            variant = (name, frozenset(n for n, v in post.items() if list(_tensors([v]))) |
+                       frozenset(n for n, s in made.items() if s is not None))
+            if self.probe and variant not in self.probed:      # once per set of passed / returned tensors
                 self._probe(idx, name, outs, pre)
                 self.probed.add(variant)
             if self.fake:
-                result = None
-                if name in RESULT:
-                    result = post["_result"] = RESULT[name](post)
+                dev = next(_tensors(list(post.values()))).device
+                for n, shape in made.items():
+                    post[n] = None if shape is None else torch.empty(shape, dtype=torch.float32, device=dev)
+                result = tuple(post[n] for n in made) if len(made) > 1 else \
+                    (post[next(iter(made))] if made else None)
                 self._fake_write(outs, pre, post)
                 label = label0
             else:
@@ -938,8 +1085,7 @@ class Shadow:
                 label = tr.records[-1]["name"] if tr.records else label0
                 if post[next(iter(post))].is_cuda:
                     torch.cuda.synchronize()
-                if name in RESULT:
-                    post["_result"] = result
+                post.update(zip(made, result if len(made) > 1 else (result,)))
             if self.mutate is not None and self.mutate[0] == name:
                 if self.mutate[1](post, outs, pre) is not False:       # False: not applicable here
                     self.mutate = None
@@ -950,11 +1096,12 @@ class Shadow:
             return result
         return launch
 
-    def _check_roles(self, idx, name, outs, post):
-        """The checker's outputs are exactly the output arguments the launch was given."""
+    def _check_roles(self, idx, name, outs, post, made):
+        """The checker's outputs are exactly the output arguments the launch was given and the
+        tensors it returns (`made`: RESULT)."""
         _, stored, accumulated = ARGS[name]
-        got = {(o.name, o.acc) for o in outs}
-        want = {(n, False) for n in stored if post.get(n) is not None or n == "_result"} | \
+        got = {(o.of, o.acc) for o in outs}
+        want = {(n, False) for n in stored if post.get(n) is not None or made.get(n) is not None} | \
             {(n, True) for n in accumulated if post.get(n) is not None}
         if got != want:
             raise CheckError(f"launch {idx}: {name}: checker outputs {sorted(got)}, declared {sorted(want)}")
@@ -1038,6 +1185,13 @@ class Shadow:
             err = (val - ref).abs()
             ratio = torch.where(bound > 0, err / bound.clamp_min(1e-300), torch.where(err > 0, math.inf, 0.0))
             ratio = torch.where(torch.isnan(g), math.inf, ratio)
+            if o.keep is not None:                    # positions the launch must not touch: bitwise
+                changed = o.keep & (_bits(got) != _bits(o.view(pre)))
+                if bool(changed.any()):
+                    j = tuple(int(c) for c in changed.nonzero()[0])
+                    self._fail(idx, name, label, f"{o.name}{list(j)}: changed outside the written positions, "
+                                                 f"got {float(got[j]):.6g}, before {float(o.view(pre)[j]):.6g}")
+                ratio = ratio.masked_fill(o.keep, 0.0)
             i = int(ratio.reshape(-1).argmax())
             worst = float(ratio.reshape(-1)[i])
             where = _where(i, tuple(ratio.shape))
@@ -1179,12 +1333,14 @@ def m_acc_lost_split(post, outs, pre):
 
 
 def m_outside_view(post, outs, pre):
-    """One element of a written tensor's storage outside the written view changed."""
+    """One element of a written tensor's storage outside the written views changed."""
     for o in outs:
         v = o.view(post)
         flat = _flat(v.untyped_storage(), v.dtype, v.device)
         mask = torch.zeros(flat.shape, dtype=torch.bool, device=v.device)
-        mask.as_strided(v.shape, v.stride(), v.storage_offset()).fill_(True)
+        for w in (o2.view(post) for o2 in outs):       # every output the launch writes into this storage
+            if _key(w) == _key(v) and w.dtype == v.dtype:
+                mask.as_strided(w.shape, w.stride(), w.storage_offset()).fill_(True)
         free = (~mask).nonzero()
         if free.numel():
             i = int(free[-1, 0])
@@ -1204,6 +1360,49 @@ def m_readonly(post, outs, pre):
     return False
 
 
+def _alternative(kind, doc, **option):
+    """A mutation that writes an alternative fp64 restatement of `kind` (CHECKERS[kind] with
+    `option`) over the outputs, rounded to their dtype."""
+    def mutate(post, outs, pre):
+        for o in CHECKERS[kind](pre, None, **option):
+            got = o.view(post)
+            got.copy_((o.ref(post)[0] if callable(o.ref) else o.ref).to(got.dtype))
+    mutate.__doc__ = doc
+    return mutate
+
+
+def m_unmasked_write(post, outs, pre):
+    """inpaint_blend: the blend also written at one position outside the mask."""
+    keep = next((o.keep for o in outs if getattr(o, "keep", None) is not None), None)
+    if keep is None or not bool(keep.any()):
+        return False
+    j = tuple(int(c) for c in keep.nonzero()[0])
+    a = pre["ab"].to(F64)
+    post["x"][j] = float(a[2] * pre["source"][j].double() + a[3] * pre["noise"][j].double())
+
+
+def m_v_chan_stride(post, outs, pre):
+    """arv_step: v read with chan's batch stride (C+1) T instead of its own C T."""
+    B, C1, T = pre["chan"].shape
+    if B < 2 or C1 < 3:
+        return False                  # one batch row, or one channel: the two strides read the same
+    _alternative("arv_step", "", v_batch_stride=C1 * T)(post, outs, pre)
+
+
 MUTATIONS = {"scale_largest": m_scale_largest, "stale_tile": m_stale_tile, "stats_slot": m_stats_slot,
              "outside_view": m_outside_view, "readonly": m_readonly, "acc_stored": m_acc_stored,
-             "acc_lost_split": m_acc_lost_split}
+             "acc_lost_split": m_acc_lost_split,
+             # kind-specific: an alternative operation written over the output
+             "mel_symmetric_pad": _alternative(
+                 "mel_spectrogram", "The edge frames cut from a symmetric pad (edge sample repeated).",
+                 symmetric=True),
+             "mel_pairs_swapped": _alternative(
+                 "mel_spectrogram", "The two frames of each FFT pair exchanged.", swap_pairs=True),
+             "to_flat_shifted": _alternative("to_flat", "The output one sample late.", shift=1),
+             "to_flat_dw_lost_row": _alternative(
+                 "to_flat_bwd", "dw without the last batch row's contribution (a lost atomic).", dw_rows=-1),
+             "blend_start_level": _alternative(
+                 "inpaint_blend", "The known region noised to the step's starting level (ab[0:2]).", level=0),
+             "blend_unmasked_write": m_unmasked_write,
+             "arv_sigma_kept": _alternative("arv_step", "The sigma channel not advanced.", advance_sigma=False),
+             "arv_v_chan_stride": m_v_chan_stride}

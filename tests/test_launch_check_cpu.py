@@ -1,9 +1,11 @@
 """The per-launch checker of tests/launch_check.py, without a GPU.
 
   * coverage: the checkers are exactly the launch kinds of the recorded inference, sampling,
-    conditioning and training programs (plus the generic sampler step and the resampler); every other launching function of `ops`
-    is listed as unchecked, and every tensor argument of a checked kind in those programs has
-    exactly one declared role;
+    conditioning and training programs plus the generic sampler step, the resampler, the vocoder
+    front-end and the VInpainter / ARVSampler steps -- every launching function of `ops` -- and
+    every tensor argument of a checked kind in those programs has exactly one declared role;
+  * the VInpainter and ARVSampler loops around the oracle's nets on fake kernels reproduce the
+    reference's golden vectors;
   * probes: changing any input a launch reads must move its reference;
   * end to end: the tiny programs run on the CPU with fake kernels that write the checker's own
     fp64 restatement rounded to the output dtype; v must match the golden vectors made from the
@@ -48,12 +50,17 @@ def test_checker_table_matches_ops():
             "arv_step"} <= fns
     recorded = {launch[0] for launch in _fixture_launches(inference_only=False)}
     assert {launch[0] for launch in _fixture_launches()} < recorded
-    # outside the recorded programs: the generic VSampler step (a net that is not a B200UNet) and the
-    # upsampler's resampling of the clip (host tensors, as recorded, take the tensor-op route)
-    assert set(lc.CHECKERS) == recorded | {"sampler_step", "fir_resample"}
+    # outside the recorded programs: the generic VSampler step (a net that is not a B200UNet), the
+    # upsampler's resampling of the clip and the vocoder front-end (host tensors, as recorded, take
+    # the tensor-op route), and the VInpainter / ARVSampler steps
+    assert set(lc.CHECKERS) == recorded | {"sampler_step", "fir_resample", "mel_spectrogram", "to_flat",
+                                           "to_flat_bwd", "inpaint_blend", "arv_step"}
     assert set(lc.ARGS) == set(lc.CHECKERS)
     assert set(lc.UNCHECKED) == fns - set(lc.CHECKERS)
-    assert set(lc.UNCHECKED) == {"to_flat", "to_flat_bwd", "mel_spectrogram", "inpaint_blend", "arv_step"}
+    assert not lc.UNCHECKED
+    for name in lc.RESULT:          # the returned tensors' names are stored roles, not parameters
+        params = set(inspect.signature(getattr(ops, name)).parameters)
+        assert not lc.ARGS[name][1] & params, name
 
 
 def _tensor_args(v):
@@ -129,7 +136,8 @@ def rel_l2(a, b):
 
 
 def _golden(golden_dir, name):
-    return {k: torch.from_numpy(np.asarray(v)) for k, v in np.load(os.path.join(golden_dir, name)).items()}
+    return {k: torch.from_numpy(np.asarray(v)) for k, v in np.load(os.path.join(golden_dir, name)).items()
+            if np.asarray(v).dtype.kind != "U"}            # numbers only (some files carry a note)
 
 
 def test_tiny_program_vs_golden(cpu_launches, oracle_port, golden_dir):
@@ -169,6 +177,67 @@ def test_text_cfg_program_vs_golden(cpu_launches, oracle_port, golden_dir):
         print(f"text_cfg: rel-L2(v) {e_v:.3e} rel-L2(branch) {e_b:.3e}")
         assert e_v <= v_tol and e_b <= b_tol
     assert {"attention", "ln_film", "stem_out"} <= {k.split(".")[0] for k in sh.records}
+
+
+def _draws_from(monkeypatch, draws):
+    """torch.randn / randn_like hand out the golden run's CPU draws, in order."""
+    it = iter(draws)
+    monkeypatch.setattr(torch, "randn", lambda *a, **kw: next(it).to(kw.get("device", "cpu")))
+    monkeypatch.setattr(torch, "randn_like", lambda t_, **kw: next(it).to(t_))
+    return it
+
+
+def test_inpainter_program_vs_golden(cpu_launches, oracle_port, golden_dir, monkeypatch):
+    """VInpainter's generic loop (sampler_step, inpaint_blend) around the oracle's tiny net, 4 steps x
+    2 resamples on fake kernels: only the fp32 rounding of the writes separates it from the golden
+    run of the unmodified reference."""
+    from audio_diffusion_pytorch_b200.diffusion import VInpainter
+    g = _golden(golden_dir, "tiny_inpaint.npz")
+    torch.manual_seed(0)
+    ref = oracle_port.DiffusionModelPort(**TINY)
+    source = torch.randn(2, 2, 4096, generator=torch.Generator().manual_seed(int(g["source_seed"])))
+    mask = torch.zeros(2, 2, 4096, dtype=torch.bool)
+    for b_, lo, hi in g["mask_spans"].tolist():
+        mask[b_, :, lo:hi] = True
+    steps, resamples = int(g["num_steps"]), int(g["num_resamples"])
+    torch.manual_seed(int(g["rng_seed"]))
+    draws = [torch.randn(2, 2, 4096) for _ in range(1 + steps * resamples)]
+    left = _draws_from(monkeypatch, draws)
+    with torch.no_grad(), lc.Shadow(fake=True, probe=True) as sh:
+        out = VInpainter(net=ref.net)(source, mask, num_steps=steps, num_resamples=resamples)
+    monkeypatch.undo()
+    print(sh.table())
+    e = rel_l2(out, g["out"])
+    print(f"VInpainter {steps} steps x {resamples} resamples on fake kernels: rel-L2 {e:.3e}")
+    assert e <= 1e-5
+    assert next(left, None) is None
+    assert sh.records["inpaint_blend.x"].count == sh.records["sampler_step.x_next"].count == steps * resamples
+    assert {k for k, _ in sh.probed} == {"sampler_step", "inpaint_blend"}
+    assert torch.equal(out[mask], source[mask])           # sigma = 0 at the end: the known region is the source
+
+
+def test_autoregressive_program_vs_golden(cpu_launches, oracle_port, golden_dir, monkeypatch):
+    """ARVSampler's generic loop (arv_step) around the oracle's DiffusionAR net: start window (4 steps)
+    and 6 ladder passes on fake kernels, against the golden run of the unmodified reference."""
+    from audio_diffusion_pytorch_b200.diffusion import ARVSampler
+    g = _golden(golden_dir, "tiny_autoregressive.npz")
+    cfg = dict(TINY, in_channels=2, length=4096, num_splits=4)
+    torch.manual_seed(0)
+    ref = oracle_port.DiffusionARPort(**cfg)
+    torch.manual_seed(int(g["sample_seed"]))
+    draws = [torch.randn(2, 2, 4096), torch.randn(2, 2, 4096)] + [torch.randn(2, 2, 1024) for _ in range(6)]
+    left = _draws_from(monkeypatch, draws)
+    sampler = ARVSampler(net=ref.net, in_channels=2, length=4096, num_splits=4)
+    with torch.no_grad(), lc.Shadow(fake=True, probe=True) as sh:
+        out = sampler(num_items=2, num_chunks=6, num_steps=4)
+    monkeypatch.undo()
+    print(sh.table())
+    e = rel_l2(out, g["sample"])
+    print(f"ARVSampler 6 chunks x 4 steps on fake kernels: rel-L2 {e:.3e}")
+    assert out.shape == (2, 2, 6144) and e <= 1e-5
+    assert next(left, None) is None
+    assert sh.records["arv_step.chan"].count == sh.records["arv_step.chan.sigma"].count == 4 + 6
+    assert {k for k, _ in sh.probed} == {"arv_step"}
 
 
 def test_unfused_program_probes(cpu_launches, oracle_port):

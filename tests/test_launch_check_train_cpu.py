@@ -1,13 +1,16 @@
 """The training half of the per-launch checker (tests/launch_check.py), without a GPU.
 
-  * every training launch kind, with and without its optional arguments, as one small direct launch
-    on fake kernels with probes: each read argument must move the restatement, and the declared roles
-    must be exactly the outputs the checker returns;
+  * every training launch kind, the vocoder front-end and the VInpainter / ARVSampler steps, with and
+    without their optional arguments, as one small direct launch on fake kernels with probes: each
+    read argument must move the restatement, and the declared roles must be exactly the outputs the
+    checker returns;
   * the restatements against float64 autograd of the forward operation they are the backward of
-    (written here from the operation's definition with plain tensor operations);
+    (written here from the operation's definition with plain tensor operations), the front-end's
+    against its float64 modules and the sampler steps' against the reference's formulas;
   * mutations: the accumulator stored instead of added, a lost share of the largest contribution, a
     scaled element, a stale tile, a write outside the view, a modified input -- each must be caught
-    on every kind it applies to, into accumulators that are non-zero before the launch.
+    on every kind it applies to, into accumulators that are non-zero before the launch -- and, for
+    the front-end and sampler steps, alternative operations written over the output.
 """
 import math
 
@@ -179,6 +182,52 @@ def _stem_out_loss(r, variant):
                                 dv=torch.empty(B, co, Tf))
 
 
+MEL = dict(n_fft=256, hop_length=64, win_length=200, sample_rate=16000, n_mel_channels=24)
+
+
+def _mel_front(normalize_log):
+    from audio_diffusion_pytorch_b200.components import MelSpectrogram
+    return MelSpectrogram(normalize_log=normalize_log, **MEL)
+
+
+def _mel_spectrogram(r, variant):
+    """15 frames (an odd count: the last FFT pair has one frame), a window shorter than n_fft."""
+    front = _mel_front(variant == "log")
+    window, fb, band = front._kernel_tables("cpu")
+    return lambda: ops.mel_spectrogram(r.f32(3, 1000), window, fb, band, MEL["n_fft"], MEL["hop_length"],
+                                       front.padding, apply_log=variant == "log")
+
+
+FLAT = dict(C=16, frames=9, win=64, hop=16, pad=24)          # t_out = 8 * 16 - 48 + 64 = 144
+
+
+def _to_flat(r, variant):
+    return lambda: ops.to_flat(r.f32(3, FLAT["C"], FLAT["frames"]), r.f32(FLAT["C"], FLAT["win"], scale=0.1),
+                               FLAT["hop"], FLAT["pad"])
+
+
+def _to_flat_bwd(r, variant):
+    return lambda: ops.to_flat_bwd(r.f32(3, FLAT["C"], FLAT["frames"]), r.f32(FLAT["C"], FLAT["win"], scale=0.1),
+                                   r.f32(3, 144), FLAT["hop"], FLAT["pad"], need_dspec=variant != "dw",
+                                   need_dw=variant != "dspec")
+
+
+def _inpaint_blend(r, variant):
+    """x is rows 1.. of a wider buffer (room outside the written view); the two alpha / beta rows differ."""
+    x = r.f32(3, 2, 500)[1:]
+    mask = (torch.rand(2, 2, 500, generator=r.g) < 0.4).to(torch.uint8)
+    return lambda: ops.inpaint_blend(x, r.f32(2, 2, 500), r.f32(2, 2, 500), mask,
+                                     torch.tensor([0.8, 0.6, 0.9, 0.43589]))
+
+
+def _arv_step(r, variant):
+    """B = 3, C = 2, T = 300; chan is rows 1.. of a wider buffer, sigma_1 <= sigma_0 per position."""
+    chan = r.f32(4, 3, 300)[1:]
+    chan[:, 2] = torch.rand(3, 300, generator=r.g)
+    sig_next = chan[:, 2] * torch.rand(3, 300, generator=r.g)
+    return lambda: ops.arv_step(chan, r.f32(3, 2, 300), sig_next)
+
+
 DIRECT = {
     "wgrad": (_wgrad, ("tap1", "taps3", "views")),
     "gn_silu_bwd": (_gn_silu_bwd, ("all",)),
@@ -195,6 +244,11 @@ DIRECT = {
     "ln_fold_bwd": (_ln_fold_bwd, ("all",)),
     "fir_resample": (_fir_resample, ("up", "down", "adjoint")),
     "stem_out": (_stem_out_loss, ("loss",)),
+    "mel_spectrogram": (_mel_spectrogram, ("log", "linear")),
+    "to_flat": (_to_flat, ("plain",)),
+    "to_flat_bwd": (_to_flat_bwd, ("both", "dspec", "dw")),
+    "inpaint_blend": (_inpaint_blend, ("all",)),
+    "arv_step": (_arv_step, ("all",)),
 }
 CASES = [(k, v) for k, (_, vs) in DIRECT.items() for v in vs]
 
@@ -205,7 +259,8 @@ def _launch(kind, variant, seed=11):
 
 
 def test_every_training_kind_has_a_direct_launch():
-    """The direct launches below cover every checked kind the inference programs do not reach."""
+    """The direct launches above cover every checked kind the recorded inference programs do not
+    reach: the training kinds, the resampler, the vocoder front-end and the two sampler steps."""
     from test_launch_check_cpu import _fixture_launches
     inference = {launch[0] for launch in _fixture_launches()} | {"sampler_step"}
     assert set(DIRECT) - {"stem_out"} == set(lc.CHECKERS) - inference
@@ -409,6 +464,65 @@ def test_small_backward_kinds_vs_autograd():
         _grad_check(o["_result"].ref, x.grad[0], f"resample adjoint {fi}->{fo}")
 
 
+def test_vocoder_front_end_vs_float64_modules():
+    """mel_spectrogram against MelSpectrogram's own tensor-op route (torchaudio STFT + MelScale after
+    F.pad reflect) in float64, with and without the log; to_flat / to_flat_bwd against
+    nn.ConvTranspose1d and its float64 autograd."""
+    r = Rand(9)
+    for log in (False, True):
+        front = _mel_front(log)
+        window, fb, band = front._kernel_tables("cpu")
+        wave = r.f32(3, 1000).double()
+        want = front.double()(wave)
+        o = _outs("mel_spectrogram", dict(wave=wave, window=window, fb=fb, band=band, n_fft=MEL["n_fft"],
+                                          hop=MEL["hop_length"], pad=front.padding, apply_log=log))
+        assert o["mel"].ref.shape == want.shape == (3, MEL["n_mel_channels"], 15)
+        _grad_check(o["mel"].ref, want, f"mel_spectrogram (log={log})")
+
+    C, frames, win, hop, pad = (FLAT[k] for k in ("C", "frames", "win", "hop", "pad"))
+    conv = torch.nn.ConvTranspose1d(C, 1, win, stride=hop, padding=pad, bias=False).double()
+    spec = r.f32(3, C, frames).double().requires_grad_()
+    out = conv(spec)
+    dout = r.f32(*out.shape).double()
+    out.backward(dout)
+    w = conv.weight.detach()[:, 0]
+    o = _outs("to_flat", dict(spec=spec.detach(), w=w, hop=hop, pad=pad))
+    _grad_check(o["out"].ref, out.detach()[:, 0], "to_flat")
+    o = _outs("to_flat_bwd", dict(spec=spec.detach(), w=w, dout=dout[:, 0], hop=hop, pad=pad, need_dspec=True,
+                                  need_dw=True))
+    _grad_check(o["dspec"].ref, spec.grad, "to_flat_bwd dspec")
+    _grad_check(o["dw"].ref, conv.weight.grad[:, 0], "to_flat_bwd dw")
+    assert set(_outs("to_flat_bwd", dict(spec=spec.detach(), w=w, dout=dout[:, 0], hop=hop, pad=pad,
+                                         need_dspec=False, need_dw=True))) == {"dw"}
+
+
+def test_sampler_steps_vs_float64_formulas():
+    """inpaint_blend and arv_step against the reference's formulas (diffusion.py, VInpainter and
+    ARVSampler) evaluated directly in float64."""
+    from audio_diffusion_pytorch_b200.diffusion import _alpha_beta
+    r = Rand(10)
+    x, src, noise = (r.f32(2, 2, 500).double() for _ in range(3))
+    mask = torch.rand(2, 2, 500, generator=r.g) < 0.4
+    sig = torch.tensor([0.7, 0.55], dtype=F64)
+    alphas, betas = _alpha_beta(sig)
+    ab = torch.stack([alphas[0], betas[0], alphas[1], betas[1]])
+    want = x.clone()
+    want[mask] = (alphas[1] * src + betas[1] * noise)[mask]
+    o = _outs("inpaint_blend", dict(x=x, source=src, noise=noise, mask_u8=mask.to(torch.uint8), ab=ab))
+    _grad_check(o["x"].ref, want, "inpaint_blend")
+    assert torch.equal(o["x"].keep, ~mask)
+
+    chan = r.f32(3, 3, 300).double()
+    chan[:, 2] = torch.rand(3, 300, generator=r.g).double()
+    v, sig_next = r.f32(3, 2, 300).double(), torch.rand(3, 300, generator=r.g).double()
+    a0, b0 = _alpha_beta(chan[:, 2:])
+    a1, b1 = _alpha_beta(sig_next[:, None])
+    x_pred, noise_pred = a0 * chan[:, :2] - b0 * v, b0 * chan[:, :2] + a0 * v
+    o = _outs("arv_step", dict(chan=chan, v=v, sig_next=sig_next))
+    _grad_check(o["chan"].ref, a1 * x_pred + b1 * noise_pred, "arv_step")
+    assert torch.equal(o["chan.sigma"].ref, sig_next) and o["chan.sigma"].exact
+
+
 # ------------------------------------------------------------------------------ mutations
 def _roles(kind):
     return lc.ARGS[kind]
@@ -423,8 +537,13 @@ MUTANTS = ([("acc_stored", k) for k in _ACC_KINDS + ["stem_out"]] +
                                         "narrow_conv_bwd", "stem_out_bwd", "attention_bwd")] +
            [("stats_slot", "skip_gate")] +
            [("outside_view", k) for k in ("wgrad", "ln_film_bwd", "colsum", "skip_gate_bwd", "cond_bwd",
-                                          "stem_out_bwd", "attention_bwd")] +
-           [("readonly", k) for k in DIRECT])
+                                          "stem_out_bwd", "attention_bwd", "inpaint_blend", "arv_step")] +
+           [("readonly", k) for k in DIRECT] +
+           # kind-specific: an alternative operation written over the output
+           [("mel_symmetric_pad", "mel_spectrogram"), ("mel_pairs_swapped", "mel_spectrogram"),
+            ("to_flat_shifted", "to_flat"), ("to_flat_dw_lost_row", "to_flat_bwd"),
+            ("blend_start_level", "inpaint_blend"), ("blend_unmasked_write", "inpaint_blend"),
+            ("arv_sigma_kept", "arv_step"), ("arv_v_chan_stride", "arv_step")])
 # the variant of each kind whose outputs leave room outside their views (column windows of wider rows)
 _VARIANT = {"wgrad": "views", "ln_film_bwd": "film", "attention_bwd": "self", "stem_out_bwd": "adapter",
             "gn_bwd_apply": "dres_colsum", "colsum": "gate", "cond_bwd": "dcond", "stem_in_bwd": "dxin"}
