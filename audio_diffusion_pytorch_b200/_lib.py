@@ -114,7 +114,7 @@ def lib() -> C.CDLL:
         "adp_arv_step": [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp],
         "adp_resample": [vp, vp, vp] + [C.c_int] * 7 + [vp],
         "adp_resample_adjoint": [vp, vp, vp] + [C.c_int] * 7 + [vp],
-        "adp_mel_spectrogram": [vp] * 5 + [C.c_int] * 8 + [vp],
+        "adp_mel_spectrogram": [vp] * 5 + [C.c_int] * 9 + [vp],
         "adp_to_flat": [vp, vp, vp] + [C.c_int] * 7 + [vp],
         "adp_to_flat_bwd": [vp] * 5 + [C.c_int] * 7 + [vp],
         "adp_f32_conv_gemm": [C.POINTER(ConvGemmArgs), vp],

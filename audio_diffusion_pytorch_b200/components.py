@@ -109,12 +109,15 @@ class MelSpectrogram(nn.Module):
         lead, t = waveform.shape[:-1], waveform.shape[-1]
         if waveform.is_cuda and not (torch.is_grad_enabled() and waveform.requires_grad):
             # one kernel: framing, window, FFT, magnitude, mel filters (+ log); autograd through
-            # the STFT (a waveform that requires grad) keeps the tensor-op route below
+            # the STFT (a waveform that requires grad) keeps the tensor-op route below.  center=True
+            # reflects the padded signal once more by n_fft // 2, as torch.stft does
             from . import ops
             window, fb, band = self._kernel_tables(waveform.device)
+            n_fft = self.to_spectrogram.n_fft
             mel = ops.mel_spectrogram(waveform.reshape(-1, t).float().contiguous(), window, fb, band,
-                                      self.to_spectrogram.n_fft, self.hop_length, self.padding,
-                                      apply_log=self.normalize_log and not self.normalize)
+                                      n_fft, self.hop_length, self.padding,
+                                      apply_log=self.normalize_log and not self.normalize,
+                                      center_pad=n_fft // 2 if self.to_spectrogram.center else 0)
             if self.normalize:
                 mel = 2 * torch.pow(mel / torch.max(mel), 0.25) - 1
                 if self.normalize_log:

@@ -2,9 +2,9 @@
 // once per call, outside the step loop, on waveform-rate data (HBM-bound, a few MB):
 //   adp_resample / _adjoint   polyphase windowed-sinc rate change (reference utils.py:82-117,
 //                             DiffusionUpsampler.reupsample / .sample)
-//   adp_mel_spectrogram       reflect-pad framing + window + radix-2 FFT in shared memory +
-//                             magnitude + triangular mel filters (+ log), reference
-//                             components.py:188-236 (DiffusionVocoder.forward)
+//   adp_mel_spectrogram       reflect-pad framing (+ stft's center pad) + window + mixed-radix
+//                             FFT in shared memory + magnitude + triangular mel filters (+ log),
+//                             reference components.py:188-236 (DiffusionVocoder.forward)
 //   adp_to_flat / _bwd        ConvTranspose1d(mel -> 1 channel, bias-free), reference
 //                             models.py:194-201, with the gradients of its weight and input
 #include "common.cuh"
@@ -70,69 +70,168 @@ resample_adjoint_kernel(const float* __restrict__ dy, const float* __restrict__ 
 
 // --------------------------------------------------------------------------- mel spectrogram
 // One CTA (256 threads) per (row, group of kMelFrames frames).  Two real frames ride through one
-// complex FFT (z = a + i b; A[k] = (Z[k] + conj Z[N-k]) / 2, B[k] = (Z[k] - conj Z[N-k]) / 2i).
-// The FFT is an in-place radix-2 decimation-in-time over bit-reversed input in shared memory
-// with a twiddle table of N/2 entries.  Each mel filter is a triangle over a contiguous bin range
-// [lo, hi) (host-computed from the filterbank's non-zeros): a thread owns one (mel, frame) output.
+// complex FFT (z = a + i b; A[k] = (Z[k] + conj Z[N-k]) / 2, B[k] = (Z[k] - conj Z[N-k]) / 2i,
+// N-k taken mod N).  The FFT is a mixed-radix Stockham transform in shared memory: N = product
+// of the plan's radices (4s, then at most one 2, then 3s, 5s, 7s), each stage reads one buffer in
+// natural order and writes the other, so no digit reversal is needed; the twiddle table holds
+// exp(-2 pi i k / N) for k < N.  Shared memory: two [N] complex buffers, the [N] twiddles and the
+// [n_mels][kMelFrames] accumulators (24 N + 32 n_mels bytes: 208 KB at N = 8192 and 512 mels);
+// the magnitudes [2][N/2 + 1] reuse the buffer the last stage read.  Each mel filter is a
+// triangle over a contiguous bin range [lo, hi) (host-computed from the filterbank's non-zeros):
+// a thread owns one (mel, frame) output.
 constexpr int kMelFrames = 8;
-constexpr int kMelMaxN = 4096;
+constexpr int kMelMaxN = 8192;
+
+__device__ __forceinline__ float2 cmul(float2 a, float2 b) {
+  return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x);
+}
+__device__ __forceinline__ float2 cadd(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
+__device__ __forceinline__ float2 csub(float2 a, float2 b) { return make_float2(a.x - b.x, a.y - b.y); }
+
+// cos and sin of 2 pi j / R for R in {3, 5, 7} and 1 <= j <= R / 2
+__host__ __device__ constexpr float dft_cos(int R, int j) {
+  return R == 3 ? -0.5f
+       : R == 5 ? (j == 1 ? 0.30901699437494745f : -0.80901699437494745f)
+       : (j == 1 ? 0.62348980185873353f : j == 2 ? -0.22252093395631440f : -0.90096886790241913f);
+}
+__host__ __device__ constexpr float dft_sin(int R, int j) {
+  return R == 3 ? 0.86602540378443865f
+       : R == 5 ? (j == 1 ? 0.95105651629515357f : 0.58778525229247313f)
+       : (j == 1 ? 0.78183148246802981f : j == 2 ? 0.97492791218182361f : 0.43388373911755812f);
+}
+
+// In-register forward DFT of R points, X_k = sum_n v_n exp(-2 pi i k n / R).  Odd R pairs
+// v_m with v_(R-m): X_k = A_k - i B_k, X_(R-k) = A_k + i B_k with A_k = v_0 + sum_m (v_m + v_(R-m))
+// cos(2 pi k m / R) and B_k = sum_m (v_m - v_(R-m)) sin(2 pi k m / R).
+template <int R>
+__device__ __forceinline__ void dft(float2 (&v)[R]) {
+  constexpr int H = R / 2;
+  float2 s[H + 1], d[H + 1];
+  const float2 x0 = v[0];
+  float2 sum = x0;
+#pragma unroll
+  for (int m = 1; m <= H; ++m) {
+    s[m] = cadd(v[m], v[R - m]);
+    d[m] = csub(v[m], v[R - m]);
+    sum = cadd(sum, s[m]);
+  }
+  v[0] = sum;
+#pragma unroll
+  for (int k = 1; k <= H; ++k) {
+    float2 a = x0, b = make_float2(0.f, 0.f);
+#pragma unroll
+    for (int m = 1; m <= H; ++m) {
+      const int j = (k * m) % R;
+      const float c = j <= H ? dft_cos(R, j) : dft_cos(R, R - j);
+      const float sn = j <= H ? dft_sin(R, j) : -dft_sin(R, R - j);
+      a = make_float2(fmaf(s[m].x, c, a.x), fmaf(s[m].y, c, a.y));
+      b = make_float2(fmaf(d[m].x, sn, b.x), fmaf(d[m].y, sn, b.y));
+    }
+    v[k] = make_float2(a.x + b.y, a.y - b.x);
+    v[R - k] = make_float2(a.x - b.y, a.y + b.x);
+  }
+}
+template <>
+__device__ __forceinline__ void dft<2>(float2 (&v)[2]) {
+  const float2 a = v[0], b = v[1];
+  v[0] = cadd(a, b);
+  v[1] = csub(a, b);
+}
+template <>
+__device__ __forceinline__ void dft<4>(float2 (&v)[4]) {
+  const float2 t0 = cadd(v[0], v[2]), t1 = csub(v[0], v[2]), t2 = cadd(v[1], v[3]), t3 = csub(v[1], v[3]);
+  const float2 mt3 = make_float2(t3.y, -t3.x);                       // -i t3
+  v[0] = cadd(t0, t2);
+  v[1] = cadd(t1, mt3);
+  v[2] = csub(t0, t2);
+  v[3] = csub(t1, mt3);
+}
+
+// One Stockham radix-R stage after sub-transforms of length Ns: butterfly j (k = j mod Ns) reads
+// src[j + r N/R], twiddles input r by exp(-2 pi i k r / (Ns R)) and writes dst[(j - k) R + k + r Ns].
+template <int R>
+__device__ __forceinline__ void fft_stage(const float2* __restrict__ src, float2* __restrict__ dst,
+                                          const float2* __restrict__ tw, int N, int Ns) {
+  const int m = N / R, step = N / (Ns * R);
+  for (int j = threadIdx.x; j < m; j += blockDim.x) {
+    const int k = j % Ns;
+    float2 v[R];
+#pragma unroll
+    for (int r = 0; r < R; ++r) v[r] = src[j + r * m];
+    if (Ns > 1) {
+#pragma unroll
+      for (int r = 1; r < R; ++r) v[r] = cmul(v[r], tw[k * r * step]);
+    }
+    dft<R>(v);
+    float2* d = dst + (j - k) * R + k;
+#pragma unroll
+    for (int r = 0; r < R; ++r) d[r * Ns] = v[r];
+  }
+}
+
+// F.pad(mode="reflect") index: the edge sample is not repeated (|j| < len assumed)
+__device__ __forceinline__ int reflect_index(int j, int len) {
+  return j < 0 ? -j : (j >= len ? 2 * (len - 1) - j : j);
+}
 
 __global__ void __launch_bounds__(256)
 mel_spectrogram_kernel(const float* __restrict__ wave, const float* __restrict__ window,
                        const float* __restrict__ fb, const int* __restrict__ band,
-                       float* __restrict__ mel, int t, int n_fft, int log2n, int hop, int pad,
-                       int frames, int n_mels, int apply_log) {
+                       float* __restrict__ mel, int t, int n_fft, unsigned long long plan, int hop,
+                       int pad, int center_pad, int frames, int n_mels, int apply_log) {
   extern __shared__ __align__(16) float smem[];
   const int N = n_fft, bins = N / 2 + 1;
-  float2* z = reinterpret_cast<float2*>(smem);                 // [N]
-  float2* tw = z + N;                                          // [N/2]
-  float* mag = reinterpret_cast<float*>(tw + N / 2);           // [2][bins]
-  float* acc = mag + 2 * bins;                                 // [n_mels][kMelFrames]
+  float2* buf0 = reinterpret_cast<float2*>(smem);              // [N] frames in, even stages' input
+  float2* buf1 = buf0 + N;                                     // [N]
+  float2* tw = buf1 + N;                                       // [N]
+  float* acc = reinterpret_cast<float*>(tw + N);               // [n_mels][kMelFrames]
   pdl_launch_dependents();
-  for (int k = threadIdx.x; k < N / 2; k += blockDim.x) {
+  for (int k = threadIdx.x; k < N; k += blockDim.x) {
     float s, c;
     sincospif(-2.f * static_cast<float>(k) / static_cast<float>(N), &s, &c);
     tw[k] = make_float2(c, s);
   }
+  int stages = 0;
+  for (unsigned long long p = plan; p; p >>= 4) ++stages;
+  const float2* z = (stages & 1) ? buf1 : buf0;                // the spectrum after the last stage
+  float* mag = reinterpret_cast<float*>((stages & 1) ? buf0 : buf1);   // [2][bins]
   pdl_wait();
   const int row = blockIdx.y;
   const int f0 = blockIdx.x * kMelFrames;
+  const int t_pad = t + 2 * pad;
   const float* wr = wave + static_cast<size_t>(row) * t;
   for (int pair = 0; pair < kMelFrames / 2; ++pair) {
     const int fa = f0 + 2 * pair, fbm = fa + 1;
     __syncthreads();
-    // windowed, reflect-padded frames -> bit-reversed positions
+    // windowed frames of the row reflect-padded by pad, then the result reflect-padded by
+    // center_pad (torch.stft's center=True after the module's own pad)
     for (int n = threadIdx.x; n < N; n += blockDim.x) {
       float va = 0.f, vb = 0.f;
       const float w = window[n];
-      if (fa < frames) {
-        int j = fa * hop + n - pad;
-        j = j < 0 ? -j : (j >= t ? 2 * (t - 1) - j : j);
-        va = wr[j] * w;
-      }
-      if (fbm < frames) {
-        int j = fbm * hop + n - pad;
-        j = j < 0 ? -j : (j >= t ? 2 * (t - 1) - j : j);
-        vb = wr[j] * w;
-      }
-      z[__brev(static_cast<unsigned>(n)) >> (32 - log2n)] = make_float2(va, vb);
+      if (fa < frames) va = wr[reflect_index(reflect_index(fa * hop + n - center_pad, t_pad) - pad, t)] * w;
+      if (fbm < frames) vb = wr[reflect_index(reflect_index(fbm * hop + n - center_pad, t_pad) - pad, t)] * w;
+      buf0[n] = make_float2(va, vb);
     }
     __syncthreads();
-    for (int s = 1; s <= log2n; ++s) {
-      const int half = 1 << (s - 1);
-      for (int i = threadIdx.x; i < N / 2; i += blockDim.x) {
-        const int grp = i >> (s - 1), pos = i & (half - 1);
-        const int a = (grp << s) + pos, b = a + half;
-        const float2 w = tw[pos << (log2n - s)];
-        const float2 u = z[a], v = z[b];
-        const float2 m = make_float2(v.x * w.x - v.y * w.y, v.x * w.y + v.y * w.x);
-        z[a] = make_float2(u.x + m.x, u.y + m.y);
-        z[b] = make_float2(u.x - m.x, u.y - m.y);
+    float2 *src = buf0, *dst = buf1;
+    int Ns = 1;
+    for (unsigned long long p = plan; p; p >>= 4) {
+      const int R = static_cast<int>(p & 15);
+      switch (R) {
+        case 4: fft_stage<4>(src, dst, tw, N, Ns); break;
+        case 2: fft_stage<2>(src, dst, tw, N, Ns); break;
+        case 3: fft_stage<3>(src, dst, tw, N, Ns); break;
+        case 5: fft_stage<5>(src, dst, tw, N, Ns); break;
+        default: fft_stage<7>(src, dst, tw, N, Ns); break;
       }
       __syncthreads();
+      float2* tmp = src;
+      src = dst;
+      dst = tmp;
+      Ns *= R;
     }
     for (int k = threadIdx.x; k < bins; k += blockDim.x) {
-      const float2 p = z[k], q = z[(N - k) & (N - 1)];
+      const float2 p = z[k], q = z[k == 0 ? 0 : N - k];
       const float ar = 0.5f * (p.x + q.x), ai = 0.5f * (p.y - q.y);     // frame a
       const float br = 0.5f * (p.y + q.y), bi = -0.5f * (p.x - q.x);    // frame b
       mag[k] = sqrtf(ar * ar + ai * ai);
@@ -158,6 +257,27 @@ mel_spectrogram_kernel(const float* __restrict__ wave, const float* __restrict__
       out[static_cast<size_t>(m) * frames + f] = v;
     }
   }
+}
+
+// Radices of n, 4 bits per stage with the first stage lowest: 4s, at most one 2, then 3s, 5s, 7s.
+// 0 when n has a prime factor above 7.
+static unsigned long long mel_fft_plan(int n) {
+  unsigned long long plan = 0;
+  int shift = 0;
+  auto take = [&](int r) {
+    while (n % r == 0 && n > 1 && shift < 64) {
+      plan |= static_cast<unsigned long long>(r) << shift;
+      shift += 4;
+      n /= r;
+      if (r == 2) break;
+    }
+  };
+  take(4);
+  take(2);
+  take(3);
+  take(5);
+  take(7);
+  return n == 1 ? plan : 0;
 }
 
 // --------------------------------------------------------------------------- to_flat
@@ -273,24 +393,25 @@ extern "C" int adp_resample_adjoint(const float* dy, const float* bank, float* d
 
 extern "C" int adp_mel_spectrogram(const float* wave, const float* window, const float* fb,
                                    const int32_t* band, float* mel, int rows, int t, int n_fft,
-                                   int hop, int pad, int frames, int n_mels, int apply_log,
-                                   adp_stream_t stream) {
+                                   int hop, int pad, int center_pad, int frames, int n_mels,
+                                   int apply_log, adp_stream_t stream) {
   ADP_CHECK(wave && window && fb && band && mel, "adp_mel_spectrogram: null pointer");
-  int log2n = 0;
-  while ((1 << log2n) < n_fft) ++log2n;
-  ADP_CHECK(n_fft >= 32 && n_fft <= kMelMaxN && (1 << log2n) == n_fft,
-            "adp_mel_spectrogram: n_fft=%d must be a power of two in [32, %d]", n_fft, kMelMaxN);
+  const unsigned long long plan = n_fft >= 32 && n_fft <= kMelMaxN ? mel_fft_plan(n_fft) : 0;
+  ADP_CHECK(plan != 0, "adp_mel_spectrogram: n_fft=%d must have prime factors 2, 3, 5, 7 only and lie in [32, %d]",
+            n_fft, kMelMaxN);
   ADP_CHECK(rows > 0 && rows <= 65535 && hop > 0 && frames > 0 && n_mels > 0 && n_mels <= 512,
             "adp_mel_spectrogram: bad sizes");
-  ADP_CHECK(pad >= 0 && pad < t && (frames - 1) * hop + n_fft - pad <= t + pad,
+  ADP_CHECK(pad >= 0 && pad < t && center_pad >= 0 && center_pad < t + 2 * pad,
+            "adp_mel_spectrogram: each reflect pad must be shorter than the signal it mirrors "
+            "(t=%d, pad=%d, center_pad=%d)", t, pad, center_pad);
+  ADP_CHECK(static_cast<int64_t>(frames - 1) * hop + n_fft <= static_cast<int64_t>(t) + 2 * pad + 2 * center_pad,
             "adp_mel_spectrogram: frames do not fit the reflect-padded signal");
-  const size_t smem = (static_cast<size_t>(n_fft) * 2 + n_fft + 2 * (n_fft / 2 + 1) +
-                       static_cast<size_t>(n_mels) * kMelFrames) * sizeof(float);
+  const size_t smem = (static_cast<size_t>(n_fft) * 6 + static_cast<size_t>(n_mels) * kMelFrames) * sizeof(float);
   static SmemAttrCache cache;
   ADP_CUDA(ensure_dyn_smem(mel_spectrogram_kernel, smem, cache));
   ADP_CUDA(launch_k(mel_spectrogram_kernel, dim3((frames + kMelFrames - 1) / kMelFrames, rows), dim3(256),
-                    smem, as_stream(stream), wave, window, fb, band, mel, t, n_fft, log2n, hop, pad,
-                    frames, n_mels, apply_log));
+                    smem, as_stream(stream), wave, window, fb, band, mel, t, n_fft, plan, hop, pad,
+                    center_pad, frames, n_mels, apply_log));
   ADP_LAUNCH_CHECK();
   return 0;
 }

@@ -472,15 +472,17 @@ def fir_resample(x: Tensor, bank: Tensor, factor_in: int, factor_out: int, half:
 
 
 def mel_spectrogram(wave: Tensor, window: Tensor, fb: Tensor, band: Tensor, n_fft: int, hop: int,
-                    pad: int, apply_log: bool) -> Tensor:
-    """wave fp32 [rows, t] -> mel fp32 [rows, n_mels, frames] (adp_mel_spectrogram)."""
+                    pad: int, apply_log: bool, center_pad: int = 0) -> Tensor:
+    """wave fp32 [rows, t] -> mel fp32 [rows, n_mels, frames] (adp_mel_spectrogram).  The row is
+    reflect-padded by `pad`, then by `center_pad` (torch.stft's center=True pads n_fft // 2)."""
     rows, t = wave.shape
     n_mels = fb.shape[1]
-    frames = 1 + (t + 2 * pad - n_fft) // hop
+    frames = 1 + (t + 2 * pad + 2 * center_pad - n_fft) // hop
     mel = torch.empty(rows, n_mels, frames, device=wave.device, dtype=torch.float32)
     _launch(lambda: _lib.lib().adp_mel_spectrogram(wave.data_ptr(), window.data_ptr(), fb.data_ptr(),
                                                    band.data_ptr(), mel.data_ptr(), rows, t, n_fft, hop, pad,
-                                                   frames, n_mels, 1 if apply_log else 0, _stream()),
+                                                   center_pad, frames, n_mels, 1 if apply_log else 0,
+                                                   _stream()),
             "adp_mel_spectrogram", lambda: (f"mel_spectrogram[n_fft={n_fft}]", 0, _nb(wave, mel)))
     return mel
 

@@ -302,13 +302,16 @@ int adp_resample(const float* x, const float* bank, float* y, int rows, int t, i
 int adp_resample_adjoint(const float* dy, const float* bank, float* dx, int rows, int t, int t_out,
                          int factor_in, int factor_out, int taps, int half, adp_stream_t stream);
 
-/* MelSpectrogram (reference components.py:188-236): reflect padding by `pad`, frames of n_fft
- * samples every `hop` (center=False), window [n_fft], |rFFT|, mel filterbank fb [n_fft/2+1, n_mels]
- * whose column m is non-zero on bins [band[2m], band[2m+1]); apply_log: log(max(mel, 1e-5)).
- * wave [rows, t] -> mel [rows, n_mels, frames].  n_fft: a power of two in [32, 4096]. */
+/* MelSpectrogram (reference components.py:188-236): reflect padding by `pad`, then (center=True)
+ * reflect padding of that signal by `center_pad` (torch.stft's n_fft/2; 0 for center=False), frames
+ * of n_fft samples every `hop`, window [n_fft], |rFFT|, mel filterbank fb [n_fft/2+1, n_mels] whose
+ * column m is non-zero on bins [band[2m], band[2m+1]); apply_log: log(max(mel, 1e-5)).
+ * wave [rows, t] -> mel [rows, n_mels, frames], frames = 1 + (t + 2*pad + 2*center_pad - n_fft)/hop.
+ * n_fft: in [32, 8192] with prime factors 2, 3, 5, 7 only (mixed-radix FFT); n_mels <= 512;
+ * pad < t and center_pad < t + 2*pad (each pad shorter than the signal it mirrors). */
 int adp_mel_spectrogram(const float* wave, const float* window, const float* fb, const int32_t* band,
-                        float* mel, int rows, int t, int n_fft, int hop, int pad, int frames,
-                        int n_mels, int apply_log, adp_stream_t stream);
+                        float* mel, int rows, int t, int n_fft, int hop, int pad, int center_pad,
+                        int frames, int n_mels, int apply_log, adp_stream_t stream);
 
 /* DiffusionVocoder.to_flat (reference models.py:194-201): ConvTranspose1d(C -> 1, kernel win,
  * stride hop, padding pad, bias-free).  spec [B, C, frames], w [C, win], out [B, t_out] with
