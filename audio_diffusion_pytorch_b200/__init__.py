@@ -6,6 +6,7 @@ Every name of the reference's export list is implemented; what is not supported 
 from .components import AppendChannelsPlugin, LTPlugin, MelSpectrogram, UNetV0
 from .diffusion import (ARVDiffusion, ARVSampler, Diffusion, Distribution, Inpainter, LinearSchedule,
                         Sampler, Schedule, UniformDistribution, VDiffusion, VInpainter, VSampler)
+from .losses import MultiResolutionSTFTLoss, STFTLoss
 from .models import (AdapterBase, DiffusionAE, DiffusionAR, DiffusionModel, DiffusionUpsampler,
                      DiffusionVocoder, EncoderBase)
 from .unet import B200UNet
@@ -16,4 +17,5 @@ XUNet = B200UNet
 __all__ = ["UNetV0", "XUNet", "LTPlugin", "MelSpectrogram", "VDiffusion", "VSampler", "VInpainter",
            "LinearSchedule", "UniformDistribution", "Diffusion", "Distribution", "Sampler",
            "Schedule", "DiffusionModel", "DiffusionUpsampler", "DiffusionVocoder", "DiffusionAE",
-           "DiffusionAR", "ARVDiffusion", "ARVSampler", "EncoderBase", "AdapterBase", "AppendChannelsPlugin", "B200UNet", "Inpainter"]
+           "DiffusionAR", "ARVDiffusion", "ARVSampler", "EncoderBase", "AdapterBase", "AppendChannelsPlugin", "B200UNet", "Inpainter",
+           "MultiResolutionSTFTLoss", "STFTLoss"]

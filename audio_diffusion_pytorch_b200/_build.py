@@ -8,7 +8,7 @@ from concurrent.futures import ThreadPoolExecutor
 PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libadp_b200.so")
-SOURCES = ["common.cu", "conv_gemm.cu", "rowwise.cu", "stem.cu", "mid_conv.cu", "attention.cu", "attention_bwd.cu", "backward.cu", "wgrad.cu", "stem_bwd.cu", "frontend.cu", "verify_f32.cu", "verify_f32_bwd.cu"]
+SOURCES = ["common.cu", "conv_gemm.cu", "rowwise.cu", "stem.cu", "mid_conv.cu", "attention.cu", "attention_bwd.cu", "backward.cu", "wgrad.cu", "stem_bwd.cu", "frontend.cu", "stft_loss.cu", "verify_f32.cu", "verify_f32_bwd.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",

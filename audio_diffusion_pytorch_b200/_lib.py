@@ -117,6 +117,8 @@ def lib() -> C.CDLL:
         "adp_mel_spectrogram": [vp] * 5 + [C.c_int] * 9 + [vp],
         "adp_to_flat": [vp, vp, vp] + [C.c_int] * 7 + [vp],
         "adp_to_flat_bwd": [vp] * 5 + [C.c_int] * 7 + [vp],
+        "adp_stft_loss_fwd": [vp] * 7 + [C.c_int] * 7 + [f32] * 5 + [C.c_int, vp],
+        "adp_stft_loss_bwd": [vp] * 8 + [C.c_int] * 7 + [f32] * 5 + [C.c_int, vp],
         "adp_f32_conv_gemm": [C.POINTER(ConvGemmArgs), vp],
         "adp_f32_gn_stats": [vp, vp, i32, i32, i32, i32, vp],
         "adp_f32_gn_silu": [vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp],
@@ -177,7 +179,8 @@ EXPORTS = ["adp_version", "adp_last_error", "adp_device_check", "adp_conv_gemm",
            "adp_gn_bwd_apply", "adp_ln_film_bwd", "adp_colsum", "adp_skip_gate",
            "adp_skip_gate_bwd", "adp_cond_bwd", "adp_narrow_conv_bwd", "adp_stem_out_bwd",
            "adp_stem_in_bwd", "adp_attention_bwd", "adp_ln_fold_bwd", "adp_inpaint_blend", "adp_arv_step", "adp_resample", "adp_resample_adjoint",
-           "adp_mel_spectrogram", "adp_to_flat", "adp_to_flat_bwd", "adp_f32_conv_gemm", "adp_f32_gn_stats",
+           "adp_mel_spectrogram", "adp_to_flat", "adp_to_flat_bwd", "adp_stft_loss_fwd", "adp_stft_loss_bwd",
+           "adp_f32_conv_gemm", "adp_f32_gn_stats",
            "adp_f32_gn_silu", "adp_f32_ln_film", "adp_f32_attention", "adp_f32_linear", "adp_f32_silu",
            "adp_f32_stem_in", "adp_f32_stem_out", "adp_step_select", "adp_step_advance",
            "adp_attention_hd", "adp_attention_bwd_hd", "adp_f32_attention_hd", "adp_f32_attention_lse",

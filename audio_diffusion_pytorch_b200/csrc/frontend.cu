@@ -8,6 +8,7 @@
 //   adp_to_flat / _bwd        ConvTranspose1d(mel -> 1 channel, bias-free), reference
 //                             models.py:194-201, with the gradients of its weight and input
 #include "common.cuh"
+#include "fft.cuh"
 #include "ptx.cuh"
 
 namespace adp {
@@ -80,99 +81,7 @@ resample_adjoint_kernel(const float* __restrict__ dy, const float* __restrict__ 
 // triangle over a contiguous bin range [lo, hi) (host-computed from the filterbank's non-zeros):
 // a thread owns one (mel, frame) output.
 constexpr int kMelFrames = 8;
-constexpr int kMelMaxN = 8192;
-
-__device__ __forceinline__ float2 cmul(float2 a, float2 b) {
-  return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x);
-}
-__device__ __forceinline__ float2 cadd(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
-__device__ __forceinline__ float2 csub(float2 a, float2 b) { return make_float2(a.x - b.x, a.y - b.y); }
-
-// cos and sin of 2 pi j / R for R in {3, 5, 7} and 1 <= j <= R / 2
-__host__ __device__ constexpr float dft_cos(int R, int j) {
-  return R == 3 ? -0.5f
-       : R == 5 ? (j == 1 ? 0.30901699437494745f : -0.80901699437494745f)
-       : (j == 1 ? 0.62348980185873353f : j == 2 ? -0.22252093395631440f : -0.90096886790241913f);
-}
-__host__ __device__ constexpr float dft_sin(int R, int j) {
-  return R == 3 ? 0.86602540378443865f
-       : R == 5 ? (j == 1 ? 0.95105651629515357f : 0.58778525229247313f)
-       : (j == 1 ? 0.78183148246802981f : j == 2 ? 0.97492791218182361f : 0.43388373911755812f);
-}
-
-// In-register forward DFT of R points, X_k = sum_n v_n exp(-2 pi i k n / R).  Odd R pairs
-// v_m with v_(R-m): X_k = A_k - i B_k, X_(R-k) = A_k + i B_k with A_k = v_0 + sum_m (v_m + v_(R-m))
-// cos(2 pi k m / R) and B_k = sum_m (v_m - v_(R-m)) sin(2 pi k m / R).
-template <int R>
-__device__ __forceinline__ void dft(float2 (&v)[R]) {
-  constexpr int H = R / 2;
-  float2 s[H + 1], d[H + 1];
-  const float2 x0 = v[0];
-  float2 sum = x0;
-#pragma unroll
-  for (int m = 1; m <= H; ++m) {
-    s[m] = cadd(v[m], v[R - m]);
-    d[m] = csub(v[m], v[R - m]);
-    sum = cadd(sum, s[m]);
-  }
-  v[0] = sum;
-#pragma unroll
-  for (int k = 1; k <= H; ++k) {
-    float2 a = x0, b = make_float2(0.f, 0.f);
-#pragma unroll
-    for (int m = 1; m <= H; ++m) {
-      const int j = (k * m) % R;
-      const float c = j <= H ? dft_cos(R, j) : dft_cos(R, R - j);
-      const float sn = j <= H ? dft_sin(R, j) : -dft_sin(R, R - j);
-      a = make_float2(fmaf(s[m].x, c, a.x), fmaf(s[m].y, c, a.y));
-      b = make_float2(fmaf(d[m].x, sn, b.x), fmaf(d[m].y, sn, b.y));
-    }
-    v[k] = make_float2(a.x + b.y, a.y - b.x);
-    v[R - k] = make_float2(a.x - b.y, a.y + b.x);
-  }
-}
-template <>
-__device__ __forceinline__ void dft<2>(float2 (&v)[2]) {
-  const float2 a = v[0], b = v[1];
-  v[0] = cadd(a, b);
-  v[1] = csub(a, b);
-}
-template <>
-__device__ __forceinline__ void dft<4>(float2 (&v)[4]) {
-  const float2 t0 = cadd(v[0], v[2]), t1 = csub(v[0], v[2]), t2 = cadd(v[1], v[3]), t3 = csub(v[1], v[3]);
-  const float2 mt3 = make_float2(t3.y, -t3.x);                       // -i t3
-  v[0] = cadd(t0, t2);
-  v[1] = cadd(t1, mt3);
-  v[2] = csub(t0, t2);
-  v[3] = csub(t1, mt3);
-}
-
-// One Stockham radix-R stage after sub-transforms of length Ns: butterfly j (k = j mod Ns) reads
-// src[j + r N/R], twiddles input r by exp(-2 pi i k r / (Ns R)) and writes dst[(j - k) R + k + r Ns].
-template <int R>
-__device__ __forceinline__ void fft_stage(const float2* __restrict__ src, float2* __restrict__ dst,
-                                          const float2* __restrict__ tw, int N, int Ns) {
-  const int m = N / R, step = N / (Ns * R);
-  for (int j = threadIdx.x; j < m; j += blockDim.x) {
-    const int k = j % Ns;
-    float2 v[R];
-#pragma unroll
-    for (int r = 0; r < R; ++r) v[r] = src[j + r * m];
-    if (Ns > 1) {
-#pragma unroll
-      for (int r = 1; r < R; ++r) v[r] = cmul(v[r], tw[k * r * step]);
-    }
-    dft<R>(v);
-    float2* d = dst + (j - k) * R + k;
-#pragma unroll
-    for (int r = 0; r < R; ++r) d[r * Ns] = v[r];
-  }
-}
-
-// F.pad(mode="reflect") index: the edge sample is not repeated (|j| < len assumed)
-__device__ __forceinline__ int reflect_index(int j, int len) {
-  return j < 0 ? -j : (j >= len ? 2 * (len - 1) - j : j);
-}
+constexpr int kMelMaxN = kFftMaxN;
 
 __global__ void __launch_bounds__(256)
 mel_spectrogram_kernel(const float* __restrict__ wave, const float* __restrict__ window,
@@ -257,27 +166,6 @@ mel_spectrogram_kernel(const float* __restrict__ wave, const float* __restrict__
       out[static_cast<size_t>(m) * frames + f] = v;
     }
   }
-}
-
-// Radices of n, 4 bits per stage with the first stage lowest: 4s, at most one 2, then 3s, 5s, 7s.
-// 0 when n has a prime factor above 7.
-static unsigned long long mel_fft_plan(int n) {
-  unsigned long long plan = 0;
-  int shift = 0;
-  auto take = [&](int r) {
-    while (n % r == 0 && n > 1 && shift < 64) {
-      plan |= static_cast<unsigned long long>(r) << shift;
-      shift += 4;
-      n /= r;
-      if (r == 2) break;
-    }
-  };
-  take(4);
-  take(2);
-  take(3);
-  take(5);
-  take(7);
-  return n == 1 ? plan : 0;
 }
 
 // --------------------------------------------------------------------------- to_flat
@@ -396,7 +284,7 @@ extern "C" int adp_mel_spectrogram(const float* wave, const float* window, const
                                    int hop, int pad, int center_pad, int frames, int n_mels,
                                    int apply_log, adp_stream_t stream) {
   ADP_CHECK(wave && window && fb && band && mel, "adp_mel_spectrogram: null pointer");
-  const unsigned long long plan = n_fft >= 32 && n_fft <= kMelMaxN ? mel_fft_plan(n_fft) : 0;
+  const unsigned long long plan = n_fft >= 32 && n_fft <= kMelMaxN ? fft_plan(n_fft) : 0;
   ADP_CHECK(plan != 0, "adp_mel_spectrogram: n_fft=%d must have prime factors 2, 3, 5, 7 only and lie in [32, %d]",
             n_fft, kMelMaxN);
   ADP_CHECK(rows > 0 && rows <= 65535 && hop > 0 && frames > 0 && n_mels > 0 && n_mels <= 512,

@@ -322,6 +322,30 @@ int adp_to_flat(const float* spec, const float* w, float* out, int B, int C, int
 int adp_to_flat_bwd(const float* spec, const float* w, const float* dout, float* dspec, float* dw,
                     int B, int C, int frames, int win, int hop, int pad, int t_out, adp_stream_t stream);
 
+/* Multi-resolution STFT loss (losses.MultiResolutionSTFTLoss), one resolution per call.  x (the
+ * input) and y (the target) [rows, t], fp32 or bf16 (in_bf16); window fp32 [n_fft]: the periodic
+ * Hann window of win_length taps zero-padded to the centre of n_fft.  Frames are taken from the
+ * rows reflect-padded by n_fft/2 (torch.stft center=True): frames = 1 + (t + 2*(n_fft/2) - n_fft)/hop.
+ * Per frame, mag = sqrt(max(re^2 + im^2, eps)) of the one-sided spectrum, and the resolution's term is
+ *   L = w_sc * mean_rows ||Ymag - Xmag|| / ||Ymag|| + w_log_mag * mean |log Xmag - log Ymag|
+ *       + w_lin_mag * mean |Xmag - Ymag|.
+ * n_fft: in [32, 8192] with prime factors 2, 3, 5, 7 only; 1 <= win_length <= n_fft; hop >= 1;
+ * t > n_fft/2; rows <= 65535.  No atomics: results are bitwise reproducible.
+ * adp_stft_loss_fwd: partials fp64 [rows][ceil(frames/8)][4] (scratch), row_stats fp64 [rows][2]
+ * (||Y - X||, ||Y|| per row, read by the backward), acc fp64 [1] and loss fp32 [1]:
+ * acc = (accumulate ? acc : 0) + scale * L, loss = acc.
+ * adp_stft_loss_bwd: dL/dx of scale * L times grad_out[0] (fp32 [1], device): frame_grad fp32
+ * [rows][frames][win_length] (scratch), dx fp32 [rows, t] (= or += with accumulate) and, when
+ * dx_bf16 is not NULL, the same values rounded to bf16 [rows, t].  The target gets no gradient. */
+int adp_stft_loss_fwd(const void* x, const void* y, const float* window, double* partials,
+                      double* row_stats, double* acc, float* loss, int rows, int t, int n_fft, int hop,
+                      int win_length, int frames, int in_bf16, float eps, float w_sc, float w_log_mag,
+                      float w_lin_mag, float scale, int accumulate, adp_stream_t stream);
+int adp_stft_loss_bwd(const void* x, const void* y, const float* window, const double* row_stats,
+                      const float* grad_out, float* frame_grad, float* dx, void* dx_bf16, int rows, int t,
+                      int n_fft, int hop, int win_length, int frames, int in_bf16, float eps, float w_sc,
+                      float w_log_mag, float w_lin_mag, float scale, int accumulate, adp_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------
  * Backward (training) entry points: VDiffusion loss.backward() through UNetV0
  * (reference diffusion.py:82-95 + autograd over the a_unet blocks).  Data gradients are
