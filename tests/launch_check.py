@@ -460,11 +460,15 @@ def _shift(t, off):
 
 
 def _gn_xhat(x, stats, groups, eps):
-    """(xhat, rstd [B, 1, C]) of GroupNorm from the statistics slots (arithmetic of _gn_coef)."""
+    """(xhat, rstd [B, 1, C], |xhat|'s magnitude) of GroupNorm from the statistics slots (arithmetic
+    of _gn_coef).  The kernels form xhat = (x - mean) rstd in fp32: its rounding is relative to
+    (|x| + |mean|) rstd, which is far above |xhat| where x lies close to its group's mean.  A sum over
+    many rows hides that; a group of one row (an innermost level of length 1 at B = 1) does not."""
     B, T, C = x.shape
     one = torch.ones(C, dtype=F64, device=x.device)
     sc, sh = _gn_coef(stats, one, torch.zeros_like(one), groups, eps, T, C)     # rstd, -mean rstd
-    return x.to(F64) * sc + sh, sc
+    xf = x.to(F64)
+    return xf * sc + sh, sc, xf.abs() * sc + sh.abs()
 
 
 def _dsilu(z):
@@ -480,12 +484,13 @@ def _group_sums(t, groups):
     return t.reshape(B, T, groups, C // groups).sum(dim=(1, 3))
 
 
-def _gn_S(xh, groups):
-    """The GroupNorm backward sums S[b, g] = (sum dxh, sum dxh xhat) of dxh AS STORED."""
+def _gn_S(xh, xha, groups):
+    """The GroupNorm backward sums S[b, g] = (sum dxh, sum dxh xhat) of dxh AS STORED (xha: the
+    magnitude of xhat, _gn_xhat)."""
     def ref(p):
         d = p["dxh"].to(F64)
         return (torch.stack([_group_sums(d, groups), _group_sums(d * xh, groups)], -1),
-                torch.stack([_group_sums(d.abs(), groups), _group_sums((d * xh).abs(), groups)], -1))
+                torch.stack([_group_sums(d.abs(), groups), _group_sums(d.abs() * xha, groups)], -1))
     return ref
 
 
@@ -504,23 +509,26 @@ def c_wgrad(a, ctx):
 
 def c_gn_silu_bwd(a, ctx):
     x, G = a["x"], a["groups"]
-    xh, _ = _gn_xhat(x, a["stats"], G, a["eps"])
+    xh, _, xha = _gn_xhat(x, a["stats"], G, a["eps"])
     ga, da = a["gamma"].to(F64), a["da"].to(F64)
     dz = da * _dsilu(xh * ga + a["beta"].to(F64))
-    return [Val("dxh", arg("dxh"), dz * ga, DSILU_MAX * (da * ga).abs()),
-            Acc("dgamma", arg("dgamma"), (dz * xh).sum((0, 1)), (dz * xh).abs().sum((0, 1))),
-            Acc("dbeta", arg("dbeta"), dz.sum((0, 1)), dz.abs().sum((0, 1))),
-            Acc("S", arg("S"), _gn_S(xh, G))]
+    # SiLU' crosses zero (z = -1.28) by cancellation: dz's rounding is relative to DSILU_MAX |da|, as for
+    # dxh and narrow_conv_bwd; a sum over one row (M = 1) shows it
+    dza = DSILU_MAX * da.abs()
+    return [Val("dxh", arg("dxh"), dz * ga, dza * ga.abs()),
+            Acc("dgamma", arg("dgamma"), (dz * xh).sum((0, 1)), (dza * xha).sum((0, 1))),
+            Acc("dbeta", arg("dbeta"), dz.sum((0, 1)), dza.sum((0, 1))),
+            Acc("S", arg("S"), _gn_S(xh, xha, G))]
 
 
 def c_gn_bwd_apply(a, ctx):
     x, G = a["x"], a["groups"]
     B, T, C = x.shape
-    xh, rstd = _gn_xhat(x, a["stats"], G, a["eps"])
+    xh, rstd, xha = _gn_xhat(x, a["stats"], G, a["eps"])
     c = (a["S"].to(F64) / float(T * (C // G))).repeat_interleave(C // G, dim=1)[:, None]     # [B, 1, C, 2]
     d = a["dxh"].to(F64)
     ref = rstd * (d - c[..., 0] - xh * c[..., 1])
-    absr = rstd.abs() * (d.abs() + c[..., 0].abs() + (xh * c[..., 1]).abs())
+    absr = rstd.abs() * (d.abs() + c[..., 0].abs() + xha * c[..., 1].abs())
     if a["dres"] is not None:
         ref, absr = ref + a["dres"].to(F64), absr + a["dres"].to(F64).abs()
     outs = [Val("dx", arg("dx"), ref, absr)]
@@ -592,7 +600,7 @@ def _conv3_t(dy, w3):
 
 def c_narrow_conv_bwd(a, ctx):
     x, G = a["x"], a["groups"]
-    xh, _ = _gn_xhat(x, a["stats_in"], G, a["gn_eps"])
+    xh, _, xha = _gn_xhat(x, a["stats_in"], G, a["gn_eps"])
     ga = a["gamma"].to(F64)
     z = xh * ga + a["beta"].to(F64)
     act, dy = _silu(z), a["dy"].to(F64)
@@ -605,9 +613,9 @@ def c_narrow_conv_bwd(a, ctx):
     # the sums of dz inherit the error of da (fp32 dot products of 3 C terms): its absref, not |dz|
     dza = DSILU_MAX * da_abs
     return [Val("dxh", arg("dxh"), dz * ga, dza * ga.abs()),
-            Acc("dgamma", arg("dgamma"), (dz * xh).sum((0, 1)), (dza * xh.abs()).sum((0, 1))),
+            Acc("dgamma", arg("dgamma"), (dz * xh).sum((0, 1)), (dza * xha).sum((0, 1))),
             Acc("dbeta", arg("dbeta"), dz.sum((0, 1)), dza.sum((0, 1))),
-            Acc("S", arg("S"), _gn_S(xh, G)),
+            Acc("S", arg("S"), _gn_S(xh, xha, G)),
             Acc("dw", arg("dw"), dw, dwa),
             Acc("dbias", arg("dbias"), dy.sum((0, 1)), dy.abs().sum((0, 1)))]
 
@@ -930,7 +938,11 @@ RESULT: Dict[str, Callable] = {"fir_resample": _fir_result, "mel_spectrogram": _
 # fp32-output epilogue has no residual (adp_conv_gemm refuses one).
 # stem_out_bwd reads the block input only for the SkipAdapter's weight gradient, and stem_in_bwd
 # the weight only for dxin; stem_out reads x un-noised only for the loss target.
+# attention over a single key (the innermost level of length 1) has softmax identically 1: its
+# output is v whatever q and k are, and only the lse rows, when the launch writes them, read q and
+# k.  attention_bwd needs no entry: its P = exp(q k * scale - lse) takes lse as an input.
 NOT_READ: Dict[str, Callable] = {
+    "attention": lambda a: {"q", "k"} if a["k"].shape[1] == 1 and a["lse"] is None else set(),
     "narrow_conv": lambda a: {"w"} if a["w_packed"] is not None else set(),
     "conv_gemm": lambda a: {"residual"} if a["out"].dtype == torch.float32 else set(),
     "stem_out_bwd": lambda a: {"x", "append", "noise", "alpha", "beta"} if a["w_adapt"] is None else set(),
