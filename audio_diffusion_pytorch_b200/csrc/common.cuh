@@ -20,9 +20,11 @@ int set_error(const char* fmt, ...);  // returns non-zero, records the message (
 #define ADP_CUDA(expr)                                                                   \
   do {                                                                                   \
     cudaError_t e_ = (expr);                                                             \
-    if (e_ != cudaSuccess)                                                               \
+    if (e_ != cudaSuccess) {                                                             \
+      (void)cudaGetLastError();  /* a refused launch's error is not the next launch's */ \
       return ::adp::set_error("%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e_),    \
                               __FILE__, __LINE__);                                       \
+    }                                                                                    \
   } while (0)
 
 #define ADP_LAUNCH_CHECK() ADP_CUDA(cudaGetLastError())

@@ -628,6 +628,10 @@ extern "C" int adp_stem_in(const adp_stem_in_args* args, adp_stream_t stream) {
   if (stem_in_narrow(a)) {
     const size_t smem = (static_cast<size_t>(a.c0) * ci_total + a.c0) * sizeof(float);
     auto kernel = ci_total <= 4 ? stem_in_kernel<4> : stem_in_kernel<kStemInNarrowIn>;
+    // with its 16.5 KiB of static shared memory the weights pass the 48 KiB default from
+    // c0 (ci_total + 1) > 7808 (c0 = 256 at 30 to 32 inputs per position)
+    static SmemAttrCache smem_cache4, smem_cache;
+    ADP_CUDA(ensure_dyn_smem(kernel, smem, ci_total <= 4 ? smem_cache4 : smem_cache));
     dim3 grid(one_wave_gx(kernel, 256, smem, a.B, (a.T / a.f + 255) / 256), a.B);
     ADP_CUDA(launch_k(kernel, grid, dim3(256), smem, as_stream(stream), a));
   } else {

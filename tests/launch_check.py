@@ -41,6 +41,28 @@ inference, sampling and training programs (forward, fused loss and backward; tau
 attention_bwd, which rounds P and dS to bf16); the tensors fir_resample, mel_spectrogram, to_flat
 and to_flat_bwd allocate and return (RESULT); and the in-place sampler steps of VSampler's generic
 loop (sampler_step), VInpainter (inpaint_blend) and ARVSampler (arv_step).
+
+Guard mode (`Shadow(guard=True)`) also holds every launch to the bytes it is given.  After the
+snapshot, each distinct storage among the tensor arguments (nested tuples such as `gn` included) is
+copied into a fresh buffer laid out as [front guard | copy | back guard], each guard GUARD_BYTES,
+the copy at its storage's address modulo GUARD_ALIGN (every TMA and vector alignment holds) and the
+back guard starting at the storage's last byte + 1.  The guards and every byte of the copy outside
+all of the launch's argument views are poisoned: POISON_FLOAT (0x7F bytes: bf16 / fp32 3.39e38, fp64
+~1.4e306, finite, so a read survives fmaxf / fminf and comparisons where a NaN would not) for
+storages only floating tensors view, POISON_INT (zero) for any storage an integer tensor views
+(`step`, `ctrl`, `mask_u8`, the mel `band`), so no poisoned value becomes an index, an address or a
+loop bound.  The launch runs on views of the copies with the original offsets, shapes and strides
+(memoised by id(): `residual is out` and `x_next=plan.x` stay aliases); the tensors the RESULT
+kinds allocate inside `ops` come from a `torch` proxy (`_TorchProxy`) that puts them between guards
+too.  Afterwards every poisoned byte must be unchanged -- a failure names the launch, the argument
+view nearest the byte, whether it lies before the start, in an unviewed gap or past the end of the
+storage, and its distance in bytes and in rows of that view -- and the viewed bytes go back to the
+original storages, where the value and side-effect checks above run unchanged: a kernel that read
+poison shows there as a huge error.  `n_guarded` counts the guarded launches.
+
+Guard mode does not cover storages a kernel reaches only through a device-side address (the
+conditioning table whose address `ctrl[0]` holds: step_select reads it in place), arguments of
+kinds listed in READS_OUTSIDE_VIEW (none), nor workspaces the C library allocates itself.
 """
 import inspect
 import math
@@ -1006,6 +1028,195 @@ class Record:
         self.count, self.worst, self.label, self.where = 0, 0.0, "", ""
 
 
+# ---------------------------------------------------------------------------- guard bands
+GUARD_BYTES = 2 << 20          # each guard: twice the largest tile store (256 rows x 2048 bf16 columns)
+GUARD_ALIGN = 4096             # a copy keeps its storage's address modulo this (TMA and vector alignment)
+POISON_FLOAT = 0x7F            # bf16 / fp32 3.39e38, fp64 ~1.4e306: finite, so fmaxf and compares keep it
+POISON_INT = 0x00              # an index, address or loop bound read from a guard stays in range
+_INT_OF_SIZE = {1: torch.int8, 2: torch.int16, 4: torch.int32, 8: torch.int64}
+
+# Kinds whose contract is to read bytes outside the views they are passed: the guard check would
+# poison those bytes.  READS_OUTSIDE_VIEW[kind](args) -> names of such arguments, left in place.
+READS_OUTSIDE_VIEW: Dict[str, Callable] = {}
+
+
+def _extent(t):
+    """[first, last + 1) byte of t's view within its storage."""
+    es = t.element_size()
+    lo = t.storage_offset() * es
+    if t.numel() == 0:
+        return lo, lo
+    return lo, lo + (sum((s - 1) * st for s, st in zip(t.shape, t.stride())) + 1) * es
+
+
+def _row_bytes(t):
+    return (t.stride(-2) if t.dim() >= 2 else max(t.numel(), 1)) * t.element_size()
+
+
+class _Guarded:
+    """One storage's copy placed as [front guard | copy | back guard] in a fresh buffer, at the
+    storage's address modulo GUARD_ALIGN; the guards and every byte of the copy outside the viewed
+    bytes (`mask`) hold the poison byte."""
+
+    def __init__(self, nbytes, device, residue, poison):
+        self.n, self.poison = nbytes, poison
+        self.buf = torch.full((2 * GUARD_BYTES + GUARD_ALIGN + nbytes,), poison, dtype=torch.uint8, device=device)
+        self.off = GUARD_BYTES + (residue - (self.buf.data_ptr() + GUARD_BYTES)) % GUARD_ALIGN
+        self.copy = self.buf[self.off:self.off + nbytes]
+        self.mask = torch.zeros(nbytes, dtype=torch.uint8, device=device)
+        self.views: List[Tuple[str, torch.Tensor]] = []          # (argument, relocated view)
+
+    def view_of(self, name, t):
+        """t's view (same storage offset, shape and strides) over the copy; its bytes marked viewed."""
+        es = t.element_size()
+        assert self.off % es == 0
+        if t.numel():
+            _flat(self.mask.untyped_storage(), _INT_OF_SIZE[es], t.device).as_strided(
+                t.shape, t.stride(), t.storage_offset()).fill_(-1)
+        r = torch.empty(0, dtype=t.dtype, device=t.device).set_(
+            self.buf.untyped_storage(), self.off // es + t.storage_offset(), t.shape, t.stride())
+        self.views.append((name, r))
+        return r
+
+    def fill_from(self, storage):
+        """The viewed bytes from `storage`, poison elsewhere."""
+        src = _flat(storage, torch.uint8, self.buf.device)
+        for lo in range(0, self.n, SIDE_CHUNK):
+            c, m = self.copy[lo:lo + SIDE_CHUNK], self.mask[lo:lo + SIDE_CHUNK]
+            c.copy_(torch.where(m.bool(), src[lo:lo + SIDE_CHUNK], self.poison))
+
+    def copy_back(self, storage):
+        """The viewed bytes of the copy into `storage`; its other bytes stay as they are."""
+        dst = _flat(storage, torch.uint8, self.buf.device)
+        for lo in range(0, self.n, SIDE_CHUNK):
+            d, m = dst[lo:lo + SIDE_CHUNK], self.mask[lo:lo + SIDE_CHUNK]
+            d.copy_(torch.where(m.bool(), self.copy[lo:lo + SIDE_CHUNK], d))
+
+    def first_damage(self):
+        """(region, buffer index) of the poisoned byte nearest the copy that changed, or None."""
+        front = (self.buf[:self.off] != self.poison).nonzero()
+        if front.numel():
+            return "before the start", int(front[-1, 0])
+        for lo in range(0, self.n, SIDE_CHUNK):
+            bad = ((self.copy[lo:lo + SIDE_CHUNK] != self.poison) & (self.mask[lo:lo + SIDE_CHUNK] == 0)).nonzero()
+            if bad.numel():
+                return "in an unviewed gap", self.off + lo + int(bad[0, 0])
+        back = (self.buf[self.off + self.n:] != self.poison).nonzero()
+        if back.numel():
+            return "past the end", self.off + self.n + int(back[0, 0])
+        return None
+
+    def describe(self, region, i):
+        """Which argument view the damaged byte i lies nearest, and how far from it."""
+        rel = i - self.off
+        best = None
+        for name, v in self.views:
+            lo, hi = (e - self.off for e in _extent(v))
+            d = lo - rel if rel < lo else (rel - hi + 1 if rel >= hi else 0)
+            if best is None or d < best[0]:
+                best = (d, name, v, "before" if rel < lo else "past the end of")
+        d, name, v, side = best
+        row = _row_bytes(v)
+        where = (f"{self.off - i} bytes before the start of the storage" if region == "before the start" else
+                 f"{rel - self.n + 1} bytes past the end of the storage" if region == "past the end" else
+                 f"storage byte {rel}")
+        return (f"`{name}` damaged {region}: {where}, {d} bytes ({d / row:.3g} rows of {row} bytes) {side} "
+                f"its view {tuple(v.shape)}, byte {int(self.buf[i]):#04x} where poison {self.poison:#04x}")
+
+
+class Guards:
+    """The storages of one launch (or one direct call) relocated between poisoned guard bands.
+
+    relocate(args) gives the arguments as views of the copies (memoised by id(): one object stays
+    one object, views of one storage stay views of one copy); alloc() makes a tensor between guards
+    for a kernel to write (`torch_proxy()` hands these out as torch.empty / empty_like /
+    zeros_like); check() reports the first poisoned byte that changed; copy_back() returns the
+    viewed bytes to the original storages."""
+
+    def __init__(self):
+        self.items: Dict[int, Tuple[_Guarded, object]] = {}     # storage key -> (copy, original storage)
+        self.made: List[_Guarded] = []
+
+    def relocate(self, args: Dict[str, object], keep=frozenset()) -> Dict[str, object]:
+        """args with every tensor (nested tuples included) but those of the arguments in `keep`
+        replaced by its view of the relocated copy of its storage."""
+        owners: Dict[int, List[Tuple[str, torch.Tensor]]] = {}
+        for n, v in args.items():
+            for t in _tensors([v] if n not in keep else []):
+                owners.setdefault(_key(t), []).append((n, t))
+        for k, ts in owners.items():
+            st = ts[0][1].untyped_storage()
+            poison = POISON_FLOAT if all(t.is_floating_point() for _, t in ts) else POISON_INT
+            self.items[k] = (_Guarded(st.nbytes(), ts[0][1].device, st.data_ptr() % GUARD_ALIGN, poison), st)
+        memo: Dict[int, torch.Tensor] = {}
+
+        def sub(n, v):
+            if n in keep:
+                return v
+            if isinstance(v, torch.Tensor):
+                if id(v) not in memo:
+                    memo[id(v)] = self.items[_key(v)][0].view_of(n, v)
+                return memo[id(v)]
+            if isinstance(v, (tuple, list)):
+                return type(v)(sub(n, x) for x in v)
+            return v
+        out = {n: sub(n, v) for n, v in args.items()}
+        for g, st in self.items.values():
+            g.fill_from(st)
+        return out
+
+    def alloc(self, shape, dtype, device, name="result", zero=False):
+        shape = tuple(shape)
+        t = torch.empty(shape, dtype=dtype, device="meta")
+        g = _Guarded(t.numel() * t.element_size(), device, 0,
+                     POISON_FLOAT if t.is_floating_point() else POISON_INT)
+        r = g.view_of(name, torch.empty(shape, dtype=dtype, device=device))
+        if zero:
+            r.zero_()
+        self.made.append(g)
+        return r
+
+    def torch_proxy(self):
+        return _TorchProxy(self)
+
+    def name(self, t, name):
+        """Names the allocated tensor t (as its launch's output) in the check's messages."""
+        for g in self.made:
+            g.views = [(name if v.data_ptr() == t.data_ptr() else n, v) for n, v in g.views]
+
+    def check(self, fail):
+        for g in [g for g, _ in self.items.values()] + self.made:
+            bad = g.first_damage()
+            if bad is not None:
+                fail(g.describe(*bad))
+
+    def copy_back(self):
+        for g, st in self.items.values():
+            g.copy_back(st)
+
+
+class _TorchProxy:
+    """`torch` for a module whose calls allocate the outputs of a guarded launch: empty, empty_like
+    and zeros_like give tensors between guard bands, every other name is torch's."""
+
+    def __init__(self, guards):
+        self._guards = guards
+
+    def empty(self, *size, dtype=None, device=None):
+        if len(size) == 1 and isinstance(size[0], (tuple, list, torch.Size)):
+            size = size[0]
+        return self._guards.alloc(size, dtype or torch.get_default_dtype(), device or "cpu")
+
+    def empty_like(self, t):
+        return self._guards.alloc(t.shape, t.dtype, t.device)
+
+    def zeros_like(self, t):
+        return self._guards.alloc(t.shape, t.dtype, t.device, zero=True)
+
+    def __getattr__(self, name):
+        return getattr(torch, name)
+
+
 class Shadow:
     """Context manager: every ops launch of a CHECKERS kind is checked (see the module docstring).
 
@@ -1013,13 +1224,14 @@ class Shadow:
     (statistics: those of the written output).  probe=True: the first launch of each kind and set
     of passed tensors also runs _probe.  mutate=(kind, fn): after the first launch of that
     kind where fn(args, outs, snapshot) applies (does not return False), fn damages what it
-    wrote (the checker's self-test)."""
+    wrote (the checker's self-test).  guard=True: each launch runs on copies of its storages
+    between poisoned guard bands (Guards; see the module docstring), and mutate's fn sees those."""
 
-    def __init__(self, fake: bool = False, mutate=None, probe: bool = False):
-        self.fake, self.mutate, self.probe = fake, mutate, probe
+    def __init__(self, fake: bool = False, mutate=None, probe: bool = False, guard: bool = False):
+        self.fake, self.mutate, self.probe, self.guard = fake, mutate, probe, guard
         self.probed = set()
         self.records: Dict[str, Record] = {}
-        self.n_launch, self.n_checked = 0, 0
+        self.n_launch, self.n_checked, self.n_guarded = 0, 0, 0
         self.labels = set()                      # trace labels of the launches seen (shapes included)
         self.known: Dict[int, torch.Tensor] = {}
 
@@ -1083,30 +1295,71 @@ class Shadow:
             if self.probe and variant not in self.probed:      # once per set of passed / returned tensors
                 self._probe(idx, name, outs, pre)
                 self.probed.add(variant)
+            guards = Guards() if self.guard else None
+            run = post                           # the arguments the launch runs on
+            if guards is not None:
+                run = guards.relocate(post, READS_OUTSIDE_VIEW[name](pre) if name in READS_OUTSIDE_VIEW else ())
             if self.fake:
                 dev = next(_tensors(list(post.values()))).device
                 for n, shape in made.items():
-                    post[n] = None if shape is None else torch.empty(shape, dtype=torch.float32, device=dev)
-                result = tuple(post[n] for n in made) if len(made) > 1 else \
-                    (post[next(iter(made))] if made else None)
-                self._fake_write(outs, pre, post)
+                    run[n] = None if shape is None else \
+                        guards.alloc(shape, torch.float32, dev, n) if guards is not None else \
+                        torch.empty(shape, dtype=torch.float32, device=dev)
+                result = tuple(run[n] for n in made) if len(made) > 1 else \
+                    (run[next(iter(made))] if made else None)
+                self._fake_write(outs, pre, run)
                 label = label0
             else:
-                with ops.trace() as tr:
-                    result = real(*args, **kwargs)
+                if guards is None:
+                    with ops.trace() as tr:
+                        result = real(*args, **kwargs)
+                else:
+                    call = inspect.BoundArguments(sig, {n: run[n] for n in b.arguments})
+                    saved = ops.torch
+                    if name in RESULT:           # the outputs ops allocates go between guards too
+                        ops.torch = guards.torch_proxy()
+                    try:
+                        with ops.trace() as tr:
+                            result = real(*call.args, **call.kwargs)
+                    finally:
+                        ops.torch = saved
                 label = tr.records[-1]["name"] if tr.records else label0
                 if post[next(iter(post))].is_cuda:
                     torch.cuda.synchronize()
-                post.update(zip(made, result if len(made) > 1 else (result,)))
+                run.update(zip(made, result if len(made) > 1 else (result,)))
             if self.mutate is not None and self.mutate[0] == name:
-                if self.mutate[1](post, outs, pre) is not False:       # False: not applicable here
+                if self.mutate[1](run, outs, pre) is not False:       # False: not applicable here
                     self.mutate = None
             self.labels.add(label)
+            if guards is not None:
+                result = self._unguard(idx, name, label, guards, post, run, made, result)
             self._check(idx, name, label, outs, pre, post, snaps)
             snaps.clear()            # `snap` refers to itself: without this the snapshots wait for the cycle collector
             self.n_checked += 1
             return result
         return launch
+
+    def _unguard(self, idx, name, label, guards, post, run, made, result):
+        """Guard check of a relocated launch; then its viewed bytes go back to the original
+        storages, the tensors it allocated are handed back as plain copies, and `result` (the
+        launch's return value) refers to those and to the original arguments."""
+        for n in made:
+            if run[n] is not None:
+                guards.name(run[n], n)
+        guards.check(lambda msg: self._fail(idx, name, label, f"guard: {msg}"))
+        guards.copy_back()
+        back = {}
+        for n, v in post.items():
+            for o, r in zip(_tensors([v]), _tensors([run[n]])):
+                back[id(r)] = o
+        for n in made:
+            post[n] = None if run[n] is None else run[n].clone()
+            if run[n] is not None:
+                back[id(run[n])] = post[n]
+        self.n_guarded += 1
+        if isinstance(result, tuple):
+            return tuple(back.get(id(r), r) if r is not None else None for r in result)
+        return back.get(id(result), result) if result is not None else None
 
     def _check_roles(self, idx, name, outs, post, made):
         """The checker's outputs are exactly the output arguments the launch was given and the
@@ -1279,7 +1532,8 @@ class Shadow:
         for k in sorted(self.records):
             r = self.records[k]
             lines.append(f"{k:28s} {r.count:6d} {r.worst:16.4f}  {r.label} {r.where}")
-        lines.append(f"launches {self.n_launch}, checked {self.n_checked}")
+        lines.append(f"launches {self.n_launch}, checked {self.n_checked}" +
+                     (f", guarded {self.n_guarded}" if self.guard else ""))
         return "\n".join(lines)
 
 
