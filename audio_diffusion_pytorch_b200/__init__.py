@@ -9,13 +9,11 @@ from .diffusion import (ARVDiffusion, ARVSampler, Diffusion, Distribution, Inpai
 from .losses import MultiResolutionSTFTLoss, STFTLoss
 from .models import (AdapterBase, DiffusionAE, DiffusionAR, DiffusionModel, DiffusionUpsampler,
                      DiffusionVocoder, EncoderBase)
+from .apex import ClassifierFreeGuidancePlugin, TimeConditioningPlugin, XUNet
 from .unet import B200UNet
-
-
-XUNet = B200UNet
 
 __all__ = ["UNetV0", "XUNet", "LTPlugin", "MelSpectrogram", "VDiffusion", "VSampler", "VInpainter",
            "LinearSchedule", "UniformDistribution", "Diffusion", "Distribution", "Sampler",
            "Schedule", "DiffusionModel", "DiffusionUpsampler", "DiffusionVocoder", "DiffusionAE",
            "DiffusionAR", "ARVDiffusion", "ARVSampler", "EncoderBase", "AdapterBase", "AppendChannelsPlugin", "B200UNet", "Inpainter",
-           "MultiResolutionSTFTLoss", "STFTLoss"]
+           "MultiResolutionSTFTLoss", "STFTLoss", "TimeConditioningPlugin", "ClassifierFreeGuidancePlugin"]

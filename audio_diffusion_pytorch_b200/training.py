@@ -340,10 +340,21 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
     finals: List = []                      # closures turning packed grads into PyTorch layout
     # one flat fp32 arena for every gradient accumulator: a single memset per backward
     n_param = sum(p.numel() for p in net.parameters())
-    # the repeated attention items of a level (counts > 1) each add a projection-gradient scratch
-    # smaller than their parameters on top of their gradients
-    n_extra = sum(p.numel() for lv in levels for it in (*lv.items_down, *lv.items_up)
-                  for am in (it.attentions()[1:] + it.crosses()[1:]) for p in am.parameters())
+    # every attention item adds a projection-gradient scratch smaller than its parameters on top of
+    # its gradients; the margin below covers the first AttentionItem and CrossAttentionItem after each
+    # ResnetItem (one UNetV0 repetition), every further one adds its parameters, and so does every
+    # attention item ahead of a chain's first ResnetItem (no ResnetItem pays for its scratch)
+    def extra_attention(chain):
+        seen = {"att", "cross"}
+        for kind, m in chain:
+            if kind == "resnet":
+                seen.clear()
+            elif kind in ("att", "cross"):
+                if kind in seen:
+                    yield m
+                seen.add(kind)
+    n_extra = sum(p.numel() for lv in levels for up in (False, True) for am in extra_attention(lv.chain(up))
+                  for p in am.parameters())
     flat = torch.zeros(int(1.25 * n_param) + n_extra + 64 * (4 * n_param // 1000 + 4096), device=dev)
     cursor = [0]
 
@@ -368,7 +379,7 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
         return t
 
     n_tot = P["cond_n"]
-    mod = net.use_modulation       # False: no ModulationItems, SkipCat merges (reference components.py:90,99)
+    mod = net.use_modulation       # False: no conditioning projection (no ModulationItem, no SkipModulate)
     ss_all = _zeros((B, max(8, ops.round_up(n_tot, 8))), dev)
     dss_all = gbuf(ss_all.shape)
     ss_stride = ss_all.shape[1]
@@ -453,14 +464,17 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
                 return dx
         return bwd
 
-    # ---- backward of one [ResnetItem, ModulationItem, InjectChannelsItem?] + AttentionItems +
-    # CrossAttentionItems from the tensors of the walk's forward
-    def item_backward(rec, ip: Dict, im, C: int, Tl: int, li: int):
-        res, inj, atts = rec
-        r_ = im.resnet
+    def cond_grads(mm, off: int, n: int) -> None:
+        """A ModulationItem's or SkipModulate's Linear is one slice of the conditioning projection."""
+        grads[id(mm.proj.weight if hasattr(mm, "proj") else mm.weight)] = ("cond_w", off, n)
+        grads[id(mm.proj.bias if hasattr(mm, "proj") else mm.bias)] = ("cond_b", off, n)
+
+    # ---- backward of a ResnetItem and the ModulationItem the walk fused into it (mm: its module)
+    def resnet_backward(res: Dict, ip: Dict, r_, mm, mp: Optional[Dict], C: int, Tl: int):
         x, h, rr, ss = res["x"], res["h"], res["r"], res["ss"]
         xs, hs = res["x_stats"], res["h_stats"]
-        dss = dss_all[:, ip["ss_off"]:] if mod else None
+        mod = mp is not None
+        dss = dss_all[:, mp["ss_off"]:] if mod else None
         S1, S2 = new_stats(), new_stats()
         dgn1 = (grad_for(r_.gn1.weight), grad_for(r_.gn1.bias))
         dgn2 = (grad_for(r_.gn2.weight), grad_for(r_.gn2.bias))
@@ -499,37 +513,49 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
                 return resnet_item_bwd(dy, x, h, rr, a1, a2, xs, hs, ip["gn1"], ip["gn2"], wd1, wd2, gw1, gw2,
                                        dgn1, dgn2, db1, db2, S1, S2, work, G, film=film)
         if mod:
-            grads[id(im.modulation.proj.weight)] = ("cond_w", ip["ss_off"], 2 * C)
-            grads[id(im.modulation.proj.bias)] = ("cond_b", ip["ss_off"], 2 * C)
-        chain = [bwd]
-        if inj is not None:
-            # a_unet InjectChannelsItem: conv1x1(cat([x, ctx])) + x, W = [W_x | W_c]
-            conv, ctxb, dctxb = im.inject, inj["ctx"], plan.dctx[li]
-            n_ctx, ctx_pad = conv.weight.shape[1] - C, ctxb.shape[-1]
-            dyi = act(B, Tl, C)
-            gw_inj = grad_for(conv.weight, (C, C + n_ctx, 1)).view(C, C + n_ctx)
-            db_inj = grad_for(conv.bias)
-            wd_x, wd_c = packed_dgrad(lambda: pack_inject_dgrad(conv.weight, C, ctx_pad))
-            # d context is summed over the items of this depth (in place through the residual)
-            chain.append(lambda d_out: inject_bwd(d_out, inj["x"], ctxb, dctxb, wd_x, wd_c, gw_inj, db_inj, dyi,
-                                                  n_ctx))
-        # every AttentionItem, then every CrossAttentionItem (the walk's order); run in reverse
-        ams = [(False, am) for am in im.attentions()] + [(True, am) for am in im.crosses()]
-        for a, (cross, am) in zip(atts, ams):
-            chain.append(attention_backward(a, am, cross, Tl, C))
+            cond_grads(mm, mp["ss_off"], 2 * C)
+        return bwd
 
-        def item_bwd(dy):
-            for fn in reversed(chain):
-                dy = fn(dy)
-            return dy
-        return item_bwd
+    # ---- backward of a ModulationItem that runs as its own ln_film pass
+    def modulation_backward(rec: Dict, mm, mp: Dict, C: int, Tl: int):
+        dx, dss = act(B, Tl, C), dss_all[:, mp["ss_off"]:]
+        cond_grads(mm, mp["ss_off"], 2 * C)
 
-    # ---- one item chain: the walk's forward (output statistics of every item, the last one
-    # included) and one backward closure per item
-    def run_items(x: Tensor, x_stats: Tensor, items_p: List[Dict], items_m, lv: LevelParams, Tl: int, li: int):
-        x, x_stats, recs = walk.items(x, x_stats, items_p, lv.ch, Tl, li, last_needs_stats=True)
-        return x, x_stats, [item_backward(rec, ip, im, lv.ch, Tl, li)
-                            for rec, ip, im in zip(recs, items_p, items_m)]
+        def bwd(dy):
+            ops.ln_film_bwd(dy, rec["x"], rec["ss"], ss_stride, dx, dss=dss, dss_stride=ss_stride,
+                            eps=net.MOD_LN_EPS)
+            return dx
+        return bwd
+
+    # ---- backward of an InjectChannelsItem: a_unet's conv1x1(cat([x, ctx])) + x, W = [W_x | W_c]
+    def inject_backward(inj: Dict, conv, C: int, Tl: int, li: int):
+        ctxb, dctxb = inj["ctx"], plan.dctx[li]
+        n_ctx, ctx_pad = conv.weight.shape[1] - C, ctxb.shape[-1]
+        dyi = act(B, Tl, C)
+        gw_inj = grad_for(conv.weight, (C, C + n_ctx, 1)).view(C, C + n_ctx)
+        db_inj = grad_for(conv.bias)
+        wd_x, wd_c = packed_dgrad(lambda: pack_inject_dgrad(conv.weight, C, ctx_pad))
+        # d context is summed over the items of this depth (in place through the residual)
+        return lambda d_out: inject_bwd(d_out, inj["x"], ctxb, dctxb, wd_x, wd_c, gw_inj, db_inj, dyi, n_ctx)
+
+    # ---- one item chain: the walk's forward (output statistics of every unit, the last one
+    # included) and one backward closure per unit, built from the walk's records
+    def run_items(x: Tensor, x_stats: Tensor, items_p: List, chain_m: List, lv: LevelParams, Tl: int, li: int):
+        C = lv.ch
+        x, x_stats, recs = walk.items(x, x_stats, items_p, C, Tl, li, last_needs_stats=True)
+        bwds = []
+        for kind, i, width, rec in recs:
+            m, pk = chain_m[i][1], items_p[i][1]
+            if kind == "resnet":
+                mm, mp = (chain_m[i + 1][1], items_p[i + 1][1]) if width == 2 else (None, None)
+                bwds.append(resnet_backward(rec, pk, m, mm, mp, C, Tl))
+            elif kind == "mod":
+                bwds.append(modulation_backward(rec, m, pk, C, Tl))
+            elif kind == "inj":
+                bwds.append(inject_backward(rec, m, C, Tl, li))
+            else:
+                bwds.append(attention_backward(rec, m, kind == "cross", Tl, C))
+        return x, x_stats, bwds
 
     # ---- recursive level walk; returns (output tensor, its stats, backward closure)
     def level(i: int, x_in: Optional[Tensor], T_in: int):
@@ -553,21 +579,24 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
             wd_down = packed_dgrad(lambda: pack_down_dgrad(lv.down.weight))
             # [co][tap][ci] (the [B, T/f, f*C] view) -> PyTorch [co][ci][tap]
             gw_down = grad_for(lv.down.weight, (C, lv.factor, lv.in_ch), (0, 2, 1)).view(C, lv.factor * lv.in_ch)
-        x, st, items_down_bwd = run_items(x0, st0, Lp["items_down"], lv.items_down, lv, Tl, li=i)
+        x, st, items_down_bwd = run_items(x0, st0, Lp["items_down"], lv.chain(up=False), lv, Tl, li=i)
         cur["down_end"] = cursor[0]
         inner = None
         skip = x
         if not innermost:
             x, st, inner = level(i + 1, skip, Tl)
         cur["inner_end"] = cursor[0]
-        x, st, items_up_bwd = run_items(x, st, Lp["items_up"], lv.items_up, lv, Tl, li=i)
-        if mod:
+        x, st, items_up_bwd = run_items(x, st, Lp["items_up"], lv.chain(up=True), lv, Tl, li=i)
+        merge = net.merge
+        if merge == "modulate":
             gate = ss_all[:, Lp["gate_off"]:]
             dgate = dss_all[:, Lp["gate_off"]:]
-            grads[id(lv.merge.weight)] = ("cond_w", Lp["gate_off"], lv.out_ch)
-            grads[id(lv.merge.bias)] = ("cond_b", Lp["gate_off"], lv.out_ch)
+            cond_grads(lv.merge, Lp["gate_off"], lv.out_ch)
         x_last = x
-        if i == 0 and not mod:
+        if i == 0 and merge == "add":
+            # SkipAdd at level 0: the stem epilogue with a unit gate, whose gradient is not used
+            gate, dgate = torch.ones(B, max(8, lv.out_ch), device=dev), gbuf((B, max(8, lv.out_ch)))
+        if i == 0 and merge == "cat":
             # SkipCat at level 0 runs in the stem kernels with the 1x1 merge conv folded into both
             # branches (B200UNet._compute_packed): they produce the gradients of the FOLDED
             # weights, unfolded below (a few hundred numbers) into merge / up / adapter gradients
@@ -589,7 +618,7 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
         else:
             db_up = grad_for(lv.up.bias)
         if i == 0:
-            if mod:
+            if merge != "cat":
                 dw_up = grad_for(lv.up.weight)
                 dwa = (grad_for(lv.adapter.weight, (lv.out_ch, lv.in_ch, 1)).view(lv.out_ch, lv.in_ch)
                        if lv.adapter is not None else None)
@@ -635,11 +664,15 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
         else:
             wd_up = packed_dgrad(lambda: ops.pack_conv_dgrad(lv.up.weight.detach()))
             gw_up = grad_for(lv.up.weight, (3, Co, C), (1, 2, 0))
-        if mod:
+        if merge == "add":
+            d_skip_of = lambda d_out: d_out      # noqa: E731
+            merge_bwd = lambda d_out: d_out      # noqa: E731  (out = x_in + y_up: both gradients are d_out)
+        elif merge == "modulate":
             d_skip_of = lambda d_out: d_out      # noqa: E731  (the skip path's gradient is d_out itself)
 
-            def merge_bwd(d_out: Tensor) -> None:
+            def merge_bwd(d_out: Tensor) -> Tensor:
                 ops.skip_gate_bwd(d_out, y_up, gate, dys, dgate)
+                return dys
         else:
             rp = max(1, 16 // Co)                # positions per GEMM row of the SkipCat merge
             d_skip = act(B, T_in, Co)
@@ -650,12 +683,12 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
             blk1, blk2 = gbuf((rp * Co, rp * Co)), gbuf((rp * Co, rp * Co))
             d_skip_of = lambda d_out: d_skip     # noqa: E731
 
-            def merge_bwd(d_out: Tensor) -> None:
+            def merge_bwd(d_out: Tensor) -> Tensor:
                 skipcat_bwd(d_out, x_in, y_up, wd_c1, wd_c2, gw_cat, db_cat, blk1, blk2, dys, d_skip, rp)
+                return dys
 
         def backward_level(d_out: Tensor) -> Tensor:
-            merge_bwd(d_out)
-            upsample_bwd(dys, x_last, wd_up, gw_up, db_up, dx_last, f)
+            upsample_bwd(merge_bwd(d_out), x_last, wd_up, gw_up, db_up, dx_last, f)
             d = dx_last
             for b_ in reversed(items_up_bwd):
                 d = b_(d)
@@ -911,6 +944,12 @@ def _time_cond(net: B200UNet, sigmas: Optional[Tensor], features: Optional[Tenso
     PyTorch ops so that autograd provides the gradients of its three [B,1024] linears."""
     if net.time is not None:
         assert sigmas is not None, "time conditioning requires the time argument"
+    if not net.use_modulation:
+        # no ModulationItem and no SkipModulate: nothing consumes the features.  An XUNet may still
+        # carry the time plugin (a_unet ignores its output then); its MLP gets no gradient
+        ref = next(net.parameters())
+        return torch.zeros(1, net.features, device=ref.device)
+    if net.time is not None:
         t = net.time
         s = sigmas.float().reshape(-1, 1)
         fr = s * t.weights * 2 * pi
@@ -918,9 +957,6 @@ def _time_cond(net: B200UNet, sigmas: Optional[Tensor], features: Optional[Tenso
         f = F.gelu(t.mlp(F.gelu(t.mlp(F.gelu(emb)))))
         if features is not None:
             f = f + features
-    elif not net.use_modulation:         # no ModulationItems: nothing consumes the features
-        ref = next(net.parameters())
-        return torch.zeros(1, net.features, device=ref.device)
     else:
         assert features is not None, "use_time_conditioning=False needs features="
         f = features

@@ -102,6 +102,10 @@ class ItemParams(nn.Module):
         return first + list(getattr(self, "extra_cross", []))
 
 
+# the a_unet item types a chain may hold, by the name the program builder knows them under
+ITEM_KINDS = ("resnet", "mod", "inj", "att", "cross")
+
+
 class LevelParams(nn.Module):
     """a_unet Block: registration order = skip_adapter, (down, items, inner, items_up, up), merge."""
 
@@ -119,6 +123,18 @@ class LevelParams(nn.Module):
         self.merge = (nn.Linear(item_kw["features"], out_ch) if item_kw.get("modulation", True)
                       else nn.Conv1d(2 * out_ch, out_ch, 1))
         self.in_ch, self.out_ch, self.ch, self.factor = in_ch, out_ch, ch, factor
+
+    def chain(self, up: bool) -> List[Tuple[str, nn.Module]]:
+        """The down (up=False) or up item chain as (kind, module) per a_unet item, in order."""
+        out = []
+        for it in (self.items_up if up else self.items_down):
+            out.append(("resnet", it.resnet))
+            if it.modulation is not None:
+                out.append(("mod", it.modulation))
+            if it.inject is not None:
+                out.append(("inj", it.inject))
+            out += [("att", a) for a in it.attentions()] + [("cross", a) for a in it.crosses()]
+        return out
 
 
 class TimeParams(nn.Module):
@@ -210,7 +226,7 @@ class _ForwardWalk:
         self.net, self.P, self.add, self.Bh, self.keep = net, P, add, Bh, keep
         self.pool = _Pool(net.net.down.weight.device, reuse=not keep, dtype=net._act_dtype())
         self.stats, self.n_stats = stats, 0
-        self.ss_all, self.ss_stride, self.mod = ss_all, ss_all.shape[1], net.use_modulation
+        self.ss_all, self.ss_stride = ss_all, ss_all.shape[1]
         self.ctx, self.embedding, self.add_ctx = ctx, embedding, add_ctx
         self.en = en         # LayerNorm(embedding), shared by all cross-attentions; made on first use
         self.G = net.groups
@@ -222,48 +238,50 @@ class _ForwardWalk:
         self.n_stats += 1
         return s
 
-    def items(self, x: Tensor, x_stats: Tensor, items_p: List[Dict], C: int, Tl: int, li: int,
+    def items(self, x: Tensor, x_stats: Tensor, chain: List[Tuple[str, Dict]], C: int, Tl: int, li: int,
               last_needs_stats: bool):
-        """One item chain of level li; returns (output, its statistics, one record per item)."""
-        recs = []
-        for idx, ip in enumerate(items_p):
-            want_stats = idx < len(items_p) - 1 or last_needs_stats
-            x, x_stats, rec = self.item(x, x_stats, ip, C, Tl, li, want_stats)
-            recs.append(rec)
+        """One item chain of level li: `chain` holds (kind, pack) per a_unet item, in order, kind in
+        ITEM_KINDS.  Returns (output, its statistics, one record per emitted unit).
+
+        The items are emitted in order, with these fusions wherever their pattern occurs: a
+        ModulationItem right after a ResnetItem runs in that ResnetItem's epilogue or its ln_film
+        pass, and that pass also writes the LayerNorm of an attention item right after it.  A unit
+        writes the GroupNorm statistics of its output only when a ResnetItem reads them (the next
+        item, or for the last one the caller's last_needs_stats).  Each record is (kind, index of
+        its first item in the chain, number of items it covers, its tensors)."""
+        recs, xn, i, n = [], None, 0, len(chain)
+        while i < n:
+            kind, pk = chain[i]
+            width = 2 if (kind == "resnet" and i + 1 < n and chain[i + 1][0] == "mod") else 1
+            j = i + width
+            want_stats = chain[j][0] == "resnet" if j < n else last_needs_stats
+            pre_norm = j < n and chain[j][0] in ("att", "cross")
+            y_stats = self.new_stats() if want_stats else None
+            if kind == "resnet":
+                rec = self._resnet(x, x_stats, pk, chain[i + 1][1] if width == 2 else None, C, Tl, y_stats,
+                                   pre_norm)
+            elif kind == "mod":
+                rec = self._modulation(x, pk, C, Tl, y_stats, pre_norm)
+            elif kind == "inj":
+                rec = self._inject(x, pk, C, Tl, li, y_stats)
+            else:
+                rec = self._attention(x, xn, pk, kind == "cross", C, Tl, y_stats)
+            x, x_stats, xn = rec["y"], y_stats, rec.get("xn") if kind in ("resnet", "mod") else None
+            recs.append((kind, i, width, rec))
+            i = j
         return x, x_stats, recs
 
-    def item(self, x: Tensor, x_stats: Tensor, ip: Dict, C: int, Tl: int, li: int, want_stats: bool):
-        """[ResnetItem, ModulationItem?, InjectChannelsItem?] + AttentionItems + CrossAttentionItems;
-        returns (output, its statistics, (resnet record, inject record or None, attention records)).
-        Only the item's last launch writes the statistics of the next GroupNorm; the first attention
-        reads the pre-norm of the Modulation pass, every later one runs its own LayerNorm."""
-        chain = [(False, ap) for ap in ip.get("att", [])] + [(True, ap) for ap in ip.get("cross", [])]
-        has_inj = "inj" in ip
-        y_stats = self.new_stats() if (want_stats and not (chain or has_inj)) else None
-        res = self._resnet(x, x_stats, ip, C, Tl, y_stats, bool(chain) and not has_inj)
-        x, x_stats, xn = res["y"], y_stats, res["xn"]
-        inj = None
-        if has_inj:
-            x_stats = self.new_stats() if (want_stats and not chain) else None
-            inj = self._inject(x, ip["inj"], C, Tl, li, x_stats)
-            x = inj["y"]
-        atts = []
-        for j, (cross, ap) in enumerate(chain):
-            x_stats = self.new_stats() if (want_stats and j == len(chain) - 1) else None
-            atts.append(self._attention(x, xn, ap, cross, C, Tl, x_stats))
-            x, xn = atts[-1]["y"], None
-        return x, x_stats, (res, inj, atts)
-
-    def _resnet(self, x: Tensor, x_stats: Tensor, ip: Dict, C: int, Tl: int, y_stats: Optional[Tensor],
-                pre_norm: bool) -> Dict:
-        """ResnetItem + ModulationItem.  pre_norm: the Modulation pass also writes the following
-        attention's LayerNorm (xn) when it runs as its own kernel."""
-        net, pool, add, G, Bh, mod = self.net, self.pool, self.add, self.G, self.Bh, self.mod
+    def _resnet(self, x: Tensor, x_stats: Tensor, ip: Dict, mp: Optional[Dict], C: int, Tl: int,
+                y_stats: Optional[Tensor], pre_norm: bool) -> Dict:
+        """ResnetItem, and the ModulationItem right after it when mp (its pack) is given.  pre_norm:
+        the Modulation pass also writes the following attention's LayerNorm (xn) when it runs as its
+        own kernel."""
+        net, pool, add, G, Bh, mod = self.net, self.pool, self.add, self.G, self.Bh, mp is not None
         narrow = C == 8 and not net.verify_fp32
         # thin levels (C = 32, 64) are HBM-bound: one fused ConvBlock kernel (mid_conv.cu)
         # instead of gn_silu -> conv_gemm (-> ln_film)
         fused = not self.keep and (narrow or (net.fuse_thin_levels and C in (32, 64) and not net.verify_fp32))
-        ss = self.ss_all[:, ip["ss_off"]:] if mod else None
+        ss = self.ss_all[:, mp["ss_off"]:] if mod else None
         (g1, be1), (g2, be2) = ip["gn1"], ip["gn2"]
         h_stats = self.new_stats()
         h = pool.get(Bh, Tl, C)
@@ -281,7 +299,7 @@ class _ForwardWalk:
         else:
             r = pool.get(Bh, Tl, C)
             y = pool.get(Bh, Tl, C) if mod else r
-            # use_modulation=False: the ResnetItem's output IS the item's output, so its
+            # no ModulationItem: the ResnetItem's output IS the unit's output, so its
             # GroupNorm statistics come out of conv2's epilogue
             rs = None if mod else y_stats
             if narrow:
@@ -312,6 +330,18 @@ class _ForwardWalk:
         pool.put(h)
         pool.put(x)             # a level's skip is the chain's *output*, never an item input
         return dict(x=x, x_stats=x_stats, h=h, h_stats=h_stats, r=r, a1=a1, a2=a2, y=y, ss=ss, xn=xn)
+
+    def _modulation(self, x: Tensor, mp: Dict, C: int, Tl: int, y_stats: Optional[Tensor], pre_norm: bool) -> Dict:
+        """A ModulationItem that does not follow a ResnetItem: y = LN(x) (1 + scale) + shift in one
+        ln_film pass, which also writes the following attention's LayerNorm when pre_norm."""
+        net, pool = self.net, self.pool
+        ss = self.ss_all[:, mp["ss_off"]:]
+        y = pool.get(self.Bh, Tl, C)
+        xn = pool.get(self.Bh, Tl, C) if pre_norm else None
+        self.add(lambda: ops.ln_film(x, y, ss, self.ss_stride, y_stats, self.G, net.MOD_LN_EPS, y2=xn,
+                                     eps2=net.ATT_LN_EPS))
+        pool.put(x)
+        return dict(x=x, y=y, ss=ss, xn=xn)
 
     def _inject(self, x: Tensor, jp: Dict, C: int, Tl: int, li: int, y_stats: Optional[Tensor]) -> Dict:
         """InjectChannelsItem: conv1x1(cat([x, ctx])) + x as two accumulating GEMMs
@@ -374,23 +404,25 @@ class _ForwardWalk:
 
     def up_merge(self, lv: "LevelParams", Lp: Dict, x: Tensor, x_in: Tensor, Tl: int, T_in: int):
         """Up conv of a level >= 1's chain output x and its merge with the level input x_in:
-        MergeModulate's gate or SkipCat.  Returns (output, its statistics, y_up = the up conv's
-        own output, None when the gate runs in its epilogue)."""
+        MergeModulate's gate, SkipCat or SkipAdd.  Returns (output, its statistics, y_up = the up
+        conv's own output, None when the merge runs in its epilogue)."""
         pool, add, G, Bh, f, C, Co = self.pool, self.add, self.G, self.Bh, lv.factor, lv.ch, lv.out_ch
         out, ost = pool.get(Bh, T_in, Co), self.new_stats()
-        gate = self.ss_all[:, Lp["gate_off"]:] if self.mod else None
+        merge = self.net.merge
+        gate = self.ss_all[:, Lp["gate_off"]:] if merge == "modulate" else None
         geom = dict(up_factor=f) if f > 1 else dict(taps=(-1, 0, 1))
 
         def phases(t):          # [Bh, T_in, Co] as the [Bh, Tl, f*Co] output of the upsample GEMM
             return t.view(Bh, Tl, f * Co)
-        if self.mod and not self.keep:
+        # SkipAdd is the epilogue's residual without a gate; its backward needs no y_up either
+        if merge == "add" or (merge == "modulate" and not self.keep):
             add(lambda: ops.conv_gemm(x, Lp["up_w"], phases(out), c_in=C, n_valid=Co, bias=Lp["up_b"],
                                       residual=phases(x_in), gate=gate, stats=ost, groups=G, **geom))
             pool.put(x)
             return out, ost, None
         y_up, tmp = pool.get(Bh, T_in, Co), None
         add(lambda: ops.conv_gemm(x, Lp["up_w"], phases(y_up), c_in=C, n_valid=Co, bias=Lp["up_b"], **geom))
-        if self.mod:
+        if merge == "modulate":
             add(lambda: ops.skip_gate(y_up, x_in, gate, out, ost, G))
         else:
             # SkipCat: tmp = Wc1 (skip * s) + bc; out = Wc2 y_up + tmp.  The tensor-core GEMM needs
@@ -462,6 +494,62 @@ class B200UNet(nn.Module):
             raise NotImplementedError(
                 "use_text_conditioning builds a T5 encoder (a_unet TextConditioningPlugin); pass "
                 "precomputed `embedding=` with use_text_conditioning=False (SURVEY.md 3.4)")
+        self._setup(in_channels, out_channels, append_channels, channels, factors, items, attentions,
+                    cross_attentions, context_channels, attention_features, attention_heads, embedding_features,
+                    resnet_groups, use_modulation, "modulate" if use_modulation else "cat",   # SkipModulate / SkipCat
+                    modulation_features, use_time_conditioning, use_embedding_cfg)
+
+        # registration order mirrors a_unet: time plugin, cfg plugin, then the recursive blocks
+        self.time = TimeParams(modulation_features) if use_time_conditioning else None
+        self.fixed_embedding = (nn.Embedding(embedding_max_length, embedding_features)
+                                if use_embedding_cfg else None)
+
+        def build(i: int):
+            if i == n:
+                return None
+            in_ch = in_channels if i == 0 else channels[i - 1]
+            out_ch = self.out_channels if i == 0 else in_ch
+            return LevelParams(in_ch, out_ch, channels[i], factors[i], items[i], build(i + 1),
+                               groups=resnet_groups, features=modulation_features,
+                               att=attentions[i], cross=cross_attentions[i],
+                               head_features=attention_features, heads=attention_heads,
+                               embedding_features=embedding_features, context=context_channels[i],
+                               modulation=use_modulation)
+
+        self.net = build(0)
+        self._init_runtime()
+
+    def _init_runtime(self) -> None:
+        """Plans, packs and the program-building attributes of a freshly built net."""
+        self._plans: Dict[Tuple, _Plan] = {}
+        self._packed = None
+        self._packed_version = None
+        self._fingerprint = None
+        self._storage_sig = None
+        self._repack_graph = None
+        self.use_cuda_graph = True
+        # GroupNorm+SiLU applied to the A tile inside the conv GEMM (adp_conv_gemm gn_*).
+        # Bit-compatible with the two-kernel path, but every N tile repeats the transform of
+        # its A rows, so it only pays for N <= BN.  Off by default.  Levels wider than
+        # MAX_FUSED_GN_C keep the two-kernel path under this flag.
+        self.fuse_groupnorm = False
+        # C = 32 / 64 ConvBlocks as ONE fused kernel (GroupNorm+SiLU -> conv3 -> +res -> LN/FiLM ->
+        # statistics, csrc/mid_conv.cu) instead of three: those levels are HBM-bound
+        self.fuse_thin_levels = True
+        self.cond_table_rows = 4096    # sampler: rows (steps x batch) of conditioning per pass
+        self.max_table_steps = 4096    # iterations per conditioning block (alpha/beta table rows)
+        self.steps_per_graph = 10      # sampling steps captured back to back in one CUDA graph
+        self._verify_fp32 = False
+
+    def _setup(self, in_channels: int, out_channels: Optional[int], append_channels: int, channels: Sequence[int],
+               factors: Sequence[int], items: Sequence[int], attentions: Sequence[int],
+               cross_attentions: Sequence[int], context_channels: Sequence[int],
+               attention_features: Optional[int], attention_heads: Optional[int],
+               embedding_features: Optional[int], resnet_groups: int, use_modulation: bool, merge: str,
+               modulation_features: int, use_time_conditioning: bool, use_embedding_cfg: bool) -> None:
+        """The net's shape attributes and the size envelope of the kernels, shared by UNetV0 and XUNet
+        (per level: `items` repetitions or items, `attentions` / `cross_attentions` counts).
+        use_modulation: the net has a conditioning projection; merge: "modulate", "cat" or "add"."""
         for c, ctx in zip(channels, context_channels):
             assert ctx == 0 or c >= 16, "InjectChannelsItem is built for levels with >= 16 channels"
         if any(attentions) or any(cross_attentions):
@@ -484,6 +572,7 @@ class B200UNet(nn.Module):
         self.embedding_features = embedding_features
         self.use_time_conditioning, self.use_embedding_cfg = use_time_conditioning, use_embedding_cfg
         self.use_modulation = use_modulation
+        self.merge = merge
         for c in self.channels:
             assert c % resnet_groups == 0 and c % 8 == 0, "channels must be multiples of 8 and groups"
         # every ResnetItem conv GEMM sums the GroupNorm statistics of its output in its epilogue,
@@ -519,43 +608,6 @@ class B200UNet(nn.Module):
                 f"embedding_features={embedding_features}: the embedding LayerNorm supports a multiple of 8 " \
                 f"up to {self.MAX_WIDTH}"
 
-        # registration order mirrors a_unet: time plugin, cfg plugin, then the recursive blocks
-        self.time = TimeParams(modulation_features) if use_time_conditioning else None
-        self.fixed_embedding = (nn.Embedding(embedding_max_length, embedding_features)
-                                if use_embedding_cfg else None)
-
-        def build(i: int):
-            if i == n:
-                return None
-            in_ch = in_channels if i == 0 else channels[i - 1]
-            out_ch = self.out_channels if i == 0 else in_ch
-            return LevelParams(in_ch, out_ch, channels[i], factors[i], items[i], build(i + 1),
-                               groups=resnet_groups, features=modulation_features,
-                               att=attentions[i], cross=cross_attentions[i],
-                               head_features=attention_features, heads=attention_heads,
-                               embedding_features=embedding_features, context=context_channels[i],
-                               modulation=use_modulation)
-
-        self.net = build(0)
-        self._plans: Dict[Tuple, _Plan] = {}
-        self._packed = None
-        self._packed_version = None
-        self._fingerprint = None
-        self._storage_sig = None
-        self._repack_graph = None
-        self.use_cuda_graph = True
-        # GroupNorm+SiLU applied to the A tile inside the conv GEMM (adp_conv_gemm gn_*).
-        # Bit-compatible with the two-kernel path, but every N tile repeats the transform of
-        # its A rows, so it only pays for N <= BN.  Off by default.  Levels wider than
-        # MAX_FUSED_GN_C keep the two-kernel path under this flag.
-        self.fuse_groupnorm = False
-        # C = 32 / 64 ConvBlocks as ONE fused kernel (GroupNorm+SiLU -> conv3 -> +res -> LN/FiLM ->
-        # statistics, csrc/mid_conv.cu) instead of three: those levels are HBM-bound
-        self.fuse_thin_levels = True
-        self.cond_table_rows = 4096    # sampler: rows (steps x batch) of conditioning per pass
-        self.max_table_steps = 4096    # iterations per conditioning block (alpha/beta table rows)
-        self.steps_per_graph = 10      # sampling steps captured back to back in one CUDA graph
-        self._verify_fp32 = False
 
     @property
     def verify_fp32(self) -> bool:
@@ -742,13 +794,10 @@ class B200UNet(nn.Module):
                 d["w_kv"], d["b_kv"] = ops.pack_linear(wkv_f), bkv.contiguous()
             return d
 
-        def pack_item(it: ItemParams, narrow: bool) -> Dict:
-            r = it.resnet
+        def pack_resnet(r: ResnetParams, narrow: bool) -> Dict:
             d: Dict = {"gn1": (f32(r.gn1.weight), f32(r.gn1.bias)),
                        "gn2": (f32(r.gn2.weight), f32(r.gn2.bias)),
                        "b1": f32(r.conv1.bias), "b2": f32(r.conv2.bias)}
-            if it.modulation is not None:
-                d["ss_off"] = add_cond(it.modulation.proj)
             if narrow:
                 d["w1"], d["w2"] = f32(r.conv1.weight), f32(r.conv2.weight)
             else:
@@ -756,21 +805,30 @@ class B200UNet(nn.Module):
                 if r.conv1.weight.shape[0] in (32, 64):    # thin levels: fused ConvBlock kernel
                     d["w1_raw"], d["w2_raw"] = f32(r.conv1.weight), f32(r.conv2.weight)
                     d["w1_mid"], d["w2_mid"] = ops.pack_mid_conv(r.conv1.weight), ops.pack_mid_conv(r.conv2.weight)
-            if it.inject is not None:
-                C_ = it.inject.weight.shape[0]
-                wi = it.inject.weight.detach().float()[:, :, 0]
-                ctx = wi.shape[1] - C_
-                wc = torch.zeros(C_, ops.round_up(ctx, 16), device=wi.device)
-                wc[:, :ctx] = wi[:, C_:]
-                d["inj"] = {"w_x": ops.pack_linear(wi[:, :C_]), "w_c": ops.pack_linear(wc),
-                            "b": f32(it.inject.bias)}
-            # one pack per attention item, in order; each cross-attention projects the context
-            # through its own K|V weights (its norm_context affine folded in)
-            if it.attention is not None:
-                d["att"] = [pack_att(a, True) for a in it.attentions()]
-            if it.cross is not None:
-                d["cross"] = [pack_att(a, False) for a in it.crosses()]
             return d
+
+        def pack_inject(conv: nn.Conv1d) -> Dict:
+            C_ = conv.weight.shape[0]
+            wi = conv.weight.detach().float()[:, :, 0]
+            ctx = wi.shape[1] - C_
+            wc = torch.zeros(C_, ops.round_up(ctx, 16), device=wi.device)
+            wc[:, :ctx] = wi[:, C_:]
+            return {"w_x": ops.pack_linear(wi[:, :C_]), "w_c": ops.pack_linear(wc), "b": f32(conv.bias)}
+
+        def pack_chain(chain, narrow: bool) -> List[Tuple[str, Dict]]:
+            """(kind, pack) per item; each cross-attention projects the context through its own K|V
+            weights (its norm_context affine folded in)."""
+            out = []
+            for kind, m in chain:
+                if kind == "resnet":
+                    out.append((kind, pack_resnet(m, narrow)))
+                elif kind == "mod":
+                    out.append((kind, {"ss_off": add_cond(m.proj)}))
+                elif kind == "inj":
+                    out.append((kind, pack_inject(m)))
+                else:
+                    out.append((kind, pack_att(m, kind == "att")))
+            return out
 
         P["levels"] = []
         for i, lvl in enumerate(self.levels()):
@@ -785,11 +843,11 @@ class B200UNet(nn.Module):
                 L["down_w"] = ops.pack_conv(lvl.down.weight.detach())
                 L["up_w"] = (ops.pack_upsample_conv(lvl.up.weight.detach(), lvl.factor)
                              if lvl.factor > 1 else ops.pack_conv(lvl.up.weight.detach()))
-            L["items_down"] = [pack_item(it, narrow) for it in lvl.items_down]
-            L["items_up"] = [pack_item(it, narrow) for it in lvl.items_up]
-            if self.use_modulation:
+            L["items_down"] = pack_chain(lvl.chain(up=False), narrow)
+            L["items_up"] = pack_chain(lvl.chain(up=True), narrow)
+            if self.merge == "modulate":
                 L["gate_off"] = add_cond(lvl.merge)
-            else:
+            elif self.merge == "cat":
                 # SkipCat: out = Wc1 (skip * s) + Wc2 y + bc,  W = [Wc1 | Wc2]
                 s_ = 2 ** -0.5
                 wm = lvl.merge.weight.detach().float()[:, :, 0]
@@ -828,7 +886,7 @@ class B200UNet(nn.Module):
             t = self.time
             kdim = t.to_out.weight.shape[1]
             kpad = ops.round_up(kdim, 8)
-            w_emb = torch.zeros(self.features, kpad, dtype=pd, device=w_all.device)
+            w_emb = torch.zeros(self.features, kpad, dtype=pd, device=t.to_out.weight.device)
             w_emb[:, :kdim] = t.to_out.weight.detach().to(pd)
             P["time"] = {"freqs": f32(t.weights), "w_emb": w_emb.contiguous(), "b_emb": f32(t.to_out.bias),
                          # a copy also in fp32: an alias would have the in-place re-pack bump the
@@ -987,7 +1045,8 @@ class B200UNet(nn.Module):
 
         h0, _ = run_level(0, None, T)
         lv0, L0 = levels[0], P["levels"][0]
-        gate0 = (ss_all[:, L0["gate_off"]:] if self.use_modulation
+        # SkipCat (folded into the stem's weights) and SkipAdd run the stem epilogue with a unit gate
+        gate0 = (ss_all[:, L0["gate_off"]:] if self.merge == "modulate"
                  else torch.ones(Bh, max(8, self.out_channels), device=dev))
 
         def final():
