@@ -74,7 +74,7 @@ def _launch(fn, what: str, meta):
         _lib.check(fn(), what)
         return
     label, flops, nbytes = meta()
-    rec = {"name": label, "flops": float(flops), "bytes": float(nbytes)}
+    rec = {"name": label, "symbol": what, "flops": float(flops), "bytes": float(nbytes)}
     if tr.timing:
         rec["e0"] = torch.cuda.Event(enable_timing=True)
         rec["e1"] = torch.cuda.Event(enable_timing=True)

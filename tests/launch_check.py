@@ -32,11 +32,45 @@ values: conv of |a| with |w|, P |V|, ...):
                    by max(ref - b, 1e-5), + 1e-5 |ref| of the log
     copies         bitwise (the step selector's rows, arv_step's sigma channel, and inpaint_blend's
                    positions outside the mask, which hold the sampler's value)
+The fp32 verification mode (B200UNet.verify_fp32: the f32_* kernels of verify_f32.cu and
+verify_f32_bwd.cu, one thread per output, fixed sequential fp32 sums) is held to fp32 round-off, none
+of the bf16 allowances above (no tau = 2^-8, no LSE_FLOOR, no bf16 rounding of operands or P):
+    f32 outputs    err <= 2^-23 |ref| + lambda sqrt(n) 2^-24 absref,   lambda = 10
+                   accumulators: + 2^-23 (|before| + |after|) (fp32), 2^-52 (...) (fp64: loss_sum, S)
+the probabilistic bound of Higham and Mary (SIAM J. Sci. Comput. 41(5), 2019): with independent
+roundings an element exceeds it with probability at most 2n exp(-lambda^2 / 2), negligible at
+lambda = 10.  n is the longest fp32 chain forming the element in that kernel:
+    kind            n                                  kind            n
+    conv_gemm       c_in * slots + 3                   wgrad           B T
+    skinny_linear   K + 2                              colsum          B T + 2
+    ln_film (y, y2) C + 4                              gn_silu_bwd     8 (dxh), B T (dgamma, dbeta), T + 8 (S)
+    attention       2 Tk + 4 (o, lse)                  gn_bwd_apply    8 (dx), B T + 8 (colsum)
+    stem_in         cin f + 3                          ln_film_bwd     C + 8 (dx), T + C (dss), B T + C (colsum)
+    stem_out        3 c0 + cin + 8                     skip_gate_bwd   8 (dys), T + 2 (dgate)
+    gn_silu, silu,  8 (F32_SHORT: a few roundings,     cond_bwd        B + 2 (dw, dbias), N + 2 (dcond)
+    skip_gate         transcendentals included)        stem_in_bwd     B T/f + 3 (dw), c0 + 1 (dxin)
+    attention_bwd   D + 2 (delta), Tk + D + 4 (dq),    stem_out_bwd    3 f co + 2 (dh), B T + 2 (dw, dbias,
+                    Tq + D + 4 (dk, dv)                                dw_adapt), co + 2 (dxin), 2 (T + 3 c0 + 2) (dgate)
+Where the arithmetic leaves that model, absref carries the magnitude the rounding is relative to,
+as the bf16 checkers do: x - mean in fp32 (gn_silu, the GroupNorm backward: |x| + |mean|), xhat
+formed in fp32 (ln_film_bwd: (|x| + mean|x|) / std), SiLU' near its zero (DSILU_MAX |da| + the
+rounding of z through |SiLU''| <= 1/2), exp(s - max) (an absolute error of the score, a D-chain over
+|q| |k| scale, is a relative one of p: attention's o and lse, attention_bwd's P and dS), and the
+stems' noising alpha x + beta noise (|alpha x| + |beta noise|).  GroupNorm statistics keep their
+check above (fp64 sums of the stored fp32 output).  attention's online softmax rounds twice per key
+(acc corr + p v, and l the same way): its n counts both.  A 2^-12 relative change of an element is
+outside the bound wherever sqrt(n) absref / |ref| < (2^-12 - 2^-23) / (lambda 2^-24) = (2^12 - 2) /
+lambda, about 409: a chain of 256 catches it while absref / |ref| < 25.
+In the fp32 mode conv_gemm, ln_film, stem_in and skip_gate make their GroupNorm statistics with a
+gn_stats launch of their own inside the ops call: it is checked once, as the caller's `stats`
+output, runs on the caller's (relocated) storages, and the caller's label names the caller.
+
 Every launch also checks that read-only arguments are bitwise unchanged and that no byte of a
 written tensor's storage outside the written view changed -- the rest of the gradient arena
 included, every accumulator being a view of that one storage.
 
-Checked kinds are every launching function of `ops` (UNCHECKED is empty): the launches of the
+Checked kinds are every launching function of `ops`, in both modes (UNCHECKED is empty: the
+launching functions without a checker; the f32 routes of a function share its checker): the launches of the
 inference, sampling and training programs (forward, fused loss and backward; tau = 2^-8 also for
 attention_bwd, which rounds P and dS to bf16); the tensors fir_resample, mel_spectrogram, to_flat
 and to_flat_bwd allocate and return (RESULT); and the in-place sampler steps of VSampler's generic
@@ -66,7 +100,7 @@ kinds listed in READS_OUTSIDE_VIEW (none), nor workspaces the C library allocate
 """
 import inspect
 import math
-from typing import Callable, Dict, FrozenSet, List, Tuple
+from typing import Callable, Dict, FrozenSet, List, Optional, Tuple
 
 import torch
 
@@ -85,10 +119,18 @@ GN_EPS = 1e-5                    # every statistics slot feeds a GroupNorm: it d
 # moves by up to 2^-9 in absolute terms.  attention_bwd rounds the P it recomputes from lse to bf16 too.
 LSE_FLOOR = 2.0 ** -9
 ACC_EPS = 2.0 ** -23              # an fp32 accumulator's own rounding, per unit of |before| + |after|
+# the fp32 verification kernels (chain = n): err <= F32_REL |ref| + F32_LAMBDA sqrt(n) F32_U absref
+F32_REL, F32_U, F32_LAMBDA = 2.0 ** -23, 2.0 ** -24, 10.0
+F32_SHORT = 8                     # chain of an element-wise f32 kernel: a few roundings, transcendentals included
+F64_ACC_EPS = 2.0 ** -52          # an fp64 accumulator's own rounding (loss_sum, S in the fp32 mode)
 SIDE_CHUNK = 1 << 28              # bytes compared at a time by the side-effect check
 ROW_TILE = 64                    # rows left stale by the mutation: half the conv GEMM's 128-row M tile
 
 UNCHECKED: Dict[str, str] = {}          # launching functions of `ops` without a checker: none
+# In the fp32 mode these kinds make their GroupNorm statistics with an adp_f32_gn_stats launch inside
+# the ops call (kind -> its statistics argument); no other launch may nest in a checked one.
+NESTED_STATS: Dict[str, str] = {"conv_gemm": "stats", "ln_film": "stats_out", "stem_in": "stats",
+                                "skip_gate": "stats"}
 
 
 class CheckError(AssertionError):
@@ -113,10 +155,11 @@ class Val:
     argument has several outputs."""
 
     def __init__(self, name, view, ref, absref=None, tau=TAU_FP32_ACC, exact=False, floor=0.0, keep=None,
-                 of=None):
+                 of=None, chain: Optional[float] = None):
         self.name, self.view, self.ref, self.absref, self.tau, self.exact = name, view, ref, absref, tau, exact
         self.acc, self.floor = False, floor      # floor: an absolute term of the bound (see LSE_FLOOR)
         self.keep, self.of = keep, of or name
+        self.chain = chain                       # an fp32 verification kernel's chain length n, or None
 
 
 class Stat:
@@ -133,9 +176,10 @@ class Acc:
     over absolute terms), or a callable(post args) -> (ref, absref) when the contribution is defined
     on another output of the launch as stored (the GroupNorm backward sums of the rounded dxh)."""
 
-    def __init__(self, name, view, ref, absref=None):
+    def __init__(self, name, view, ref, absref=None, chain: Optional[float] = None):
         self.name, self.view, self.ref, self.absref = name, view, ref, absref
         self.acc, self.exact, self.of, self.keep = True, False, name, None
+        self.chain = chain
 
 
 def arg(name):
@@ -194,7 +238,7 @@ def _layer_norm(x, eps):
 # ----------------------------------------------------------------------------- checkers
 def c_conv_gemm(a, ctx):
     x, w, out = a["a"], a["w"], a["out"]
-    assert x.dtype == torch.bfloat16, "the fp32 verification mode is not checked here"
+    f32 = x.dtype == torch.float32         # f32_conv_gemm: fp32 operands, residual read, statistics a gn_stats pass
     B, T, _ = x.shape
     c_in, n_valid, taps, up = a["c_in"], a["n_valid"], tuple(a["taps"]), a["up_factor"]
     phases = up if up > 1 else 1
@@ -235,7 +279,7 @@ def c_conv_gemm(a, ctx):
     if gate is not None:
         ref *= gate
         absr *= gate.abs()
-    if a["residual"] is not None and out.dtype != torch.float32:
+    if a["residual"] is not None and (f32 or out.dtype != torch.float32):
         r = a["residual"][..., :phases * n_valid].to(F64).reshape(B, T, phases, n_valid)
         ref += r
         absr += r.abs()
@@ -243,7 +287,9 @@ def c_conv_gemm(a, ctx):
 
     def view(args):
         return args["out"][..., :ncols]
-    outs = [Val("out", view, ref.reshape(B, T, ncols), absr.reshape(B, T, ncols), tau)]
+    # f32: one fmaf chain of c_in per tap slot, the slots added in turn (+ bias, gate, residual)
+    chain = c_in * (2 if up > 1 else len(taps)) + 3 if f32 else None
+    outs = [Val("out", view, ref.reshape(B, T, ncols), absr.reshape(B, T, ncols), tau, chain=chain)]
     if a["stats"] is not None:
         outs.append(Stat("stats", arg("stats"),
                          lambda p: p["out"][..., :ncols].reshape(B, T * phases, n_valid), a["groups"]))
@@ -255,6 +301,10 @@ def c_gn_silu(a, ctx):
     B, T, C = x.shape
     sc, sh = _gn_coef(a["stats"], a["gamma"], a["beta"], a["groups"], a["eps"], T, C)
     z = x.to(F64) * sc + sh
+    if x.dtype == torch.float32:         # f32_gn_silu forms x - mean in fp32: relative to |x| + |mean|
+        be = a["beta"].to(F64)[None, None]
+        return [Val("y", arg("y"), _silu(z), 1.2 * ((x.to(F64) * sc).abs() + (be - sh).abs() + be.abs()),
+                    chain=F32_SHORT)]
     return [Val("y", arg("y"), _silu(z), 1.2 * ((x.to(F64) * sc).abs() + sh.abs()))]
 
 
@@ -265,18 +315,19 @@ def c_gn_stats(a, ctx):
 def c_ln_film(a, ctx):
     x = a["x"]
     B, T, C = x.shape
+    chain = C + 4 if x.dtype == torch.float32 else None      # f32_ln_film: the row sums over C
     xn, _, lnabs = _layer_norm(x.to(F64), a["eps"])
     ref, absr = xn, lnabs
     if a["scale_shift"] is not None:
         ss = a["scale_shift"].to(F64)
         s, t = ss[:, None, :C], ss[:, None, C:2 * C]
         ref, absr = xn * (1 + s) + t, lnabs * (1 + s).abs() + t.abs()
-    outs = [Val("y", arg("y"), ref, absr)]
+    outs = [Val("y", arg("y"), ref, absr, chain=chain)]
     if a["y2"] is not None:
         def ref2(p, eps2=a["eps2"]):
             y2, _, y2abs = _layer_norm(p["y"].to(F64), eps2)
             return y2, y2abs
-        outs.append(Val("y2", arg("y2"), ref2))
+        outs.append(Val("y2", arg("y2"), ref2, chain=chain))
     if a["stats_out"] is not None:
         outs.append(Stat("stats_out", arg("stats_out"), arg("y"), a["groups"]))
     return outs
@@ -286,6 +337,7 @@ def c_attention(a, ctx):
     q, k, v = a["q"], a["k"], a["v"]
     H, D, scale = a["heads"], a["head_dim"], a["scale"]
     B, Tq, Tk, mid = q.shape[0], q.shape[1], k.shape[1], a["heads"] * a["head_dim"]
+    f32 = q.dtype == torch.float32
     ref = torch.empty(B, Tq, mid, dtype=F64, device=q.device)
     absr = torch.empty_like(ref)
     lse = torch.empty(B, H, Tq, dtype=F64, device=q.device) if a["lse"] is not None else None
@@ -298,9 +350,22 @@ def c_attention(a, ctx):
         P = torch.softmax(S, dim=-1)
         ref[b] = (P @ V).transpose(0, 1).reshape(Tq, mid)
         absr[b] = (P @ V.abs()).transpose(0, 1).reshape(Tq, mid)
+        if f32:
+            # exp(s - max) turns an absolute error e_j of the score (a D-chain over |q| |k| scale)
+            # into a relative one of p_j: o moves by sum_j p_j e_j (v_j - o), at most 2 max_j e_j P|V|
+            smax = ((Q.abs() @ K.abs().transpose(1, 2)) * scale).amax(-1)                   # [H, Tq]
+            absr[b] *= (1 + 2 * math.sqrt(D / (2 * Tk)) * smax).transpose(0, 1).repeat_interleave(D, dim=1)
         if lse is not None:
             lse[b] = torch.logsumexp(S, dim=-1)
-            lse_abs[b] = S.abs().amax(-1)
+            # f32: max + logf(l): the score error, l's relative error (a Tk-chain) and the log's rounding
+            lse_abs[b] = S.abs().amax(-1) if not f32 else \
+                math.sqrt(D / (2 * Tk)) * smax + 1 + lse[b].abs()
+    if f32:
+        # each key rounds twice (acc * corr + p v; l * corr + p): n = 2 Tk
+        outs = [Val("o", lambda p: p["o"][..., :mid], ref, absr, chain=2 * Tk + 4)]
+        if lse is not None:
+            outs.append(Val("lse", arg("lse"), lse, lse_abs, chain=2 * Tk + 4))
+        return outs
     outs = [Val("o", lambda p: p["o"][..., :mid], ref, absr, TAU_BF16_OPERAND)]
     if lse is not None:
         outs.append(Val("lse", arg("lse"), lse, lse_abs, floor=LSE_FLOOR))
@@ -319,7 +384,8 @@ def c_skinny_linear(a, ctx):
     if a["bias"] is not None:
         pre = pre + a["bias"].to(F64)[:N]
         absr = absr + a["bias"].to(F64)[:N].abs()
-    return [Val("y", lambda p: p["y"][:, :N], fout(pre), gout * absr)]
+    chain = K + 2 if w.dtype == torch.float32 else None          # f32_linear: one fmaf chain over K
+    return [Val("y", lambda p: p["y"][:, :N], fout(pre), gout * absr, chain=chain)]
 
 
 def c_time_features(a, ctx):
@@ -336,29 +402,41 @@ def c_time_features(a, ctx):
 
 def c_silu_bf16(a, ctx):
     x = a["x"].to(F64)
-    return [Val("y", arg("y"), _silu(x).reshape(a["y"].shape), 1.2 * x.abs().reshape(a["y"].shape))]
+    chain = F32_SHORT if a["y"].dtype == torch.float32 else None
+    return [Val("y", arg("y"), _silu(x).reshape(a["y"].shape), 1.2 * x.abs().reshape(a["y"].shape), chain=chain)]
 
 
-def _stem_input(a):
-    """cat([alpha x + beta noise, append]) fp64 [B, cin, T] (VDiffusion noising in the stems)."""
+def _stem_input(a, absolute=False):
+    """cat([alpha x + beta noise, append]) fp64 [B, cin, T] (VDiffusion noising in the stems);
+    absolute=True: its magnitude |alpha x| + |beta noise| (the fp32 kernels round the noising)."""
     x = a["x"].to(F64)
+    if absolute:
+        x = x.abs()
     if a["noise"] is not None:
-        x = a["alpha"].to(F64)[:, None, None] * x + a["beta"].to(F64)[:, None, None] * a["noise"].to(F64)
+        al, be, nz = a["alpha"].to(F64), a["beta"].to(F64), a["noise"].to(F64)
+        if absolute:
+            al, be, nz = al.abs(), be.abs(), nz.abs()
+        x = al[:, None, None] * x + be[:, None, None] * nz
     if a["append"] is not None:
-        x = torch.cat([x, a["append"].to(F64)], dim=1)
+        x = torch.cat([x, a["append"].to(F64).abs() if absolute else a["append"].to(F64)], dim=1)
     return x
 
 
 def c_stem_in(a, ctx):
     xin, w, f = _stem_input(a), a["w"].to(F64), a["f"]
+    f32 = a["out"].dtype == torch.float32
     B, cin, T = xin.shape
     c0 = w.shape[0]
-    xr = xin.reshape(B, cin, T // f, f).permute(0, 2, 1, 3).reshape(B, T // f, cin * f)
+
+    def rows(t):
+        return t.reshape(B, cin, T // f, f).permute(0, 2, 1, 3).reshape(B, T // f, cin * f)
+    xr = rows(xin)
+    xa = rows(_stem_input(a, absolute=True)) if f32 else xr.abs()
     Wm = w.reshape(c0, cin * f)
-    ref, absr = xr @ Wm.t(), xr.abs() @ Wm.abs().t()
+    ref, absr = xr @ Wm.t(), xa @ Wm.abs().t()
     if a["bias"] is not None:
         ref, absr = ref + a["bias"].to(F64), absr + a["bias"].to(F64).abs()
-    outs = [Val("out", arg("out"), ref, absr)]
+    outs = [Val("out", arg("out"), ref, absr, chain=cin * f + 3 if f32 else None)]
     if a["stats"] is not None:
         outs.append(Stat("stats", arg("stats"), arg("out"), a["groups"]))
     return outs
@@ -367,17 +445,22 @@ def c_stem_in(a, ctx):
 def c_stem_out(a, ctx):
     h, f = a["h"], a["f"]
     xin = _stem_input(a)
-    B, _, T = xin.shape
+    f32 = h.dtype == torch.float32
+    xin_abs = _stem_input(a, absolute=True) if f32 else xin.abs()
+    B, cin, T = xin.shape
     w = a["w"].to(F64)
     co = w.shape[0]
+    # f32_stem_out: the branch is one fmaf chain over 3 c0, the adapter one over cin; then the
+    # merge, the guidance combine, the sampler update or the loss term
+    chain = 3 * h.shape[-1] + cin + 8 if f32 else None
     w3 = w.permute(2, 0, 1)                                    # [3, co, c0]
     bias = a["bias"].to(F64) if a["bias"] is not None else None
     if a["w_adapt"] is not None:
         wa = a["w_adapt"].to(F64)
         skip = torch.einsum("oc,bct->bot", wa, xin) + a["b_adapt"].to(F64)[None, :, None]
-        skip_abs = torch.einsum("oc,bct->bot", wa.abs(), xin.abs()) + a["b_adapt"].to(F64).abs()[None, :, None]
+        skip_abs = torch.einsum("oc,bct->bot", wa.abs(), xin_abs) + a["b_adapt"].to(F64).abs()[None, :, None]
     else:
-        skip, skip_abs = xin[:, :co], xin[:, :co].abs()
+        skip, skip_abs = xin[:, :co], xin_abs[:, :co]
     gate = a["gate"].to(F64)[:, :co]
 
     def branch(b):               # gate * conv3(nearest_up(h)) of trunk row b -> [co, T]
@@ -399,23 +482,27 @@ def c_stem_out(a, ctx):
             vabs[b] = (abs(s) + abs(1 - s)) * skip_abs[b] + abs(s) * yca + abs(1 - s) * yma
     outs = []
     if a["v_out"] is not None:
-        outs.append(Val("v_out", arg("v_out"), v, vabs))
+        outs.append(Val("v_out", arg("v_out"), v, vabs, chain=chain))
     if a["x_next"] is not None:
         a0, b0, a1, b1 = a["ab"].to(F64).tolist()
         xs = xin[:, :co]
         xn = a1 * (a0 * xs - b0 * v) + b1 * (b0 * xs + a0 * v)
         xna = (abs(a1 * a0) + abs(b1 * b0)) * xs.abs() + (abs(a1 * b0) + abs(b1 * a0)) * vabs
-        outs.append(Val("x_next", arg("x_next"), xn, xna))
+        outs.append(Val("x_next", arg("x_next"), xn, xna, chain=chain))
     if a["loss_sum"] is not None:      # VDiffusion: sum (v - (alpha noise - beta x))^2, dv = 2 (v - target) / numel
         al, be = a["alpha"].to(F64)[:, None, None], a["beta"].to(F64)[:, None, None]
         nz, x0 = a["noise"].to(F64), a["x"].to(F64)
         d = v - (al * nz - be * x0)
         dabs = vabs + (al * nz).abs() + (be * x0).abs()
-        # an error e of v within its fp32 bound moves d^2 by 2 |d| e: carried at the same weight
-        outs.append(Acc("loss_sum", arg("loss_sum"), (d * d).sum().reshape(1),
-                        ((d * d).sum() + (FP32_TAU / STATS_TOL) * (2 * d.abs() * dabs).sum()).reshape(1)))
+        if f32:        # d^2 summed in fp64: an error e of d (its chain bound) moves a term by 2 |d| e
+            outs.append(Acc("loss_sum", arg("loss_sum"), (d * d).sum().reshape(1),
+                            (2 * d.abs() * dabs).sum().reshape(1), chain=chain))
+        else:
+            # an error e of v within its fp32 bound moves d^2 by 2 |d| e: carried at the same weight
+            outs.append(Acc("loss_sum", arg("loss_sum"), (d * d).sum().reshape(1),
+                            ((d * d).sum() + (FP32_TAU / STATS_TOL) * (2 * d.abs() * dabs).sum()).reshape(1)))
         if a["dv"] is not None:
-            outs.append(Val("dv", arg("dv"), 2 * d / d.numel(), 2 * dabs / d.numel()))
+            outs.append(Val("dv", arg("dv"), 2 * d / d.numel(), 2 * dabs / d.numel(), chain=chain))
     return outs
 
 
@@ -518,29 +605,34 @@ def _gn_S(xh, xha, groups):
 
 def c_wgrad(a, ctx):
     g, x, n, k = a["g"], a["x"], a["n"], a["k"]
-    assert g.dtype == torch.bfloat16, "the fp32 verification mode is not checked here"
+    chain = g.shape[0] * g.shape[1] if g.dtype == torch.float32 else None     # f32_wgrad: one chain over B T
     G = g[..., a["g_col0"]:a["g_col0"] + n].to(F64).reshape(-1, n)
     X = x[..., a["x_col0"]:a["x_col0"] + k].to(F64)
     taps = 3 if a["ntaps"] == 3 else 1
     ref = [G.t() @ _shift(X, a["off"] + j).reshape(-1, k) for j in range(taps)]
     absr = [G.abs().t() @ _shift(X.abs(), a["off"] + j).reshape(-1, k) for j in range(taps)]
     if taps == 3:
-        return [Acc("dw", lambda p: p["dw"][:, :n, :k], torch.stack(ref), torch.stack(absr))]
-    return [Acc("dw", lambda p: p["dw"][:n, :k], ref[0], absr[0])]
+        return [Acc("dw", lambda p: p["dw"][:, :n, :k], torch.stack(ref), torch.stack(absr), chain=chain)]
+    return [Acc("dw", lambda p: p["dw"][:n, :k], ref[0], absr[0], chain=chain)]
 
 
 def c_gn_silu_bwd(a, ctx):
     x, G = a["x"], a["groups"]
+    B, T, _ = x.shape
     xh, _, xha = _gn_xhat(x, a["stats"], G, a["eps"])
-    ga, da = a["gamma"].to(F64), a["da"].to(F64)
-    dz = da * _dsilu(xh * ga + a["beta"].to(F64))
+    ga, da, be = a["gamma"].to(F64), a["da"].to(F64), a["beta"].to(F64)
+    dz = da * _dsilu(xh * ga + be)
     # SiLU' crosses zero (z = -1.28) by cancellation: dz's rounding is relative to DSILU_MAX |da|, as for
     # dxh and narrow_conv_bwd; a sum over one row (M = 1) shows it
     dza = DSILU_MAX * da.abs()
-    return [Val("dxh", arg("dxh"), dz * ga, dza * ga.abs()),
-            Acc("dgamma", arg("dgamma"), (dz * xh).sum((0, 1)), (dza * xha).sum((0, 1))),
-            Acc("dbeta", arg("dbeta"), dz.sum((0, 1)), dza.sum((0, 1))),
-            Acc("S", arg("S"), _gn_S(xh, xha, G))]
+    f32 = x.dtype == torch.float32
+    if f32:            # + z's own rounding (relative to |xhat gamma| + |beta|) through |SiLU''| <= 1/2
+        dza = dza + 0.5 * da.abs() * (xha * ga.abs() + be.abs())
+    c = (lambda n: n) if f32 else (lambda n: None)
+    return [Val("dxh", arg("dxh"), dz * ga, dza * ga.abs(), chain=c(F32_SHORT)),
+            Acc("dgamma", arg("dgamma"), (dz * xh).sum((0, 1)), (dza * xha).sum((0, 1)), chain=c(B * T)),
+            Acc("dbeta", arg("dbeta"), dz.sum((0, 1)), dza.sum((0, 1)), chain=c(B * T)),
+            Acc("S", arg("S"), _gn_S(xh, xha, G), chain=c(T + F32_SHORT))]
 
 
 def c_gn_bwd_apply(a, ctx):
@@ -553,45 +645,53 @@ def c_gn_bwd_apply(a, ctx):
     absr = rstd.abs() * (d.abs() + c[..., 0].abs() + xha * c[..., 1].abs())
     if a["dres"] is not None:
         ref, absr = ref + a["dres"].to(F64), absr + a["dres"].to(F64).abs()
-    outs = [Val("dx", arg("dx"), ref, absr)]
+    f32 = x.dtype == torch.float32
+    outs = [Val("dx", arg("dx"), ref, absr, chain=F32_SHORT if f32 else None)]
     if a["colsum"] is not None:        # the kernel sums the values before they are rounded to bf16
-        outs.append(Acc("colsum", cols("colsum", C), ref.sum((0, 1)), absr.sum((0, 1))))
+        outs.append(Acc("colsum", cols("colsum", C), ref.sum((0, 1)), absr.sum((0, 1)),
+                        chain=B * T + F32_SHORT if f32 else None))
     return outs
 
 
 def c_ln_film_bwd(a, ctx):
     x = a["x"]
     B, T, C = x.shape
-    xh, std, _ = _layer_norm(x.to(F64), a["eps"])
+    xh, std, lnabs = _layer_norm(x.to(F64), a["eps"])
     dy = a["dy"].to(F64)
     f = 1 + a["scale_shift"].to(F64)[:, None, :C] if a["scale_shift"] is not None else 1.0
     g = dy * f
     m1, m2 = g.mean(-1, keepdim=True), (g * xh).mean(-1, keepdim=True)
     ref = (g - m1 - xh * m2) / std
-    absr = (g.abs() + g.abs().mean(-1, keepdim=True) + xh.abs() * (g * xh).abs().mean(-1, keepdim=True)) / std
+    f32 = x.dtype == torch.float32
+    # f32_ln_film_bwd forms xhat in fp32: its rounding is relative to lnabs ((|x| + mean|x|) / std)
+    xa = lnabs if f32 else xh.abs()
+    absr = (g.abs() + g.abs().mean(-1, keepdim=True) + xa * (g.abs() * xa).mean(-1, keepdim=True)) / std
     if a["dres"] is not None:
         ref, absr = ref + a["dres"].to(F64), absr + a["dres"].to(F64).abs()
-    outs = [Val("dx", arg("dx"), ref, absr)]
+    c = (lambda n: n) if f32 else (lambda n: None)
+    outs = [Val("dx", arg("dx"), ref, absr, chain=c(C + F32_SHORT))]
     if a["dss"] is not None:
         outs.append(Acc("dss", cols("dss", 2 * C), torch.cat([(dy * xh).sum(1), dy.sum(1)], -1),
-                        torch.cat([(dy * xh).abs().sum(1), dy.abs().sum(1)], -1)))
+                        torch.cat([(dy.abs() * xa).sum(1), dy.abs().sum(1)], -1), chain=c(T + C)))
     if a["colsum"] is not None:
-        outs.append(Acc("colsum", cols("colsum", C), ref.sum((0, 1)), absr.sum((0, 1))))
+        outs.append(Acc("colsum", cols("colsum", C), ref.sum((0, 1)), absr.sum((0, 1)), chain=c(B * T + C)))
     return outs
 
 
 def c_colsum(a, ctx):
     x = a["x"].to(F64)
-    C = x.shape[-1]
+    B, T, C = x.shape
+    chain = B * T + 2 if a["x"].dtype == torch.float32 else None      # f32_colsum: B T-sums, gated, summed
     if a["gate"] is not None:
         x = x * a["gate"].to(F64)[:, None, :C]
-    return [Acc("out", cols("out", C), x.sum((0, 1)), x.abs().sum((0, 1)))]
+    return [Acc("out", cols("out", C), x.sum((0, 1)), x.abs().sum((0, 1)), chain=chain)]
 
 
 def c_skip_gate(a, ctx):
     y, skip = a["y"].to(F64), a["skip"].to(F64)
     gy = a["gate"].to(F64)[:, None, :y.shape[-1]] * y
-    outs = [Val("out", arg("out"), skip + gy, skip.abs() + gy.abs())]
+    chain = F32_SHORT if a["y"].dtype == torch.float32 else None
+    outs = [Val("out", arg("out"), skip + gy, skip.abs() + gy.abs(), chain=chain)]
     if a["stats"] is not None:
         outs.append(Stat("stats", arg("stats"), arg("out"), a["groups"]))
     return outs
@@ -599,19 +699,22 @@ def c_skip_gate(a, ctx):
 
 def c_skip_gate_bwd(a, ctx):
     d, y = a["dout"].to(F64), a["y"].to(F64)
-    C = y.shape[-1]
+    T, C = y.shape[1], y.shape[-1]
     ref = a["gate"].to(F64)[:, None, :C] * d
-    return [Val("dys", arg("dys"), ref, ref.abs()),
-            Acc("dgate", cols("dgate", C), (d * y).sum(1), (d * y).abs().sum(1))]
+    c = (lambda n: n) if a["y"].dtype == torch.float32 else (lambda n: None)
+    return [Val("dys", arg("dys"), ref, ref.abs(), chain=c(F32_SHORT)),
+            Acc("dgate", cols("dgate", C), (d * y).sum(1), (d * y).abs().sum(1), chain=c(T + 2))]
 
 
 def c_cond_bwd(a, ctx):
     N = a["N"]
     d, c, W = a["dss"][:, :N].to(F64), a["cond"].to(F64), a["w"][:N].to(F64)
-    outs = [Val("dw", lambda p: p["dw"][:N], d.t() @ c, d.abs().t() @ c.abs()),
-            Val("dbias", lambda p: p["dbias"][:N], d.sum(0), d.abs().sum(0))]
+    B = d.shape[0]
+    f = (lambda n: n) if a["w"].dtype == torch.float32 else (lambda n: None)
+    outs = [Val("dw", lambda p: p["dw"][:N], d.t() @ c, d.abs().t() @ c.abs(), chain=f(B + 2)),
+            Val("dbias", lambda p: p["dbias"][:N], d.sum(0), d.abs().sum(0), chain=f(B + 2))]
     if a["dcond"] is not None:
-        outs.append(Acc("dcond", arg("dcond"), d @ W, d.abs() @ W.abs()))
+        outs.append(Acc("dcond", arg("dcond"), d @ W, d.abs() @ W.abs(), chain=f(N + 2)))
     return outs
 
 
@@ -660,17 +763,23 @@ def c_stem_out_bwd(a, ctx):
     T = up.shape[1]
     dw = torch.stack([dy.reshape(-1, co).t() @ _shift(up, k - 1).reshape(-1, c0) for k in range(3)], -1)
     dwa = torch.stack([dy.abs().reshape(-1, co).t() @ _shift(up.abs(), k - 1).reshape(-1, c0) for k in range(3)], -1)
-    outs = [Val("dh", arg("dh"), dup.reshape(B, Tl, f, c0).sum(2), dupa.reshape(B, Tl, f, c0).sum(2)),
-            Acc("dw", arg("dw"), dw, dwa),
-            Acc("dbias", cols("dbias", co), dy.sum((0, 1)), dy.abs().sum((0, 1))),
-            Acc("dgate", cols("dgate", co), (dvs * y).sum(1), (dvs.abs() * ya).sum(1))]
+    # f32_stem_out_bwd: dh sums f 3 co terms, the parameter gradients B T terms; dgate's terms carry
+    # the branch y, itself a chain over 3 c0: (sqrt(T) + sqrt(3 c0))^2 <= 2 (T + 3 c0)
+    f32 = h.dtype == torch.float32
+    c = (lambda n: n) if f32 else (lambda n: None)
+    outs = [Val("dh", arg("dh"), dup.reshape(B, Tl, f, c0).sum(2), dupa.reshape(B, Tl, f, c0).sum(2),
+                chain=c(3 * f * co + 2)),
+            Acc("dw", arg("dw"), dw, dwa, chain=c(B * T + 2)),
+            Acc("dbias", cols("dbias", co), dy.sum((0, 1)), dy.abs().sum((0, 1)), chain=c(B * T + 2)),
+            Acc("dgate", cols("dgate", co), (dvs * y).sum(1), (dvs.abs() * ya).sum(1), chain=c(2 * (T + 3 * c0 + 2)))]
     xin = None
     if a["w_adapt"] is not None:
         xin = _stem_input(a).transpose(1, 2)                    # [B, T, cin]
+        xin_abs = _stem_input(a, absolute=True).transpose(1, 2) if f32 else xin.abs()
         cin = xin.shape[-1]
         outs += [Acc("dw_adapt", arg("dw_adapt"), dvs.reshape(-1, co).t() @ xin.reshape(-1, cin),
-                     dvs.abs().reshape(-1, co).t() @ xin.abs().reshape(-1, cin)),
-                 Acc("db_adapt", arg("db_adapt"), dvs.sum((0, 1)), dvs.abs().sum((0, 1)))]
+                     dvs.abs().reshape(-1, co).t() @ xin_abs.reshape(-1, cin), chain=c(B * T + 3)),
+                 Acc("db_adapt", arg("db_adapt"), dvs.sum((0, 1)), dvs.abs().sum((0, 1)), chain=c(B * T + 1))]
     if a["dxin"] is not None:          # through the skip path only, stored
         cin = a["dxin"].shape[1]
         if a["w_adapt"] is not None:
@@ -679,25 +788,32 @@ def c_stem_out_bwd(a, ctx):
         else:
             ref = torch.cat([dvs, dvs.new_zeros(B, T, cin - co)], -1)
             absr = ref.abs()
-        outs.append(Val("dxin", arg("dxin"), ref.transpose(1, 2), absr.transpose(1, 2)))
+        outs.append(Val("dxin", arg("dxin"), ref.transpose(1, 2), absr.transpose(1, 2), chain=c(co + 2)))
     return outs
 
 
 def c_stem_in_bwd(a, ctx):
     f = a["f"]
     xin, d = _stem_input(a), a["dout"].to(F64)
+    f32 = a["dout"].dtype == torch.float32
     B, cin, T = xin.shape
     c0 = d.shape[-1]
-    xr = xin.reshape(B, cin, T // f, f).permute(0, 2, 1, 3).reshape(-1, cin * f)
+
+    def rows(t):
+        return t.reshape(B, cin, T // f, f).permute(0, 2, 1, 3).reshape(-1, cin * f)
+    xr = rows(xin)
+    xa = rows(_stem_input(a, absolute=True)) if f32 else xr.abs()
     d2 = d.reshape(-1, c0)
-    outs = [Acc("dw", arg("dw"), (d2.t() @ xr).reshape(c0, cin, f), (d2.abs().t() @ xr.abs()).reshape(c0, cin, f)),
-            Acc("dbias", arg("dbias"), d2.sum(0), d2.abs().sum(0))]
+    c = (lambda n: n) if f32 else (lambda n: None)
+    outs = [Acc("dw", arg("dw"), (d2.t() @ xr).reshape(c0, cin, f), (d2.abs().t() @ xa).reshape(c0, cin, f),
+                chain=c(d2.shape[0] + 3)),
+            Acc("dbias", arg("dbias"), d2.sum(0), d2.abs().sum(0), chain=c(d2.shape[0] + 1))]
     if a["dxin"] is not None:
         Wm = a["w"].to(F64).reshape(c0, cin * f)
 
         def back(t):
             return t.reshape(B, T // f, cin, f).permute(0, 2, 1, 3).reshape(B, cin, T)
-        outs.append(Acc("dxin", arg("dxin"), back(d2 @ Wm), back(d2.abs() @ Wm.abs())))
+        outs.append(Acc("dxin", arg("dxin"), back(d2 @ Wm), back(d2.abs() @ Wm.abs()), chain=c(c0 + 1)))
     return outs
 
 
@@ -706,6 +822,7 @@ def c_attention_bwd(a, ctx):
     H, D, scale = a["heads"], a["head_dim"], a["scale"]
     B, Tq, Tk, mid = q.shape[0], q.shape[1], k.shape[1], H * D
     dev = q.device
+    f32 = q.dtype == torch.float32
     r = {n: torch.empty(B, t, mid, dtype=F64, device=dev) for n, t in
          (("dq", Tq), ("dk", Tk), ("dv", Tk), ("dqa", Tq), ("dka", Tk), ("dva", Tk))}
     delta = torch.empty(B, H, Tq, dtype=F64, device=dev)
@@ -723,13 +840,24 @@ def c_attention_bwd(a, ctx):
         dl, dla = (dO * O).sum(-1), (dO * O).abs().sum(-1)
         dS = P * (dO @ V.transpose(1, 2) - dl[..., None])
         dSa = P * (dO.abs() @ V.abs().transpose(1, 2) + dla[..., None])
+        Pa = P
+        if f32:
+            # the f32 kernels recompute s (a D-chain over |q| |k| scale): its absolute error is a
+            # relative one of P = exp(s - lse), carried into P and dS at the weight of one chain
+            sa = 1 + (Q.abs() @ K.abs().transpose(1, 2)) * scale
+            Pa, dSa = P * sa, dSa * sa
         delta[b], delta_abs[b] = dl, dla
-        r["dv"][b], r["dva"][b] = rows(P.transpose(1, 2) @ dO, Tk), rows(P.transpose(1, 2) @ dO.abs(), Tk)
+        r["dv"][b], r["dva"][b] = rows(P.transpose(1, 2) @ dO, Tk), rows(Pa.transpose(1, 2) @ dO.abs(), Tk)
         r["dq"][b], r["dqa"][b] = rows(dS @ K * scale, Tq), rows(dSa @ K.abs() * scale, Tq)
         r["dk"][b], r["dka"][b] = rows(dS.transpose(1, 2) @ Q * scale, Tk), rows(dSa.transpose(1, 2) @ Q.abs() * scale, Tk)
     # P and dS are rounded to bf16 for the second GEMMs
     def delta_view(p):       # a flat workspace sized for the largest item: this launch's rows come first
         return p["delta"].reshape(-1)[:B * H * Tq].view(B, H, Tq)
+    if f32:                  # dq sums Tk terms, dk and dv Tq terms, each over a D-chain of s and dO.v
+        return [Val("delta", delta_view, delta, delta_abs, chain=D + 2),
+                Val("dq", cols("dq", mid), r["dq"], r["dqa"], chain=Tk + D + 4),
+                Val("dk", cols("dk", mid), r["dk"], r["dka"], chain=Tq + D + 4),
+                Val("dv", cols("dv", mid), r["dv"], r["dva"], chain=Tq + D + 4)]
     return [Val("delta", delta_view, delta, delta_abs),
             Val("dq", cols("dq", mid), r["dq"], r["dqa"], TAU_BF16_OPERAND),
             Val("dk", cols("dk", mid), r["dk"], r["dka"], TAU_BF16_OPERAND),
@@ -956,8 +1084,9 @@ RESULT: Dict[str, Callable] = {"fir_resample": _fir_result, "mel_spectrogram": _
                                "to_flat": _to_flat_result, "to_flat_bwd": _to_flat_bwd_result}
 
 # Read arguments the kernel does not read for some argument combinations (the probe skips them):
-# narrow_conv copies the host-packed bf16 image instead of converting `w`, and the conv GEMM's
-# fp32-output epilogue has no residual (adp_conv_gemm refuses one).
+# narrow_conv copies the host-packed bf16 image instead of converting `w`, and the tensor-core conv
+# GEMM's fp32-output epilogue has no residual (adp_conv_gemm refuses one); f32_conv_gemm, whose
+# operands are fp32 too, adds it.
 # stem_out_bwd reads the block input only for the SkipAdapter's weight gradient, and stem_in_bwd
 # the weight only for dxin; stem_out reads x un-noised only for the loss target.
 # attention over a single key (the innermost level of length 1) has softmax identically 1: its
@@ -966,7 +1095,8 @@ RESULT: Dict[str, Callable] = {"fir_resample": _fir_result, "mel_spectrogram": _
 NOT_READ: Dict[str, Callable] = {
     "attention": lambda a: {"q", "k"} if a["k"].shape[1] == 1 and a["lse"] is None else set(),
     "narrow_conv": lambda a: {"w"} if a["w_packed"] is not None else set(),
-    "conv_gemm": lambda a: {"residual"} if a["out"].dtype == torch.float32 else set(),
+    "conv_gemm": lambda a: {"residual"} if a["out"].dtype == torch.float32 and a["a"].dtype != torch.float32
+    else set(),
     "stem_out_bwd": lambda a: {"x", "append", "noise", "alpha", "beta"} if a["w_adapt"] is None else set(),
     "stem_in_bwd": lambda a: {"w"} if a["dxin"] is None else set(),
     "cond_bwd": lambda a: {"w"} if a["dcond"] is None else set(),     # the weights serve dcond only
@@ -1233,7 +1363,9 @@ class Shadow:
         self.records: Dict[str, Record] = {}
         self.n_launch, self.n_checked, self.n_guarded = 0, 0, 0
         self.labels = set()                      # trace labels of the launches seen (shapes included)
+        self.symbols = set()                     # C entry points the checked launches called (ops._launch)
         self.known: Dict[int, torch.Tensor] = {}
+        self._depth = 0                          # > 0 inside a checked launch (a nested launch: see _wrap)
 
     # ---- install
     def __enter__(self):
@@ -1262,6 +1394,8 @@ class Shadow:
         sig = inspect.signature(real)
 
         def launch(*args, **kwargs):
+            if self._depth:           # a launch made by a checked launch's own ops call: part of it
+                return real(*args, **kwargs)
             if name not in CHECKERS:
                 raise CheckError(f"launch {self.n_launch}: {name} has no checker ({UNCHECKED.get(name, '?')})")
             b = sig.bind(*args, **kwargs)
@@ -1310,20 +1444,32 @@ class Shadow:
                 self._fake_write(outs, pre, run)
                 label = label0
             else:
-                if guards is None:
-                    with ops.trace() as tr:
-                        result = real(*args, **kwargs)
-                else:
-                    call = inspect.BoundArguments(sig, {n: run[n] for n in b.arguments})
-                    saved = ops.torch
-                    if name in RESULT:           # the outputs ops allocates go between guards too
-                        ops.torch = guards.torch_proxy()
-                    try:
+                self._depth += 1
+                try:
+                    if guards is None:
                         with ops.trace() as tr:
-                            result = real(*call.args, **call.kwargs)
-                    finally:
-                        ops.torch = saved
-                label = tr.records[-1]["name"] if tr.records else label0
+                            result = real(*args, **kwargs)
+                    else:
+                        call = inspect.BoundArguments(sig, {n: run[n] for n in b.arguments})
+                        saved = ops.torch
+                        if name in RESULT:           # the outputs ops allocates go between guards too
+                            ops.torch = guards.torch_proxy()
+                        try:
+                            with ops.trace() as tr:
+                                result = real(*call.args, **call.kwargs)
+                        finally:
+                            ops.torch = saved
+                finally:
+                    self._depth -= 1
+                # the first record is the launch itself; a nested one (gn_stats) follows it
+                label = tr.records[0]["name"] if tr.records else label0
+                nested = [r["symbol"] for r in tr.records[1:]]
+                if nested and (nested != ["adp_f32_gn_stats"] or name not in NESTED_STATS
+                               or post[NESTED_STATS[name]] is None):
+                    self._fail(idx, name, label, f"launches {nested} inside the ops call: only the fp32 "
+                                                 f"statistics pass of {sorted(NESTED_STATS)} is checked as part of "
+                                                 f"its caller")
+                self.symbols.update(r["symbol"] for r in tr.records)
                 if post[next(iter(post))].is_cuda:
                     torch.cuda.synchronize()
                 run.update(zip(made, result if len(made) > 1 else (result,)))
@@ -1434,7 +1580,15 @@ class Shadow:
                 self._note(key, 0.0, label, "")
                 continue
             g = got.to(F64)
-            if isinstance(o, Acc):                    # the launch's own contribution
+            if o.chain is not None:                   # an fp32 verification kernel (f32_*)
+                bound = F32_REL * ref.abs() + (F32_LAMBDA * math.sqrt(o.chain) * F32_U) * absr
+                val = g
+                if isinstance(o, Acc):
+                    before = o.view(pre).to(F64)
+                    val = g - before
+                    eps = F64_ACC_EPS if got.dtype == torch.float64 else ACC_EPS
+                    bound = bound + eps * (before.abs() + g.abs())
+            elif isinstance(o, Acc):                  # the launch's own contribution
                 before = o.view(pre).to(F64)
                 val = g - before
                 if got.dtype == torch.float64:
@@ -1626,6 +1780,22 @@ def m_readonly(post, outs, pre):
     return False
 
 
+def m_scale_largest_f32(post, outs, pre):
+    """The largest-|ref| element of the first stored output scaled by 1 + 2^-12 (an fp32 output
+    one bf16-class rounding off, which the fp32 bound must see)."""
+    o = next((o for o in outs if isinstance(o, (Val, Acc)) and not o.exact), None)
+    if o is None:
+        return False
+    ref = o.ref(post)[0] if callable(o.ref) else o.ref
+    g = o.view(post)
+    idx = _where(int(ref.abs().to(F64).reshape(-1).argmax()), tuple(g.shape))
+    if isinstance(o, Acc):                     # the launch's contribution, not the value before it
+        old = o.view(pre)[idx].to(F64)
+        g[idx] = (old + (g[idx].to(F64) - old) * (1 + 2 ** -12)).to(g.dtype)
+    else:
+        g[idx] = (g[idx].to(F64) * (1 + 2 ** -12)).to(g.dtype)
+
+
 def _alternative(kind, doc, **option):
     """A mutation that writes an alternative fp64 restatement of `kind` (CHECKERS[kind] with
     `option`) over the outputs, rounded to their dtype."""
@@ -1657,7 +1827,7 @@ def m_v_chan_stride(post, outs, pre):
 
 MUTATIONS = {"scale_largest": m_scale_largest, "stale_tile": m_stale_tile, "stats_slot": m_stats_slot,
              "outside_view": m_outside_view, "readonly": m_readonly, "acc_stored": m_acc_stored,
-             "acc_lost_split": m_acc_lost_split,
+             "acc_lost_split": m_acc_lost_split, "scale_largest_f32": m_scale_largest_f32,
              # kind-specific: an alternative operation written over the output
              "mel_symmetric_pad": _alternative(
                  "mel_spectrogram", "The edge frames cut from a symmetric pad (edge sample repeated).",
