@@ -61,7 +61,9 @@ __device__ __forceinline__ uint64_t v_desc_mnmajor(uint32_t addr) {
   else return gmma_desc_mnmajor_sw128(addr, D == 64 ? 1024 : kKT * 128);
 }
 
-template <int D>
+// LSE: the training forward, which also writes the log-sum-exp rows (p.lse); the inference
+// instantiation keeps no second row sum.
+template <int D, bool LSE>
 __global__ void __launch_bounds__(kAttnThreads, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                  const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
@@ -125,7 +127,10 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   const int row_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // fragment rows row_lo, row_lo + 8
   const int cq = 2 * (lane & 3);
   const uint64_t q_desc = gmma_desc_kmajor<kSW>(smem_u32(q_s) + wg * 64 * kSW);
-  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  // l_run: row sum of P as rounded to bf16 for the P V GEMM (it normalises o, so o is consistent
+  // with what the tensor cores saw); e_run: the same sum before that rounding (lse).  When the
+  // terms of a row round the same way (near-equal scores) the two differ by up to 2^-8.
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f}, e_run[2] = {0.f, 0.f};
   float o[D / 2];
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
@@ -168,7 +173,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     }
     // p = 2^(s*c - m*c) -> bf16 A fragments of P V (16 keys per fragment)
     uint32_t pa[kKT / 16][4];
-    float l_tile[2] = {0.f, 0.f};
+    float l_tile[2] = {0.f, 0.f}, e_tile[2] = {0.f, 0.f};
 #pragma unroll
     for (int kk = 0; kk < kKT / 16; ++kk) {
 #pragma unroll
@@ -180,10 +185,14 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
         pa[kk][q] = pack_bf16(p0, p1);
         const float2 pr = unpack_bf16(pa[kk][q]);   // sum what the MMA will actually see
         l_tile[r] += pr.x + pr.y;
+        if constexpr (LSE) e_tile[r] += p0 + p1;
       }
     }
-    l_run[0] = l_run[0] * alpha[0] + l_tile[0];
-    l_run[1] = l_run[1] * alpha[1] + l_tile[1];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      l_run[r] = l_run[r] * alpha[r] + l_tile[r];
+      if constexpr (LSE) e_run[r] = e_run[r] * alpha[r] + e_tile[r];
+    }
 
     const uint64_t v_desc = v_desc_mnmajor<D>(smem_u32(v_s + s * kKVBytes));
     wgmma_fence();
@@ -201,15 +210,19 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   for (int r = 0; r < 2; ++r) {
     l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
     l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
+    if constexpr (LSE) {
+      e_run[r] += __shfl_xor_sync(0xffffffffu, e_run[r], 1);
+      e_run[r] += __shfl_xor_sync(0xffffffffu, e_run[r], 2);
+    }
   }
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const int t = t0 + row_lo + 8 * r;
     if (t >= p.Tq) continue;
     const float inv_l = 1.f / l_run[r];
-    if (p.lse != nullptr && (lane & 3) == 0)    // natural-log units (adp_attention_bwd)
+    if (LSE && (lane & 3) == 0)                  // natural-log units (adp_attention_bwd)
       p.lse[(static_cast<size_t>(b) * gridDim.y + h) * p.Tq + t] =
-          (m_run[r] * p.scale_log2 + log2f(l_run[r])) * 0.6931471805599453f;
+          (m_run[r] * p.scale_log2 + log2f(e_run[r])) * 0.6931471805599453f;
     __nv_bfloat16* orow = p.o + (static_cast<size_t>(b) * p.Tq + t) * p.ldo + h * D;
 #pragma unroll
     for (int jb = 0; jb < D / 8; ++jb)
@@ -246,8 +259,9 @@ int attention_launch(const void* q, const void* k, const void* v, void* o, int32
     const uint64_t str[2] = {(uint64_t)ldv * 2, (uint64_t)Tk * ldv * 2};
     if (int e = make_tmap_bf16(&tmV, v, 3, dims, str, box, S::kSW)) return e;
   }
-  static SmemAttrCache smem_cache;
-  ADP_CUDA(ensure_dyn_smem(attention_kernel<D>, (size_t)S::kSmem, smem_cache));
+  auto kernel = lse != nullptr ? attention_kernel<D, true> : attention_kernel<D, false>;
+  static SmemAttrCache smem_cache, smem_cache_lse;
+  ADP_CUDA(ensure_dyn_smem(kernel, (size_t)S::kSmem, lse != nullptr ? smem_cache_lse : smem_cache));
   AttnParams p;
   p.o = static_cast<__nv_bfloat16*>(o);
   p.lse = lse;
@@ -256,7 +270,7 @@ int attention_launch(const void* q, const void* k, const void* v, void* o, int32
   p.ldo = ldo;
   p.scale_log2 = scale * 1.4426950408889634f;
   dim3 grid((Tq + kQT - 1) / kQT, H, B);
-  ADP_CUDA(launch_k(attention_kernel<D>, grid, dim3(kAttnThreads), (size_t)S::kSmem, as_stream(stream), tmQ, tmK, tmV, p));
+  ADP_CUDA(launch_k(kernel, grid, dim3(kAttnThreads), (size_t)S::kSmem, as_stream(stream), tmQ, tmK, tmV, p));
   ADP_LAUNCH_CHECK();
   return 0;
 }

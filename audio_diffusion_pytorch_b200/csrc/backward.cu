@@ -427,12 +427,14 @@ skip_gate_kernel(const uint4* __restrict__ y, const uint4* __restrict__ skip,
                  double* __restrict__ stats, int T, int C, int groups) {
   pdl_launch_dependents();
   pdl_wait();
-  extern __shared__ __align__(16) float s_bw[];     // 2 x C: per-channel sum / sum of squares of out
-  float* s_s1 = s_bw;
-  float* s_s2 = s_bw + C;
+  // 2 x C: per-channel sum / sum of squares of out, fp64 (the per-thread sums are pivot-shifted
+  // fp32, PivotStat, and come back unshifted in fp64)
+  extern __shared__ __align__(16) float s_bw[];
+  double* s_s1 = reinterpret_cast<double*>(s_bw);
+  double* s_s2 = s_s1 + C;
   const int b = blockIdx.y;
   if (stats) {                                     // no shared memory without statistics
-    for (int c = threadIdx.x; c < C; c += blockDim.x) { s_s1[c] = 0.f; s_s2[c] = 0.f; }
+    for (int c = threadIdx.x; c < C; c += blockDim.x) { s_s1[c] = 0.0; s_s2[c] = 0.0; }
   }
   __syncthreads();
   const int vpr = C >> 3, gsz = groups > 0 ? C / groups : C;
@@ -441,10 +443,12 @@ skip_gate_kernel(const uint4* __restrict__ y, const uint4* __restrict__ skip,
   const size_t nthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
   const size_t stride = chan_stride(nthreads, vpr);
   const int c0 = static_cast<int>(tid % vpr) << 3;
-  float g8[8], s1[8], s2[8];
+  float g8[8];
+  PivotStat st[8];
+  int n = 0;
 #pragma unroll
-  for (int j = 0; j < 8; ++j) { g8[j] = gate[static_cast<size_t>(b) * ld_gate + c0 + j]; s1[j] = 0.f; s2[j] = 0.f; }
-  for (size_t i = tid; tid < stride && i < nvec; i += stride) {
+  for (int j = 0; j < 8; ++j) g8[j] = gate[static_cast<size_t>(b) * ld_gate + c0 + j];
+  for (size_t i = tid; tid < stride && i < nvec; i += stride, ++n) {
     float fy[8], fs[8], o[8];
     unpack8(__ldg(y + boff + i), fy);
     unpack8(__ldg(skip + boff + i), fs);
@@ -456,15 +460,20 @@ skip_gate_kernel(const uint4* __restrict__ y, const uint4* __restrict__ skip,
       float orr[8];
       unpack8(ov, orr);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) { s1[j] += orr[j]; s2[j] += orr[j] * orr[j]; }
+      for (int j = 0; j < 8; ++j) st[j].add(orr[j], n == 0);
     }
   }
   if (stats) {
     const bool fold = fold_ok(vpr);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      float v1 = s1[j], v2 = s2[j];
-      if (fold) { v1 = fold_lanes(v1, vpr); v2 = fold_lanes(v2, vpr); }
+      double v1 = st[j].sum(n), v2 = st[j].sumsq(n);
+      if (fold) {
+        for (int o = vpr; o < 32; o <<= 1) {
+          v1 += __shfl_xor_sync(0xffffffffu, v1, o);
+          v2 += __shfl_xor_sync(0xffffffffu, v2, o);
+        }
+      }
       if (!fold || (threadIdx.x & 31) < vpr) {
         atomicAdd(&s_s1[c0 + j], v1);
         atomicAdd(&s_s2[c0 + j], v2);
@@ -473,10 +482,10 @@ skip_gate_kernel(const uint4* __restrict__ y, const uint4* __restrict__ skip,
     __syncthreads();
     if (threadIdx.x < 2 * groups) {
       const int g = threadIdx.x >> 1, which = threadIdx.x & 1;
-      const float* src = which ? s_s2 : s_s1;
-      float tot = 0.f;
+      const double* src = which ? s_s2 : s_s1;
+      double tot = 0.0;
       for (int c = g * gsz; c < (g + 1) * gsz; ++c) tot += src[c];
-      atomicAdd(stats + static_cast<size_t>(b) * 2 * groups + threadIdx.x, static_cast<double>(tot));
+      atomicAdd(stats + static_cast<size_t>(b) * 2 * groups + threadIdx.x, tot);
     }
   }
 }
@@ -698,7 +707,7 @@ extern "C" int adp_skip_gate(const void* y, const void* skip, const float* gate,
   ADP_CHECK(!stats || (groups > 0 && groups <= 64 && C % groups == 0 && C <= kBwMaxC),
             "adp_skip_gate: C=%d groups=%d (statistics need C <= %d)", C, groups, kBwMaxC);
   dim3 grid(grid_for(static_cast<size_t>(T) * (C / 8), B, C / 8), B);
-  const size_t smem = stats ? 2 * static_cast<size_t>(C) * sizeof(float) : 0;
+  const size_t smem = stats ? 2 * static_cast<size_t>(C) * sizeof(double) : 0;
   static SmemAttrCache smem_cache;
   ADP_CUDA(ensure_dyn_smem(skip_gate_kernel, smem, smem_cache));
   ADP_CUDA(launch_k(skip_gate_kernel, grid, dim3(256), smem, as_stream(stream),

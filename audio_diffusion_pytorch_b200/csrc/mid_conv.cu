@@ -63,14 +63,13 @@ __global__ void __launch_bounds__(NTH, 512 / NTH) mid_conv_kernel(const adp_narr
   __shared__ __align__(16) float s_ga[C], s_de[C];   // GroupNorm a, d per channel
   __shared__ __align__(16) float s_sc[C], s_sh[C];   // FiLM 1+scale, shift
   __shared__ float s_bias[C];
-  __shared__ float s_stats[2 * 64];
+  __shared__ float s_part[NTH / 32][C / 4][2];     // (sum, sumsq) per 4-channel block, one row per warp
   const int b = blockIdx.y;
   const int tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, q = lane & 3;
   const bool has_res = a.residual != nullptr, has_film = a.scale_shift != nullptr;
 
-  if (tid < 128) s_stats[tid] = 0.f;
   if (a.w_packed) {            // bf16 [C][3C] image prepared by the host: straight 16-byte copy
     constexpr int VPRW = 3 * C * 2 / 16;             // 16-byte vectors per W row
     const uint4* wp = static_cast<const uint4*>(a.w_packed);
@@ -285,7 +284,8 @@ __global__ void __launch_bounds__(NTH, 512 / NTH) mid_conv_kernel(const adp_narr
   }
   if (a.stats_out) {
     const int gsz = C / a.groups;
-    // lanes el, el+LPR, ... of a warp hold the same channels: fold, then one atomic per (warp, half)
+    // lanes el, el+LPR, ... of a warp hold the same channels: fold, then lane el writes its two
+    // 4-channel blocks into the warp's own row
 #pragma unroll
     for (int hf = 0; hf < 2; ++hf) {
 #pragma unroll
@@ -294,13 +294,20 @@ __global__ void __launch_bounds__(NTH, 512 / NTH) mid_conv_kernel(const adp_narr
         st_q[hf] += __shfl_xor_sync(0xffffffffu, st_q[hf], o);
       }
       if (lane < LPR) {
-        const int gi = (el * 8 + hf * 4) / gsz;
-        atomicAdd(&s_stats[2 * gi], st_s[hf]);
-        atomicAdd(&s_stats[2 * gi + 1], st_q[hf]);
+        s_part[warp][el * 2 + hf][0] = st_s[hf];
+        s_part[warp][el * 2 + hf][1] = st_q[hf];
       }
     }
     __syncthreads();
-    flush_group_stats(s_stats, a.stats_out, b, a.groups);
+    // warps and blocks summed in a fixed order (fp64; the host requires gsz % 4 == 0): the
+    // block's contribution does not depend on the order the warps finish in
+    if (tid < 2 * a.groups) {
+      const int gi = tid >> 1, which = tid & 1;
+      double tot = 0.0;
+      for (int w = 0; w < NTH / 32; ++w)
+        for (int k = gi * gsz / 4; k < (gi + 1) * gsz / 4; ++k) tot += s_part[w][k][which];
+      if (tot != 0.0) atomicAdd(a.stats_out + static_cast<size_t>(b) * 2 * a.groups + tid, tot);
+    }
   }
 }
 

@@ -325,6 +325,26 @@ struct GroupStatAcc {
   }
 };
 
+// One channel's (sum, sumsq) over the rows a thread visits, shifted by a pivot: the fp32 sums
+// run over d = x - c, c the first value the thread sees, and come back unshifted in fp64
+// (sum x = s + n c, sum x^2 = q + 2 c s + n c^2).  A group whose values sit close together
+// (|mean| >> std, or all equal) then keeps its variance: the fp32 sums carry the spread, not the
+// offset, and a constant group gives E[x^2] - mean^2 = 0 to fp64 round-off.
+struct PivotStat {
+  float c = 0.f, s = 0.f, q = 0.f;
+  __device__ __forceinline__ void add(float x, bool first) {
+    if (first) c = x;
+    const float d = x - c;
+    s += d;
+    q += d * d;
+  }
+  __device__ __forceinline__ double sum(int n) const { return static_cast<double>(s) + n * static_cast<double>(c); }
+  __device__ __forceinline__ double sumsq(int n) const {
+    const double cd = c;
+    return static_cast<double>(q) + 2.0 * cd * s + n * cd * cd;
+  }
+};
+
 // The block's shared-memory bins s_stats[2 * groups] -> the fp64 statistics of batch element b
 // (one atomic per non-zero bin).  After a __syncthreads that follows the last bin update.
 __device__ __forceinline__ void flush_group_stats(const float* s_stats, double* stats, int b, int groups) {

@@ -123,12 +123,13 @@ gn_stats_kernel(const uint4* __restrict__ x, double* __restrict__ stats, int T, 
                 int groups) {
   pdl_launch_dependents();
   pdl_wait();
-  // each thread keeps a fixed channel-vector (stride is a multiple of vectors-per-row)
-  __shared__ float s_acc[2 * 64];
+  // each thread keeps a fixed channel-vector (stride is a multiple of vectors-per-row); its
+  // per-channel sums are pivot-shifted fp32 (PivotStat), everything after them fp64
+  __shared__ double s_acc[2 * 64];
   const int b = blockIdx.y;
   const int gsz = C / groups;
   const int vpr = C >> 3;
-  if (threadIdx.x < 2 * groups) s_acc[threadIdx.x] = 0.f;
+  if (threadIdx.x < 2 * groups) s_acc[threadIdx.x] = 0.0;
   __syncthreads();
   const size_t nvec = static_cast<size_t>(T) * vpr;
   const uint4* xb = x + static_cast<size_t>(b) * nvec;
@@ -136,32 +137,39 @@ gn_stats_kernel(const uint4* __restrict__ x, double* __restrict__ stats, int T, 
   const size_t tid = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   const size_t nthreads = static_cast<size_t>(gridDim.x) * blockDim.x;
   const size_t stride = nthreads / vpr * vpr;      // round DOWN: threads >= stride sit out (host: vpr <= 256)
-  float s[8], q[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) { s[j] = 0.f; q[j] = 0.f; }
+  PivotStat st[8];
+  int n = 0;
   if (tid < stride) {
-    for (size_t i = tid; i < nvec; i += stride) {
+    for (size_t i = tid; i < nvec; i += stride, ++n) {
       const uint4 u = __ldg(xb + i);
       const uint32_t in[4] = {u.x, u.y, u.z, u.w};
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const float2 f = unpack_bf16(in[j]);
-        s[2 * j] += f.x; q[2 * j] += f.x * f.x;
-        s[2 * j + 1] += f.y; q[2 * j + 1] += f.y * f.y;
+        st[2 * j].add(f.x, n == 0);
+        st[2 * j + 1].add(f.y, n == 0);
       }
     }
     const int c = static_cast<int>(tid % vpr) << 3;
+    int gcur = c / gsz;
+    double a1 = 0.0, a2 = 0.0;                      // this thread's channels of group gcur
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const int g = (c + j) / gsz;
-      atomicAdd(&s_acc[2 * g], s[j]);
-      atomicAdd(&s_acc[2 * g + 1], q[j]);
+      if (g != gcur) {
+        atomicAdd(&s_acc[2 * gcur], a1);
+        atomicAdd(&s_acc[2 * gcur + 1], a2);
+        a1 = 0.0; a2 = 0.0; gcur = g;
+      }
+      a1 += st[j].sum(n);
+      a2 += st[j].sumsq(n);
     }
+    atomicAdd(&s_acc[2 * gcur], a1);
+    atomicAdd(&s_acc[2 * gcur + 1], a2);
   }
   __syncthreads();
   if (threadIdx.x < 2 * groups)
-    atomicAdd(stats + static_cast<size_t>(b) * 2 * groups + threadIdx.x,
-              static_cast<double>(s_acc[threadIdx.x]));
+    atomicAdd(stats + static_cast<size_t>(b) * 2 * groups + threadIdx.x, s_acc[threadIdx.x]);
 }
 
 // --------------------------------------------------------------------------- ln_film

@@ -241,12 +241,11 @@ __global__ void __launch_bounds__(256) narrow_conv_kernel(const adp_narrow_conv_
   constexpr int TB = 256;
   __shared__ __align__(128) uint4 s_rows[2][TB + 2];     // bf16 activated rows t0-1 .. t0+TB
   __shared__ float s_a[C], s_d[C];
-  __shared__ float s_stats[2 * C];
+  __shared__ float s_part[TB / 32][2 * C];               // (sum, sumsq) per channel, one row per warp
   const int b = blockIdx.y;
   const int tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, q = lane & 3;
-  if (tid < 2 * C) s_stats[tid] = 0.f;
   if (tid < C) {
     const int c = tid;
     const int gsz = C / a.groups, gi = c / gsz;
@@ -392,15 +391,19 @@ __global__ void __launch_bounds__(256) narrow_conv_kernel(const adp_narrow_conv_
       cs0 += __shfl_xor_sync(0xffffffffu, cs0, o); cq0 += __shfl_xor_sync(0xffffffffu, cq0, o);
       cs1 += __shfl_xor_sync(0xffffffffu, cs1, o); cq1 += __shfl_xor_sync(0xffffffffu, cq1, o);
     }
-    if (lane < 4) {            // lane == q: channels 2q, 2q+1
-      atomicAdd(&s_stats[2 * (2 * q)], cs0);     atomicAdd(&s_stats[2 * (2 * q) + 1], cq0);
-      atomicAdd(&s_stats[2 * (2 * q + 1)], cs1); atomicAdd(&s_stats[2 * (2 * q + 1) + 1], cq1);
+    if (lane < 4) {            // lane == q: channels 2q, 2q+1, into the warp's own row
+      s_part[warp][2 * (2 * q)] = cs0;     s_part[warp][2 * (2 * q) + 1] = cq0;
+      s_part[warp][2 * (2 * q + 1)] = cs1; s_part[warp][2 * (2 * q + 1) + 1] = cq1;
     }
     __syncthreads();
-    if (tid < 2 * C && s_stats[tid] != 0.f) {    // tid = 2*channel + {sum, sumsq}
-      const int c = tid >> 1, gi = c / (C / a.groups);
-      atomicAdd(a.stats_out + (static_cast<size_t>(b) * a.groups + gi) * 2 + (tid & 1),
-                static_cast<double>(s_stats[tid]));
+    // warps and channels summed in a fixed order (fp64): the block's contribution does not
+    // depend on the order the warps finish in, so a run repeats itself up to the fp64 atomics
+    if (tid < 2 * a.groups) {  // tid = 2*group + {sum, sumsq}
+      const int gi = tid >> 1, gsz = C / a.groups;
+      double tot = 0.0;
+      for (int w = 0; w < TB / 32; ++w)
+        for (int c = gi * gsz; c < (gi + 1) * gsz; ++c) tot += s_part[w][2 * c + (tid & 1)];
+      if (tot != 0.0) atomicAdd(a.stats_out + (static_cast<size_t>(b) * a.groups + gi) * 2 + (tid & 1), tot);
     }
   }
 }

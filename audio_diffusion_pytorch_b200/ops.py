@@ -158,7 +158,11 @@ def conv_gemm(a: Tensor, w: Tensor, out: Tensor, *, c_in: int, n_valid: int,
               residual: Optional[Tensor] = None, gate: Optional[Tensor] = None,
               stats: Optional[Tensor] = None, groups: int = 8, block_n: int = 0,
               gn: Optional[tuple] = None) -> Tensor:
-    """a: bf16 [B, T, lda]; w: packed bf16 [phases*n_pad, k_total]; out: [B, T, ldo]."""
+    """a: bf16 [B, T, lda]; w: packed bf16 [phases*n_pad, k_total]; out: [B, T, ldo].
+
+    stats: the epilogue adds the output's (sum, sumsq) per group in single-pass fp32 partials, so
+    E[x^2] - mean^2 keeps the variance within 1e-3 (var + 1e-5) for groups with |mean| / std up to
+    256 (tests/test_numeric_edges_gpu.py); at ~1000 its relative error reaches ~1.5e-2."""
     B, T, lda = a.shape
     phases = up_factor if up_factor > 1 else 1
     args = ConvGemmArgs()
@@ -215,6 +219,9 @@ def gn_silu(x: Tensor, y: Tensor, stats: Tensor, gamma: Tensor, beta: Tensor, gr
 
 
 def gn_stats(x: Tensor, stats: Tensor, groups: int) -> Tensor:
+    """stats [B, groups, 2] += (sum, sumsq) of x per group.  The per-thread sums are shifted by a
+    pivot (the first value each thread sees) and return to fp64 unshifted, so near-constant groups
+    keep their variance (|mean| / std ~1000: relative error ~1e-10; constant groups: 0)."""
     B, T, Cc = x.shape
     if x.dtype == torch.float32:
         assert x.is_contiguous()

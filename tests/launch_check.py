@@ -114,9 +114,10 @@ FP32_REL, FP32_TAU = 1e-5, 2.0 ** -14
 STATS_TOL = 1e-4
 VAR_TOL = 1e-3
 GN_EPS = 1e-5                    # every statistics slot feeds a GroupNorm: it divides by sqrt(var + eps)
-# attention's lse is log of the row sum of P AS ROUNDED TO bf16 for the P V GEMM (the sum that
-# normalises o): every term carries a relative rounding of up to 2^-9, so does the sum, and its log
-# moves by up to 2^-9 in absolute terms.  attention_bwd rounds the P it recomputes from lse to bf16 too.
+# attention's lse is log of the fp32 row sum of P, taken before P is rounded to bf16 for the P V GEMM
+# (the rounded sum normalises o only: when a row's terms all round the same way, near-equal scores,
+# the two sums differ by up to 2^-8).  LSE_FLOOR is the absolute allowance of 2^-9 kept for the log;
+# attention_bwd rounds the P it recomputes from lse to bf16.
 LSE_FLOOR = 2.0 ** -9
 ACC_EPS = 2.0 ** -23              # an fp32 accumulator's own rounding, per unit of |before| + |after|
 # the fp32 verification kernels (chain = n): err <= F32_REL |ref| + F32_LAMBDA sqrt(n) F32_U absref

@@ -267,6 +267,8 @@ def test_small_under_launch_checker(adp, case):
 
 # ------------------------------------------------------------------ c. full size under the checker
 def _room(gib):
+    gc.collect()                # this process's cached blocks are free to the test: release them first
+    torch.cuda.empty_cache()
     free = torch.cuda.mem_get_info()[0] / 2 ** 30
     assert free >= gib, f"{free:.1f} GiB of device memory free, this test needs about {gib} GiB"
 
