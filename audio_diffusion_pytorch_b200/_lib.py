@@ -76,6 +76,80 @@ class AttentionBwdArgs(C.Structure):
                 ("lddk", i32), ("lddv", i32), ("scale", f32)]
 
 
+# argtypes of every entry point of include/adp_b200.h that returns a status (0 = success): all but
+# adp_version and adp_last_error.  tests/test_abi_cpu.py checks each against its prototype.
+SIGNATURES = {
+    "adp_device_check": [],
+    "adp_debug_set": [i32, i32],
+    "adp_conv_gemm": [C.POINTER(ConvGemmArgs), vp],
+    "adp_gn_silu": [vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp],
+    "adp_gn_stats": [vp, vp, i32, i32, i32, i32, vp],
+    "adp_ln_film": [vp, vp, vp, i32, vp, i32, i32, i32, i32, f32, vp],
+    "adp_ln_film_dual": [vp, vp, vp, vp, i32, vp, i32, i32, i32, i32, f32, f32, vp],
+    "adp_attention": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, f32, vp, vp],
+    "adp_attention_hd": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, f32, vp, vp],
+    "adp_attention_bwd": [C.POINTER(AttentionBwdArgs), vp],
+    "adp_attention_bwd_hd": [C.POINTER(AttentionBwdArgs), i32, vp],
+    "adp_ln_fold_bwd": [vp, vp, vp, vp, i32, vp, vp, vp, vp, i32, i32, vp],
+    "adp_skinny_linear": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp],
+    "adp_time_features": [vp, vp, vp, i32, i32, i32, vp],
+    "adp_stem_in": [C.POINTER(StemInArgs), vp],
+    "adp_stem_out": [C.POINTER(StemOutArgs), vp],
+    "adp_narrow_conv": [C.POINTER(NarrowConvArgs), vp],
+    "adp_sampler_step": [vp, vp, vp, vp, C.c_int64, vp],
+    "adp_inpaint_blend": [vp, vp, vp, vp, vp, C.c_int64, vp],
+    "adp_arv_step": [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp],
+    "adp_resample": [vp, vp, vp] + [C.c_int] * 7 + [vp],
+    "adp_resample_adjoint": [vp, vp, vp] + [C.c_int] * 7 + [vp],
+    "adp_mel_spectrogram": [vp] * 5 + [C.c_int] * 9 + [vp],
+    "adp_to_flat": [vp, vp, vp] + [C.c_int] * 7 + [vp],
+    "adp_to_flat_bwd": [vp] * 5 + [C.c_int] * 7 + [vp],
+    "adp_stft_loss_fwd": [vp] * 7 + [C.c_int] * 7 + [f32] * 5 + [C.c_int, vp],
+    "adp_stft_loss_bwd": [vp] * 8 + [C.c_int] * 7 + [f32] * 5 + [C.c_int, vp],
+    "adp_f32_conv_gemm": [C.POINTER(ConvGemmArgs), vp],
+    "adp_f32_gn_stats": [vp, vp, i32, i32, i32, i32, vp],
+    "adp_f32_gn_silu": [vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp],
+    "adp_f32_ln_film": [vp, vp, vp, vp, i32, i32, i32, i32, f32, f32, vp],
+    "adp_f32_attention": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, f32, vp],
+    "adp_f32_attention_hd": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, f32, vp],
+    "adp_f32_linear": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp],
+    "adp_f32_silu": [vp, vp, C.c_int64, vp],
+    "adp_f32_stem_in": [C.POINTER(StemInArgs), vp],
+    "adp_f32_stem_out": [C.POINTER(StemOutArgs), vp],
+    "adp_f32_attention_lse": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, f32, vp, vp],
+    "adp_f32_stem_in_train": [C.POINTER(StemInArgs), vp],
+    "adp_f32_stem_out_train": [C.POINTER(StemOutArgs), vp],
+    "adp_f32_wgrad": [C.POINTER(WgradArgs), vp],
+    "adp_f32_gn_silu_bwd": [vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp],
+    "adp_f32_gn_bwd_apply": [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp],
+    "adp_f32_ln_film_bwd": [vp, vp, vp, i32, vp, vp, i32, vp, vp, i32, i32, i32, f32, vp],
+    "adp_f32_colsum": [vp, vp, i32, vp, i32, i32, i32, vp],
+    "adp_f32_skip_gate": [vp, vp, vp, i32, vp, vp, i32, i32, i32, i32, vp],
+    "adp_f32_skip_gate_bwd": [vp, vp, vp, i32, vp, vp, i32, i32, i32, i32, vp],
+    "adp_f32_cond_bwd": [vp, i32, vp, vp, vp, vp, vp, i32, i32, i32, vp],
+    "adp_f32_stem_out_bwd": [C.POINTER(StemOutBwdArgs), vp],
+    "adp_f32_stem_in_bwd": [C.POINTER(StemInBwdArgs), vp],
+    "adp_f32_attention_bwd": [C.POINTER(AttentionBwdArgs), i32, vp],
+    "adp_step_select": [vp, vp, vp, vp, vp, C.c_int64, vp],
+    "adp_step_advance": [vp, vp],
+    "adp_silu_bf16": [vp, vp, C.c_int64, vp],
+    "adp_wgrad": [C.POINTER(WgradArgs), vp],
+    "adp_gn_silu_bwd": [vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp],
+    "adp_gn_bwd_apply": [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp],
+    "adp_ln_film_bwd": [vp, vp, vp, i32, vp, vp, i32, vp, vp, i32, i32, i32, f32, vp],
+    "adp_colsum": [vp, vp, i32, vp, i32, i32, i32, vp],
+    "adp_skip_gate": [vp, vp, vp, i32, vp, vp, i32, i32, i32, i32, vp],
+    "adp_skip_gate_bwd": [vp, vp, vp, i32, vp, vp, i32, i32, i32, i32, vp],
+    "adp_cond_bwd": [vp, i32, vp, vp, vp, vp, vp, i32, i32, i32, vp],
+    "adp_narrow_conv_bwd": [C.POINTER(NarrowConvBwdArgs), vp],
+    "adp_stem_out_bwd": [C.POINTER(StemOutBwdArgs), vp],
+    "adp_stem_in_bwd": [C.POINTER(StemInBwdArgs), vp],
+}
+
+# every symbol include/adp_b200.h declares
+EXPORTS = ["adp_version", "adp_last_error"] + list(SIGNATURES)
+
+
 _lib = None
 
 
@@ -91,78 +165,9 @@ def lib() -> C.CDLL:
     L = C.CDLL(LIB_PATH)
     L.adp_last_error.restype = C.c_char_p
     L.adp_version.restype = i32
-    sig = {
-        "adp_device_check": [],
-        "adp_debug_set": [i32, i32],
-        "adp_conv_gemm": [C.POINTER(ConvGemmArgs), vp],
-        "adp_gn_silu": [vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp],
-        "adp_gn_stats": [vp, vp, i32, i32, i32, i32, vp],
-        "adp_ln_film": [vp, vp, vp, i32, vp, i32, i32, i32, i32, f32, vp],
-        "adp_ln_film_dual": [vp, vp, vp, vp, i32, vp, i32, i32, i32, i32, f32, f32, vp],
-        "adp_attention": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, f32, vp, vp],
-        "adp_attention_hd": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, f32, vp, vp],
-        "adp_attention_bwd": [C.POINTER(AttentionBwdArgs), vp],
-        "adp_attention_bwd_hd": [C.POINTER(AttentionBwdArgs), i32, vp],
-        "adp_ln_fold_bwd": [vp, vp, vp, vp, i32, vp, vp, vp, vp, i32, i32, vp],
-        "adp_skinny_linear": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp],
-        "adp_time_features": [vp, vp, vp, i32, i32, i32, vp],
-        "adp_stem_in": [C.POINTER(StemInArgs), vp],
-        "adp_stem_out": [C.POINTER(StemOutArgs), vp],
-        "adp_narrow_conv": [C.POINTER(NarrowConvArgs), vp],
-        "adp_sampler_step": [vp, vp, vp, vp, C.c_int64, vp],
-        "adp_inpaint_blend": [vp, vp, vp, vp, vp, C.c_int64, vp],
-        "adp_arv_step": [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp],
-        "adp_resample": [vp, vp, vp] + [C.c_int] * 7 + [vp],
-        "adp_resample_adjoint": [vp, vp, vp] + [C.c_int] * 7 + [vp],
-        "adp_mel_spectrogram": [vp] * 5 + [C.c_int] * 9 + [vp],
-        "adp_to_flat": [vp, vp, vp] + [C.c_int] * 7 + [vp],
-        "adp_to_flat_bwd": [vp] * 5 + [C.c_int] * 7 + [vp],
-        "adp_stft_loss_fwd": [vp] * 7 + [C.c_int] * 7 + [f32] * 5 + [C.c_int, vp],
-        "adp_stft_loss_bwd": [vp] * 8 + [C.c_int] * 7 + [f32] * 5 + [C.c_int, vp],
-        "adp_f32_conv_gemm": [C.POINTER(ConvGemmArgs), vp],
-        "adp_f32_gn_stats": [vp, vp, i32, i32, i32, i32, vp],
-        "adp_f32_gn_silu": [vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp],
-        "adp_f32_ln_film": [vp, vp, vp, vp, i32, i32, i32, i32, f32, f32, vp],
-        "adp_f32_attention": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, f32, vp],
-        "adp_f32_attention_hd": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, f32, vp],
-        "adp_f32_linear": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp],
-        "adp_f32_silu": [vp, vp, C.c_int64, vp],
-        "adp_f32_stem_in": [C.POINTER(StemInArgs), vp],
-        "adp_f32_stem_out": [C.POINTER(StemOutArgs), vp],
-        "adp_f32_attention_lse": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, f32, vp, vp],
-        "adp_f32_stem_in_train": [C.POINTER(StemInArgs), vp],
-        "adp_f32_stem_out_train": [C.POINTER(StemOutArgs), vp],
-        "adp_f32_wgrad": [C.POINTER(WgradArgs), vp],
-        "adp_f32_gn_silu_bwd": [vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp],
-        "adp_f32_gn_bwd_apply": [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp],
-        "adp_f32_ln_film_bwd": [vp, vp, vp, i32, vp, vp, i32, vp, vp, i32, i32, i32, f32, vp],
-        "adp_f32_colsum": [vp, vp, i32, vp, i32, i32, i32, vp],
-        "adp_f32_skip_gate": [vp, vp, vp, i32, vp, vp, i32, i32, i32, i32, vp],
-        "adp_f32_skip_gate_bwd": [vp, vp, vp, i32, vp, vp, i32, i32, i32, i32, vp],
-        "adp_f32_cond_bwd": [vp, i32, vp, vp, vp, vp, vp, i32, i32, i32, vp],
-        "adp_f32_stem_out_bwd": [C.POINTER(StemOutBwdArgs), vp],
-        "adp_f32_stem_in_bwd": [C.POINTER(StemInBwdArgs), vp],
-        "adp_f32_attention_bwd": [C.POINTER(AttentionBwdArgs), i32, vp],
-        "adp_step_select": [vp, vp, vp, vp, vp, C.c_int64, vp],
-        "adp_step_advance": [vp, vp],
-        "adp_silu_bf16": [vp, vp, C.c_int64, vp],
-        "adp_wgrad": [C.POINTER(WgradArgs), vp],
-        "adp_gn_silu_bwd": [vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp],
-        "adp_gn_bwd_apply": [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp],
-        "adp_ln_film_bwd": [vp, vp, vp, i32, vp, vp, i32, vp, vp, i32, i32, i32, f32, vp],
-        "adp_colsum": [vp, vp, i32, vp, i32, i32, i32, vp],
-        "adp_skip_gate": [vp, vp, vp, i32, vp, vp, i32, i32, i32, i32, vp],
-        "adp_skip_gate_bwd": [vp, vp, vp, i32, vp, vp, i32, i32, i32, i32, vp],
-        "adp_cond_bwd": [vp, i32, vp, vp, vp, vp, vp, i32, i32, i32, vp],
-        "adp_narrow_conv_bwd": [C.POINTER(NarrowConvBwdArgs), vp],
-        "adp_stem_out_bwd": [C.POINTER(StemOutBwdArgs), vp],
-        "adp_stem_in_bwd": [C.POINTER(StemInBwdArgs), vp],
-    }
-    for name, argtypes in sig.items():
-        if hasattr(L, name):
-            fn = getattr(L, name)
-            fn.argtypes = argtypes
-            fn.restype = i32
+    for name, argtypes in SIGNATURES.items():
+        fn = getattr(L, name)           # a symbol the library lacks raises here, naming it
+        fn.argtypes, fn.restype = argtypes, i32
     _lib = L
     return L
 
@@ -170,21 +175,3 @@ def lib() -> C.CDLL:
 def check(rc: int, what: str) -> None:
     if rc != 0:
         raise RuntimeError(f"{what} failed: {lib().adp_last_error().decode()}")
-
-
-EXPORTS = ["adp_version", "adp_last_error", "adp_device_check", "adp_conv_gemm", "adp_gn_silu",
-           "adp_gn_stats", "adp_ln_film", "adp_ln_film_dual", "adp_attention", "adp_skinny_linear",
-           "adp_time_features", "adp_stem_in", "adp_stem_out", "adp_narrow_conv",
-           "adp_sampler_step", "adp_silu_bf16", "adp_debug_set", "adp_wgrad", "adp_gn_silu_bwd",
-           "adp_gn_bwd_apply", "adp_ln_film_bwd", "adp_colsum", "adp_skip_gate",
-           "adp_skip_gate_bwd", "adp_cond_bwd", "adp_narrow_conv_bwd", "adp_stem_out_bwd",
-           "adp_stem_in_bwd", "adp_attention_bwd", "adp_ln_fold_bwd", "adp_inpaint_blend", "adp_arv_step", "adp_resample", "adp_resample_adjoint",
-           "adp_mel_spectrogram", "adp_to_flat", "adp_to_flat_bwd", "adp_stft_loss_fwd", "adp_stft_loss_bwd",
-           "adp_f32_conv_gemm", "adp_f32_gn_stats",
-           "adp_f32_gn_silu", "adp_f32_ln_film", "adp_f32_attention", "adp_f32_linear", "adp_f32_silu",
-           "adp_f32_stem_in", "adp_f32_stem_out", "adp_step_select", "adp_step_advance",
-           "adp_attention_hd", "adp_attention_bwd_hd", "adp_f32_attention_hd", "adp_f32_attention_lse",
-           "adp_f32_stem_in_train", "adp_f32_stem_out_train", "adp_f32_wgrad", "adp_f32_gn_silu_bwd",
-           "adp_f32_gn_bwd_apply", "adp_f32_ln_film_bwd", "adp_f32_colsum", "adp_f32_skip_gate",
-           "adp_f32_skip_gate_bwd", "adp_f32_cond_bwd", "adp_f32_stem_out_bwd", "adp_f32_stem_in_bwd",
-           "adp_f32_attention_bwd"]

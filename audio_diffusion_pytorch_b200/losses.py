@@ -26,7 +26,7 @@ from typing import List, Sequence, Tuple
 import torch
 from torch import Tensor, nn
 
-from . import _lib, ops
+from . import ops
 
 # auraloss options this module does not implement, with the value that means "off": passing that
 # value is accepted, anything else is refused with the option named
@@ -97,11 +97,11 @@ def _fwd(x: Tensor, y: Tensor, res, weights, eps: float, scale: float, acc: Tens
     window = _window(n_fft, win, x.device)
     partials = torch.empty(rows, (frames + 7) // 8, 4, device=x.device, dtype=torch.float64)
     stats = torch.empty(rows, 2, device=x.device, dtype=torch.float64)
-    ops._launch(lambda: _lib.lib().adp_stft_loss_fwd(
+    ops._launch("adp_stft_loss_fwd", (
         x.data_ptr(), y.data_ptr(), window.data_ptr(), partials.data_ptr(), stats.data_ptr(), acc.data_ptr(),
         loss.data_ptr(), rows, t, n_fft, hop, win, frames, 1 if x.dtype == torch.bfloat16 else 0, eps,
-        *weights, scale, 1 if accumulate else 0, ops._stream()),
-        "adp_stft_loss_fwd", lambda: (f"stft_loss_fwd[n_fft={n_fft}]", 0, ops._nb(x, y)))
+        *weights, scale, 1 if accumulate else 0),
+        lambda: (f"stft_loss_fwd[n_fft={n_fft}]", 0, ops._nb(x, y)))
     return stats
 
 
@@ -113,11 +113,11 @@ def _bwd(x: Tensor, y: Tensor, res, weights, eps: float, scale: float, stats: Te
     frames = _frames(t, n_fft, hop)
     window = _window(n_fft, win, x.device)
     frame_grad = torch.empty(rows, frames, win, device=x.device, dtype=torch.float32)
-    ops._launch(lambda: _lib.lib().adp_stft_loss_bwd(
+    ops._launch("adp_stft_loss_bwd", (
         x.data_ptr(), y.data_ptr(), window.data_ptr(), stats.data_ptr(), grad_out.data_ptr(),
         frame_grad.data_ptr(), dx.data_ptr(), ops._p(dx_bf16), rows, t, n_fft, hop, win, frames,
-        1 if x.dtype == torch.bfloat16 else 0, eps, *weights, scale, 1 if accumulate else 0, ops._stream()),
-        "adp_stft_loss_bwd", lambda: (f"stft_loss_bwd[n_fft={n_fft}]", 0, ops._nb(x, y, dx)))
+        1 if x.dtype == torch.bfloat16 else 0, eps, *weights, scale, 1 if accumulate else 0),
+        lambda: (f"stft_loss_bwd[n_fft={n_fft}]", 0, ops._nb(x, y, dx)))
 
 
 class _STFTLossFunction(torch.autograd.Function):

@@ -67,22 +67,30 @@ class trace:
         return out
 
 
-def _launch(fn, what: str, meta):
-    """meta: callable -> (label, flops, bytes); evaluated only while tracing."""
+def _launch(symbol: str, args: tuple, meta):
+    """Calls the C entry point `symbol` with args + (the current stream,) and raises on a non-zero
+    status.  meta: callable -> (label, flops, bytes); evaluated only while tracing."""
+    fn = getattr(_lib.lib(), symbol)
     tr = _TRACE
     if tr is None:
-        _lib.check(fn(), what)
+        _lib.check(fn(*args, _stream()), symbol)
         return
     label, flops, nbytes = meta()
-    rec = {"name": label, "symbol": what, "flops": float(flops), "bytes": float(nbytes)}
+    rec = {"name": label, "symbol": symbol, "flops": float(flops), "bytes": float(nbytes)}
     if tr.timing:
         rec["e0"] = torch.cuda.Event(enable_timing=True)
         rec["e1"] = torch.cuda.Event(enable_timing=True)
         rec["e0"].record()
-    _lib.check(fn(), what)
+    _lib.check(fn(*args, _stream()), symbol)
     if tr.timing:
         rec["e1"].record()
     tr.records.append(rec)
+
+
+def _f32(t: Tensor) -> str:
+    """The trace-label prefix of the fp32 verification mode (adp_f32_* entry points) when t is fp32,
+    else the empty string."""
+    return "f32_" if t.dtype == torch.float32 else ""
 
 
 def _nb(*tensors) -> int:
@@ -190,31 +198,25 @@ def conv_gemm(a: Tensor, w: Tensor, out: Tensor, *, c_in: int, n_valid: int,
             + rows * phases * n_valid * out.element_size() * (2 if residual is not None else 1)
         return f"conv_gemm[{kind} M={rows} K={c_in} N={n_valid}x{phases}]", flops, nbytes
 
-    if a.dtype == torch.float32:       # fp32 verification mode (csrc/verify_f32.cu)
+    f32 = _f32(a)
+    if f32:                            # fp32 verification mode (csrc/verify_f32.cu)
         assert w.dtype == torch.float32 and out.dtype == torch.float32 and gn is None
         assert residual is None or residual.dtype == torch.float32
         args.stats, args.out_fp32 = None, 0
-        _launch(lambda: _lib.lib().adp_f32_conv_gemm(C.byref(args), _stream()), "adp_f32_conv_gemm", meta)
-        if stats is not None:
-            assert out.shape[-1] == phases * n_valid, "statistics need a dense output"
-            gn_stats(out.reshape(B, -1, n_valid), stats, groups)
-        return out
-    _launch(lambda: _lib.lib().adp_conv_gemm(C.byref(args), _stream()), "adp_conv_gemm", meta)
+    _launch("adp_f32_conv_gemm" if f32 else "adp_conv_gemm", (C.byref(args),), meta)
+    if f32 and stats is not None:
+        assert out.shape[-1] == phases * n_valid, "statistics need a dense output"
+        gn_stats(out.reshape(B, -1, n_valid), stats, groups)
     return out
 
 
 def gn_silu(x: Tensor, y: Tensor, stats: Tensor, gamma: Tensor, beta: Tensor, groups: int,
             eps: float = 1e-5) -> Tensor:
     B, T, Cc = x.shape
-    if x.dtype == torch.float32:
-        _launch(lambda: _lib.lib().adp_f32_gn_silu(x.data_ptr(), y.data_ptr(), stats.data_ptr(), gamma.data_ptr(),
-                                                   beta.data_ptr(), B, T, Cc, groups, eps, _stream()),
-                "adp_f32_gn_silu", lambda: (f"f32_gn_silu[M={B * T} C={Cc}]", 0, _nb(x, y)))
-        return y
-    _launch(lambda: _lib.lib().adp_gn_silu(x.data_ptr(), y.data_ptr(), stats.data_ptr(),
-                                           gamma.data_ptr(), beta.data_ptr(), B, T, Cc, groups,
-                                           eps, _stream()), "adp_gn_silu",
-            lambda: (f"gn_silu[M={B * T} C={Cc}]", 0, _nb(x, y)))
+    f32 = _f32(x)
+    _launch("adp_f32_gn_silu" if f32 else "adp_gn_silu",
+            (x.data_ptr(), y.data_ptr(), stats.data_ptr(), gamma.data_ptr(), beta.data_ptr(), B, T, Cc, groups, eps),
+            lambda: (f"{f32}gn_silu[M={B * T} C={Cc}]", 0, _nb(x, y)))
     return y
 
 
@@ -223,14 +225,11 @@ def gn_stats(x: Tensor, stats: Tensor, groups: int) -> Tensor:
     pivot (the first value each thread sees) and return to fp64 unshifted, so near-constant groups
     keep their variance (|mean| / std ~1000: relative error ~1e-10; constant groups: 0)."""
     B, T, Cc = x.shape
-    if x.dtype == torch.float32:
+    f32 = _f32(x)
+    if f32:
         assert x.is_contiguous()
-        _launch(lambda: _lib.lib().adp_f32_gn_stats(x.data_ptr(), stats.data_ptr(), B, T, Cc, groups, _stream()),
-                "adp_f32_gn_stats", lambda: (f"f32_gn_stats[M={B * T} C={Cc}]", 0, _nb(x)))
-        return stats
-    _launch(lambda: _lib.lib().adp_gn_stats(x.data_ptr(), stats.data_ptr(), B, T, Cc, groups,
-                                            _stream()), "adp_gn_stats",
-            lambda: (f"gn_stats[M={B * T} C={Cc}]", 0, _nb(x)))
+    _launch("adp_f32_gn_stats" if f32 else "adp_gn_stats", (x.data_ptr(), stats.data_ptr(), B, T, Cc, groups),
+            lambda: (f"{f32}gn_stats[M={B * T} C={Cc}]", 0, _nb(x)))
     return stats
 
 
@@ -239,22 +238,20 @@ def ln_film(x: Tensor, y: Tensor, scale_shift: Optional[Tensor] = None, ss_strid
             y2: Optional[Tensor] = None, eps2: float = 1e-5) -> Tensor:
     """y = LN(x)*(1+scale)+shift; with y2 also y2 = LN(y; eps2) in the same pass."""
     B, T, Cc = x.shape
-    if x.dtype == torch.float32:
-        _launch(lambda: _lib.lib().adp_f32_ln_film(x.data_ptr(), y.data_ptr(), _p(y2), _p(scale_shift), ss_stride,
-                                                   B, T, Cc, eps, eps2, _stream()),
-                "adp_f32_ln_film", lambda: (f"f32_ln_film[M={B * T} C={Cc}]", 0, _nb(x, y, y2)))
+    if x.dtype == torch.float32:       # no statistics argument: they are a gn_stats pass of their own
+        _launch("adp_f32_ln_film", (x.data_ptr(), y.data_ptr(), _p(y2), _p(scale_shift), ss_stride, B, T, Cc, eps,
+                                    eps2),
+                lambda: (f"f32_ln_film[M={B * T} C={Cc}]", 0, _nb(x, y, y2)))
         if stats_out is not None:
             gn_stats(y, stats_out, groups)
-        return y
-    if y2 is None:
-        _launch(lambda: _lib.lib().adp_ln_film(x.data_ptr(), y.data_ptr(), _p(scale_shift), ss_stride,
-                                               _p(stats_out), B, T, Cc, groups, eps, _stream()),
-                "adp_ln_film", lambda: (f"ln_film[M={B * T} C={Cc}]", 0, _nb(x, y)))
+    elif y2 is None:
+        _launch("adp_ln_film", (x.data_ptr(), y.data_ptr(), _p(scale_shift), ss_stride, _p(stats_out), B, T, Cc,
+                                groups, eps),
+                lambda: (f"ln_film[M={B * T} C={Cc}]", 0, _nb(x, y)))
     else:
-        _launch(lambda: _lib.lib().adp_ln_film_dual(x.data_ptr(), y.data_ptr(), y2.data_ptr(),
-                                                    _p(scale_shift), ss_stride, _p(stats_out), B, T, Cc,
-                                                    groups, eps, eps2, _stream()),
-                "adp_ln_film_dual", lambda: (f"ln_film_dual[M={B * T} C={Cc}]", 0, _nb(x, y, y2)))
+        _launch("adp_ln_film_dual", (x.data_ptr(), y.data_ptr(), y2.data_ptr(), _p(scale_shift), ss_stride,
+                                     _p(stats_out), B, T, Cc, groups, eps, eps2),
+                lambda: (f"ln_film_dual[M={B * T} C={Cc}]", 0, _nb(x, y, y2)))
     return y
 
 
@@ -270,25 +267,18 @@ def attention(q: Tensor, k: Tensor, v: Tensor, o: Tensor, heads: int, scale: flo
     B, Tq = q.shape[0], q.shape[1]
     Tk = k.shape[1]
     D, tag = head_dim, _hd_tag(head_dim)
+    args = (q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), B, heads, D, Tq, Tk, q.stride(1), k.stride(1),
+            v.stride(1), o.stride(1), scale)
     if q.dtype == torch.float32:
         if lse is not None:            # training forward: also the log-sum-exp rows
-            _launch(lambda: _lib.lib().adp_f32_attention_lse(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
-                                                             B, heads, D, Tq, Tk, q.stride(1), k.stride(1),
-                                                             v.stride(1), o.stride(1), scale, lse.data_ptr(),
-                                                             _stream()),
-                    "adp_f32_attention_lse", lambda: (f"f32_attention[B={B} H={heads} Tq={Tq} Tk={Tk}{tag} +lse]",
-                                                      4.0 * B * heads * Tq * Tk * D, 0))
-            return o
-        _launch(lambda: _lib.lib().adp_f32_attention_hd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
-                                                        B, heads, D, Tq, Tk, q.stride(1), k.stride(1),
-                                                        v.stride(1), o.stride(1), scale, _stream()),
-                "adp_f32_attention", lambda: (f"f32_attention[B={B} H={heads} Tq={Tq} Tk={Tk}{tag}]",
-                                              4.0 * B * heads * Tq * Tk * D, 0))
+            _launch("adp_f32_attention_lse", args + (lse.data_ptr(),),
+                    lambda: (f"f32_attention[B={B} H={heads} Tq={Tq} Tk={Tk}{tag} +lse]",
+                             4.0 * B * heads * Tq * Tk * D, 0))
+        else:
+            _launch("adp_f32_attention_hd", args,
+                    lambda: (f"f32_attention[B={B} H={heads} Tq={Tq} Tk={Tk}{tag}]", 4.0 * B * heads * Tq * Tk * D, 0))
         return o
-    _launch(lambda: _lib.lib().adp_attention_hd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
-                                                B, heads, D, Tq, Tk, q.stride(1), k.stride(1),
-                                                v.stride(1), o.stride(1), scale, _p(lse), _stream()),
-            "adp_attention",
+    _launch("adp_attention_hd", args + (_p(lse),),
             lambda: (f"attention[B={B} H={heads} Tq={Tq} Tk={Tk}{tag}]", 4.0 * B * heads * Tq * Tk * D,
                      (2 * B * Tq + 2 * B * Tk) * heads * D * 2))
     return o
@@ -296,36 +286,26 @@ def attention(q: Tensor, k: Tensor, v: Tensor, o: Tensor, heads: int, scale: flo
 
 def skinny_linear(x: Tensor, w: Tensor, bias: Optional[Tensor], y: Tensor, K: int, N: int,
                   in_act: int = ACT_NONE, out_act: int = ACT_NONE) -> Tensor:
-    if w.dtype == torch.float32:
-        _launch(lambda: _lib.lib().adp_f32_linear(x.data_ptr(), w.data_ptr(), _p(bias), y.data_ptr(), x.shape[0],
-                                                  K, N, x.stride(0), w.stride(0), y.stride(0), in_act, out_act,
-                                                  _stream()),
-                "adp_f32_linear", lambda: (f"f32_linear[B={x.shape[0]} K={K} N={N}]", 2.0 * x.shape[0] * K * N,
-                                           _nb(w)))
-        return y
-    _launch(lambda: _lib.lib().adp_skinny_linear(x.data_ptr(), w.data_ptr(), _p(bias), y.data_ptr(),
-                                                 x.shape[0], K, N, x.stride(0), w.stride(0),
-                                                 y.stride(0), in_act, out_act, _stream()),
-            "adp_skinny_linear",
-            lambda: (f"skinny_linear[B={x.shape[0]} K={K} N={N}]", 2.0 * x.shape[0] * K * N, _nb(w)))
+    f32 = _f32(w)
+    _launch("adp_f32_linear" if f32 else "adp_skinny_linear",
+            (x.data_ptr(), w.data_ptr(), _p(bias), y.data_ptr(), x.shape[0], K, N, x.stride(0), w.stride(0),
+             y.stride(0), in_act, out_act),
+            lambda: (f"{'f32_linear' if f32 else 'skinny_linear'}[B={x.shape[0]} K={K} N={N}]",
+                     2.0 * x.shape[0] * K * N, _nb(w)))
     return y
 
 
 def time_features(sigma: Tensor, freqs: Tensor, out: Tensor) -> Tensor:
-    _launch(lambda: _lib.lib().adp_time_features(sigma.data_ptr(), freqs.data_ptr(), out.data_ptr(),
-                                                 sigma.shape[0], freqs.shape[0], out.stride(0),
-                                                 _stream()), "adp_time_features",
+    _launch("adp_time_features",
+            (sigma.data_ptr(), freqs.data_ptr(), out.data_ptr(), sigma.shape[0], freqs.shape[0], out.stride(0)),
             lambda: ("time_features", 0, _nb(out)))
     return out
 
 
 def silu_bf16(x: Tensor, y: Tensor) -> Tensor:
-    if y.dtype == torch.float32:
-        _launch(lambda: _lib.lib().adp_f32_silu(x.data_ptr(), y.data_ptr(), x.numel(), _stream()),
-                "adp_f32_silu", lambda: ("f32_silu", 0, _nb(x, y)))
-        return y
-    _launch(lambda: _lib.lib().adp_silu_bf16(x.data_ptr(), y.data_ptr(), x.numel(), _stream()),
-            "adp_silu_bf16", lambda: ("silu_bf16", 0, _nb(x, y)))
+    f32 = _f32(y)
+    _launch("adp_f32_silu" if f32 else "adp_silu_bf16", (x.data_ptr(), y.data_ptr(), x.numel()),
+            lambda: ("f32_silu" if f32 else "silu_bf16", 0, _nb(x, y)))
     return y
 
 
@@ -339,21 +319,18 @@ def stem_in(x: Tensor, w: Tensor, bias: Optional[Tensor], out: Tensor, f: int, *
     a.B, a.cx, a.T = x.shape
     a.ca = 0 if append is None else append.shape[1]
     a.c0, a.f, a.groups = w.shape[0], f, groups
-    if out.dtype == torch.float32:
+    f32 = _f32(out)
+    train = f32 and noise is not None  # the fp32 training forward: the VDiffusion noising
+    if f32:                            # the statistics are a gn_stats pass of their own
         a.stats = None
-        if noise is not None:          # training forward: the VDiffusion noising
-            _launch(lambda: _lib.lib().adp_f32_stem_in_train(C.byref(a), _stream()), "adp_f32_stem_in_train",
-                    lambda: (f"f32_stem_in[B={x.shape[0]} T={x.shape[2]} c0={w.shape[0]} +noise]", 0,
-                             _nb(x, append, noise, out)))
-        else:
-            _launch(lambda: _lib.lib().adp_f32_stem_in(C.byref(a), _stream()), "adp_f32_stem_in",
-                    lambda: (f"f32_stem_in[B={x.shape[0]} T={x.shape[2]} c0={w.shape[0]}]", 0, _nb(x, append, out)))
-        if stats is not None:
-            gn_stats(out, stats, groups)
-        return out
-    _launch(lambda: _lib.lib().adp_stem_in(C.byref(a), _stream()), "adp_stem_in",
-            lambda: (f"stem_in[B={x.shape[0]} T={x.shape[2]} c0={w.shape[0]}]",
-                     2.0 * out.numel() * w.shape[1] * w.shape[2], _nb(x, append, noise, out)))
+        symbol = "adp_f32_stem_in_train" if train else "adp_f32_stem_in"
+    else:
+        symbol = "adp_stem_in"
+    _launch(symbol, (C.byref(a),),
+            lambda: (f"{f32}stem_in[B={x.shape[0]} T={x.shape[2]} c0={w.shape[0]}{' +noise' if train else ''}]",
+                     0 if f32 else 2.0 * out.numel() * w.shape[1] * w.shape[2], _nb(x, append, noise, out)))
+    if f32 and stats is not None:
+        gn_stats(out, stats, groups)
     return out
 
 
@@ -375,19 +352,16 @@ def stem_out(h: Tensor, x: Tensor, w: Tensor, bias: Optional[Tensor], gate: Tens
     a.ca = 0 if append is None else append.shape[1]
     a.c0, a.co, a.f = h.shape[-1], w.shape[0], f
     a.ld_gate = gate.stride(0)
-    if h.dtype == torch.float32:
-        if noise is not None or loss_sum is not None or dv is not None:    # training forward
-            _launch(lambda: _lib.lib().adp_f32_stem_out_train(C.byref(a), _stream()), "adp_f32_stem_out_train",
-                    lambda: (f"f32_stem_out[B={x.shape[0]} T={x.shape[2]} c0={h.shape[-1]} +loss]", 0,
-                             _nb(h, x, noise, v_out, dv)))
-            return
-        _launch(lambda: _lib.lib().adp_f32_stem_out(C.byref(a), _stream()), "adp_f32_stem_out",
-                lambda: (f"f32_stem_out[B={x.shape[0]} T={x.shape[2]} c0={h.shape[-1]}]", 0, _nb(h, x, v_out)))
-        return
-    _launch(lambda: _lib.lib().adp_stem_out(C.byref(a), _stream()), "adp_stem_out",
-            lambda: (f"stem_out[B={x.shape[0]} T={x.shape[2]} c0={h.shape[-1]}]",
-                     2.0 * h.shape[0] * x.shape[2] * w.numel(),
-                     _nb(h, x, append, noise, v_out, x_next, dv)))
+    f32 = _f32(h)
+    train = f32 and (noise is not None or loss_sum is not None or dv is not None)    # the fp32 training forward
+    if f32:
+        symbol = "adp_f32_stem_out_train" if train else "adp_f32_stem_out"
+    else:
+        symbol = "adp_stem_out"
+    _launch(symbol, (C.byref(a),),
+            lambda: (f"{f32}stem_out[B={x.shape[0]} T={x.shape[2]} c0={h.shape[-1]}{' +loss' if train else ''}]",
+                     0 if f32 else 2.0 * h.shape[0] * x.shape[2] * w.numel(),
+                     _nb(h, x, noise, v_out, dv) if f32 else _nb(h, x, append, noise, v_out, x_next, dv)))
 
 
 def narrow_conv(x: Tensor, y: Tensor, stats_in: Tensor, gamma: Tensor, beta: Tensor, w: Tensor,
@@ -403,7 +377,7 @@ def narrow_conv(x: Tensor, y: Tensor, stats_in: Tensor, gamma: Tensor, beta: Ten
     a.ss_stride = ss_stride
     a.B, a.T, a.C = x.shape
     a.groups, a.gn_eps, a.ln_eps = groups, gn_eps, ln_eps
-    _launch(lambda: _lib.lib().adp_narrow_conv(C.byref(a), _stream()), "adp_narrow_conv",
+    _launch("adp_narrow_conv", (C.byref(a),),
             lambda: (f"narrow_conv[M={x.shape[0] * x.shape[1]} C={x.shape[2]}"
                      f"{' +res+film' if residual is not None else ''}]",
                      2.0 * x.numel() * 3 * x.shape[2], _nb(x, y, residual)))
@@ -418,29 +392,28 @@ def pack_mid_conv(w: Tensor) -> Tensor:
 
 
 def sampler_step(x: Tensor, v: Tensor, ab: Tensor, x_next: Tensor) -> Tensor:
-    _launch(lambda: _lib.lib().adp_sampler_step(x.data_ptr(), v.data_ptr(), ab.data_ptr(),
-                                                x_next.data_ptr(), x.numel(), _stream()),
-            "adp_sampler_step", lambda: ("sampler_step", 0, _nb(x, v, x_next)))
+    _launch("adp_sampler_step", (x.data_ptr(), v.data_ptr(), ab.data_ptr(), x_next.data_ptr(), x.numel()),
+            lambda: ("sampler_step", 0, _nb(x, v, x_next)))
     return x_next
 
 
 def step_select(step: Tensor, ctrl: Tensor, ab_table: Tensor, ab_out: Tensor, ss_out: Tensor) -> None:
     """ss_out <- table[step // ctrl[1]], ab_out <- ab_table[step]  (table address in ctrl[0])."""
-    _launch(lambda: _lib.lib().adp_step_select(step.data_ptr(), ctrl.data_ptr(), ab_table.data_ptr(),
-                                               ab_out.data_ptr(), ss_out.data_ptr(), ss_out.numel(), _stream()),
-            "adp_step_select", lambda: ("step_select", 0, 2 * _nb(ss_out)))
+    _launch("adp_step_select", (step.data_ptr(), ctrl.data_ptr(), ab_table.data_ptr(), ab_out.data_ptr(),
+                                ss_out.data_ptr(), ss_out.numel()),
+            lambda: ("step_select", 0, 2 * _nb(ss_out)))
 
 
 def step_advance(step: Tensor) -> None:
-    _launch(lambda: _lib.lib().adp_step_advance(step.data_ptr(), _stream()), "adp_step_advance",
+    _launch("adp_step_advance", (step.data_ptr(),),
             lambda: ("step_advance", 0, 4))
 
 
 def inpaint_blend(x: Tensor, source: Tensor, noise: Tensor, mask_u8: Tensor, ab: Tensor) -> Tensor:
     """In place: x = ab[2]*source + ab[3]*noise where mask (VInpainter, reference diffusion.py:346-350)."""
-    _launch(lambda: _lib.lib().adp_inpaint_blend(x.data_ptr(), source.data_ptr(), noise.data_ptr(),
-                                                 mask_u8.data_ptr(), ab.data_ptr(), x.numel(), _stream()),
-            "adp_inpaint_blend", lambda: ("inpaint_blend", 0, _nb(x, source, noise, mask_u8)))
+    _launch("adp_inpaint_blend",
+            (x.data_ptr(), source.data_ptr(), noise.data_ptr(), mask_u8.data_ptr(), ab.data_ptr(), x.numel()),
+            lambda: ("inpaint_blend", 0, _nb(x, source, noise, mask_u8)))
     return x
 
 
@@ -448,9 +421,8 @@ def arv_step(chan: Tensor, v: Tensor, sig_next: Tensor) -> Tensor:
     """In place on chan [B, C+1, T] (current | sigma_i): the ARVSampler update with per-position
     noise levels (reference diffusion.py:231-235); channel C becomes sig_next [B, T]."""
     B, C1, T = chan.shape
-    _launch(lambda: _lib.lib().adp_arv_step(chan.data_ptr(), v.data_ptr(), sig_next.data_ptr(), B, C1 - 1,
-                                            T, _stream()),
-            "adp_arv_step", lambda: ("arv_step", 0, 2 * _nb(chan) + _nb(v)))
+    _launch("adp_arv_step", (chan.data_ptr(), v.data_ptr(), sig_next.data_ptr(), B, C1 - 1, T),
+            lambda: ("arv_step", 0, 2 * _nb(chan) + _nb(v)))
     return chan
 
 
@@ -461,21 +433,14 @@ def fir_resample(x: Tensor, bank: Tensor, factor_in: int, factor_out: int, half:
     (adp_resample); with adjoint_of = t the transposed map [rows, t_out] -> [rows, t]."""
     rows = x.shape[0]
     taps = bank.shape[1]
-    if adjoint_of is None:
-        t = x.shape[1]
-        y = torch.empty(rows, t_out, device=x.device, dtype=torch.float32)
-        _launch(lambda: _lib.lib().adp_resample(x.data_ptr(), bank.data_ptr(), y.data_ptr(), rows, t, t_out,
-                                                factor_in, factor_out, taps, half, _stream()),
-                "adp_resample", lambda: (f"resample[{factor_in}->{factor_out}]", 2.0 * rows * t_out * taps,
-                                         _nb(x, y)))
-        return y
-    t = adjoint_of
-    dx = torch.empty(rows, t, device=x.device, dtype=torch.float32)
-    _launch(lambda: _lib.lib().adp_resample_adjoint(x.data_ptr(), bank.data_ptr(), dx.data_ptr(), rows, t,
-                                                    t_out, factor_in, factor_out, taps, half, _stream()),
-            "adp_resample_adjoint", lambda: (f"resample_adjoint[{factor_in}->{factor_out}]",
-                                             2.0 * rows * t_out * taps, _nb(x, dx)))
-    return dx
+    adjoint = adjoint_of is not None
+    t = adjoint_of if adjoint else x.shape[1]
+    y = torch.empty(rows, t if adjoint else t_out, device=x.device, dtype=torch.float32)
+    _launch("adp_resample_adjoint" if adjoint else "adp_resample",
+            (x.data_ptr(), bank.data_ptr(), y.data_ptr(), rows, t, t_out, factor_in, factor_out, taps, half),
+            lambda: (f"resample{'_adjoint' if adjoint else ''}[{factor_in}->{factor_out}]",
+                     2.0 * rows * t_out * taps, _nb(x, y)))
+    return y
 
 
 def mel_spectrogram(wave: Tensor, window: Tensor, fb: Tensor, band: Tensor, n_fft: int, hop: int,
@@ -486,11 +451,10 @@ def mel_spectrogram(wave: Tensor, window: Tensor, fb: Tensor, band: Tensor, n_ff
     n_mels = fb.shape[1]
     frames = 1 + (t + 2 * pad + 2 * center_pad - n_fft) // hop
     mel = torch.empty(rows, n_mels, frames, device=wave.device, dtype=torch.float32)
-    _launch(lambda: _lib.lib().adp_mel_spectrogram(wave.data_ptr(), window.data_ptr(), fb.data_ptr(),
-                                                   band.data_ptr(), mel.data_ptr(), rows, t, n_fft, hop, pad,
-                                                   center_pad, frames, n_mels, 1 if apply_log else 0,
-                                                   _stream()),
-            "adp_mel_spectrogram", lambda: (f"mel_spectrogram[n_fft={n_fft}]", 0, _nb(wave, mel)))
+    _launch("adp_mel_spectrogram", (wave.data_ptr(), window.data_ptr(), fb.data_ptr(), band.data_ptr(),
+                                    mel.data_ptr(), rows, t, n_fft, hop, pad, center_pad, frames, n_mels,
+                                    1 if apply_log else 0),
+            lambda: (f"mel_spectrogram[n_fft={n_fft}]", 0, _nb(wave, mel)))
     return mel
 
 
@@ -500,9 +464,8 @@ def to_flat(spec: Tensor, w: Tensor, hop: int, pad: int) -> Tensor:
     win = w.shape[1]
     t_out = (frames - 1) * hop - 2 * pad + win
     out = torch.empty(B, t_out, device=spec.device, dtype=torch.float32)
-    _launch(lambda: _lib.lib().adp_to_flat(spec.data_ptr(), w.data_ptr(), out.data_ptr(), B, Cc, frames, win,
-                                           hop, pad, t_out, _stream()),
-            "adp_to_flat", lambda: ("to_flat", 2.0 * B * t_out * Cc * (win // hop), _nb(spec, out)))
+    _launch("adp_to_flat", (spec.data_ptr(), w.data_ptr(), out.data_ptr(), B, Cc, frames, win, hop, pad, t_out),
+            lambda: ("to_flat", 2.0 * B * t_out * Cc * (win // hop), _nb(spec, out)))
     return out
 
 
@@ -513,9 +476,9 @@ def to_flat_bwd(spec: Tensor, w: Tensor, dout: Tensor, hop: int, pad: int, need_
     t_out = dout.shape[1]
     dspec = torch.empty_like(spec) if need_dspec else None
     dw = torch.zeros_like(w) if need_dw else None
-    _launch(lambda: _lib.lib().adp_to_flat_bwd(spec.data_ptr(), w.data_ptr(), dout.data_ptr(), _p(dspec),
-                                               _p(dw), B, Cc, frames, win, hop, pad, t_out, _stream()),
-            "adp_to_flat_bwd", lambda: ("to_flat_bwd", 4.0 * B * Cc * frames * win, _nb(spec, dout)))
+    _launch("adp_to_flat_bwd", (spec.data_ptr(), w.data_ptr(), dout.data_ptr(), _p(dspec), _p(dw), B, Cc, frames,
+                                win, hop, pad, t_out),
+            lambda: ("to_flat_bwd", 4.0 * B * Cc * frames * win, _nb(spec, dout)))
     return dspec, dw
 
 
@@ -539,33 +502,24 @@ def wgrad(g: Tensor, x: Tensor, dw: Tensor, *, n: int, k: int, off: int = 0, g_c
     a.ldg, a.ldx, a.ldw = g.stride(1), x.stride(1), dw.stride(-2)
     a.g_cols, a.x_cols = g.shape[2], x.shape[2]
     a.g_col0, a.x_col0, a.off = g_col0, x_col0, off
-    if g.dtype == torch.float32:       # fp32 verification mode (csrc/verify_f32_bwd.cu)
+    f32 = _f32(g)
+    if f32:                            # fp32 verification mode (csrc/verify_f32_bwd.cu)
         assert x.dtype == torch.float32
-        _launch(lambda: _lib.lib().adp_f32_wgrad(C.byref(a), _stream()), "adp_f32_wgrad",
-                lambda: (f"f32_wgrad[M={g.shape[0] * g.shape[1]} n={n} k={k}{' x3' if ntaps == 3 else ''}]",
-                         2.0 * g.shape[0] * g.shape[1] * n * k * ntaps, 0))
-        return dw
-    _launch(lambda: _lib.lib().adp_wgrad(C.byref(a), _stream()), "adp_wgrad",
-            lambda: (f"wgrad[M={g.shape[0] * g.shape[1]} n={n} k={k}{' x3' if ntaps == 3 else ''}]",
-                     2.0 * g.shape[0] * g.shape[1] * n * k * ntaps, (g.shape[0] * g.shape[1]) * (n + k) * 2))
+    _launch("adp_f32_wgrad" if f32 else "adp_wgrad", (C.byref(a),),
+            lambda: (f"{f32}wgrad[M={g.shape[0] * g.shape[1]} n={n} k={k}{' x3' if ntaps == 3 else ''}]",
+                     2.0 * g.shape[0] * g.shape[1] * n * k * ntaps,
+                     0 if f32 else (g.shape[0] * g.shape[1]) * (n + k) * 2))
     return dw
 
 
 def gn_silu_bwd(da: Tensor, x: Tensor, stats: Tensor, gamma: Tensor, beta: Tensor, dxh: Tensor,
                 dgamma: Tensor, dbeta: Tensor, S: Tensor, groups: int, eps: float = 1e-5) -> Tensor:
     B, T, Cc = x.shape
-    if x.dtype == torch.float32:
-        _launch(lambda: _lib.lib().adp_f32_gn_silu_bwd(da.data_ptr(), x.data_ptr(), stats.data_ptr(),
-                                                       gamma.data_ptr(), beta.data_ptr(), dxh.data_ptr(),
-                                                       dgamma.data_ptr(), dbeta.data_ptr(), S.data_ptr(),
-                                                       B, T, Cc, groups, eps, _stream()),
-                "adp_f32_gn_silu_bwd", lambda: (f"f32_gn_silu_bwd[M={B * T} C={Cc}]", 0, _nb(da, x, dxh)))
-        return dxh
-    _launch(lambda: _lib.lib().adp_gn_silu_bwd(da.data_ptr(), x.data_ptr(), stats.data_ptr(),
-                                               gamma.data_ptr(), beta.data_ptr(), dxh.data_ptr(),
-                                               dgamma.data_ptr(), dbeta.data_ptr(), S.data_ptr(),
-                                               B, T, Cc, groups, eps, _stream()),
-            "adp_gn_silu_bwd", lambda: (f"gn_silu_bwd[M={B * T} C={Cc}]", 0, _nb(da, x, dxh)))
+    f32 = _f32(x)
+    _launch("adp_f32_gn_silu_bwd" if f32 else "adp_gn_silu_bwd",
+            (da.data_ptr(), x.data_ptr(), stats.data_ptr(), gamma.data_ptr(), beta.data_ptr(), dxh.data_ptr(),
+             dgamma.data_ptr(), dbeta.data_ptr(), S.data_ptr(), B, T, Cc, groups, eps),
+            lambda: (f"{f32}gn_silu_bwd[M={B * T} C={Cc}]", 0, _nb(da, x, dxh)))
     return dxh
 
 
@@ -573,16 +527,11 @@ def gn_bwd_apply(dxh: Tensor, x: Tensor, stats: Tensor, S: Tensor, dx: Tensor, g
                  dres: Optional[Tensor] = None, colsum: Optional[Tensor] = None,
                  eps: float = 1e-5) -> Tensor:
     B, T, Cc = x.shape
-    if x.dtype == torch.float32:
-        _launch(lambda: _lib.lib().adp_f32_gn_bwd_apply(dxh.data_ptr(), x.data_ptr(), stats.data_ptr(),
-                                                        S.data_ptr(), _p(dres), dx.data_ptr(), _p(colsum),
-                                                        B, T, Cc, groups, eps, _stream()),
-                "adp_f32_gn_bwd_apply", lambda: (f"f32_gn_bwd_apply[M={B * T} C={Cc}]", 0, _nb(dxh, x, dres, dx)))
-        return dx
-    _launch(lambda: _lib.lib().adp_gn_bwd_apply(dxh.data_ptr(), x.data_ptr(), stats.data_ptr(),
-                                                S.data_ptr(), _p(dres), dx.data_ptr(), _p(colsum),
-                                                B, T, Cc, groups, eps, _stream()),
-            "adp_gn_bwd_apply", lambda: (f"gn_bwd_apply[M={B * T} C={Cc}]", 0, _nb(dxh, x, dres, dx)))
+    f32 = _f32(x)
+    _launch("adp_f32_gn_bwd_apply" if f32 else "adp_gn_bwd_apply",
+            (dxh.data_ptr(), x.data_ptr(), stats.data_ptr(), S.data_ptr(), _p(dres), dx.data_ptr(), _p(colsum),
+             B, T, Cc, groups, eps),
+            lambda: (f"{f32}gn_bwd_apply[M={B * T} C={Cc}]", 0, _nb(dxh, x, dres, dx)))
     return dx
 
 
@@ -591,78 +540,54 @@ def ln_film_bwd(dy: Tensor, x: Tensor, scale_shift: Optional[Tensor], ss_stride:
                 colsum: Optional[Tensor] = None, dres: Optional[Tensor] = None,
                 eps: float = 1e-6) -> Tensor:
     B, T, Cc = x.shape
-    if x.dtype == torch.float32:
-        _launch(lambda: _lib.lib().adp_f32_ln_film_bwd(dy.data_ptr(), x.data_ptr(), _p(scale_shift),
-                                                       ss_stride, dx.data_ptr(), _p(dss), dss_stride,
-                                                       _p(colsum), _p(dres), B, T, Cc, eps, _stream()),
-                "adp_f32_ln_film_bwd", lambda: (f"f32_ln_film_bwd[M={B * T} C={Cc}]", 0, _nb(dy, x, dx)))
-        return dx
-    _launch(lambda: _lib.lib().adp_ln_film_bwd(dy.data_ptr(), x.data_ptr(), _p(scale_shift),
-                                               ss_stride, dx.data_ptr(), _p(dss), dss_stride,
-                                               _p(colsum), _p(dres), B, T, Cc, eps, _stream()),
-            "adp_ln_film_bwd", lambda: (f"ln_film_bwd[M={B * T} C={Cc}]", 0, _nb(dy, x, dx)))
+    f32 = _f32(x)
+    _launch("adp_f32_ln_film_bwd" if f32 else "adp_ln_film_bwd",
+            (dy.data_ptr(), x.data_ptr(), _p(scale_shift), ss_stride, dx.data_ptr(), _p(dss), dss_stride,
+             _p(colsum), _p(dres), B, T, Cc, eps),
+            lambda: (f"{f32}ln_film_bwd[M={B * T} C={Cc}]", 0, _nb(dy, x, dx)))
     return dx
 
 
 def colsum(x: Tensor, out: Tensor, gate: Optional[Tensor] = None) -> Tensor:
     B, T, Cc = x.shape
-    if x.dtype == torch.float32:
-        _launch(lambda: _lib.lib().adp_f32_colsum(x.data_ptr(), _p(gate), 0 if gate is None else gate.stride(0),
-                                                  out.data_ptr(), B, T, Cc, _stream()),
-                "adp_f32_colsum", lambda: (f"f32_colsum[M={B * T} C={Cc}]", 0, _nb(x)))
-        return out
-    _launch(lambda: _lib.lib().adp_colsum(x.data_ptr(), _p(gate), 0 if gate is None else gate.stride(0),
-                                          out.data_ptr(), B, T, Cc, _stream()),
-            "adp_colsum", lambda: (f"colsum[M={B * T} C={Cc}]", 0, _nb(x)))
+    f32 = _f32(x)
+    _launch("adp_f32_colsum" if f32 else "adp_colsum",
+            (x.data_ptr(), _p(gate), 0 if gate is None else gate.stride(0), out.data_ptr(), B, T, Cc),
+            lambda: (f"{f32}colsum[M={B * T} C={Cc}]", 0, _nb(x)))
     return out
 
 
 def skip_gate(y: Tensor, skip: Tensor, gate: Tensor, out: Tensor, stats: Optional[Tensor],
               groups: int) -> Tensor:
     B, T, Cc = y.shape
-    if y.dtype == torch.float32:       # the statistics of out are their own pass, as in conv_gemm
-        _launch(lambda: _lib.lib().adp_f32_skip_gate(y.data_ptr(), skip.data_ptr(), gate.data_ptr(),
-                                                     gate.stride(0), out.data_ptr(), None, B, T, Cc, groups,
-                                                     _stream()),
-                "adp_f32_skip_gate", lambda: (f"f32_skip_gate[M={B * T} C={Cc}]", 0, _nb(y, skip, out)))
-        if stats is not None:
-            gn_stats(out, stats, groups)
-        return out
-    _launch(lambda: _lib.lib().adp_skip_gate(y.data_ptr(), skip.data_ptr(), gate.data_ptr(),
-                                             gate.stride(0), out.data_ptr(), _p(stats), B, T, Cc,
-                                             groups, _stream()),
-            "adp_skip_gate", lambda: (f"skip_gate[M={B * T} C={Cc}]", 0, _nb(y, skip, out)))
+    f32 = _f32(y)                      # fp32: the statistics of out are their own pass, as in conv_gemm
+    _launch("adp_f32_skip_gate" if f32 else "adp_skip_gate",
+            (y.data_ptr(), skip.data_ptr(), gate.data_ptr(), gate.stride(0), out.data_ptr(),
+             None if f32 else _p(stats), B, T, Cc, groups),
+            lambda: (f"{f32}skip_gate[M={B * T} C={Cc}]", 0, _nb(y, skip, out)))
+    if f32 and stats is not None:
+        gn_stats(out, stats, groups)
     return out
 
 
 def skip_gate_bwd(dout: Tensor, y: Tensor, gate: Tensor, dys: Tensor, dgate: Tensor) -> Tensor:
     B, T, Cc = y.shape
-    if y.dtype == torch.float32:
-        _launch(lambda: _lib.lib().adp_f32_skip_gate_bwd(dout.data_ptr(), y.data_ptr(), gate.data_ptr(),
-                                                         gate.stride(0), dys.data_ptr(), dgate.data_ptr(),
-                                                         dgate.stride(0), B, T, Cc, _stream()),
-                "adp_f32_skip_gate_bwd", lambda: (f"f32_skip_gate_bwd[M={B * T} C={Cc}]", 0, _nb(dout, y, dys)))
-        return dys
-    _launch(lambda: _lib.lib().adp_skip_gate_bwd(dout.data_ptr(), y.data_ptr(), gate.data_ptr(),
-                                                 gate.stride(0), dys.data_ptr(), dgate.data_ptr(),
-                                                 dgate.stride(0), B, T, Cc, _stream()),
-            "adp_skip_gate_bwd", lambda: (f"skip_gate_bwd[M={B * T} C={Cc}]", 0, _nb(dout, y, dys)))
+    f32 = _f32(y)
+    _launch("adp_f32_skip_gate_bwd" if f32 else "adp_skip_gate_bwd",
+            (dout.data_ptr(), y.data_ptr(), gate.data_ptr(), gate.stride(0), dys.data_ptr(), dgate.data_ptr(),
+             dgate.stride(0), B, T, Cc),
+            lambda: (f"{f32}skip_gate_bwd[M={B * T} C={Cc}]", 0, _nb(dout, y, dys)))
     return dys
 
 
 def cond_bwd(dss: Tensor, cond: Tensor, w: Tensor, dw: Tensor, dbias: Tensor, dcond: Optional[Tensor],
              N: int) -> None:
     B, K = cond.shape
-    if w.dtype == torch.float32:       # the fp32 verification mode's packed projection
-        _launch(lambda: _lib.lib().adp_f32_cond_bwd(dss.data_ptr(), dss.stride(0), cond.data_ptr(),
-                                                    w.data_ptr(), dw.data_ptr(), dbias.data_ptr(),
-                                                    _p(dcond), B, N, K, _stream()),
-                "adp_f32_cond_bwd", lambda: (f"f32_cond_bwd[B={B} N={N} K={K}]", 4.0 * B * N * K, 0))
-        return
-    _launch(lambda: _lib.lib().adp_cond_bwd(dss.data_ptr(), dss.stride(0), cond.data_ptr(),
-                                            w.data_ptr(), dw.data_ptr(), dbias.data_ptr(),
-                                            _p(dcond), B, N, K, _stream()),
-            "adp_cond_bwd", lambda: (f"cond_bwd[B={B} N={N} K={K}]", 4.0 * B * N * K, N * K * 6))
+    f32 = _f32(w)                      # fp32: the fp32 verification mode's packed projection
+    _launch("adp_f32_cond_bwd" if f32 else "adp_cond_bwd",
+            (dss.data_ptr(), dss.stride(0), cond.data_ptr(), w.data_ptr(), dw.data_ptr(), dbias.data_ptr(),
+             _p(dcond), B, N, K),
+            lambda: (f"{f32}cond_bwd[B={B} N={N} K={K}]", 4.0 * B * N * K, 0 if f32 else N * K * 6))
 
 
 def narrow_conv_bwd(dy: Tensor, x: Tensor, stats_in: Tensor, gamma: Tensor, beta: Tensor,
@@ -676,7 +601,7 @@ def narrow_conv_bwd(dy: Tensor, x: Tensor, stats_in: Tensor, gamma: Tensor, beta
     a.dw, a.dbias = dw.data_ptr(), dbias.data_ptr()
     a.B, a.T, a.C = x.shape
     a.groups, a.gn_eps = groups, gn_eps
-    _launch(lambda: _lib.lib().adp_narrow_conv_bwd(C.byref(a), _stream()), "adp_narrow_conv_bwd",
+    _launch("adp_narrow_conv_bwd", (C.byref(a),),
             lambda: (f"narrow_conv_bwd[M={x.shape[0] * x.shape[1]}]", 4.0 * x.numel() * 24, _nb(dy, x, dxh)))
     return dxh
 
@@ -699,12 +624,9 @@ def stem_out_bwd(dv: Tensor, h: Tensor, x: Tensor, w: Tensor, bias: Optional[Ten
     a.ca = 0 if append is None else append.shape[1]
     a.c0, a.co, a.f = h.shape[-1], w.shape[0], f
     a.ld_gate, a.ld_dgate = gate.stride(0), dgate.stride(0)
-    if h.dtype == torch.float32:
-        _launch(lambda: _lib.lib().adp_f32_stem_out_bwd(C.byref(a), _stream()), "adp_f32_stem_out_bwd",
-                lambda: ("f32_stem_out_bwd", 0, _nb(dv, h, x, dh)))
-        return dh
-    _launch(lambda: _lib.lib().adp_stem_out_bwd(C.byref(a), _stream()), "adp_stem_out_bwd",
-            lambda: ("stem_out_bwd", 0, _nb(dv, h, x, dh)))
+    f32 = _f32(h)
+    _launch("adp_f32_stem_out_bwd" if f32 else "adp_stem_out_bwd", (C.byref(a),),
+            lambda: (f"{f32}stem_out_bwd", 0, _nb(dv, h, x, dh)))
     return dh
 
 
@@ -720,12 +642,9 @@ def stem_in_bwd(dout: Tensor, x: Tensor, dw: Tensor, dbias: Tensor, f: int, *,
     a.B, a.cx, a.T = x.shape
     a.ca = 0 if append is None else append.shape[1]
     a.c0, a.f = dout.shape[-1], f
-    if dout.dtype == torch.float32:
-        _launch(lambda: _lib.lib().adp_f32_stem_in_bwd(C.byref(a), _stream()), "adp_f32_stem_in_bwd",
-                lambda: ("f32_stem_in_bwd", 0, _nb(dout, x)))
-        return
-    _launch(lambda: _lib.lib().adp_stem_in_bwd(C.byref(a), _stream()), "adp_stem_in_bwd",
-            lambda: ("stem_in_bwd", 0, _nb(dout, x)))
+    f32 = _f32(dout)
+    _launch("adp_f32_stem_in_bwd" if f32 else "adp_stem_in_bwd", (C.byref(a),),
+            lambda: (f"{f32}stem_in_bwd", 0, _nb(dout, x)))
 
 
 def attention_bwd(q: Tensor, k: Tensor, v: Tensor, o: Tensor, d_o: Tensor, lse: Tensor, delta: Tensor,
@@ -741,21 +660,16 @@ def attention_bwd(q: Tensor, k: Tensor, v: Tensor, o: Tensor, d_o: Tensor, lse: 
     a.scale = scale
     B, Tq, Tk = a.B, a.Tq, a.Tk
     D, tag = head_dim, _hd_tag(head_dim)
-    if q.dtype == torch.float32:
-        _launch(lambda: _lib.lib().adp_f32_attention_bwd(C.byref(a), D, _stream()), "adp_f32_attention_bwd",
-                lambda: (f"f32_attention_bwd[B={B} H={heads} Tq={Tq} Tk={Tk}{tag}]",
-                         14.0 * B * heads * Tq * Tk * D, 0))
-        return
-    _launch(lambda: _lib.lib().adp_attention_bwd_hd(C.byref(a), D, _stream()), "adp_attention_bwd",
-            lambda: (f"attention_bwd[B={B} H={heads} Tq={Tq} Tk={Tk}{tag}]", 14.0 * B * heads * Tq * Tk * D,
-                     (4 * B * Tq + 4 * B * Tk) * heads * D * 2))
+    f32 = _f32(q)
+    _launch("adp_f32_attention_bwd" if f32 else "adp_attention_bwd_hd", (C.byref(a), D),
+            lambda: (f"{f32}attention_bwd[B={B} H={heads} Tq={Tq} Tk={Tk}{tag}]", 14.0 * B * heads * Tq * Tk * D,
+                     0 if f32 else (4 * B * Tq + 4 * B * Tk) * heads * D * 2))
 
 
 def ln_fold_bwd(w: Tensor, g: Tensor, b: Tensor, dwf: Tensor, dbf: Tensor, dw: Tensor, dg: Tensor,
                 db: Tensor) -> None:
     """Unfolds the gradient of a LayerNorm-affine-folded projection (see adp_ln_fold_bwd)."""
     N, Cc = w.shape
-    _launch(lambda: _lib.lib().adp_ln_fold_bwd(w.data_ptr(), g.data_ptr(), b.data_ptr(), dwf.data_ptr(),
-                                               dwf.stride(0), dbf.data_ptr(), dw.data_ptr(),
-                                               dg.data_ptr(), db.data_ptr(), N, Cc, _stream()),
-            "adp_ln_fold_bwd", lambda: (f"ln_fold_bwd[N={N} C={Cc}]", 0, 3 * N * Cc * 4))
+    _launch("adp_ln_fold_bwd", (w.data_ptr(), g.data_ptr(), b.data_ptr(), dwf.data_ptr(), dwf.stride(0),
+                                dbf.data_ptr(), dw.data_ptr(), dg.data_ptr(), db.data_ptr(), N, Cc),
+            lambda: (f"ln_fold_bwd[N={N} C={Cc}]", 0, 3 * N * Cc * 4))

@@ -18,7 +18,7 @@
      rel-L2 <= 1e-5 for the tiny, ragged, XUNet, SkipCat and upsampler nets, 1e-4 for the README,
      widths and wide-boundary nets, times |s| + |1 - s| under guidance s; 1e-4 rel-L2 of the sample;
   d. coverage: every adp_f32_* entry point `ops` can call is reached by a checked edge launch, by
-     the name ops._launch records for it (adp_f32_attention_hd's launches are named adp_f32_attention).
+     the name ops._launch records for it (the C function called).
 """
 import inspect
 import re
@@ -516,7 +516,7 @@ def test_f32_training_under_checker(adp, oracle_port, golden_dir, monkeypatch, n
 def test_every_f32_entry_point_is_checked(ops):
     """One probe pass over every edge case: the C entry points its checked launches call."""
     src = inspect.getsource(ops)
-    callable_ = set(re.findall(r'"(adp_f32_\w+)"', src))   # the names ops._launch records (_hd: adp_f32_attention)
+    callable_ = set(re.findall(r'"(adp_f32_\w+)"', src))   # the symbols ops._launch calls and records
     reached = set()
     for case in ALL:
         reached |= _run(ops, case, "probe", 100 + ALL.index(case)).symbols
