@@ -7,7 +7,7 @@ graph per step; with any other `net` the same algebra runs as the generic fused
 `adp_sampler_step` kernel after the net call.
 """
 from math import pi
-from typing import Any, Optional, Tuple
+from typing import Any, List, Optional, Tuple
 
 import torch
 import torch.nn as nn
@@ -66,6 +66,17 @@ class Sampler(nn.Module):
 def _alpha_beta(sigmas: Tensor) -> Tuple[Tensor, Tensor]:
     angle = sigmas * pi / 2          # reference diffusion.py:77-80
     return torch.cos(angle), torch.sin(angle)
+
+
+def _progress(label: str, num_steps: int, host_sig: Optional[List[float]]):
+    """range(num_steps) through a tqdm bar, shown when `host_sig` is given: a host copy of the
+    schedule, made once per call, whose next value the bar's description shows after each step (the
+    reference formats a device scalar every step = one sync per step, reference diffusion.py:188)."""
+    bar = tqdm(range(num_steps), disable=host_sig is None)
+    for i in bar:
+        yield i
+        if host_sig is not None:
+            bar.set_description(f"{label} (noise={host_sig[i + 1]:.2f})")
 
 
 def _inner_b200(net: nn.Module) -> Optional[B200UNet]:
@@ -170,21 +181,13 @@ class ARVSampler(Sampler):
 
     def sample_loop(self, current: Tensor, sigmas: Tensor, show_progress: bool = False, **kwargs) -> Tensor:
         num_steps = sigmas.shape[0] - 1
-        host_sig = sigmas[:, 0, 0, 0].tolist() if show_progress else None
-        bar = tqdm(range(num_steps), disable=not show_progress)
-
-        def progress():
-            for i in bar:
-                yield i
-                if host_sig is not None:
-                    bar.set_description(f"Sampling (noise={host_sig[i + 1]:.2f})")
-
+        progress = _progress("Sampling", num_steps, sigmas[:, 0, 0, 0].tolist() if show_progress else None)
         net = _inner_b200(self.net)
         if net is not None:
-            return net.arv_loop(current, sigmas, progress=progress() if show_progress else None, **kwargs)
+            return net.arv_loop(current, sigmas, progress=progress if show_progress else None, **kwargs)
         chan = torch.cat([current, sigmas[0]], dim=1).float().contiguous()
         sig = sigmas.float().reshape(num_steps + 1, current.shape[0], -1).contiguous()
-        for i in progress():
+        for i in progress:
             v = self.net(chan, **kwargs).float().contiguous()                                 # :231-232
             ops.arv_step(chan, v, sig[i + 1])                                                 # :233-235
         return chan[:, : current.shape[1]].to(current.dtype)
@@ -245,24 +248,16 @@ class VInpainter(Inpainter):
         sigmas_1d = self.schedule(num_steps + 1, device=x_noisy.device)              # :333
         sigmas = sigmas_1d[:, None].expand(-1, b)
         alphas, betas = _alpha_beta(sigmas_1d)
-        host_sig = sigmas_1d.tolist() if show_progress else None
-        bar = tqdm(range(num_steps), disable=not show_progress)
-
-        def progress():
-            for i in bar:
-                yield i
-                if host_sig is not None:
-                    bar.set_description(f"Inpainting (noise={host_sig[i + 1]:.2f})")
-
+        progress = _progress("Inpainting", num_steps, sigmas_1d.tolist() if show_progress else None)
         net = _inner_b200(self.net)
         if net is not None:
             return net.inpaint_loop(x_noisy, source, mask, sigmas, alphas, betas, num_resamples,
-                                    progress=progress() if show_progress else None, **kwargs)
+                                    progress=progress if show_progress else None, **kwargs)
         x = x_noisy.float().contiguous().clone()
         src = source.float().expand_as(x).contiguous()
         mask_u8 = mask.expand_as(x).to(torch.uint8).contiguous()
         a, bt = alphas.float(), betas.float()
-        for i in progress():
+        for i in progress:
             for r in range(num_resamples):
                 j = int(r == num_resamples - 1)
                 ab = torch.stack([a[i], bt[i], a[i + j], bt[i + j]]).contiguous()
@@ -293,24 +288,14 @@ class VSampler(Sampler):
         sigmas_1d = self.schedule(num_steps + 1, device=x_noisy.device)           # :177
         sigmas = sigmas_1d[:, None].expand(-1, b)                                 # :178
         alphas, betas = _alpha_beta(sigmas_1d)                                    # :180
-        # the bar shows the schedule value from a host copy made once, before the loop
-        # (the reference formats a device scalar every step = one sync per step, :188)
-        host_sig = sigmas_1d.tolist() if show_progress else None
-        bar = tqdm(range(num_steps), disable=not show_progress)
-
-        def progress():
-            for i in bar:
-                yield i
-                if host_sig is not None:
-                    bar.set_description(f"Sampling (noise={host_sig[i + 1]:.2f})")
-
+        progress = _progress("Sampling", num_steps, sigmas_1d.tolist() if show_progress else None)
         net = _inner_b200(self.net)
         if net is not None:
             return net.sample_loop(x_noisy, sigmas, alphas, betas,
-                                   progress=progress() if show_progress else None, **kwargs)
+                                   progress=progress if show_progress else None, **kwargs)
         ab = torch.stack([alphas[:-1], betas[:-1], alphas[1:], betas[1:]], 1).float().contiguous()
         x = x_noisy.float().contiguous().clone()
-        for i in progress():
+        for i in progress:
             v = self.net(x, sigmas[i], **kwargs).float().contiguous()             # :184
             ops.sampler_step(x, v, ab[i], x)                                      # :185-187
         return x.to(x_noisy.dtype)

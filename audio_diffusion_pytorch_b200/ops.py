@@ -32,6 +32,11 @@ def device_check() -> None:
     _lib.check(_lib.lib().adp_device_check(), "adp_device_check")
 
 
+def require_cuda(x: Tensor) -> None:
+    """The input check of every entry point of the net."""
+    assert x.is_cuda, "the CUDA path runs on a CUDA device only (no CPU fallback)"
+
+
 # -------------------------------------------------------------------------------- tracing
 _TRACE = None
 

@@ -33,18 +33,23 @@ import torch.nn.functional as F
 from torch import Tensor
 
 from . import ops
-from .unet import B200UNet, LevelParams, _ForwardWalk, _capture, _pad_to
+from .unet import B200UNet, LevelParams, _ForwardWalk, _Graphed, _pad_to, _refreshed
 
 
 class _TrainPlan:
     def __init__(self):
         self.fwd: List = []
-        self.graph_f = self.graph_b = None
-        self.runs_f = self.runs_b = 0
+        self.forward = _Graphed(self.run_forward, early_weights=False)
+        self.backward = _Graphed(lambda: self.backward_program(), early_weights=False)
+        self.refresh_graph = None
         self.generation = 0
         self.on_mark = None          # callable(interval) while a gradient all-reduce is overlapped
         self.seg_graphs = None       # backward captured as segments cut at the flush marks
         self.mark_log: List = []     # intervals in execution order (recorded on the eager run)
+
+    def run_forward(self) -> None:
+        for fn in self.fwd:
+            fn()
 
     def mark(self, interval) -> None:
         """A contiguous range [start, end) of the gradient arena is final (see level())."""
@@ -741,26 +746,7 @@ def _refresh_dgrad_packs(plan: _TrainPlan, net: B200UNet) -> None:
     def refresh():
         for r in plan.refreshers:
             r()
-    if not net.use_cuda_graph:
-        refresh()
-    elif getattr(plan, "refresh_graph", None) is None:
-        refresh()
-        plan.refresh_graph = _capture(refresh)
-    else:
-        plan.refresh_graph.replay()
-
-
-def _run(plan: _TrainPlan, which: str, use_graph: bool) -> None:
-    """Eager on the first call, captured on the second, replayed afterwards (which: 'f' / 'b')."""
-    prog = (lambda: [f() for f in plan.fwd]) if which == "f" else plan.backward_program
-    runs = getattr(plan, "runs_" + which)
-    if not use_graph or runs == 0:
-        prog()
-    else:
-        if getattr(plan, "graph_" + which) is None:
-            setattr(plan, "graph_" + which, _capture(prog))
-        getattr(plan, "graph_" + which).replay()
-    setattr(plan, "runs_" + which, runs + 1)
+    plan.refresh_graph = _refreshed(plan.refresh_graph, refresh, net.use_cuda_graph)
 
 
 def _run_backward_synced(plan: _TrainPlan, net: B200UNet, sync) -> None:
@@ -823,7 +809,7 @@ def _run_backward_synced(plan: _TrainPlan, net: B200UNet, sync) -> None:
             g.replay()
             if todo:
                 reduce_now(todo)
-    plan.runs_b += 1
+    plan.backward.runs += 1
     sync.conditioning_gradients(plan)
     for w in works:
         w.wait()
@@ -870,7 +856,7 @@ class _UNetFn(torch.autograd.Function):
         for d_, c_ in zip(ctx_depths, context):      # [B, ctx, T_d] -> channels-last
             plan.ctx[d_][:, :, : c_.shape[1]].copy_(c_.transpose(1, 2))
         plan.cond.copy_(cond)
-        _run(plan, "f", net.use_cuda_graph)
+        plan.forward(net.use_cuda_graph)
         plan.generation += 1
         ctx.plan, ctx.net, ctx.mode, ctx.generation = plan, net, mode, plan.generation
         ctx.params = params
@@ -896,7 +882,7 @@ class _UNetFn(torch.autograd.Function):
             plan.dv.copy_(grad_out)
         sync = getattr(net, "_grad_sync", None)
         if sync is None:
-            _run(plan, "b", net.use_cuda_graph)
+            plan.backward(net.use_cuda_graph)
         else:
             _run_backward_synced(plan, net, sync)
         for fin in plan.finals:
@@ -1006,7 +992,7 @@ def fused_v_loss(net: B200UNet, x: Tensor, noise: Tensor, sigmas: Tensor, *,
                  embedding: Optional[Tensor] = None, embedding_scale: float = 1.0,
                  embedding_mask_proba: float = 0.0, channels=None) -> Tensor:
     """mse(net(alpha*x + beta*noise, sigma), alpha*noise - beta*x)  (reference diffusion.py:90-95)."""
-    assert x.is_cuda, "the CUDA path runs on a CUDA device only (no CPU fallback)"
+    ops.require_cuda(x)
     if net.use_embedding_cfg and embedding_scale != 1.0:
         # guidance inside the training objective = two differentiable evaluations (a_unet CFG
         # plugin); no fused-loss form: take the generic route
@@ -1029,7 +1015,7 @@ def differentiable_forward(net: B200UNet, x: Tensor, time: Optional[Tensor], *,
                            embedding_scale: float = 1.0, embedding_mask_proba: float = 0.0,
                            append_channels: Optional[Tensor] = None, channels=None) -> Tensor:
     """v = net(x, time, ...) with autograd support (custom loss_fn / diffusion_t)."""
-    assert x.is_cuda, "the CUDA path runs on a CUDA device only (no CPU fallback)"
+    ops.require_cuda(x)
     cond = _time_cond(net, time, features)
     emb, fixed = _train_embedding(net, x.shape[0], embedding, embedding_mask_proba)
     params = _net_params(net)

@@ -171,16 +171,34 @@ class _Pool:
             self.free.setdefault((tuple(t.shape), t.dtype), []).append(t)
 
 
-class _Plan:
+class _Graphed:
+    """A program that runs eagerly on its first call (every launch is validated), is captured into a
+    CUDA graph on the second and replayed from then on.  With use_graph False it runs eagerly."""
+
+    def __init__(self, run: Callable[[], None], early_weights: bool):
+        self.run, self.early_weights = run, early_weights
+        self.graph: Optional[torch.cuda.CUDAGraph] = None
+        self.runs = 0
+
+    def __call__(self, use_graph: bool) -> None:
+        if not use_graph or self.runs == 0:
+            self.run()
+        else:
+            if self.graph is None:
+                self.graph = _capture(self.run, self.early_weights)
+            self.graph.replay()
+        self.runs += 1
+
+
+class _Plan(_Graphed):
     """Everything tied to one input shape: static I/O buffers, workspaces, the launch list and
     (after warm-up) its CUDA graph."""
 
     def __init__(self):
+        super().__init__(self.run_eager, early_weights=True)
         self.prog: List[Callable[[], None]] = []
-        self.graph: Optional[torch.cuda.CUDAGraph] = None
         self.n_launches = 0
         self.n_kernels = 0
-        self.runs = 0
 
     def add(self, fn: Callable[[], None]) -> None:
         self.prog.append(fn)
@@ -189,6 +207,21 @@ class _Plan:
     def run_eager(self) -> None:
         for fn in self.prog:
             fn()
+
+
+def _refreshed(graph: Optional[torch.cuda.CUDAGraph], run: Callable[[], None],
+               use_graph: bool) -> Optional[torch.cuda.CUDAGraph]:
+    """One in-place refresh of packed weights; returns the graph to keep for the next one.  The
+    first refresh runs eagerly (the allocator warms up) and is then captured without a replay;
+    later ones replay that graph.  With use_graph False it runs eagerly."""
+    if not use_graph:
+        run()
+    elif graph is None:
+        run()
+        graph = _capture(run)
+    else:
+        graph.replay()
+    return graph
 
 
 def _capture(run: Callable[[], None], early_weights: bool = False) -> torch.cuda.CUDAGraph:
@@ -745,14 +778,9 @@ class B200UNet(nn.Module):
         fold launches whose HOST cost
         dwarfs their device time: sources (the parameters) and destinations (the packs) have
         fixed addresses, so the whole sequence is captured once into a CUDA graph and replayed."""
-        if not (self.use_cuda_graph and self.net.down.weight.is_cuda):
-            _copy_tree(self._packed, self._compute_packed())
-            return
-        if self._repack_graph is None:
-            _copy_tree(self._packed, self._compute_packed())       # eager once: allocator warm
-            self._repack_graph = _capture(lambda: _copy_tree(self._packed, self._compute_packed()))
-        else:
-            self._repack_graph.replay()
+        self._repack_graph = _refreshed(self._repack_graph,
+                                        lambda: _copy_tree(self._packed, self._compute_packed()),
+                                        self.use_cuda_graph and self.net.down.weight.is_cuda)
 
     @torch.no_grad()
     def _compute_packed(self):
@@ -1088,19 +1116,14 @@ class B200UNet(nn.Module):
         return table
 
     def _execute(self, plan: _Plan) -> None:
-        """First call eager (validates every launch), second call captures, then replays."""
-        if not self.use_cuda_graph:
-            plan.run_eager()
-        elif plan.graph is not None:
-            plan.graph.replay()
-        elif plan.runs == 0:
-            with ops.trace() as tr:          # also counts the kernels of one net evaluation
-                plan.run_eager()
+        """One evaluation of the plan (_Graphed); the first eager run under graphs also counts the
+        kernels of one net evaluation."""
+        if self.use_cuda_graph and plan.runs == 0:
+            with ops.trace() as tr:
+                plan(True)
             plan.n_kernels = len(tr.records)
         else:
-            plan.graph = _capture(plan.run_eager, early_weights=True)
-            plan.graph.replay()
-        plan.runs += 1
+            plan(self.use_cuda_graph)
 
     def _execute_steps(self, plan: _Plan, n: int) -> None:
         """n consecutive sampling steps of a 'sample' plan.  Once the single-step graph exists, a
@@ -1187,7 +1210,6 @@ class B200UNet(nn.Module):
                 embedding: Optional[Tensor] = None, embedding_scale: float = 1.0,
                 embedding_mask_proba: float = 0.0, channels=None,
                 append_channels: Optional[Tensor] = None) -> Tensor:
-        assert x.is_cuda, "the CUDA path runs on a CUDA device only (no CPU fallback)"
         if self.use_embedding_cfg:
             assert exists(embedding), "ClassiferFreeGuidancePlugin requires embedding"
         ctx_list = [c for c in (channels or []) if exists(c)]
@@ -1200,147 +1222,119 @@ class B200UNet(nn.Module):
                                           embedding_scale=embedding_scale,
                                           embedding_mask_proba=embedding_mask_proba,
                                           append_channels=append_channels, channels=channels)
-        return self._forward_inference(x, time, features, embedding, embedding_scale,
-                                       embedding_mask_proba, append_channels, channels)
+        with torch.no_grad():
+            plan = self._prelude(x, "v", time, features=features, embedding=embedding,
+                                 embedding_scale=embedding_scale, embedding_mask_proba=embedding_mask_proba,
+                                 append_channels=append_channels, channels=channels)
+            self._execute(plan)
+            return plan.v.clone().to(x.dtype)
 
-    @torch.no_grad()
-    def _forward_inference(self, x, time, features, embedding, embedding_scale,
-                           embedding_mask_proba, append_channels, channels=None) -> Tensor:
+    def _prelude(self, x: Tensor, mode: str, time: Optional[Tensor], **kwargs) -> _Plan:
+        """What every inference entry point does before its first evaluation: checks the input device
+        and the weights, picks the plan of x's shape, stages the inputs and runs the plan's
+        step-invariant launches (plan.pre: the cross-attention context K/V of a sampling plan, once
+        per call).  kwargs: forward's keyword arguments."""
+        ops.require_cuda(x)
         self._check_untracked_updates()
-        B, T, Bh, M = self._shape_key(x, embedding, embedding_scale)
-        plan = self._plan(B, T, Bh, M, "v", (float(embedding_scale) if Bh != B else None,
-                                             exists(features)))
-        self._stage_inputs(plan, x.float(), time, features, embedding, embedding_scale,
-                           embedding_mask_proba, append_channels, channels)
-        self._execute(plan)
-        return plan.v.clone().to(x.dtype)
+        embedding, scale, features = kwargs.get("embedding"), kwargs.get("embedding_scale", 1.0), kwargs.get("features")
+        B, T, Bh, M = self._shape_key(x, embedding, scale)
+        plan = self._plan(B, T, Bh, M, mode, (float(scale) if Bh != B else None, exists(features)))
+        self._stage_inputs(plan, x.float(), time, features, embedding, scale,
+                           kwargs.get("embedding_mask_proba", 0.0), kwargs.get("append_channels"),
+                           kwargs.get("channels"))
+        for fn in plan.pre:
+            fn()
+        return plan
+
+    def _table_steps(self, plan: _Plan, sigmas: Tensor, ab_rows: Tensor, share: int, progress,
+                     each: Optional[Callable[[], None]] = None) -> None:
+        """The steps of a 'sample' plan from sigmas [N+1, B]: `share` evaluations per step, each
+        followed by each(); ab_rows [N * share, 4] holds every evaluation's alpha/beta.  The
+        conditioning table is evaluated in blocks of <= ~4096 rows (190 KB of fp32 per row for the
+        README net); inside a block the device picks each step's rows: graph launches only, no host
+        sync.  Without a progress iterator and each(), _execute_steps runs a block's steps."""
+        B, Bh = plan.x.shape[0], plan.sigma.shape[0]
+        num_steps = sigmas.shape[0] - 1
+        sig = sigmas.float().repeat(1, Bh // B).contiguous()      # [N+1, Bh]
+        block = max(1, min(self.cond_table_rows // Bh, self.max_table_steps // share))
+        ticks = _ticks(progress, num_steps)
+        for first in range(0, num_steps, block):
+            n = min(block, num_steps - first)
+            feats = plan.features_in.repeat(n, 1) if plan.use_features_in else None
+            table = self._cond_table(sig[first:first + n].reshape(-1), feats).view(n, Bh, -1)
+            self._set_step_tables(plan, table, ab_rows[first * share:(first + n) * share], share)
+            if progress is None and each is None:
+                self._execute_steps(plan, n)
+                continue
+            for _ in range(n):         # progress bar: one graph launch per evaluation
+                next(ticks)
+                for _ in range(share):
+                    self._execute(plan)
+                    if each is not None:
+                        each()
+        for _ in ticks:
+            pass
 
     @torch.no_grad()
     def sample_loop(self, x_noisy: Tensor, sigmas: Tensor, alphas: Tensor, betas: Tensor,
                     progress=None, **kwargs) -> Tensor:
         """VSampler's loop (reference diffusion.py:183-188) with the per-step update fused into
         the net's last kernel: one graph launch per step, no host sync inside the loop."""
-        assert x_noisy.is_cuda, "the CUDA path runs on a CUDA device only (no CPU fallback)"
-        self._check_untracked_updates()
-        embedding = kwargs.get("embedding")
-        scale = kwargs.get("embedding_scale", 1.0)
-        B, T, Bh, M = self._shape_key(x_noisy, embedding, scale)
-        plan = self._plan(B, T, Bh, M, "sample", (float(scale) if Bh != B else None,
-                                                  exists(kwargs.get("features"))))
-        self._stage_inputs(plan, x_noisy.float(), sigmas[0], kwargs.get("features"), embedding, scale,
-                           kwargs.get("embedding_mask_proba", 0.0), kwargs.get("append_channels"),
-                           kwargs.get("channels"))
-        for fn in plan.pre:          # cross-attention context K/V: once per call
-            fn()
-        num_steps = sigmas.shape[0] - 1
+        plan = self._prelude(x_noisy, "sample", sigmas[0], **kwargs)
         ab = torch.stack([alphas[:-1], betas[:-1], alphas[1:], betas[1:]], dim=1).float().contiguous()
-        sig = sigmas.float().repeat(1, Bh // B).contiguous()      # [N+1, Bh]
-        # conditioning table in blocks of <= ~4096 rows (190 KB of fp32 per row for the README net);
-        # inside a block the device picks each step's rows: graph launches only, no host sync
-        block = max(1, min(self.cond_table_rows // Bh, self.max_table_steps))
-        it = iter(progress) if progress is not None else None
-        for first in range(0, num_steps, block):
-            n = min(block, num_steps - first)
-            feats = plan.features_in.repeat(n, 1) if plan.use_features_in else None
-            table = self._cond_table(sig[first:first + n].reshape(-1), feats).view(n, Bh, -1)
-            self._set_step_tables(plan, table, ab[first:first + n])
-            if it is None:
-                self._execute_steps(plan, n)
-            else:                      # progress bar: one graph launch per step
-                for _ in range(n):
-                    next(it)
-                    self._execute(plan)
-        if it is not None:
-            for _ in it:               # let the progress generator finish (last description update)
-                pass
+        self._table_steps(plan, sigmas, ab, 1, progress)
         return plan.x.clone().to(x_noisy.dtype)
 
+    @torch.no_grad()
+    def inpaint_loop(self, x_noisy: Tensor, source: Tensor, mask: Tensor, sigmas: Tensor, alphas: Tensor,
+                     betas: Tensor, num_resamples: int, progress=None, **kwargs) -> Tensor:
+        """VInpainter's loop (reference diffusion.py:338-352): per step `num_resamples` net
+        evaluations; each one advances x to the level of the NEXT step only on the last resample
+        (otherwise it is re-noised back to the current level), then the known region (mask) is
+        replaced by the source noised to that level.  One graph launch + one blend kernel per
+        evaluation; the noise is drawn with torch.randn_like(source) in the reference's order."""
+        plan = self._prelude(x_noisy, "sample", sigmas[0], **kwargs)
+        a, b = alphas.float(), betas.float()
+        # ab[i][j]: coefficients of a step from level i to level i + j (j = 0: stay, re-noise)
+        ab = torch.stack([torch.stack([a[:-1], b[:-1], a[:-1], b[:-1]], 1),
+                          torch.stack([a[:-1], b[:-1], a[1:], b[1:]], 1)], 1).contiguous()
+        # per iteration (step i, resample r): alpha/beta row = ab[i][r is the last]
+        last = torch.zeros(num_resamples, dtype=torch.long, device=ab.device)
+        last[-1] = 1
+        src = source.float().expand_as(plan.x).contiguous()
+        mask_u8 = mask.expand_as(plan.x).to(torch.uint8).contiguous()
 
-def _inpaint_loop(self, x_noisy: Tensor, source: Tensor, mask: Tensor, sigmas: Tensor, alphas: Tensor,
-                  betas: Tensor, num_resamples: int, progress=None, **kwargs) -> Tensor:
-    """VInpainter's loop (reference diffusion.py:338-352): per step `num_resamples` net evaluations;
-    each one advances x to the level of the NEXT step only on the last resample (otherwise it is
-    re-noised back to the current level), then the known region (mask) is replaced by the source
-    noised to that level.  One graph launch + one blend kernel per evaluation; the noise is drawn
-    with torch.randn_like(source) in the reference's order."""
-    assert x_noisy.is_cuda, "the CUDA path runs on a CUDA device only (no CPU fallback)"
-    self._check_untracked_updates()
-    embedding = kwargs.get("embedding")
-    scale = kwargs.get("embedding_scale", 1.0)
-    B, T, Bh, M = self._shape_key(x_noisy, embedding, scale)
-    plan = self._plan(B, T, Bh, M, "sample", (float(scale) if Bh != B else None,
-                                              exists(kwargs.get("features"))))
-    self._stage_inputs(plan, x_noisy.float(), sigmas[0], kwargs.get("features"), embedding, scale,
-                       kwargs.get("embedding_mask_proba", 0.0), kwargs.get("append_channels"),
-                       kwargs.get("channels"))
-    for fn in plan.pre:
-        fn()
-    num_steps = sigmas.shape[0] - 1
-    a, b = alphas.float(), betas.float()
-    # ab[i][j]: coefficients of a step from level i to level i + j (j = 0: stay, re-noise)
-    ab = torch.stack([torch.stack([a[:-1], b[:-1], a[:-1], b[:-1]], 1),
-                      torch.stack([a[:-1], b[:-1], a[1:], b[1:]], 1)], 1).contiguous()
-    sig = sigmas.float().repeat(1, Bh // B).contiguous()
-    src = source.float().expand_as(plan.x).contiguous()
-    mask_u8 = mask.expand_as(plan.x).to(torch.uint8).contiguous()
-    block = max(1, min(self.cond_table_rows // Bh, self.max_table_steps // max(1, num_resamples)))
-    # per iteration (step i, resample r): alpha/beta row = ab[i][r is the last]
-    last = torch.zeros(num_resamples, dtype=torch.long, device=ab.device)
-    last[-1] = 1
-    it = iter(progress) if progress is not None else None
-    for first in range(0, num_steps, block):
-        n = min(block, num_steps - first)
-        feats = plan.features_in.repeat(n, 1) if plan.use_features_in else None
-        table = self._cond_table(sig[first:first + n].reshape(-1), feats).view(n, Bh, -1)
-        ab_rows = ab[first:first + n][:, last].reshape(n * num_resamples, 4)
-        self._set_step_tables(plan, table, ab_rows, share=num_resamples)
-        for _ in range(n):
-            if it is not None:
-                next(it)
-            for r in range(num_resamples):
-                self._execute(plan)
-                ops.inpaint_blend(plan.x, src, torch.randn_like(source).float().expand_as(plan.x).contiguous(),
-                                  mask_u8, plan.ab)
-    if it is not None:
-        for _ in it:
-            pass
-    return plan.x.clone().to(x_noisy.dtype)
+        def blend():
+            ops.inpaint_blend(plan.x, src, torch.randn_like(source).float().expand_as(plan.x).contiguous(),
+                              mask_u8, plan.ab)
+        self._table_steps(plan, sigmas, ab[:, last].reshape(-1, 4), num_resamples, progress, blend)
+        return plan.x.clone().to(x_noisy.dtype)
+
+    @torch.no_grad()
+    def arv_loop(self, current: Tensor, sigmas: Tensor, progress=None, **kwargs) -> Tensor:
+        """ARVSampler.sample_loop (reference diffusion.py:223-238): the net input is cat([current,
+        sigma_i]) with a noise level PER POSITION (sigmas [N+1, B, 1, T]) and no time conditioning.
+        The plan's input buffer holds that concatenation for the whole loop: one graph launch (the
+        net) + one adp_arv_step (the update, which also writes sigma_{i+1} into the last channel)."""
+        B, C, T = current.shape
+        assert C + 1 == self.x_channels and sigmas.shape[1:] == (B, 1, T)
+        plan = self._prelude(torch.cat([current.float(), sigmas[0].float()], dim=1), "v", None, **kwargs)
+        sig = sigmas.float().reshape(sigmas.shape[0], B, T).contiguous()
+        for i in _ticks(progress, sigmas.shape[0] - 1):
+            self._execute(plan)
+            ops.arv_step(plan.x, plan.v, sig[i + 1])
+        return plan.x[:, :C].clone().to(current.dtype)
 
 
-B200UNet.inpaint_loop = torch.no_grad()(_inpaint_loop)
-
-
-def _arv_loop(self, current: Tensor, sigmas: Tensor, progress=None, **kwargs) -> Tensor:
-    """ARVSampler.sample_loop (reference diffusion.py:223-238): the net input is cat([current,
-    sigma_i]) with a noise level PER POSITION (sigmas [N+1, B, 1, T]) and no time conditioning.
-    The plan's input buffer holds that concatenation for the whole loop: one graph launch (the
-    net) + one adp_arv_step (the update, which also writes sigma_{i+1} into the last channel)."""
-    assert current.is_cuda, "the CUDA path runs on a CUDA device only (no CPU fallback)"
-    self._check_untracked_updates()
-    embedding = kwargs.get("embedding")
-    scale = kwargs.get("embedding_scale", 1.0)
-    B, C, T = current.shape
-    assert C + 1 == self.x_channels and sigmas.shape[1:] == (B, 1, T)
-    plan_x = torch.cat([current.float(), sigmas[0].float()], dim=1)
-    _, _, Bh, M = self._shape_key(plan_x, embedding, scale)
-    plan = self._plan(B, T, Bh, M, "v", (float(scale) if Bh != B else None, exists(kwargs.get("features"))))
-    self._stage_inputs(plan, plan_x, None, kwargs.get("features"), embedding, scale,
-                       kwargs.get("embedding_mask_proba", 0.0), kwargs.get("append_channels"),
-                       kwargs.get("channels"))
-    sig = sigmas.float().reshape(sigmas.shape[0], B, T).contiguous()
-    it = iter(progress) if progress is not None else None
-    for i in range(sigmas.shape[0] - 1):
-        if it is not None:
-            next(it)
-        self._execute(plan)
-        ops.arv_step(plan.x, plan.v, sig[i + 1])
-    if it is not None:
-        for _ in it:
-            pass
-    return plan.x[:, :C].clone().to(current.dtype)
-
-
-B200UNet.arv_loop = torch.no_grad()(_arv_loop)
+def _ticks(progress, n: int):
+    """n steps: advances `progress` (any iterable) before each, then lets it finish (a progress
+    generator's last description update runs after the last step)."""
+    it = iter(progress if progress is not None else range(n))
+    for i in range(n):
+        next(it)
+        yield i
+    for _ in it:
+        pass
 
 
 _OPTIMIZER_STEPS = [0]

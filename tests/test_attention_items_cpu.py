@@ -16,7 +16,7 @@ import torch
 
 import launch_check as lc
 from audio_diffusion_pytorch_b200 import _lib, ops, training
-from audio_diffusion_pytorch_b200.diffusion import _alpha_beta
+from audio_diffusion_pytorch_b200.diffusion import VSampler
 from audio_diffusion_pytorch_b200.models import DiffusionModel
 from audio_diffusion_pytorch_b200.unet import UNetV0
 from test_launch_check_cpu import rel_l2
@@ -126,6 +126,7 @@ def oracle_kw(emb, channels, scale=1.0):
 @pytest.fixture
 def cpu_launches(monkeypatch):
     monkeypatch.setattr(ops, "device_check", lambda: None)
+    monkeypatch.setattr(ops, "require_cuda", lambda x: None)
 
     def no_library():
         raise AssertionError("a launch reached the CUDA library")
@@ -137,6 +138,7 @@ def pair(oracle_port, cfg):
     ref = oracle_port.DiffusionModelPort(**cfg)
     model = DiffusionModel(net_t=UNetV0, **cfg)
     model.net.load_reference_parameters(ref.net)
+    model.net.use_cuda_graph = False           # every call runs the plan's launches eagerly
     return ref, model.net
 
 
@@ -201,34 +203,6 @@ def test_reference_checkpoint_loads(oracle_port, tmp_path, name):
 
 
 # ------------------------------------------------------------------------------ programs
-def run_v(net, x, sigma, emb=None, scale=1.0, channels=None):
-    """One eager evaluation of the 'v' plan (what net(x, sigma, ...) runs on a GPU)."""
-    B, T, Bh, M = net._shape_key(x, emb, scale)
-    plan = net._plan(B, T, Bh, M, "v", (float(scale) if Bh != B else None, False))
-    net._stage_inputs(plan, x.float(), sigma, None, emb, scale, 0.0, None, channels)
-    plan.run_eager()
-    return plan.v.clone()
-
-
-def run_sample(net, x, num_steps, emb=None, channels=None):
-    """What sample_loop runs on a GPU: the step-invariant launches (cross-attention K|V), the
-    conditioning table, the device step selector and one eager evaluation per step."""
-    B, T, Bh, M = net._shape_key(x, emb, 1.0)
-    sig1 = torch.linspace(1, 0, num_steps + 1)
-    alphas, betas = _alpha_beta(sig1)
-    plan = net._plan(B, T, Bh, M, "sample", (None, False))
-    net._stage_inputs(plan, x.float(), sig1[:1].expand(B), None, emb, 1.0, 0.0, None, channels)
-    for fn in plan.pre:
-        fn()
-    ab = torch.stack([alphas[:-1], betas[:-1], alphas[1:], betas[1:]], 1).float().contiguous()
-    sig = sig1[:, None].expand(-1, B).float().contiguous()
-    table = net._cond_table(sig[:num_steps].reshape(-1), None).view(num_steps, B, -1)
-    net._set_step_tables(plan, table, ab)
-    for _ in range(num_steps):
-        plan.run_eager()
-    return plan.x.clone()
-
-
 def _oracle_v(ref, x, sigma, kw):
     return ref.net(x, sigma, **kw) if sigma is not None else ref.net(x, **kw)
 
@@ -247,7 +221,7 @@ def test_program_vs_oracle(cpu_launches, oracle_port, name):
         for scale, v_tol, b_tol in cases:
             want = _oracle_v(ref, x, sigma, oracle_kw(emb, channels, scale))
             with lc.Shadow(fake=True) as sh:
-                v = run_v(net, x, sigma, emb, scale, channels)
+                v = net(x, sigma, **oracle_kw(emb, channels, scale))
             assert sh.n_checked == sh.n_launch > 0
             assert sh.records["attention.o"].count == n_items(cfg, "attentions") + n_items(cfg, "cross_attentions")
             e_v, e_b = rel_l2(v, want), rel_l2(v - x[:, :v.shape[1]], want - x[:, :v.shape[1]])
@@ -263,7 +237,7 @@ def test_sampling_program_vs_oracle(cpu_launches, oracle_port, name):
     with torch.no_grad():
         want = ref.sample(noise, num_steps=3, **oracle_kw(emb, channels))
         with lc.Shadow(fake=True) as sh:
-            s = run_sample(net, noise, 3, emb, channels)
+            s = VSampler(net=net)(noise, num_steps=3, **oracle_kw(emb, channels))
     assert sh.n_checked == sh.n_launch > 0
     e = rel_l2(s, want)
     print(f"{name} 3-step sample: rel-L2 {e:.3e}")

@@ -235,7 +235,7 @@ def test_guard_mutation_is_caught(cpu_launches, tiny_nets, mutation, kind, progr
     with torch.no_grad(), lc.Shadow(fake=True, guard=True, mutate=(kind, mutation)) as sh:
         with pytest.raises(lc.CheckError) as err:
             if program == "v":
-                lcc.run_v(tiny_nets["fused"], torch.randn(2, 2, 4096, generator=g), torch.rand(2, generator=g))
+                tiny_nets["fused"](torch.randn(2, 2, 4096, generator=g), torch.rand(2, generator=g))
             else:
                 {"arena": _arena_step, "to_flat": _to_flat, "fir_resample": _fir_resample}[program]()
     assert sh.mutate is None, f"{mutation.__name__} never applied to a {kind} launch"

@@ -23,6 +23,7 @@ import torch
 
 import launch_check as lc
 from audio_diffusion_pytorch_b200 import _lib, ops
+from audio_diffusion_pytorch_b200.diffusion import VSampler
 from audio_diffusion_pytorch_b200.models import DiffusionModel
 from audio_diffusion_pytorch_b200.unet import UNetV0
 from test_launch_programs_cpu import FIXTURE, LAUNCHES, TINY, TINY_TEXT
@@ -89,6 +90,7 @@ def test_every_tensor_argument_is_classified():
 @pytest.fixture
 def cpu_launches(monkeypatch):
     monkeypatch.setattr(ops, "device_check", lambda: None)
+    monkeypatch.setattr(ops, "require_cuda", lambda x: None)
 
     def no_library():
         raise AssertionError("a launch reached the CUDA library")
@@ -100,34 +102,8 @@ def _model(oracle_port, cfg):
     ref = oracle_port.DiffusionModelPort(**cfg)
     model = DiffusionModel(net_t=UNetV0, **cfg)
     model.net.load_reference_parameters(ref.net)
+    model.net.use_cuda_graph = False           # every call runs the plan's launches eagerly
     return model.net
-
-
-def run_v(net, x, sigma, embedding=None, scale=1.0):
-    """One eager evaluation of the 'v' plan (what net(x, sigma) runs on a GPU)."""
-    B, T, Bh, M = net._shape_key(x, embedding, scale)
-    plan = net._plan(B, T, Bh, M, "v", (float(scale) if Bh != B else None, False))
-    net._stage_inputs(plan, x.float(), sigma, None, embedding, scale, 0.0, None)
-    plan.run_eager()
-    return plan.v.clone()
-
-
-def run_sample(net, x, num_steps):
-    """What sample_loop runs on a GPU: the conditioning table, the device step selector and the
-    sampling plan, one eager evaluation per step."""
-    from audio_diffusion_pytorch_b200.diffusion import _alpha_beta
-    B, T = x.shape[0], x.shape[2]
-    sig1 = torch.linspace(1, 0, num_steps + 1)
-    alphas, betas = _alpha_beta(sig1)
-    plan = net._plan(B, T, B, 0, "sample", (None, False))
-    net._stage_inputs(plan, x.float(), sig1[:1].expand(B), None, None, 1.0, 0.0, None)
-    ab = torch.stack([alphas[:-1], betas[:-1], alphas[1:], betas[1:]], 1).float().contiguous()
-    sig = sig1[:, None].expand(-1, B).float().contiguous()
-    table = net._cond_table(sig[:num_steps].reshape(-1), None).view(num_steps, B, -1)
-    net._set_step_tables(plan, table, ab)
-    for _ in range(num_steps):
-        plan.run_eager()
-    return plan.x.clone()
 
 
 def rel_l2(a, b):
@@ -144,7 +120,7 @@ def test_tiny_program_vs_golden(cpu_launches, oracle_port, golden_dir):
     g = _golden(golden_dir, "tiny_unconditional.npz")
     net = _model(oracle_port, TINY)
     with torch.no_grad(), lc.Shadow(fake=True, probe=True) as sh:
-        v = run_v(net, g["x"], g["sigma"])
+        v = net(g["x"], g["sigma"])
     print(sh.table())
     e_v, e_b = rel_l2(v, g["v"]), rel_l2(v - g["x"], g["v"] - g["x"])
     print(f"tiny: rel-L2(v) {e_v:.3e} rel-L2(branch) {e_b:.3e}")
@@ -157,7 +133,7 @@ def test_tiny_sampling_program_vs_golden(cpu_launches, oracle_port, golden_dir):
     g = _golden(golden_dir, "tiny_unconditional.npz")
     net = _model(oracle_port, TINY)
     with torch.no_grad(), lc.Shadow(fake=True, probe=True) as sh:
-        s = run_sample(net, g["noise"], 5)
+        s = VSampler(net=net)(g["noise"], num_steps=5)
     print(sh.table())
     e = rel_l2(s, g["sample5"])
     print(f"tiny 5-step sample: rel-L2 {e:.3e}")
@@ -169,8 +145,8 @@ def test_text_cfg_program_vs_golden(cpu_launches, oracle_port, golden_dir):
     g = _golden(golden_dir, "tiny_text_cfg.npz")
     net = _model(oracle_port, TINY_TEXT)
     with torch.no_grad(), lc.Shadow(fake=True, probe=True) as sh:
-        v1 = run_v(net, g["x"], g["sigma"], g["embedding"])
-        v5 = run_v(net, g["x"], g["sigma"], g["embedding"], 5.0)
+        v1 = net(g["x"], g["sigma"], embedding=g["embedding"])
+        v5 = net(g["x"], g["sigma"], embedding=g["embedding"], embedding_scale=5.0)
     print(sh.table())
     for v, want, v_tol, b_tol in ((v1, g["v_scale1"], V_TOL, BRANCH_TOL), (v5, g["v_scale5"], 3e-4, 3e-2)):
         e_v, e_b = rel_l2(v, want), rel_l2(v - g["x"], want - g["x"])
@@ -250,7 +226,7 @@ def test_unfused_program_probes(cpu_launches, oracle_port):
         for k, v in attrs.items():
             setattr(net, k, v)
         with torch.no_grad(), lc.Shadow(fake=True, probe=True) as sh:
-            run_v(net, x, sigma)
+            net(x, sigma)
         assert kinds <= {k for k, _ in sh.probed}
         if attrs.get("fuse_groupnorm"):
             assert any(k == "conv_gemm" and "gn" in args for k, args in sh.probed)
@@ -324,9 +300,9 @@ def test_mutation_is_caught(cpu_launches, tiny_nets, mutation, kind):
             if kind in _DIRECT_KINDS:
                 _direct(kind)
             elif kind in _SAMPLE_KINDS:
-                run_sample(net, x, 2)
+                VSampler(net=net)(x, num_steps=2)
             else:
-                run_v(net, x, sigma)
+                net(x, sigma)
     assert sh.mutate is None, f"{mutation} never applied to a {kind} launch"
     assert f"): {kind}:" in str(err.value), str(err.value)
     print(f"caught {mutation} in {kind}: {err.value}")

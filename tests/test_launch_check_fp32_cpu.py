@@ -23,9 +23,9 @@ import torch.nn.functional as F
 
 import launch_check as lc
 from audio_diffusion_pytorch_b200 import _lib, ops, training
+from audio_diffusion_pytorch_b200.diffusion import VSampler
 from audio_diffusion_pytorch_b200.models import DiffusionModel
 from audio_diffusion_pytorch_b200.unet import UNetV0
-from test_launch_check_cpu import run_sample, run_v
 from test_launch_programs_cpu import NETS, TINY, TINY_TEXT, build_net, install
 from test_train_fp32_cpu import record_train
 
@@ -38,6 +38,7 @@ LOSS_TOL, GRAD_TOL = 1e-5, 1e-4
 @pytest.fixture
 def cpu_launches(monkeypatch):
     monkeypatch.setattr(ops, "device_check", lambda: None)
+    monkeypatch.setattr(ops, "require_cuda", lambda x: None)
 
     def no_library():
         raise AssertionError("a launch reached the CUDA library")
@@ -133,7 +134,7 @@ def test_tiny_v_fp32(cpu_launches, oracle_port):
     ref, net = _pair(oracle_port, TINY)
     x, _, sigma = _inputs(1)
     with torch.no_grad(), lc.Shadow(fake=True, probe=True) as sh:
-        v = run_v(net, x, sigma)
+        v = net(x, sigma)
     want = ref.net(x.double(), sigma.double())
     print(sh.table())
     e = rel_l2(v - x, want - x.double())
@@ -148,7 +149,7 @@ def test_text_cfg5_fp32(cpu_launches, oracle_port):
     x, _, sigma = _inputs(2)
     emb = torch.randn(2, 8, 32, generator=torch.Generator().manual_seed(3))
     with torch.no_grad(), lc.Shadow(fake=True, probe=True) as sh:
-        v = run_v(net, x, sigma, emb, 5.0)
+        v = net(x, sigma, embedding=emb, embedding_scale=5.0)
     want = ref.net(x.double(), sigma.double(), embedding=emb.double(), embedding_scale=5.0)
     e = rel_l2(v - x, want - x.double())
     print(f"text net fp32 CFG 5 on fake kernels: branch rel-L2 {e:.3e}")
@@ -160,19 +161,12 @@ def test_tiny_sample_fp32(cpu_launches, oracle_port):
     ref, net = _pair(oracle_port, TINY)
     noise, _, _ = _inputs(4)
     with torch.no_grad(), lc.Shadow(fake=True, probe=True) as sh:
-        s = run_sample(net, noise, 5)
+        s = VSampler(net=net)(noise, num_steps=5)
     want = ref.sample(noise.double(), num_steps=5)
     e = rel_l2(s, want)
     print(f"tiny fp32 5-step sample on fake kernels: rel-L2 {e:.3e}")
     assert e <= SAMPLE_TOL
     assert {"step_select", "step_advance", "stem_out"} <= _f32_kinds(sh)
-
-
-def _loss_program(net, x, noise, sigma):
-    cond = training._time_cond(net, sigma, None)
-    e, _ = training._train_embedding(net, x.shape[0], None, 0.0)
-    return training._UNetFn.apply(net, "loss", x.float(), noise.float(), sigma, None, cond, e, (),
-                                  *training._net_params(net))
 
 
 def test_tiny_training_step_fp32(cpu_launches, oracle_port):
@@ -183,7 +177,7 @@ def test_tiny_training_step_fp32(cpu_launches, oracle_port):
     loss_ref = F.mse_loss(ref.net(a64 * x64 + b64 * n64, sigma.double()), a64 * n64 - b64 * x64)
     loss_ref.backward()
     with lc.Shadow(fake=True, probe=True) as sh:
-        loss = _loss_program(net, x, noise, sigma)
+        loss = training.fused_v_loss(net, x, noise, sigma)
         loss.backward()
     assert sh.n_checked == sh.n_launch > 0
     rel = abs(float(loss) - float(loss_ref)) / float(loss_ref)
@@ -281,10 +275,10 @@ def test_fp32_mutation_is_caught(cpu_launches, tiny_fp32, mutation, kind):
     with lc.Shadow(fake=True, mutate=(kind, lc.MUTATIONS[mutation])) as sh:
         with pytest.raises(lc.CheckError) as err:
             if kind in _TRAIN + _LONG:
-                _loss_program(net, x, noise, sigma).backward()
+                training.fused_v_loss(net, x, noise, sigma).backward()
             else:
                 with torch.no_grad():
-                    run_v(net, x, sigma)
+                    net(x, sigma)
     assert sh.mutate is None, f"{mutation} never applied to a {kind} launch"
     assert f"): {kind}:" in str(err.value), str(err.value)
     print(f"caught {mutation} in {kind}: {err.value}")
@@ -314,7 +308,7 @@ def test_long_chain_resolution(cpu_launches, tiny_fp32):
         mp.setitem(lc.CHECKERS, k, spy(k))
     try:
         with lc.Shadow(fake=True):
-            _loss_program(net, x, noise, sigma).backward()
+            training.fused_v_loss(net, x, noise, sigma).backward()
     finally:
         mp.undo()
     for k, r in sorted(seen.items()):

@@ -20,7 +20,7 @@ import torch.nn.functional as F
 
 import launch_check as lc
 from audio_diffusion_pytorch_b200 import _lib, ops, training
-from audio_diffusion_pytorch_b200.diffusion import _alpha_beta
+from audio_diffusion_pytorch_b200.diffusion import VSampler
 from audio_diffusion_pytorch_b200.models import DiffusionModel
 from audio_diffusion_pytorch_b200.unet import UNetV0
 from test_lengths_gpu import FULL, NETS, SMALL, level_lengths
@@ -99,6 +99,7 @@ def test_power_of_two_grid_misses_the_ragged_edges():
 @pytest.fixture
 def cpu_launches(monkeypatch):
     monkeypatch.setattr(ops, "device_check", lambda: None)
+    monkeypatch.setattr(ops, "require_cuda", lambda x: None)
 
     def no_library():
         raise AssertionError("a launch reached the CUDA library")
@@ -175,42 +176,6 @@ def _inputs(cfg, B, T, seed):
     return x, noise, sigma, emb
 
 
-def run_v(net, x, sigma, emb=None, scale=1.0):
-    """One eager evaluation of the 'v' plan (what net(x, sigma, ...) runs on a GPU)."""
-    B, T, Bh, M = net._shape_key(x, emb, scale)
-    plan = net._plan(B, T, Bh, M, "v", (float(scale) if Bh != B else None, False))
-    net._stage_inputs(plan, x.float(), sigma, None, emb, scale, 0.0, None)
-    plan.run_eager()
-    return plan.v.clone()
-
-
-def run_sample(net, x, num_steps, emb=None, scale=1.0):
-    """What sample_loop runs on a GPU, guidance included: the step-invariant launches, the
-    conditioning table of all Bh rows, the device step selector and one eager evaluation per step."""
-    B, T, Bh, M = net._shape_key(x, emb, scale)
-    sig1 = torch.linspace(1, 0, num_steps + 1)
-    alphas, betas = _alpha_beta(sig1)
-    plan = net._plan(B, T, Bh, M, "sample", (float(scale) if Bh != B else None, False))
-    net._stage_inputs(plan, x.float(), sig1[:1].expand(B), None, emb, scale, 0.0, None)
-    for fn in plan.pre:
-        fn()
-    ab = torch.stack([alphas[:-1], betas[:-1], alphas[1:], betas[1:]], 1).float().contiguous()
-    sig = sig1[:, None].expand(-1, Bh).float().contiguous()
-    table = net._cond_table(sig[:num_steps].reshape(-1), None).view(num_steps, Bh, -1)
-    net._set_step_tables(plan, table, ab)
-    for _ in range(num_steps):
-        plan.run_eager()
-    return plan.x.clone()
-
-
-def loss_program(net, x, noise, sigma, emb=None):
-    """fused_v_loss without its device check: the training plan's forward, loss and backward."""
-    cond = training._time_cond(net, sigma, None)
-    e, _ = training._train_embedding(net, x.shape[0], emb, 0.0)
-    return training._UNetFn.apply(net, "loss", x.float(), noise.float(), sigma, None, cond, e, (),
-                                  *training._net_params(net))
-
-
 def rel_l2(a, b):
     a, b = a.double(), b.double()
     return float((a - b).norm() / b.norm().clamp_min(1e-30))
@@ -250,13 +215,13 @@ def test_tiny_programs_vs_oracle(cpu_launches, oracle_port, case):
     kw = dict(embedding=emb) if emb is not None else {}
     what = f"{name} B={B} T={T}"
     with torch.no_grad(), lc.Shadow(fake=True, probe=True) as sh:
-        per_row(run_v(net, x, sigma, emb), ref.net(x, sigma, **kw), f"{what} v/branch", BRANCH_TOL, x, V_TOL)
+        per_row(net(x, sigma, embedding=emb), ref.net(x, sigma, **kw), f"{what} v/branch", BRANCH_TOL, x, V_TOL)
         scale = GUIDANCE if emb is not None else 1.0
         if emb is not None:
-            per_row(run_v(net, x, sigma, emb, scale), ref.net(x, sigma, embedding_scale=scale, **kw),
+            per_row(net(x, sigma, embedding=emb, embedding_scale=scale), ref.net(x, sigma, embedding_scale=scale, **kw),
                     f"{what} guidance {scale}", CFG_BRANCH_TOL, x, CFG_V_TOL)
         want = ref.sample(x, num_steps=3, **(dict(kw, embedding_scale=scale) if kw else {}))
-        per_row(run_sample(net, x, 3, emb, scale), want, f"{what} 3-step sample", SAMPLE_TOL)
+        per_row(VSampler(net=net)(x, num_steps=3, embedding=emb, embedding_scale=scale), want, f"{what} 3-step sample", SAMPLE_TOL)
     assert sh.n_checked == sh.n_launch > 0
     labels = " ".join(sh.labels)
     t_att = level_lengths(cfg, T)[-1]
@@ -296,7 +261,7 @@ def test_tiny_training_step_vs_oracle(cpu_launches, oracle_port, case):
     loss_ref = F.mse_loss(ref.net(a * x + b * noise, sigma, **kw), a * noise - b * x)
     loss_ref.backward()
     with lc.Shadow(fake=True) as sh:
-        loss = loss_program(net, x, noise, sigma, emb)
+        loss = training.fused_v_loss(net, x, noise, sigma, embedding=emb)
         loss.backward()
     assert sh.n_checked == sh.n_launch > 0
     assert {"wgrad", "cond_bwd", "attention_bwd", "stem_in_bwd"} <= {k.split(".")[0] for k in sh.records}
@@ -317,7 +282,7 @@ def test_readme_v_program_vs_oracle(cpu_launches, oracle_port, T):
     ref, net = _pair(oracle_port, NETS["readme"])
     x, _, sigma, _ = _inputs(NETS["readme"], 3, T, 2)
     with torch.no_grad(), lc.Shadow(fake=True) as sh:
-        v = run_v(net, x, sigma)
+        v = net(x, sigma)
         want = ref.net(x, sigma)
     assert sh.n_checked == sh.n_launch > 0
     per_row(v, want, f"README B=3 T={T} v/branch", BRANCH_TOL, x, V_TOL)

@@ -31,15 +31,15 @@ def repack():
     with torch.no_grad():
         for r in plan.refreshers: r()
 timeit("repack fwd+dgrad weights", repack)
-timeit("forward graph", lambda: plan.graph_f.replay())
-timeit("backward graph", lambda: plan.graph_b.replay())
+timeit("forward graph", lambda: plan.forward.graph.replay())
+timeit("backward graph", lambda: plan.backward.graph.replay())
 timeit("finals", lambda: [f() for f in plan.finals])
 timeit("optimizer step", lambda: opt.step())
 timeit("reupsample", lambda: model.reupsample(audio))
 
 def graph_table(which):
-    prog = (lambda: [f() for f in plan.fwd]) if which == "f" else plan.backward_program
-    graph = plan.graph_f if which == "f" else plan.graph_b
+    graphed = plan.forward if which == "f" else plan.backward
+    prog, graph = graphed.run, graphed.graph
     with ops.trace() as tr:
         prog()
     torch.cuda.synchronize()
