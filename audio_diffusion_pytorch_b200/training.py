@@ -33,23 +33,19 @@ import torch.nn.functional as F
 from torch import Tensor
 
 from . import ops
-from .unet import B200UNet, LevelParams, _ForwardWalk, _Graphed, _pad_to, _refreshed
+from .unet import B200UNet, _ForwardWalk, _Graphed, _Plan, _refreshed
 
 
 class _TrainPlan:
     def __init__(self):
-        self.fwd: List = []
-        self.forward = _Graphed(self.run_forward, early_weights=False)
+        self.forward = _Plan(early_weights=False)
+        self.fwd = self.forward.prog     # the forward's launch list (the same list object)
         self.backward = _Graphed(lambda: self.backward_program(), early_weights=False)
         self.refresh_graph = None
         self.generation = 0
         self.on_mark = None          # callable(interval) while a gradient all-reduce is overlapped
         self.seg_graphs = None       # backward captured as segments cut at the flush marks
         self.mark_log: List = []     # intervals in execution order (recorded on the eager run)
-
-    def run_forward(self) -> None:
-        for fn in self.fwd:
-            fn()
 
     def mark(self, interval) -> None:
         """A contiguous range [start, end) of the gradient arena is final (see level())."""
@@ -298,9 +294,8 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
 
     # ---- static I/O
     cin = net.x_channels + net.append_channels
-    plan.x = _zeros((B, net.x_channels, T), dev)
+    net._static_io(plan, B, B, T, M)
     plan.noise = _zeros((B, net.x_channels, T), dev) if loss_mode else None
-    plan.append = _zeros((B, net.append_channels, T), dev) if net.append_channels else None
     plan.alpha = _zeros((B,), dev) if loss_mode else None
     plan.beta = _zeros((B,), dev) if loss_mode else None
     plan.cond = _zeros((B, Fm), dev)                      # SiLU(features), fp32 master
@@ -312,20 +307,14 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
     plan.dcond = _zeros((B, Fm), dev)
     plan.dxin = _zeros((B, cin, T), dev) if want_dxin else None
     E = net.embedding_features
-    plan.embedding = torch.zeros(B, M, E, dtype=adt, device=dev) if M else None
     plan.demb = torch.zeros(B, M, E, dtype=adt, device=dev) if M else None
-    # InjectChannelsItem context per depth (channels-last, channels zero-padded to 16) + gradient
-    plan.ctx, plan.dctx, t_l = {}, {}, T
-    for i, c in enumerate(net.context_channels):
-        t_l //= net.factors[i]
-        if c > 0:
-            plan.ctx[i] = torch.zeros(B, t_l, ops.round_up(c, 16), dtype=adt, device=dev)
-            plan.dctx[i] = torch.zeros(B, t_l, ops.round_up(c, 16), dtype=adt, device=dev)
+    plan.dctx = {i: torch.zeros_like(c) for i, c in plan.ctx.items()}     # d InjectChannelsItem context
 
     # ---- statistics + gradient arenas
     n_items = sum(len(lv.items_down) + len(lv.items_up) for lv in levels)
     arena = torch.zeros(7 * n_items + 4 * len(levels) + 8, B, G, 2, dtype=torch.float64, device=dev)
-    plan.fwd.append(lambda: (arena.zero_(), plan.loss_sum.zero_()))
+    add = plan.forward.add
+    add(lambda: (arena.zero_(), plan.loss_sum.zero_()))
     refreshers: List = []                  # re-pack the dgrad weights in place after a weight update
 
     def packed_dgrad(make_any):
@@ -385,24 +374,24 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
 
     n_tot = P["cond_n"]
     mod = net.use_modulation       # False: no conditioning projection (no ModulationItem, no SkipModulate)
-    ss_all = _zeros((B, max(8, ops.round_up(n_tot, 8))), dev)
+    ss_all = net._ss_all(P, B)
     dss_all = gbuf(ss_all.shape)
     ss_stride = ss_all.shape[1]
     if mod:
-        cond_bias = _pad_to(P["cond_b"], ss_all.shape[1])
-        plan.fwd.append(lambda: plan.cond_bf.copy_(plan.cond.view(1, B, Fm)))
-        plan.fwd.append(lambda: ops.conv_gemm(plan.cond_bf, P["cond_w"], ss_all.view(1, B, -1), c_in=Fm,
-                                              n_valid=ss_all.shape[1], bias=cond_bias))
+        add(lambda: plan.cond_bf.copy_(plan.cond.view(1, B, Fm)))
+        net._project_conditioning(add, P, plan.cond_bf, ss_all)
 
     # ---- cross-attention context: LayerNorm(embedding) once per forward (the per-item
     # norm_context affines are folded into each item's to_kv weights)
     en = den = None
     if M:
         en, den = act(B, M, E), torch.zeros(B, M, E, dtype=adt, device=dev)
-        plan.fwd.append(lambda: ops.ln_film(plan.embedding, en, None, 0, None, G, net.ATT_LN_EPS))
+        add(lambda: ops.ln_film(plan.embedding, en, None, 0, None, G, net.ATT_LN_EPS))
     # the forward launches; every intermediate the backward reads stays live
-    walk = _ForwardWalk(net, P, plan.fwd.append, B, arena, ss_all, keep=True, ctx=plan.ctx,
-                        embedding=plan.embedding, add_ctx=plan.fwd.append, en=en)
+    walk = _ForwardWalk(net, P, plan, add, B, arena, ss_all, keep=True, add_ctx=add, en=en)
+    trunk = walk.trunk(lambda: dict(loss_sum=plan.loss_sum if loss_mode else None,
+                                    dv=plan.dv if loss_mode else None, v_out=plan.v),
+                       noise=plan.noise, alpha=plan.alpha, beta=plan.beta)
     new_stats = walk.new_stats
     delta_ws = [None]    # shared fp32 workspace of adp_attention_bwd, sized for the largest item
 
@@ -543,11 +532,8 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
         # d context is summed over the items of this depth (in place through the residual)
         return lambda d_out: inject_bwd(d_out, inj["x"], ctxb, dctxb, wd_x, wd_c, gw_inj, db_inj, dyi, n_ctx)
 
-    # ---- one item chain: the walk's forward (output statistics of every unit, the last one
-    # included) and one backward closure per unit, built from the walk's records
-    def run_items(x: Tensor, x_stats: Tensor, items_p: List, chain_m: List, lv: LevelParams, Tl: int, li: int):
-        C = lv.ch
-        x, x_stats, recs = walk.items(x, x_stats, items_p, C, Tl, li, last_needs_stats=True)
+    # ---- one backward closure per unit of an item chain, built from the walk's records
+    def chain_backward(recs: List, items_p: List, chain_m: List, C: int, Tl: int, li: int) -> List:
         bwds = []
         for kind, i, width, rec in recs:
             m, pk = chain_m[i][1], items_p[i][1]
@@ -560,13 +546,13 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
                 bwds.append(inject_backward(rec, m, C, Tl, li))
             else:
                 bwds.append(attention_backward(rec, m, kind == "cross", Tl, C))
-        return x, x_stats, bwds
+        return bwds
 
-    # ---- recursive level walk; returns (output tensor, its stats, backward closure)
-    def level(i: int, x_in: Optional[Tensor], T_in: int):
-        lv, Lp = levels[i], P["levels"][i]
-        Tl, C = T_in // lv.factor, lv.ch
-        innermost = i == len(levels) - 1
+    # ---- backward of one level from the walk's record (_ForwardWalk.trunk); level 0's closure
+    # takes no argument, that of a level >= 1 maps d(its output) to d(its input)
+    def level(rec: Dict):
+        i, lv, Lp, Tl, T_in = rec["i"], rec["lv"], rec["Lp"], rec["Tl"], rec["T_in"]
+        x_in, x_last, gate, C = rec["x_in"], rec["x"], rec["gate"], lv.ch
         # gradient-arena cursor at the level's sequence points: the arena is laid out in FORWARD
         # build order, so "down part", "inner levels" and "up part" of a level are three
         # contiguous ranges; the backward finishes them in the order up, inner, down and
@@ -574,39 +560,43 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
         cur = {"entry": cursor[0]}
         db_down = grad_for(lv.down.bias)
         if i == 0:
-            x0, st0 = walk.pool.get(B, Tl, C), new_stats()
             dw_down = grad_for(lv.down.weight)
-            plan.fwd.append(lambda: ops.stem_in(plan.x, Lp["down_w"], Lp["down_b"], x0, lv.factor,
-                                                append=plan.append, noise=plan.noise, alpha=plan.alpha,
-                                                beta=plan.beta, stats=st0, groups=G))
         else:
-            x0, st0 = walk.down(lv, Lp, x_in, Tl)
             wd_down = packed_dgrad(lambda: pack_down_dgrad(lv.down.weight))
             # [co][tap][ci] (the [B, T/f, f*C] view) -> PyTorch [co][ci][tap]
             gw_down = grad_for(lv.down.weight, (C, lv.factor, lv.in_ch), (0, 2, 1)).view(C, lv.factor * lv.in_ch)
-        x, st, items_down_bwd = run_items(x0, st0, Lp["items_down"], lv.chain(up=False), lv, Tl, li=i)
+        items_down_bwd = chain_backward(rec["down"], Lp["items_down"], lv.chain(up=False), C, Tl, i)
         cur["down_end"] = cursor[0]
-        inner = None
-        skip = x
-        if not innermost:
-            x, st, inner = level(i + 1, skip, Tl)
+        inner = level(rec["inner"]) if rec["inner"] is not None else None
         cur["inner_end"] = cursor[0]
-        x, st, items_up_bwd = run_items(x, st, Lp["items_up"], lv.chain(up=True), lv, Tl, li=i)
+        items_up_bwd = chain_backward(rec["up"], Lp["items_up"], lv.chain(up=True), C, Tl, i)
+
+        def chains(d: Tensor) -> Tensor:
+            """d(up chain output) -> d(down chain input), through the inner level."""
+            for b_ in reversed(items_up_bwd):
+                d = b_(d)
+            if inner is not None:
+                plan.mark((cur["inner_end"], cur["exit"]))
+                d = inner(d)
+            for b_ in reversed(items_down_bwd):
+                d = b_(d)
+            return d
+
+        def mark_down() -> None:
+            plan.mark((cur["entry"], cur["down_end"] if inner is not None else cur["exit"]))
+
         merge = net.merge
         if merge == "modulate":
-            gate = ss_all[:, Lp["gate_off"]:]
             dgate = dss_all[:, Lp["gate_off"]:]
             cond_grads(lv.merge, Lp["gate_off"], lv.out_ch)
-        x_last = x
-        if i == 0 and merge == "add":
-            # SkipAdd at level 0: the stem epilogue with a unit gate, whose gradient is not used
-            gate, dgate = torch.ones(B, max(8, lv.out_ch), device=dev), gbuf((B, max(8, lv.out_ch)))
+        elif i == 0:
+            # SkipAdd and SkipCat at level 0: the stem epilogue with a unit gate, whose gradient is not used
+            dgate = gbuf(gate.shape)
         if i == 0 and merge == "cat":
             # SkipCat at level 0 runs in the stem kernels with the 1x1 merge conv folded into both
             # branches (B200UNet._compute_packed): they produce the gradients of the FOLDED
             # weights, unfolded below (a few hundred numbers) into merge / up / adapter gradients
             Co, Ci = lv.out_ch, lv.in_ch
-            gate, dgate = torch.ones(B, max(8, Co), device=dev), gbuf((B, max(8, Co)))
             dw_up, db_up = gbuf((Co, C, 3)), gbuf((Co,))
             dwa, dba = gbuf((Co, Ci)), gbuf((Co,))
 
@@ -629,35 +619,22 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
                        if lv.adapter is not None else None)
                 dba = grad_for(lv.adapter.bias) if lv.adapter is not None else None
             dh0 = act(B, Tl, C)
-            plan.fwd.append(lambda: ops.stem_out(
-                x_last, plan.x, Lp["up_w"], Lp["up_b"], gate, lv.factor, append=plan.append,
-                w_adapt=Lp.get("adapt_w"), b_adapt=Lp.get("adapt_b"), noise=plan.noise,
-                alpha=plan.alpha, beta=plan.beta, loss_sum=plan.loss_sum if loss_mode else None,
-                dv=plan.dv if loss_mode else None, v_out=plan.v))
 
             def backward_level0():
                 ops.stem_out_bwd(plan.dv, x_last, plan.x, Lp["up_w"], Lp["up_b"], gate, lv.factor, dh0,
                                  dw_up, db_up, dgate, gscale=plan.gscale, append=plan.append,
                                  noise=plan.noise, alpha=plan.alpha, beta=plan.beta,
                                  w_adapt=Lp.get("adapt_w"), dw_adapt=dwa, db_adapt=dba, dxin=plan.dxin)
-                d = dh0
-                for b_ in reversed(items_up_bwd):
-                    d = b_(d)
-                if inner is not None:
-                    plan.mark((cur["inner_end"], cur["exit"]))
-                    d = inner(d)
-                for b_ in reversed(items_down_bwd):
-                    d = b_(d)
+                d = chains(dh0)
                 ops.stem_in_bwd(d, plan.x, dw_down, db_down, lv.factor, append=plan.append,
                                 noise=plan.noise, alpha=plan.alpha, beta=plan.beta,
                                 w=Lp["down_w"], dxin=plan.dxin)
-                plan.mark((cur["entry"], cur["down_end"] if inner is not None else cur["exit"]))
+                mark_down()
             cur["exit"] = cursor[0]
-            return None, None, backward_level0
+            return backward_level0
 
-        # levels >= 1: the up conv writes y_up (pre-gate), the merge combines it with the level's input
-        f, Co = lv.factor, lv.out_ch
-        out, ost, y_up = walk.up_merge(lv, Lp, x_last, x_in, Tl, T_in)
+        # levels >= 1: the up conv wrote y_up (pre-gate), the merge combined it with the level's input
+        f, Co, y_up = lv.factor, lv.out_ch, rec["y_up"]
         dys, dx_last, d_xin = act(B, T_in, Co), act(B, Tl, C), act(B, T_in, lv.in_ch)
         if f > 1:
             wd_up = packed_dgrad(lambda: pack_upsample_dgrad(lv.up.weight, f))
@@ -694,24 +671,16 @@ def build_train_plan(net: B200UNet, B: int, T: int, M: int, mode: str, want_dxin
 
         def backward_level(d_out: Tensor) -> Tensor:
             upsample_bwd(merge_bwd(d_out), x_last, wd_up, gw_up, db_up, dx_last, f)
-            d = dx_last
-            for b_ in reversed(items_up_bwd):
-                d = b_(d)
-            if inner is not None:
-                plan.mark((cur["inner_end"], cur["exit"]))
-                d = inner(d)
-            for b_ in reversed(items_down_bwd):
-                d = b_(d)
+            d = chains(dx_last)
             # gradient w.r.t. the level input = dgrad(down conv) + the skip path
             downsample_bwd(d, x_in, wd_down, gw_down, db_down, d_xin, d_skip_of(d_out), lv.factor,
-                           wgrad_done=lambda: plan.mark((cur["entry"],
-                                                         cur["down_end"] if inner is not None else cur["exit"])))
+                           wgrad_done=mark_down)
             return d_xin
 
         cur["exit"] = cursor[0]
-        return out, ost, backward_level
+        return backward_level
 
-    _, _, backward0 = level(0, None, T)
+    backward0 = level(trunk)
     plan.flat = flat
     plan.refreshers, plan.version = refreshers, net._version()
     plan.grads, plan.finals, plan.specs = grads, finals, specs

@@ -191,11 +191,12 @@ class _Graphed:
 
 
 class _Plan(_Graphed):
-    """Everything tied to one input shape: static I/O buffers, workspaces, the launch list and
-    (after warm-up) its CUDA graph."""
+    """A launch list and (after warm-up) its CUDA graph; an inference or sampling plan also holds
+    everything tied to its input shape: static I/O buffers and workspaces.  early_weights: see
+    _capture; the training forward is captured without it."""
 
-    def __init__(self):
-        super().__init__(self.run_eager, early_weights=True)
+    def __init__(self, early_weights: bool = True):
+        super().__init__(self.run_eager, early_weights)
         self.prog: List[Callable[[], None]] = []
         self.n_launches = 0
         self.n_kernels = 0
@@ -243,24 +244,27 @@ def _capture(run: Callable[[], None], early_weights: bool = False) -> torch.cuda
 
 class _ForwardWalk:
     """Emits the trunk's forward launches, shared by the inference / sampling plans
-    (B200UNet._build_plan) and the training plan (training.build_train_plan): the item chains,
-    the down conv of levels >= 1 and their up conv + merge.  Each caller walks the levels itself
-    and owns the level-0 stems, the conditioning and its static I/O.  Every emitter returns the
-    tensors it used; the training plan builds its backward from them.
+    (B200UNet._build_plan) and the training plan (training.build_train_plan): `trunk` walks the
+    levels and emits the level-0 stems, the item chains, the down conv of levels >= 1 and their up
+    conv + merge.  The callers own the conditioning, the statistics arena and the static I/O (`io`:
+    x, append, embedding, ctx, from B200UNet._static_io), and pass the stems their mode's inputs and
+    outputs.  Every emitter returns the tensors it used; the training plan builds its backward from
+    them.
 
     keep=False: dead activations are reused, and the fusions that never write a tensor are used
     (FiLM in the narrow / thin-level conv, the thin-level kernel, the GroupNorm A-transform, the
-    merge gate in the up-conv epilogue).  keep=True: every buffer stays live, every tensor the
-    backward reads is written, and attention keeps its log-sum-exp."""
+    merge gate in the up-conv epilogue); only the innermost down chain ends with GroupNorm
+    statistics (the next level's ResnetItem reads them).  keep=True: every buffer stays live, every
+    tensor the backward reads is written, every chain end writes its statistics and attention keeps
+    its log-sum-exp."""
 
-    def __init__(self, net: "B200UNet", P: Dict, add: Callable, Bh: int, stats: Tensor, ss_all: Tensor,
-                 keep: bool, ctx: Dict[int, Tensor], embedding: Optional[Tensor], add_ctx: Callable,
-                 en: Optional[Tensor] = None):
-        self.net, self.P, self.add, self.Bh, self.keep = net, P, add, Bh, keep
+    def __init__(self, net: "B200UNet", P: Dict, io, add: Callable, Bh: int, stats: Tensor, ss_all: Tensor,
+                 keep: bool, add_ctx: Callable, en: Optional[Tensor] = None):
+        self.net, self.P, self.io, self.add, self.Bh, self.keep = net, P, io, add, Bh, keep
         self.pool = _Pool(net.net.down.weight.device, reuse=not keep, dtype=net._act_dtype())
         self.stats, self.n_stats = stats, 0
         self.ss_all, self.ss_stride = ss_all, ss_all.shape[1]
-        self.ctx, self.embedding, self.add_ctx = ctx, embedding, add_ctx
+        self.add_ctx = add_ctx
         self.en = en         # LayerNorm(embedding), shared by all cross-attentions; made on first use
         self.G = net.groups
         self.D = net.head_features or 64
@@ -270,6 +274,51 @@ class _ForwardWalk:
         s = self.stats[self.n_stats]
         self.n_stats += 1
         return s
+
+    def trunk(self, outputs: Callable[[], Dict], **noising) -> Dict:
+        """The whole trunk: stem_in (once per half of the rows under classifier-free guidance), the
+        levels' chains, down and up convs, and stem_out.  noising: the fused loss's noise, alpha and
+        beta, for both stems; outputs() -> stem_out's output arguments, called when the launch runs
+        (a plan's cfg_scale is set after it is built).  Returns level 0's record: the level (i, lv,
+        Lp), Tl, T_in, its input x_in, the unit records of its "down" and "up" chains, the "inner"
+        level's record, the up chain's output x, the merge gate and, for levels >= 1, up_merge's
+        out, ost and y_up."""
+        io, G, Bh, levels = self.io, self.G, self.Bh, self.net.levels()
+        B, _, T = io.x.shape
+
+        def level(i: int, x_in: Optional[Tensor], T_in: int) -> Dict:
+            lv, Lp = levels[i], self.P["levels"][i]
+            Tl, innermost = T_in // lv.factor, i == len(levels) - 1
+            rec = dict(i=i, lv=lv, Lp=Lp, Tl=Tl, T_in=T_in, x_in=x_in, inner=None)
+            if i == 0:
+                x, st = self.pool.get(Bh, Tl, lv.ch), self.new_stats()
+                for h in range(Bh // B):
+                    self.add(lambda x=x[h * B:(h + 1) * B], st=st[h * B:(h + 1) * B]: ops.stem_in(
+                        io.x, Lp["down_w"], Lp["down_b"], x, lv.factor, append=io.append, stats=st, groups=G,
+                        **noising))
+            else:
+                x, st = self.down(lv, Lp, x_in, Tl)
+            x, st, rec["down"] = self.items(x, st, Lp["items_down"], lv.ch, Tl, i,
+                                            last_needs_stats=self.keep or innermost)
+            if not innermost:
+                skip = x
+                rec["inner"] = level(i + 1, skip, Tl)
+                x, st = rec["inner"]["out"], rec["inner"]["ost"]
+                self.pool.put(skip)
+            x, st, rec["up"] = self.items(x, st, Lp["items_up"], lv.ch, Tl, i, last_needs_stats=self.keep)
+            gate = self.ss_all[:, Lp["gate_off"]:] if self.net.merge == "modulate" else None
+            if i == 0 and gate is None:
+                # SkipCat (folded into the stem's weights) and SkipAdd run the stem epilogue with a unit gate
+                gate = torch.ones(Bh, max(8, lv.out_ch), device=x.device)
+            rec.update(x=x, gate=gate)
+            if i > 0:
+                rec["out"], rec["ost"], rec["y_up"] = self.up_merge(lv, Lp, x, x_in, Tl, T_in, gate)
+            else:
+                self.add(lambda: ops.stem_out(x, io.x, Lp["up_w"], Lp["up_b"], gate, lv.factor, append=io.append,
+                                              w_adapt=Lp.get("adapt_w"), b_adapt=Lp.get("adapt_b"), **noising,
+                                              **outputs()))
+            return rec
+        return level(0, None, T)
 
     def items(self, x: Tensor, x_stats: Tensor, chain: List[Tuple[str, Dict]], C: int, Tl: int, li: int,
               last_needs_stats: bool):
@@ -379,7 +428,7 @@ class _ForwardWalk:
     def _inject(self, x: Tensor, jp: Dict, C: int, Tl: int, li: int, y_stats: Optional[Tensor]) -> Dict:
         """InjectChannelsItem: conv1x1(cat([x, ctx])) + x as two accumulating GEMMs
         (W = [W_x | W_c]): tmp = ctx W_c^T + b + x ; y = x W_x^T + tmp."""
-        pool, ctxb = self.pool, self.ctx[li]
+        pool, ctxb = self.pool, self.io.ctx[li]
         tmp, y = pool.get(self.Bh, Tl, C), pool.get(self.Bh, Tl, C)
         self.add(lambda: ops.conv_gemm(ctxb, jp["w_c"], tmp, c_in=ctxb.shape[-1], n_valid=C, bias=jp["b"],
                                        residual=x))
@@ -408,11 +457,11 @@ class _ForwardWalk:
         else:
             # context K/V do not depend on x or sigma: in sampling mode they are projected ONCE per
             # sample() call (plan.pre), not once per step
-            E, M = net.embedding_features, self.embedding.shape[1]
+            E, M = net.embedding_features, self.io.embedding.shape[1]
             q = pool.get(Bh, Tl, mid)
             if self.en is None:
                 self.en = torch.empty(Bh, M, E, dtype=pool.dtype, device=x.device)
-                self.add_ctx(lambda en=self.en: ops.ln_film(self.embedding, en, None, 0, None, self.G,
+                self.add_ctx(lambda en=self.en: ops.ln_film(self.io.embedding, en, None, 0, None, self.G,
                                                             net.ATT_LN_EPS))
             en = self.en
             kv = torch.empty(Bh, M, 2 * mid, dtype=pool.dtype, device=x.device)
@@ -435,14 +484,14 @@ class _ForwardWalk:
                                        bias=Lp["down_b"], stats=st, groups=self.G))
         return x, st
 
-    def up_merge(self, lv: "LevelParams", Lp: Dict, x: Tensor, x_in: Tensor, Tl: int, T_in: int):
+    def up_merge(self, lv: "LevelParams", Lp: Dict, x: Tensor, x_in: Tensor, Tl: int, T_in: int,
+                 gate: Optional[Tensor]):
         """Up conv of a level >= 1's chain output x and its merge with the level input x_in:
-        MergeModulate's gate, SkipCat or SkipAdd.  Returns (output, its statistics, y_up = the up
-        conv's own output, None when the merge runs in its epilogue)."""
+        MergeModulate's `gate`, SkipCat or SkipAdd (gate None).  Returns (output, its statistics,
+        y_up = the up conv's own output, None when the merge runs in its epilogue)."""
         pool, add, G, Bh, f, C, Co = self.pool, self.add, self.G, self.Bh, lv.factor, lv.ch, lv.out_ch
         out, ost = pool.get(Bh, T_in, Co), self.new_stats()
         merge = self.net.merge
-        gate = self.ss_all[:, Lp["gate_off"]:] if merge == "modulate" else None
         geom = dict(up_factor=f) if f > 1 else dict(taps=(-1, 0, 1))
 
         def phases(t):          # [Bh, T_in, Co] as the [Bh, Tl, f*Co] output of the upsample GEMM
@@ -929,8 +978,7 @@ class B200UNet(nn.Module):
         gate of the network, concatenated)."""
         dev = plan.sigma.device
         Fm = self.features
-        n_tot = P["cond_n"]
-        ss_all = torch.zeros(Bh, ops.round_up(n_tot, 8), device=dev)
+        ss_all = self._ss_all(P, Bh)
         cond_bf = torch.zeros(1, Bh, Fm, dtype=self._act_dtype(), device=dev)
         fvec = torch.zeros(Bh, Fm, device=dev)
         plan.use_features_in = False
@@ -953,22 +1001,44 @@ class B200UNet(nn.Module):
         else:
             plan.add(lambda: fvec.copy_(plan.features_in))
         plan.add(lambda: ops.silu_bf16(fvec, cond_bf))
-        cond_bias = _pad_to(P["cond_b"], ss_all.shape[1])
-        plan.add(lambda: ops.conv_gemm(cond_bf, P["cond_w"], ss_all.view(1, Bh, -1), c_in=Fm,
-                                       n_valid=ss_all.shape[1], bias=cond_bias))
+        self._project_conditioning(plan.add, P, cond_bf, ss_all)
         return ss_all
+
+    def _ss_all(self, P: Dict, rows: int) -> Tensor:
+        """A zeroed ss_all [rows, n] fp32: the conditioning projection's output, n = its outputs padded
+        to 8 (8 without a projection: the step selector and the walk keep one layout)."""
+        return torch.zeros(rows, max(8, ops.round_up(P["cond_n"], 8)), device=self.net.down.weight.device)
+
+    def _project_conditioning(self, add: Callable, P: Dict, cond_bf: Tensor, ss_all: Tensor) -> None:
+        """Appends the conditioning projection ss_all = W_all cond_bf + b_all (cond_bf [1, rows,
+        features] = SiLU(features), in the activation dtype) through `add`."""
+        cond_bias = _pad_to(P["cond_b"], ss_all.shape[1])
+        add(lambda: ops.conv_gemm(cond_bf, P["cond_w"], ss_all.view(1, ss_all.shape[0], -1), c_in=self.features,
+                                  n_valid=ss_all.shape[1], bias=cond_bias))
+
+    def _static_io(self, io, B: int, Bh: int, T: int, M: int) -> None:
+        """The input buffers of a plan, set on `io`: x [B, x channels, T] and append (fp32, as the
+        caller passes them), the embedding tokens [Bh, M, embedding_features] (M = 0: None) and the
+        InjectChannelsItem context of each depth d, ctx[d] [Bh, T_d, channels padded to 16] (both in
+        the activation dtype)."""
+        dev, adt = self.net.down.weight.device, self._act_dtype()
+        io.x = torch.zeros(B, self.x_channels, T, device=dev)
+        io.append = torch.zeros(B, self.append_channels, T, device=dev) if self.append_channels else None
+        io.embedding = torch.zeros(Bh, M, self.embedding_features, dtype=adt, device=dev) if M else None
+        io.ctx = {i: torch.zeros(Bh, T // _prod(self.factors[:i + 1]), ops.round_up(c, 16), dtype=adt, device=dev)
+                  for i, c in enumerate(self.context_channels) if c > 0}
 
     def _cond_table(self, sigmas: Tensor, features_in: Optional[Tensor]) -> Tensor:
         """ss_all for every row of `sigmas` [R] in one pass (the 97 MB of conditioning weights of
         the README network are read once per sample() call instead of once per step)."""
         R = sigmas.shape[0]
         key = ("cond", R)
-        self.packed()
+        P = self.packed()
         if not self.use_modulation:       # nothing to evaluate: a dummy table keeps the step selector uniform
             plan = self._plans.get(key)
             if plan is None:
                 plan = self._plans[key] = _Plan()
-                plan.ss_all = torch.zeros(R, 8, device=sigmas.device)
+                plan.ss_all = self._ss_all(P, R)
             return plan.ss_all
         plan = self._plans.get(key)
         if plan is None:
@@ -976,7 +1046,7 @@ class B200UNet(nn.Module):
             plan = _Plan()
             plan.sigma = torch.zeros(R, device=sigmas.device)
             plan.features_in = torch.zeros(R, self.features, device=sigmas.device)
-            plan.ss_all = self._add_conditioning(plan, self.packed(), R)
+            plan.ss_all = self._add_conditioning(plan, P, R)
             self._plans[key] = plan
         plan.sigma.copy_(sigmas)
         plan.use_features_in = features_in is not None
@@ -992,31 +1062,22 @@ class B200UNet(nn.Module):
         dev = self.net.down.weight.device
         P = self.packed()
         plan = _Plan()
-        G, Fm = self.groups, self.features
         levels = self.levels()
-        total_f = 1
-        for lv in levels:
-            total_f *= lv.factor
+        total_f = _prod(self.factors)
         assert T % total_f == 0, f"length {T} must be divisible by the product of factors {total_f}"
 
         # ---- static I/O
-        plan.x = torch.zeros(B, self.x_channels, T, device=dev)
-        plan.append = torch.zeros(B, self.append_channels, T, device=dev) if self.append_channels else None
+        self._static_io(plan, B, Bh, T, M)
         plan.sigma = torch.zeros(Bh, device=dev)
-        plan.features_in = torch.zeros(Bh, Fm, device=dev)
+        plan.features_in = torch.zeros(Bh, self.features, device=dev)
         plan.v = torch.zeros(B, self.out_channels, T, device=dev)
         plan.ab = torch.zeros(4, device=dev)
-        adt = self._act_dtype()
-        plan.embedding = torch.zeros(Bh, M, self.embedding_features, dtype=adt, device=dev) if M else None
         plan.cfg_scale = None
-        plan.ctx = {i: torch.zeros(Bh, (T // _prod(self.factors[:i + 1])), ops.round_up(c, 16),
-                                   dtype=adt, device=dev)
-                    for i, c in enumerate(self.context_channels) if c > 0}
         plan.pre = []                        # step-invariant launches of a sampling plan
 
         # ---- statistics arena (zeroed once per forward)
         n_slots = 2 + sum(3 * (len(lv.items_down) + len(lv.items_up)) + 3 for lv in levels)
-        arena = torch.zeros(n_slots, Bh, G, 2, dtype=torch.float64, device=dev)
+        arena = torch.zeros(n_slots, Bh, self.groups, 2, dtype=torch.float64, device=dev)
         if mode == "sample":
             # the step's conditioning rows and alpha/beta are picked ON THE DEVICE from tables by a
             # step counter, so the captured graph is identical for every step (the host only
@@ -1031,64 +1092,22 @@ class B200UNet(nn.Module):
         # The sampler knows every sigma_i up front and evaluates this ONCE for all steps
         # (_cond_table): its plan only receives the step's rows of the table.
         if mode == "sample":
-            ss_all = torch.zeros(Bh, max(8, ops.round_up(P["cond_n"], 8)), device=dev)
-            plan.ss_all = ss_all
+            ss_all = plan.ss_all = self._ss_all(P, Bh)
             plan.use_features_in = False
             plan.add(lambda: ops.step_select(plan.step, plan.ctrl, plan.ab_table, plan.ab, ss_all))
         elif self.use_modulation:
             ss_all = self._add_conditioning(plan, P, Bh)
         else:
-            ss_all = torch.zeros(Bh, 8, device=dev)
+            ss_all = self._ss_all(P, Bh)
             plan.use_features_in = False
-        walk = _ForwardWalk(self, P, plan.add, Bh, arena, ss_all, keep=False, ctx=plan.ctx,
-                            embedding=plan.embedding,
+        walk = _ForwardWalk(self, P, plan, plan.add, Bh, arena, ss_all, keep=False,
                             add_ctx=plan.pre.append if mode == "sample" else plan.add)
-        pool = walk.pool
-
-        # ---- recursive level walk
-        def run_level(i: int, x_in: Optional[Tensor], T_in: int) -> Tuple[Tensor, Optional[Tensor]]:
-            """Returns the level's output [Bh, T_in, out_ch] (+ its stats) for i >= 1 and the
-            output of level 0's item chain (the input of stem_out) for i = 0."""
-            lv, Lp = levels[i], P["levels"][i]
-            Tl = T_in // lv.factor
-            innermost = i == len(levels) - 1
-            if i == 0:
-                x, st = pool.get(Bh, Tl, lv.ch), walk.new_stats()
-                for half in range(Bh // B):
-                    plan.add(lambda half=half, x=x, st=st: ops.stem_in(
-                        plan.x, Lp["down_w"], Lp["down_b"], x[half * B:(half + 1) * B], lv.factor,
-                        append=plan.append, stats=st[half * B:(half + 1) * B], groups=G))
-            else:
-                x, st = walk.down(lv, Lp, x_in, Tl)
-            x, st, _ = walk.items(x, st, Lp["items_down"], lv.ch, Tl, i, last_needs_stats=innermost)
-            if not innermost:
-                skip = x
-                x, st = run_level(i + 1, skip, Tl)
-                pool.put(skip)
-            x, st, _ = walk.items(x, st, Lp["items_up"], lv.ch, Tl, i, last_needs_stats=False)
-            if i == 0:
-                return x, None
-            out, ost, _ = walk.up_merge(lv, Lp, x, x_in, Tl, T_in)
-            return out, ost
-
-        h0, _ = run_level(0, None, T)
-        lv0, L0 = levels[0], P["levels"][0]
-        # SkipCat (folded into the stem's weights) and SkipAdd run the stem epilogue with a unit gate
-        gate0 = (ss_all[:, L0["gate_off"]:] if self.merge == "modulate"
-                 else torch.ones(Bh, max(8, self.out_channels), device=dev))
-
-        def final():
-            kw = dict(append=plan.append, w_adapt=L0.get("adapt_w"), b_adapt=L0.get("adapt_b"),
-                      cfg_scale=plan.cfg_scale)
-            if mode == "sample":   # v and the VSampler update in one pass; x advanced in place
-                ops.stem_out(h0, plan.x, L0["up_w"], L0["up_b"], gate0, lv0.factor, x_next=plan.x, ab=plan.ab,
-                             **kw)
-            else:
-                ops.stem_out(h0, plan.x, L0["up_w"], L0["up_b"], gate0, lv0.factor, v_out=plan.v, **kw)
-        plan.add(final)
-        if mode == "sample":
+        if mode == "sample":       # v and the VSampler update in one pass; x advanced in place
+            walk.trunk(lambda: dict(x_next=plan.x, ab=plan.ab, cfg_scale=plan.cfg_scale))
             plan.add(lambda: ops.step_advance(plan.step))
-        plan.workspace_bytes = pool.total_bytes
+        else:
+            walk.trunk(lambda: dict(v_out=plan.v, cfg_scale=plan.cfg_scale))
+        plan.workspace_bytes = walk.pool.total_bytes
         return plan
 
     def _plan(self, B: int, T: int, Bh: int, M: int, mode: str, baked: Tuple = ()) -> _Plan:
