@@ -97,6 +97,7 @@ SIGNATURES = {
     "adp_stem_out": [C.POINTER(StemOutArgs), vp],
     "adp_narrow_conv": [C.POINTER(NarrowConvArgs), vp],
     "adp_sampler_step": [vp, vp, vp, vp, C.c_int64, vp],
+    "adp_dpm_step": [vp, vp, vp, vp, vp, i32, C.c_int64, vp],
     "adp_inpaint_blend": [vp, vp, vp, vp, vp, C.c_int64, vp],
     "adp_arv_step": [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp],
     "adp_resample": [vp, vp, vp] + [C.c_int] * 7 + [vp],

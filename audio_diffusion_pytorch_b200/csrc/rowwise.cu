@@ -517,6 +517,63 @@ __global__ void sampler_step_kernel(const float* __restrict__ x, const float* __
   }
 }
 
+// DPM-Solver++(2M) step (DPMSolverSampler), in place on x and on the history h of the previous
+// step's x0.  Row r = min(*step, rows - 1) of `table` holds (alpha_i, beta_i, c1, c2, k):
+//   x0 = alpha_i x - beta_i v,   x = c1 x + c2 ((1 + k) x0 - k h),   h = x0.
+// With k == 0 (first step, last step to sigma = 0, after an infinite log-SNR step) h is not read,
+// so an uninitialised or NaN history cannot reach x.
+constexpr int kDpmRow = 5;
+
+struct DpmCoef { float a, b, c1, c2, k; };
+
+__device__ __forceinline__ float dpm_elem(const DpmCoef& c, bool second, float& xv, float vv, float hv) {
+  const float x0 = c.a * xv - c.b * vv;
+  const float d = second ? (1.f + c.k) * x0 - c.k * hv : x0;
+  xv = c.c1 * xv + c.c2 * d;
+  return x0;
+}
+
+template <bool kVec>
+__global__ void dpm_step_kernel(float* __restrict__ x, const float* __restrict__ v, float* __restrict__ hist,
+                                const float* __restrict__ table, const int* __restrict__ step, int rows,
+                                int64_t n) {
+  pdl_launch_dependents();
+  pdl_wait();
+  int r = *step;
+  r = r < 0 ? 0 : (r < rows ? r : rows - 1);
+  const float* row = table + static_cast<size_t>(r) * kDpmRow;
+  const DpmCoef c{row[0], row[1], row[2], row[3], row[4]};
+  const bool second = c.k != 0.f;
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+  const int64_t tid = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  int64_t done = 0;
+  if (kVec) {
+    const int64_t n4 = n >> 2;
+    float4* x4 = reinterpret_cast<float4*>(x);
+    const float4* v4 = reinterpret_cast<const float4*>(v);
+    float4* h4 = reinterpret_cast<float4*>(hist);
+    for (int64_t i = tid; i < n4; i += stride) {
+      float4 xv = x4[i];
+      const float4 vv = v4[i];
+      const float4 hv = second ? h4[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+      float4 x0;
+      x0.x = dpm_elem(c, second, xv.x, vv.x, hv.x);
+      x0.y = dpm_elem(c, second, xv.y, vv.y, hv.y);
+      x0.z = dpm_elem(c, second, xv.z, vv.z, hv.z);
+      x0.w = dpm_elem(c, second, xv.w, vv.w, hv.w);
+      x4[i] = xv;
+      h4[i] = x0;
+    }
+    done = n4 << 2;
+  }
+  for (int64_t i = done + tid; i < n; i += stride) {
+    float xv = x[i];
+    const float hv = second ? hist[i] : 0.f;
+    hist[i] = dpm_elem(c, second, xv, v[i], hv);
+    x[i] = xv;
+  }
+}
+
 // Per-step inputs of the captured sampling step, selected ON THE DEVICE: the step graph is the same
 // for every step (and several steps can be captured back to back), the host only replays it.
 //   ctrl[0] = address of the conditioning table rows [n][ss_elems] (fp32), ctrl[1] = steps that
@@ -782,6 +839,22 @@ extern "C" int adp_sampler_step(const float* x, const float* v, const float* ab,
   ADP_CHECK(x && v && ab && x_next && n > 0, "adp_sampler_step: bad args");
   ADP_CUDA(launch_k(sampler_step_kernel, dim3(pick_grid(static_cast<size_t>(n), 256 * 4, num_sms() * 8)),
                     dim3(256), (size_t)0, as_stream(stream), x, v, ab, x_next, n));
+  ADP_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int adp_dpm_step(float* x, const float* v, float* hist, const float* table, const int32_t* step,
+                            int32_t rows, int64_t n, adp_stream_t stream) {
+  ADP_CHECK(x && v && hist && table && step && rows > 0 && n > 0, "adp_dpm_step: bad args");
+  const bool vec = ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(v) |
+                     reinterpret_cast<uintptr_t>(hist)) & 15) == 0;
+  const dim3 grid(pick_grid(static_cast<size_t>(vec ? (n + 3) / 4 : n), 256, num_sms() * 8));
+  if (vec)
+    ADP_CUDA(launch_k(dpm_step_kernel<true>, grid, dim3(256), (size_t)0, as_stream(stream), x, v, hist, table,
+                      step, (int)rows, n));
+  else
+    ADP_CUDA(launch_k(dpm_step_kernel<false>, grid, dim3(256), (size_t)0, as_stream(stream), x, v, hist, table,
+                      step, (int)rows, n));
   ADP_LAUNCH_CHECK();
   return 0;
 }

@@ -4,9 +4,10 @@ VDiffusion and VSampler keep the reference constructors and call signatures
 (reference diffusion.py:68-95, :158-190).  When the wrapped net is the CUDA U-Net the
 per-step arithmetic is fused into the net's last kernel and the loop launches one CUDA
 graph per step; with any other `net` the same algebra runs as the generic fused
-`adp_sampler_step` kernel after the net call.
+`adp_sampler_step` kernel after the net call.  DPMSolverSampler (DPM-Solver++(2M)) takes the same
+slot: its update is the `adp_dpm_step` kernel, inside the step graph with the CUDA U-Net.
 """
-from math import pi
+from math import inf, isfinite, log, pi, sin
 from typing import Any, List, Optional, Tuple
 
 import torch
@@ -298,4 +299,102 @@ class VSampler(Sampler):
         for i in progress:
             v = self.net(x, sigmas[i], **kwargs).float().contiguous()             # :184
             ops.sampler_step(x, v, ab[i], x)                                      # :185-187
+        return x.to(x_noisy.dtype)
+
+
+def _log_snr(a: float, b: float) -> float:
+    """lambda = log(alpha / beta): -inf at alpha = 0 (sigma = 1), +inf at beta = 0 (sigma = 0)."""
+    if a <= 0.0:
+        return -inf
+    return inf if b <= 0.0 else log(a) - log(b)
+
+
+def dpm_coefficients(sigmas: Tensor) -> Tensor:
+    """The per-step rows (alpha_i, beta_i, c1, c2, k) of DPM-Solver++(2M) (Lu et al. 2022, Algorithm
+    2) for a schedule sigmas [N + 1] in [0, 1], computed in float64 on the host and returned as fp32
+    [N, 5] on the host.  With alpha = cos(pi sigma / 2), beta = sin(pi sigma / 2) and lambda =
+    log(alpha / beta), step i (sigma_i -> sigma_i+1, h_i = lambda_i+1 - lambda_i) is
+        x0_i = alpha_i x_i - beta_i v_i
+        x_i+1 = c1 x_i + c2 ((1 + k) x0_i - k x0_i-1),   c1 = beta_i+1 / beta_i,   c2 = alpha_i+1 - alpha_i c1
+    with k = h_i / (2 h_i-1), except k = 0 on the first step, on a last step to sigma = 0 (as
+    k-diffusion's sample_dpmpp_2m) and after a step with h = inf.  alpha is evaluated as
+    sin(pi (1 - sigma) / 2), clamped to >= 0, so that it is exactly 0 at sigma = 1: lambda = -inf
+    there and the step from sigma = 1 has h = inf (cos(pi / 2) rounds to 6e-17 instead).  With
+    k = 0 the step is VSampler's."""
+    s = [float(v) for v in sigmas.detach().double().cpu()]
+    a = [max(sin(pi * (1.0 - v) / 2), 0.0) for v in s]
+    b = [sin(pi * v / 2) for v in s]
+    lam = [_log_snr(ai, bi) for ai, bi in zip(a, b)]
+    n = len(s) - 1
+    rows = []
+    h_prev = None
+    for i in range(n):
+        h = lam[i + 1] - lam[i]
+        c1 = b[i + 1] / b[i]
+        k = 0.0
+        if h_prev is not None and isfinite(h_prev) and not (i == n - 1 and s[n] == 0.0):
+            k = h / (2 * h_prev)
+        rows.append([a[i], b[i], c1, a[i + 1] - a[i] * c1, k])
+        h_prev = h
+    return torch.tensor(rows, dtype=torch.float64).float()
+
+
+def _dpm_step(x: Tensor, v: Tensor, hist: Tensor, table: Tensor, step: Tensor, rows: int) -> None:
+    """One DPM-Solver++(2M) update (adp_dpm_step), in place on x and hist: the coefficients are row
+    min(step[0], rows - 1) of table [rows, 5] (dpm_coefficients), step a device int32 counter."""
+    ops._launch("adp_dpm_step", (x.data_ptr(), v.data_ptr(), hist.data_ptr(), table.data_ptr(),
+                                 step.data_ptr(), rows, x.numel()),
+                lambda: ("dpm_step", 0, ops._nb(x, v, hist, x, hist)))
+
+
+def _check_schedule(sigmas: Tensor) -> None:
+    s = sigmas.detach().double().cpu()
+    if s.numel() < 2 or not bool(torch.all(s[1:] < s[:-1])):
+        raise ValueError(f"DPMSolverSampler: the schedule must be strictly decreasing (got {s.tolist()})")
+    if not bool(torch.all((s >= 0) & (s <= 1))):
+        raise ValueError(f"DPMSolverSampler: the schedule leaves [0, 1] (got {s.tolist()})")
+
+
+class DPMSolverSampler(Sampler):
+    """Second-order multistep sampling of v-diffusion: DPM-Solver++(2M) (Lu et al. 2022, Algorithm
+    2; the edge steps of k-diffusion's sample_dpmpp_2m), one net evaluation per step like VSampler
+    and the same call.  The update (dpm_coefficients) runs as adp_dpm_step after the net: with the
+    CUDA U-Net inside its sampling step graph (B200UNet.dpm_loop), with any other net after
+    `net(x, sigma_i)`.  For num_steps <= 2 on a schedule from 1 to 0 it is VSampler's update."""
+
+    diffusion_types = [VDiffusion]
+
+    def __init__(self, net: nn.Module, schedule: Schedule = LinearSchedule()):
+        super().__init__()
+        self.net = net
+        self.schedule = schedule
+
+    def get_alpha_beta(self, sigmas: Tensor) -> Tuple[Tensor, Tensor]:
+        return _alpha_beta(sigmas)
+
+    @torch.no_grad()
+    def forward(self, x_noisy: Tensor, num_steps: int, show_progress: bool = False,
+                **kwargs) -> Tensor:
+        b, c = x_noisy.shape[0], x_noisy.shape[1]
+        out_channels = getattr(self.net, "out_channels", c)
+        if out_channels != c:
+            raise ValueError(f"DPMSolverSampler: the net's out_channels={out_channels} differs from the {c} "
+                             f"channels of x (the update needs v of x's shape)")
+        sigmas_1d = self.schedule(num_steps + 1, device=x_noisy.device)
+        _check_schedule(sigmas_1d)
+        sigmas = sigmas_1d[:, None].expand(-1, b)
+        coef = dpm_coefficients(sigmas_1d).to(x_noisy.device)
+        progress = _progress("Sampling", num_steps, sigmas_1d.tolist() if show_progress else None)
+        net = _inner_b200(self.net)
+        if net is not None:
+            return net.dpm_loop(x_noisy, sigmas, coef, progress=progress if show_progress else None, **kwargs)
+        x = x_noisy.float().contiguous().clone()
+        hist = torch.empty_like(x)
+        step = torch.zeros(1, dtype=torch.int32, device=x.device)
+        for i in progress:
+            v = self.net(x, sigmas[i], **kwargs).float().contiguous()
+            if v.shape != x.shape:
+                raise ValueError(f"DPMSolverSampler: the net returned {tuple(v.shape)} for x of shape "
+                                 f"{tuple(x.shape)} (the update needs v of x's shape)")
+            _dpm_step(x, v, hist, coef[i:], step, num_steps - i)
         return x.to(x_noisy.dtype)

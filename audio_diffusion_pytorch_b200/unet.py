@@ -1058,7 +1058,9 @@ class B200UNet(nn.Module):
     # --------------------------------------------------------------------- plan
     def _build_plan(self, B: int, T: int, Bh: int, M: int, mode: str) -> _Plan:
         """B = batch of x; Bh = rows the trunk runs (2B under classifier-free guidance);
-        M = embedding tokens (0 if none); mode in {'v', 'sample'}."""
+        M = embedding tokens (0 if none); mode in {'v', 'sample', 'sample_dpm'}.  'sample_dpm' is the
+        'sample' plan with stem_out writing v and the DPM-Solver++(2M) update (adp_dpm_step, on
+        x, a history buffer and a coefficient table picked by the step counter) before step_advance."""
         dev = self.net.down.weight.device
         P = self.packed()
         plan = _Plan()
@@ -1078,7 +1080,8 @@ class B200UNet(nn.Module):
         # ---- statistics arena (zeroed once per forward)
         n_slots = 2 + sum(3 * (len(lv.items_down) + len(lv.items_up)) + 3 for lv in levels)
         arena = torch.zeros(n_slots, Bh, self.groups, 2, dtype=torch.float64, device=dev)
-        if mode == "sample":
+        sampling = mode in ("sample", "sample_dpm")
+        if sampling:
             # the step's conditioning rows and alpha/beta are picked ON THE DEVICE from tables by a
             # step counter, so the captured graph is identical for every step (the host only
             # replays it, and several steps are captured back to back: _execute_steps)
@@ -1086,12 +1089,16 @@ class B200UNet(nn.Module):
             plan.ctrl = torch.zeros(3, dtype=torch.int64, device=dev)
             plan.ab_table = torch.zeros(self.max_table_steps, 4, device=dev)
             plan.multi_graph, plan.multi_steps = None, 0
+        if mode == "sample_dpm":
+            from . import diffusion
+            plan.dpm_table = torch.zeros(self.max_table_steps, 5, device=dev)
+            plan.hist = torch.zeros_like(plan.x)          # x0 of the previous step
         plan.add(lambda: arena.zero_())
 
         # ---- conditioning: f = MLP(GELU(embed(sigma))) (+features); ss = W_all SiLU(f) + b.
         # The sampler knows every sigma_i up front and evaluates this ONCE for all steps
         # (_cond_table): its plan only receives the step's rows of the table.
-        if mode == "sample":
+        if sampling:
             ss_all = plan.ss_all = self._ss_all(P, Bh)
             plan.use_features_in = False
             plan.add(lambda: ops.step_select(plan.step, plan.ctrl, plan.ab_table, plan.ab, ss_all))
@@ -1101,9 +1108,14 @@ class B200UNet(nn.Module):
             ss_all = self._ss_all(P, Bh)
             plan.use_features_in = False
         walk = _ForwardWalk(self, P, plan, plan.add, Bh, arena, ss_all, keep=False,
-                            add_ctx=plan.pre.append if mode == "sample" else plan.add)
+                            add_ctx=plan.pre.append if sampling else plan.add)
         if mode == "sample":       # v and the VSampler update in one pass; x advanced in place
             walk.trunk(lambda: dict(x_next=plan.x, ab=plan.ab, cfg_scale=plan.cfg_scale))
+            plan.add(lambda: ops.step_advance(plan.step))
+        elif mode == "sample_dpm":
+            walk.trunk(lambda: dict(v_out=plan.v, cfg_scale=plan.cfg_scale))
+            plan.add(lambda: diffusion._dpm_step(plan.x, plan.v, plan.hist, plan.dpm_table, plan.step,
+                                                 plan.dpm_table.shape[0]))
             plan.add(lambda: ops.step_advance(plan.step))
         else:
             walk.trunk(lambda: dict(v_out=plan.v, cfg_scale=plan.cfg_scale))
@@ -1164,11 +1176,15 @@ class B200UNet(nn.Module):
                 self._execute(plan)
                 n -= 1
 
-    def _set_step_tables(self, plan: _Plan, table: Tensor, ab_rows: Tensor, share: int = 1) -> None:
+    def _set_step_tables(self, plan: _Plan, table: Tensor, ab_rows: Tensor, share: int = 1,
+                         dpm_rows: Optional[Tensor] = None) -> None:
         """Points the plan's step selector at a block of conditioning rows [n, Bh, stride] and its
-        alpha/beta rows [n_iterations, 4]; resets the device step counter."""
+        alpha/beta rows [n_iterations, 4] (and a 'sample_dpm' plan's update at its coefficient rows
+        [n_iterations, 5]); resets the device step counter."""
         assert ab_rows.shape[0] <= plan.ab_table.shape[0], "too many iterations per conditioning block"
         plan.ab_table[: ab_rows.shape[0]].copy_(ab_rows, non_blocking=True)
+        if dpm_rows is not None:
+            plan.dpm_table[: dpm_rows.shape[0]].copy_(dpm_rows, non_blocking=True)
         plan.ctrl.copy_(torch.tensor([table.data_ptr(), share, table.shape[0]], dtype=torch.int64),
                         non_blocking=True)
         plan.step.zero_()
@@ -1266,9 +1282,10 @@ class B200UNet(nn.Module):
         return plan
 
     def _table_steps(self, plan: _Plan, sigmas: Tensor, ab_rows: Tensor, share: int, progress,
-                     each: Optional[Callable[[], None]] = None) -> None:
+                     each: Optional[Callable[[], None]] = None, dpm_rows: Optional[Tensor] = None) -> None:
         """The steps of a 'sample' plan from sigmas [N+1, B]: `share` evaluations per step, each
-        followed by each(); ab_rows [N * share, 4] holds every evaluation's alpha/beta.  The
+        followed by each(); ab_rows [N * share, 4] holds every evaluation's alpha/beta (dpm_rows
+        [N, 5] a 'sample_dpm' plan's update coefficients, re-based per block like ab_rows).  The
         conditioning table is evaluated in blocks of <= ~4096 rows (190 KB of fp32 per row for the
         README net); inside a block the device picks each step's rows: graph launches only, no host
         sync.  Without a progress iterator and each(), _execute_steps runs a block's steps."""
@@ -1281,7 +1298,8 @@ class B200UNet(nn.Module):
             n = min(block, num_steps - first)
             feats = plan.features_in.repeat(n, 1) if plan.use_features_in else None
             table = self._cond_table(sig[first:first + n].reshape(-1), feats).view(n, Bh, -1)
-            self._set_step_tables(plan, table, ab_rows[first * share:(first + n) * share], share)
+            self._set_step_tables(plan, table, ab_rows[first * share:(first + n) * share], share,
+                                  None if dpm_rows is None else dpm_rows[first:first + n])
             if progress is None and each is None:
                 self._execute_steps(plan, n)
                 continue
@@ -1302,6 +1320,18 @@ class B200UNet(nn.Module):
         plan = self._prelude(x_noisy, "sample", sigmas[0], **kwargs)
         ab = torch.stack([alphas[:-1], betas[:-1], alphas[1:], betas[1:]], dim=1).float().contiguous()
         self._table_steps(plan, sigmas, ab, 1, progress)
+        return plan.x.clone().to(x_noisy.dtype)
+
+    @torch.no_grad()
+    def dpm_loop(self, x_noisy: Tensor, sigmas: Tensor, coefficients: Tensor, progress=None, **kwargs) -> Tensor:
+        """DPMSolverSampler's loop: per step one graph launch of the 'sample_dpm' plan (the net's v,
+        then adp_dpm_step on x and the history with row i of `coefficients` [N, 5], from
+        diffusion.dpm_coefficients), no host sync inside the loop."""
+        assert self.out_channels == self.x_channels, \
+            f"out_channels={self.out_channels} differs from the {self.x_channels} channels of x"
+        plan = self._prelude(x_noisy, "sample_dpm", sigmas[0], **kwargs)
+        unused_ab = torch.zeros(coefficients.shape[0], 4, device=plan.x.device)   # stem_out writes v: plan.ab is not read
+        self._table_steps(plan, sigmas, unused_ab, 1, progress, dpm_rows=coefficients)
         return plan.x.clone().to(x_noisy.dtype)
 
     @torch.no_grad()

@@ -236,6 +236,14 @@ int adp_silu_bf16(const float* x, void* y, int64_t n, adp_stream_t stream);
 int adp_sampler_step(const float* x, const float* v, const float* ab, float* x_next, int64_t n,
                      adp_stream_t stream);
 
+/* DPM-Solver++(2M) step (DPMSolverSampler), in place, fp32 [n] each.  Row r = min(step[0], rows - 1)
+ * of table fp32 [rows][5] holds (alpha_i, beta_i, c1, c2, k):
+ *   x0 = alpha_i*x - beta_i*v,   x = c1*x + c2*((1 + k)*x0 - k*hist),   hist = x0.
+ * With k == 0 hist is not read (it may hold anything, NaN included).  step is the device step
+ * counter of adp_step_select, so one captured graph serves every step. */
+int adp_dpm_step(float* x, const float* v, float* hist, const float* table, const int32_t* step,
+                 int32_t rows, int64_t n, adp_stream_t stream);
+
 /* The sampling loop's per-step inputs selected on the device (reference diffusion.py:183-187 indexes
  * sigmas[i], alphas[i], betas[i] on the host): step[0] = iterations done since the host reset it,
  * ctrl[0] = device address of the conditioning table rows fp32 [n][ss_elems], ctrl[1] = iterations
